@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — Mpps of the subscriber-dataplane hot path on B200 (BASELINE.json metric).
+"""bench.py — Mpps of the subscriber-dataplane hot path on H100 (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--workload pipeline_imix] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--workload pipeline_imix] [--impl reference] [--dump-outputs DIR]
 
 A *step* is one batch of 2^22 synthetic frames per GPU through the program of
 the chosen workload (default: the full pipeline antispoof -> NAT44 -> QoS on
@@ -11,6 +11,8 @@ whole-job Mpps with frames resident in HBM when the timed region starts
 metric through the C-ABI call with pinned HOST buffers, host<->device copies
 inside the timed region.  `--impl reference` times the reference's own eBPF C
 (oracle/_ref, or the port where that library is absent) on the host cores.
+`--dump-outputs DIR` writes what the last timed step of the headline computed
+(dump_outputs) so that two builds can be compared output for output.
 Prints ONE JSON line.
 """
 from __future__ import annotations
@@ -37,7 +39,7 @@ def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not a measured peak"
 
 
 # ---------------------------------------------------------------------------
@@ -279,13 +281,41 @@ def _traffic(name, kernel, world, reference_capacities):
     The capture is of ONE configuration (N = 1, workload-sized tables): any other run reports null."""
     tp = os.path.join(ROOT, "profiles", "ncu_traffic.json")
     if not os.path.exists(tp) or world != 1 or reference_capacities:
-        return None, "not captured for this configuration (profiles/ncu_traffic.json holds the N=1 workload-sized run)"
+        return None, "no ncu capture stored for this configuration (profiles/ncu_traffic.json, N = 1, workload-sized tables)"
     ent = json.load(open(tp)).get(name, {}).get(kernel)
     if ent is None:
         return None, "no capture of this kernel"
     if isinstance(ent, dict):
         return ent.get("bytes"), ent.get("source")
     return ent, "profiles/ncu_traffic.json"
+
+
+DUMP_MAX_FRAMES = 1 << 22   # verdict.npy and len.npy: 16 MiB each in float32
+DUMP_HEADER_BYTES = 24 << 20  # headers.npy: a seeded sample of rows of rewritten header bytes
+
+
+def dump_outputs(out_dir, arena_d, len_d, verdict_d, off_d, stride, hw):
+    """What one bng_prog_run call hands back to its caller, as float32 .npy files: the verdict and the (possibly
+    rewritten) length of every frame and the first `hw` bytes of every frame after the program rewrote them.  Batches
+    above DUMP_MAX_FRAMES and the header bytes are sampled with a fixed seed (index.npy / header_index.npy name the
+    frames), so the files stay under 64 MB and two runs with the same arguments dump the same frames."""
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    n = int(verdict_d.numel())
+    rng = np.random.default_rng(0x5EED)
+    idx = np.arange(n) if n <= DUMP_MAX_FRAMES else np.sort(rng.choice(n, DUMP_MAX_FRAMES, replace=False))
+    rows = np.sort(rng.choice(idx, min(idx.size, DUMP_HEADER_BYTES // (4 * hw)), replace=False))
+    dev = arena_d.device
+    rows_d = torch.from_numpy(rows).to(dev)
+    start = off_d[rows_d].long() * 16 if off_d is not None else rows_d * stride
+    headers = arena_d[start[:, None] + torch.arange(hw, device=dev)[None, :]]
+    idx_d = torch.from_numpy(idx).to(dev)
+    out = {"verdict": verdict_d[idx_d], "len": len_d[idx_d], "headers": headers}
+    for name, t in out.items():
+        np.save(os.path.join(out_dir, name + ".npy"), t.cpu().numpy().astype(np.float32))
+    np.save(os.path.join(out_dir, "header_index.npy"), rows.astype(np.float64))
+    if idx.size < n:
+        np.save(os.path.join(out_dir, "index.npy"), idx.astype(np.float64))
 
 
 def measure(a, name, frames, steps, warmup, *, wl=None, reference_capacities=False, subs_scale=1, keep=False):
@@ -378,6 +408,9 @@ def measure(a, name, frames, steps, warmup, *, wl=None, reference_capacities=Fal
         evs.append((e0, e1))
     dp.sync()
     torch.cuda.synchronize()
+    if keep and a.dump_outputs:
+        out_dir = a.dump_outputs if world == 1 else os.path.join(a.dump_outputs, f"rank{rank}")
+        dump_outputs(out_dir, arena_d, len_d, verdict_d, off_d, stride, hw)
     launches = dp.launch_count - launches0
     step_ms = [e0.elapsed_time(e1) for e0, e1 in evs]
     tmax = torch.tensor([sum(step_ms)], dtype=torch.float64, device=dev)
@@ -748,6 +781,8 @@ def main():
                     help="diagnostic: run ONE GPU as shard R of an N-GPU job (its subscribers, its frames) without the other ranks")
     ap.add_argument("--no-extra", action="store_true",
                     help="only the headline: skip the reference-capacities variant, the per-GPU-constant variant and the other configs")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the verdicts, lengths and rewritten headers of the headline's last timed step to DIR/*.npy")
     a = ap.parse_args()
     a.warmup = max(a.warmup, 3) if a.impl == "ours" else a.warmup
     if a.as_shard:

@@ -1,4 +1,4 @@
-"""bng_b200 — B200-native subscriber dataplane (antispoof, NAT44, QoS, DHCP fast path).
+"""bng_b200 — H100-native subscriber dataplane (antispoof, NAT44, QoS, DHCP fast path).
 
 The product is ``libbng_b200.so`` (C ABI in ``include/bng_b200.h``);
 :class:`Dataplane` is its ctypes binding.  Importing this package never

@@ -1,6 +1,6 @@
 // bng_b200 — device-side building blocks shared by every kernel:
 // table descriptors, the open-addressing hash, packet access, statistics and
-// event staging.  sm_100a only; no host fallback exists for anything here.
+// event staging.  sm_90a only; no host fallback exists for anything here.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -77,7 +77,7 @@ struct Tbl {
 // nat_sessions slots are 128 B, laid out by what the per-frame paths touch (DESIGN.md §4):
 //   sector 0 [0,32)   key 16 | nat_ip 4 | nat_port 2 | epoch 2 | out_lo 8
 //            everything an upstream HIT needs — probe, translation and the out-direction counters — is
-//            ONE 32-byte sector: one 256-bit load plus one 64-bit atomic on the same sector.
+//            ONE 32-byte sector: one 32-byte load plus one 64-bit atomic on the same sector.
 //   sector 1 [32,64)  last_seen 8 | orig_ip 4 | state word 4 | orig_port 2 | pad 6 | in_lo 8
 //            what a downstream hit adds (original tuple, TCP state, in-direction counters), and last_seen.
 //   sector 2 [64,96)  out_hi 8 | in_hi 8 | created 8 | dest_ip 4 | dest_port 2 | _pad1 2   (creation / carries / ABI)
@@ -401,8 +401,7 @@ __device__ __forceinline__ bool tbl_evict_near(const Tbl &t, u32 home, u64 *stat
 // The state words of PROBE_W consecutive slots are requested together: in a table that lives in DRAM every probe
 // step is a full memory round trip, and the longest chain among a warp's 32 lanes (3-4 steps at load 0.25) costs
 // that many round trips per lookup.  Every speculative slot is a 64-byte DRAM burst, though, and the cold-start
-// kernel moves 46 G bursts/s — the part's scattered-access limit: 4 slots per step measured 0.637 ms per 2^20 new
-// flows, 2 slots 0.567, 1 slot 0.574 (profiles/r02_notes.md).
+// kernel is bound by the rate of scattered DRAM bursts, so the window stays narrow (-DPROBE_W=1|2|4 to compare).
 #ifndef PROBE_W
 #define PROBE_W 2
 #endif
@@ -490,8 +489,8 @@ __device__ __forceinline__ void tbl_unreserve(const Tbl &t, u32 n) {
 
 // tbl_find for code that goes on for hundreds of instructions after the lookup: the lanes that entered together
 // leave together (lanes whose probe ended wait for the longest chain), so what follows runs once for the warp, not
-// once per distinct chain length — without it the compiler's tail duplication made dhcp_fastpath execute its body
-// 2.4 times per warp with 13 lanes active (ncu source view, profiles/r02_notes.md).  Read-only tables.
+// once per distinct chain length — without it the compiler's tail duplication can make dhcp_fastpath execute its
+// body several times per warp with few lanes active.  Read-only tables.
 template <int KW>
 __device__ __forceinline__ const u8 *tbl_find_conv(const Tbl &t, const u64 *k) {
     const unsigned m = __activemask();
@@ -741,15 +740,16 @@ __device__ __forceinline__ void hdr_store_chunk(const Hdr64 &h, u8 *p, int c) {
     *(uint4 *)(p + c * 16) = make_uint4(h.w[4 * c], h.w[4 * c + 1], h.w[4 * c + 2], h.w[4 * c + 3]);
 }
 
-// 256-bit global accesses (sm_100: LDG/STG.E.ENL2.256).  One instruction moves a whole 32-byte sector per
-// lane; the per-frame kernels are bound by the number of divergent memory instructions they issue
-// (l1tex wavefronts), so a sector is never fetched piecemeal.  p must be 32-byte aligned.
+// 32-byte global accesses: one whole sector per lane, issued as two back-to-back 128-bit accesses (the
+// widest global load/store sm_90 has: LDG/STG.E.128).  Both halves are issued before either result is
+// used, so a sector costs one round trip and is never fetched piecemeal across dependent loads.
+// p must be 32-byte aligned.
 struct __align__(16) U256 {
     u32 w[8];
 };
-// L2 eviction priority of a 256-bit access (sm_100: LDG/STG.E.{EN,EF,EL}L2.256).  Frames stream through once:
-// evict-first keeps them from pushing the flow table's hot sectors (touched ~6 times per batch) out of the
-// 126 MB L2; the flow-table probe asks to stay (evict-last).
+// L2 eviction priority of a 32-byte access (ld/st.global.L2::evict_{first,last}).  Frames stream through
+// once: evict-first keeps them from pushing the flow table's hot sectors (touched ~6 times per batch) out
+// of the 50 MB L2; the flow-table probe asks to stay (evict-last).
 enum { L2_NORMAL = 0, L2_FIRST = 1, L2_LAST = 2 };
 #ifndef FRAME_POLICY
 #define FRAME_POLICY L2_NORMAL
@@ -757,38 +757,45 @@ enum { L2_NORMAL = 0, L2_FIRST = 1, L2_LAST = 2 };
 #ifndef SES_POLICY
 #define SES_POLICY L2_NORMAL
 #endif
+#define BNG_LDG128(HINT, r, q)                                                                                   \
+    asm volatile("ld.global" HINT ".v4.u32 {%0,%1,%2,%3}, [%4];"                                                 \
+                 : "=r"((r)[0]), "=r"((r)[1]), "=r"((r)[2]), "=r"((r)[3])                                        \
+                 : "l"(q)                                                                                        \
+                 : "memory")
+#define BNG_STG128(HINT, q, w)                                                                                   \
+    asm volatile("st.global" HINT ".v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(q), "r"((w)[0]), "r"((w)[1]), "r"((w)[2]), \
+                 "r"((w)[3])                                                                                     \
+                 : "memory")
 template <int POLICY = L2_NORMAL>
 __device__ __forceinline__ U256 ldg256(const void *p) {
     U256 r;
-    if (POLICY == L2_FIRST)
-        asm volatile("ld.global.L2::evict_first.v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                     : "=r"(r.w[0]), "=r"(r.w[1]), "=r"(r.w[2]), "=r"(r.w[3]), "=r"(r.w[4]), "=r"(r.w[5]), "=r"(r.w[6]), "=r"(r.w[7])
-                     : "l"(p)
-                     : "memory");
-    else if (POLICY == L2_LAST)
-        asm volatile("ld.global.L2::evict_last.v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                     : "=r"(r.w[0]), "=r"(r.w[1]), "=r"(r.w[2]), "=r"(r.w[3]), "=r"(r.w[4]), "=r"(r.w[5]), "=r"(r.w[6]), "=r"(r.w[7])
-                     : "l"(p)
-                     : "memory");
-    else
-        asm volatile("ld.global.v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                     : "=r"(r.w[0]), "=r"(r.w[1]), "=r"(r.w[2]), "=r"(r.w[3]), "=r"(r.w[4]), "=r"(r.w[5]), "=r"(r.w[6]), "=r"(r.w[7])
-                     : "l"(p)
-                     : "memory");
+    const u8 *q = (const u8 *)p;
+    if (POLICY == L2_FIRST) {
+        BNG_LDG128(".L2::evict_first", &r.w[0], q);
+        BNG_LDG128(".L2::evict_first", &r.w[4], q + 16);
+    } else if (POLICY == L2_LAST) {
+        BNG_LDG128(".L2::evict_last", &r.w[0], q);
+        BNG_LDG128(".L2::evict_last", &r.w[4], q + 16);
+    } else {
+        BNG_LDG128("", &r.w[0], q);
+        BNG_LDG128("", &r.w[4], q + 16);
+    }
     return r;
 }
 template <int POLICY = L2_NORMAL>
 __device__ __forceinline__ void stg256(void *p, const u32 *w) {
-    if (POLICY == L2_FIRST)
-        asm volatile("st.global.L2::evict_first.v8.u32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3]),
-                     "r"(w[4]), "r"(w[5]), "r"(w[6]), "r"(w[7])
-                     : "memory");
-    else
-        asm volatile("st.global.v8.u32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3]), "r"(w[4]),
-                     "r"(w[5]), "r"(w[6]), "r"(w[7])
-                     : "memory");
+    u8 *q = (u8 *)p;
+    if (POLICY == L2_FIRST) {
+        BNG_STG128(".L2::evict_first", q, &w[0]);
+        BNG_STG128(".L2::evict_first", q + 16, &w[4]);
+    } else {
+        BNG_STG128("", q, &w[0]);
+        BNG_STG128("", q + 16, &w[4]);
+    }
 }
-// Frame header load: two 256-bit loads when the whole warp's frames allow it (32-byte aligned and 64
+#undef BNG_LDG128
+#undef BNG_STG128
+// Frame header load: two 32-byte loads when the whole warp's frames allow it (32-byte aligned and 64
 // bytes inside the arena), 16-byte chunks otherwise.  `wide` must be warp-uniform.
 __device__ __forceinline__ void hdr_load_wide(Hdr64 &h, const u8 *p, u32 len, bool wide) {
     if (wide) {
@@ -840,7 +847,7 @@ __device__ __forceinline__ u16 csum_upd16(u16 csum, u16 old_val, u16 new_val) {
 }
 
 // ---------------------------------------------------------------------------
-// TMA bulk copy of a small global image into shared memory (sm_90+/sm_100a):
+// TMA bulk copy of a small global image into shared memory (sm_90):
 // one thread arms an mbarrier with the byte count and issues cp.async.bulk;
 // everyone waits on the barrier's phase 0.
 // ---------------------------------------------------------------------------

@@ -396,8 +396,7 @@ uint32_t bng_shard_of_mac(uint64_t mac_key, uint32_t world) {
 // Pinned, GPU-mapped host memory for frame arenas (BNG_MEM_HOST batches are then read in place, zero-copy).
 // The arena is backed by 2 MB transparent huge pages and registered with cudaHostRegister: behind an IOMMU in
 // translated mode the GPU's scattered 64-byte header reads cost one translation per page touched, and a
-// receive ring in 4 KB pages thrashes the IOTLB (measured on the bench box: 228 -> 289 Mpps end to end for
-// IMIX frames, 207 -> 397 Mpps for the contiguous DMA path).  Falls back to cudaHostAlloc when huge pages or
+// receive ring in 4 KB pages thrashes the IOTLB.  Falls back to cudaHostAlloc when huge pages or
 // registration are not available.  BNG_HOST_ARENA=pinned forces the fallback.
 namespace {
 struct HostArena {
@@ -422,8 +421,8 @@ void *bng_host_alloc(size_t bytes) {
             madvise(p, size, MADV_HUGEPAGE);
 #endif
             for (size_t o = 0; o < size; o += 4096) p[o] = 0; // first touch on the caller's (NUMA-bound) thread
-            // Whether the fault path found free 2 MB pages is luck (the same process was seen with one arena in huge
-            // pages and the next in 4 KB pages: 320 vs 65 Mpps end to end).  MADV_COLLAPSE (Linux 6.1+) collapses
+            // Whether the fault path found free 2 MB pages is luck (the same process can get one arena in huge
+            // pages and the next in 4 KB pages).  MADV_COLLAPSE (Linux 6.1+) collapses
             // the range synchronously, compacting memory if it has to; best effort, errors ignored.
 #ifndef MADV_COLLAPSE
 #define MADV_COLLAPSE 25
@@ -538,8 +537,8 @@ bng_ctx *bng_open(const bng_open_opts *o) {
     OPEN_CU(cudaSetDevice(dev));
     cudaDeviceProp prop;
     OPEN_CU(cudaGetDeviceProperties(&prop, dev));
-    if (prop.major < 10) {
-        fail(nullptr, 0, "device %d is sm_%d%d; this library is built for sm_100a (B200) only", dev, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0) { // sm_90a code runs on compute capability 9.0 alone
+        fail(nullptr, 0, "device %d is sm_%d%d; this library is built for sm_90a (H100) only", dev, prop.major, prop.minor);
         bng_close(c);
         return nullptr;
     }
@@ -1023,8 +1022,8 @@ static int run_host_zero_copy(bng_ctx *c, int prog, bng_batch *bb, u8 *arena_dev
     const bool contiguous = !bb->off16 && bb->stride <= hb_need;
     const u32 hb = contiguous ? bb->stride : hb_need;         // compact slot stride
     // The TC programs write below byte 16 only in flagged frames (ihl = 0), but the first 16 bytes are written back
-    // all the same: ONE 64-byte PCIe write per frame is cheaper than a 16- and a 32-byte one (338 -> 355 Mpps end to
-    // end; what the link counts is TLPs, not bytes).  BNG_ZC_SKIP_CH0=1 restores the 48-byte write-back for A/B runs.
+    // all the same: ONE 64-byte PCIe write per frame rather than a 16- and a 32-byte one (what the link counts is
+    // TLPs, not bytes).  BNG_ZC_SKIP_CH0=1 restores the 48-byte write-back for A/B runs.
     static const bool skip_ch0 = getenv("BNG_ZC_SKIP_CH0") != nullptr;
     const u32 first_chunk = (tc && skip_ch0) ? 1u : 0u;
     if (!c->s_in) {

@@ -273,8 +273,8 @@ __device__ __forceinline__ int dhcp_one(const DevCtx &c, BlockStats &bs, u8 *p, 
     return XDP_TX_;
 }
 
-// Tile kernel (one mbarrier per block; per-thread barriers without any block-wide synchronisation were measured
-// in round 2 and are SLOWER: 1.19 vs 0.96 ms per 2^22 requests): a request is up to ~350 bytes that the program reads sparsely and rewrites almost
+// Tile kernel (one mbarrier per block rather than per-thread barriers without any block-wide synchronisation): a
+// request is up to ~350 bytes that the program reads sparsely and rewrites almost
 // entirely (L2 headers, BOOTP fixed part, 192 zeroed bytes, options), so frames are staged through
 // shared memory with the TMA: every thread bulk-copies its frame (cp.async.bulk, completion on an
 // mbarrier), runs the program on the shared-memory copy, and bulk-stores it back.  HBM sees two
@@ -287,8 +287,8 @@ __device__ __forceinline__ int dhcp_one(const DevCtx &c, BlockStats &bs, u8 *p, 
 
 // DHCP_TILE_TMA: in a fixed-stride arena (a receive ring: what a NIC fills) the 128 frames of a tile are one
 // contiguous run, so the whole tile moves with ONE bulk copy each way instead of one per frame — the per-frame
-// version issues 2 x 2^22 TMA operations per batch, ~32 cycles apart on every SM, and that, not HBM, is what
-// bounded it (double-buffering the per-frame copies made it slower, 0.97 -> 1.43 ms: profiles/r02_notes.md).
+// version issues 2 x 2^22 TMA operations per batch, a few dozen cycles apart on every SM, and that, not HBM,
+// bounds it.
 #ifndef DHCP_TILE_TMA
 #define DHCP_TILE_TMA 1
 #endif
@@ -386,7 +386,7 @@ __global__ void __launch_bounds__(DH_TILE) k_dhcp_fastpath(const __grid_constant
 }
 
 // (A double-buffered variant — two staging slots per thread, the load of tile i+1 issued before the program runs on
-// tile i — was measured in round 2 and dropped: 0.97 -> 1.43 ms per 2^22 requests, profiles/r02_notes.md.)
+// tile i — was tried and dropped: it was slower.)
 
 cudaError_t run_dhcp_fastpath(Launcher &L, const DevCtx &c, const DevBatch &b) {
     const int smem = DH_TILE * DH_SLOT;
@@ -396,7 +396,7 @@ cudaError_t run_dhcp_fastpath(Launcher &L, const DevCtx &c, const DevBatch &b) {
         L.dhcp_smem_set = 1;
     }
     long want = ((long)b.n + DH_TILE - 1) / DH_TILE;
-    long cap = (long)L.num_sms * 4; // 4 x 50 KB of staging per SM
+    long cap = (long)L.num_sms * 4; // 4 x 50 KB of staging per SM (of the 228 KB an H100 SM has)
     int grid = (int)(want < cap ? (want < 1 ? 1 : want) : cap);
     prof_begin(L, "k_dhcp_fastpath");
     k_dhcp_fastpath<<<grid, DH_TILE, smem, L.stream>>>(c, b);

@@ -72,12 +72,10 @@ __global__ void __launch_bounds__(256) k_scatter_frames(u8 *__restrict__ arena, 
     }
 }
 
-// Both kernels are bound by PCIe, not by the SMs: one 256-thread block per SM (600 KB of 16-byte accesses in flight)
-// moves as much as eight did (tools/e2e_chunk_sweep.sh), and leaves the SMs to the program kernels of the chunk in
-// between.  What limits the pipeline is the link itself: alone, the gather of 2^19 IMIX frames takes 0.69-0.82 ms
-// (41-48 GB/s of 64-byte read completions) and the scatter 0.70 ms (36 GB/s of 48-byte writes); together they take
-// 1.4 and 1.0 ms (BNG_ZC_TRACE=1) — the gather's read requests and the scatter's small write TLPs share the upstream
-// direction.  Copy-engine traffic (a header-split ring, moved with cudaMemcpyAsync) overlaps cleanly.
+// Both kernels are bound by PCIe, not by the SMs: one 256-thread block per SM keeps hundreds of KB of 16-byte
+// accesses in flight (tools/e2e_chunk_sweep.sh sweeps the count), and leaves the SMs to the program kernels of the
+// chunk in between.  What limits the pipeline is the link itself (BNG_ZC_TRACE=1 times the stages): the gather's
+// read requests and the scatter's small write TLPs share the upstream direction.  Copy-engine traffic (a header-split ring, moved with cudaMemcpyAsync) overlaps cleanly.
 cudaError_t run_gather_frames(cudaStream_t st, int blocks, const u8 *arena, const u32 *off16, const u32 *len, u32 stride,
                               u32 n, u32 slot, bool tc, u8 *dst, u32 *need) {
     k_gather_frames<<<blocks, 256, 0, st>>>(arena, off16, len, stride, n, slot, tc ? 1u : 0u, dst, need);

@@ -5,7 +5,7 @@
 // order.  Three phases run back to back on the context's stream:
 //   CLASSIFY  one thread per frame over a persistent grid (a multiple of the
 //             SM count).  The first 64 bytes of the frame are held in
-//             registers (2 x 256-bit loads, or 4 x 128-bit for unaligned
+//             registers (2 x 32-byte loads, or 4 x 16-byte for unaligned
 //             frames), the first probe slot of every table the frame may need
 //             is fetched up front as whole 32-byte sectors so the loads are in
 //             flight together, and everything whose effect commutes is
@@ -90,7 +90,7 @@ __global__ void __launch_bounds__(BLOCK, AS_MINB) k_antispoof(const __grid_const
     u32 cfg = *(const u16 *)c.as_config;
     AsCnt cn = {0, 0};
     const u32 lane = threadIdx.x & 31;
-    // warp-uniform trip count: the warp decides together whether its frames allow 256-bit loads
+    // warp-uniform trip count: the warp decides together whether its frames allow 32-byte loads
     for (u32 base = (blockIdx.x * BLOCK + (threadIdx.x & ~31u)) * AS_UNROLL; base < b.n; base += gridDim.x * BLOCK * AS_UNROLL) {
         if (*(volatile u32 *)&sq.n >= 32) spoof_flush(c, sq); // (warp-uniform: the queue is the warp's own)
         Hdr64 h[AS_UNROLL];
@@ -187,7 +187,7 @@ __global__ void __launch_bounds__(BLOCK)
 // ---------------------------------------------------------------------------
 // nat44_ingress, nat44_hairpin_xdp
 // ---------------------------------------------------------------------------
-// Header in registers, whole-sector probes (nat_reverse slot = key + original tuple in one 256-bit load,
+// Header in registers, whole-sector probes (nat_reverse slot = key + original tuple in one 32-byte load,
 // nat_sessions sector 0 = key + translation + last_seen), the TCP state CAS only when the state would
 // change, the rewrite stored back as whole sectors.  Frames with IPv4 options take nat_ingress_one().
 __global__ void __launch_bounds__(BLOCK) k_nat_ingress(const __grid_constant__ DevCtx c, const __grid_constant__ DevBatch b) {

@@ -15,11 +15,9 @@
 // gather-heavy kernel like this one.
 #pragma once
 
-// Resident blocks per SM each instantiation is compiled for (registers: 65536 / (256 x blocks)).  Measured at the
-// end of round 2 for the pipeline instantiations (ms per 2^22 frames): 2 blocks 0.429, 3 blocks 0.355 (78 registers,
-// nothing spilled), 4 blocks 0.363 (64 registers, 24 bytes spilled), 5 blocks 0.44.  3 is 2 % faster; the default
-// stays at 4 because the round's GPU time ran out before the parity suite could be re-run on that build
-// (-DCLASSIFY_BLOCKS=3 is the whole change).
+// Resident blocks per SM each instantiation is compiled for (registers: 65536 / (256 x blocks)).  At 4 blocks the
+// pipeline instantiations get 64 registers and spill a few bytes; at 3 they get 85 and spill nothing.  Which is faster
+// on H100 has not been measured (-DCLASSIFY_BLOCKS=3 is the whole change).
 #ifndef CLASSIFY_BLOCKS
 #define CLASSIFY_BLOCKS 4
 #endif
@@ -29,7 +27,7 @@
 #define CLASSIFY_BPS(AS) ((AS) ? CLASSIFY_BLOCKS : CLASSIFY_BLOCKS_NAT)
 // CLASSIFY_PAIR: fetch the home PAIR of slots of the bindings table / subscriber directory with the first probe
 #ifndef CLASSIFY_PAIR
-#define CLASSIFY_PAIR 0 // measured (profiles/r02_notes.md): the 16 extra registers spill, 0.373 -> 0.425 ms
+#define CLASSIFY_PAIR 0 // the 16 extra registers spill
 #endif
 
 // AS: run antispoof_ingress first; QOS: honour the qos_ingress bucket.  <false,false> is the

@@ -42,7 +42,7 @@ __device__ __forceinline__ void ascnt_flush(BlockStats &bs, const AsCnt &n) { //
     warp_stat_flush(bs, ST_AS_V6_VIOL, v6);
     warp_stat_flush(bs, ST_AS_DROPPED, v4 + v6);
 }
-// ... which bounds the batch: 1023 trips of the persistent grid (148 x 4 x 256 threads) = 155 M frames
+// ... which bounds the batch: 1023 trips of the persistent grid (132 x 4 x 256 threads on an H100 SXM) = 138 M frames
 __device__ __forceinline__ void ascnt_spill(BlockStats &bs, AsCnt &n) { // called once per trip; keeps the 10-bit fields from wrapping
     if (__any_sync(0xffffffffu, ((n.rare & 1023u) | ((n.rare >> 10) & 1023u) | (n.rare >> 20)) >= 1000u)) {
         AsCnt t = n;
@@ -58,7 +58,7 @@ __device__ __forceinline__ void ascnt_spill(BlockStats &bs, AsCnt &n) { // calle
 
 // log_violation(), bpf/antispoof.c:150-175.  A violating frame used to reserve its record with an atomicAdd on the
 // ring's one counter and wait for the answer before its warp could go on: 40 k same-address atomics per 4 M frames
-// at 1 % violations, a quarter of k_antispoof's time (0.114 ms with logging, 0.084 without).  The lanes now drop
+// at 1 % violations, all serialised on one address.  The lanes now drop
 // what the record needs into a queue of their WARP in shared memory, and the warp writes a batch of records at a
 // time — one atomic for the batch, one lane per record, 64-byte records side by side (spoof_flush).  The order of the
 // records in the ring is immaterial: the drain sorts by (batch, frame).
@@ -74,7 +74,7 @@ __device__ __forceinline__ void spoofq_init(SpoofQ *q) { // q: this block's queu
     __syncwarp();
 }
 // q == nullptr: the record is reserved and written on the spot (the pipeline's classify kernel, where the queue's
-// shared memory and the per-trip check cost more than the 1 % of frames that log gain: 0.363 -> 0.369 ms).
+// shared memory and the per-trip check cost more than the 1 % of frames that log gain).
 __device__ __forceinline__ void spoof_log(const DevCtx &c, SpoofQ *q, AsCnt &cn, u32 idx, u64 now, const Hdr64 &h, u32 spoofed,
                                           u32 allowed_ip, bool v6) {
     // the record is emitted, then packets_logged is bumped whether or not the output succeeded (:171-174)
@@ -132,7 +132,7 @@ __device__ __forceinline__ void spoof_flush(const DevCtx &c, SpoofQ &q) {
 // `bind` is the subscriber_bindings slot of the frame's source MAC (or null),
 // `cfg` = default_mode | log_violations << 8; packets_allowed is counted in the
 // caller's register counter n_allowed (flushed once per thread).
-// A subscriber_bindings slot (32 B: key, then struct subscriber_binding) as one 256-bit load.
+// A subscriber_bindings slot (32 B: key, then struct subscriber_binding) as one 32-byte load.
 struct BindVal {
     bool has;
     U256 s; // w[0..1] key, w[2] ipv4_addr, w[3..6] ipv6_addr, w[7] ipv4_valid | ipv6_valid << 8 | mode << 16
@@ -599,7 +599,7 @@ __device__ __forceinline__ u32 nat_chunk_coop(const DevCtx &c, BlockStats &bs, c
     const bool stamped = b.nowv != nullptr;
     const u32 dlen = frame_dlen(b, len);
     // ---- parse.  The common frame (ihl = 5, classify has already vetted it: not ALG traffic, L4 header in bounds)
-    //      comes in with two 256-bit loads and is rewritten in registers, like classify does; anything else takes
+    //      comes in with two 32-byte loads and is rewritten in registers, like classify does; anything else takes
     //      the byte-wise parse of the sequential code ----
     NatFlow f;
     f.ok = f.alg = false;

@@ -1,4 +1,4 @@
-/* bng_b200 — C ABI of the B200-native subscriber dataplane.
+/* bng_b200 — C ABI of the H100-native subscriber dataplane.
  *
  * This is the drop-in boundary for the reference's eBPF hot path: everything
  * the Go control plane does to the dataplane goes through cilium/ebpf

@@ -91,7 +91,7 @@ def main():
                                                              f"N=1, 2^22 frames, workload-sized tables)"}}
     json.dump(traffic, open(os.path.join(DST, "ncu_traffic.json"), "w"), indent=1)
 
-    L = [f"# Measured on B200 — round {R}", ""]
+    L = [f"# Measured on H100 — round {R}", ""]
     p = os.path.join(DST, f"{R}_bench.json")
     if os.path.exists(p):
         j = json.loads(open(p).readline())

@@ -5,9 +5,13 @@ A *script* is a deterministic list of steps (map commands and batch runs).
 oracle, or the GPU dataplane — and returns everything observable: per-run
 verdicts / rewritten frames / lengths / priorities, return codes of map
 commands, final counters, table contents and event streams.  ``compare``
-asserts two result sets are bit-identical (compiler padding masked).
+asserts two result sets are bit-identical (compiler padding masked);
+``compare_digest`` does the same against a stored ``digest`` of one.
 """
 from __future__ import annotations
+
+import hashlib
+import os
 
 import numpy as np
 
@@ -283,6 +287,39 @@ def compare(a: dict, b: dict, what: str = ""):
     if diffs:
         lines = "\n".join(f"  {k}: {msg}" for k, msg in diffs[:40])
         raise AssertionError(f"{what}: {len(diffs)} result keys differ\n{lines}")
+
+
+def _key_digest(k: str, v) -> int:
+    v = np.ascontiguousarray(v)
+    body = b"" if v.shape[0] == 0 else repr(v.shape).encode() + v.tobytes()  # empty results are equal, as in diff_keys
+    return int.from_bytes(hashlib.sha256(k.encode() + b"\0" + body).digest()[:4], "little")
+
+
+def digest(res: dict) -> np.ndarray:
+    """Compact fingerprint of a result set: a 32-bit SHA-256 prefix of each key's name, shape and bytes, in sorted
+    key order."""
+    return np.array([_key_digest(k, res[k]) for k in sorted(res)], dtype=np.uint32)
+
+
+def compare_digest(stored: np.ndarray, res: dict, what: str = ""):
+    """Asserts that a result set matches a stored digest(); the failure message names every differing key."""
+    got = digest(res)
+    if np.array_equal(got, stored):
+        return
+    keys = sorted(res)
+    if len(keys) != len(stored):
+        raise AssertionError(f"{what}: {len(keys)} result keys, the stored results have {len(stored)}")
+    bad = [k for k, x, y in zip(keys, got, stored) if x != y]
+    raise AssertionError(f"{what}: {len(bad)} result keys differ from the stored results: {bad[:40]}")
+
+
+REFERENCE_DIGESTS = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_digests.npz")
+
+
+def reference_digest(name: str) -> np.ndarray:
+    """The reference oracle's digest() of a corpus, as tests/golden/make_golden.py stored it."""
+    with np.load(REFERENCE_DIGESTS) as z:
+        return z[name]
 
 
 def save_golden(path: str, res: dict):

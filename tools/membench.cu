@@ -1,11 +1,11 @@
 // Micro-benchmark of the access patterns the dataplane kernels are made of, to
-// calibrate what "HBM roofline" means for gather-bound integer work on B200:
+// calibrate what "HBM roofline" means for gather-bound integer work on H100:
 //   seq       coalesced 16 B/thread streaming read                      (copy-like)
 //   hdr       each thread reads G contiguous bytes at a stride of S bytes (frame headers in an IMIX arena)
 //   gather    each thread reads G bytes at R independent pseudo-random slots of a big table
 //   chain     gather with a dependent chain of D steps (probe -> value -> ...)
 //   red       each thread issues atomicAdd(u64) to a pseudo-random slot
-// Prints GB/s of useful bytes and M accesses/s.  Build: nvcc -O3 -gencode arch=compute_100a,code=sm_100a
+// Prints GB/s of useful bytes and M accesses/s.  Build: nvcc -O3 -gencode arch=compute_90a,code=sm_90a
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
