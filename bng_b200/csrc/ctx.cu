@@ -91,6 +91,11 @@ struct bng_ctx {
     u64 staged_total = 0, staged_errors = 0, staged_flushes = 0;
     u64 rebuilds = 0; // flow-table rebuilds (tombstone compaction) so far
     u64 evict_at_rebuild = 0; // ST_LRU_EVICT when the flow tables were last rebuilt
+    // BNG_MEM_DEVICE batches do not synchronise: each one queues a copy of ST_LRU_EVICT into evict_word and records
+    // evict_ev; a later call looks at the copy once the event has completed (poll_compact_locked)
+    u64 *evict_word = nullptr; // pinned
+    cudaEvent_t evict_ev = nullptr;
+    bool evict_pending = false;
     bool small_dirty = false; // a map feeding the SmallTabs image changed since the image was built
     // grow-only scratch of map dumps (no cudaMalloc / cudaFree per call)
     u8 *dump_k = nullptr, *dump_v = nullptr;
@@ -485,6 +490,8 @@ int bng_close(bng_ctx *c) {
         for (void *p : sp)
             if (p) cudaFree(p);
         if (c->io_host) cudaFreeHost(c->io_host);
+        if (c->evict_word) cudaFreeHost(c->evict_word);
+        if (c->evict_ev) cudaEventDestroy(c->evict_ev);
         for (int i = 0; i < ZC_BUFS; i++) {
             void *zp[] = {c->zc_hdr[i], c->zc_verdict[i], c->zc_off[i], c->zc_len[i], c->zc_len0[i], c->zc_prio[i], c->zc_now[i]};
             for (void *p : zp)
@@ -1013,6 +1020,8 @@ static int dispatch(bng_ctx *c, int prog, const DevBatch &b) {
 // program can touch ever cross the bus.
 #define ZC_CHUNK (c->zc_chunk)
 static int maybe_compact_locked(bng_ctx *c);
+static int poll_compact_locked(bng_ctx *c);
+static int queue_evict_read_locked(bng_ctx *c);
 static int run_host_zero_copy(bng_ctx *c, int prog, bng_batch *bb, u8 *arena_dev) {
     // Bytes of a frame a program can touch (hostio.cu): 96 for the TC programs (Ethernet + IPv4 with options + 20
     // bytes of L4), 448 for dhcp_fastpath_prog.  Frames that ARE a fixed slot no larger than that (64-byte
@@ -1148,6 +1157,7 @@ int bng_prog_run(bng_ctx *c, int prog, bng_batch *bb) {
     cudaSetDevice(c->device);
     int r = ensure_scratch(c, bb->n);
     if (r) return r;
+    if ((r = poll_compact_locked(c)) != 0) return r;     // what an earlier device-resident batch left to compact
     if ((r = flush_staged_locked(c, -1)) != 0) return r; // the batch boundary: staged upserts become visible
     if (c->small_dirty && (r = small_refresh_p(c)) != 0) return r; // ... and the shared-memory image of the small maps is rebuilt
     c->dev.batch_seq++;
@@ -1171,7 +1181,9 @@ int bng_prog_run(bng_ctx *c, int prog, bng_batch *bb) {
         b.len = bb->len;
         b.verdict = bb->verdict;
         b.priority = bb->priority;
-        return dispatch(c, prog, b);
+        if ((r = dispatch(c, prog, b)) != 0) return r;
+        // only the programs that create flows evict from the flow tables
+        return (prog == P_NAT_EG || prog == P_PIPE_UP || prog == P_PIPE_TC) ? queue_evict_read_locked(c) : 0;
     }
     if (bb->mem != BNG_MEM_HOST) return -EINVAL;
     {
@@ -1356,19 +1368,46 @@ static int table_rebuild_locked(bng_ctx *c, Tbl *t) {
 }
 
 // Tombstone compaction between batches: every eviction from a full LRU table leaves a tombstone, and a table that
-// churns at capacity runs out of EMPTY slots (every lookup of an absent key then walks the whole table).  Called
-// where the stream is synchronised anyway; rebuilds the three flow tables once the evictions since the last rebuild
-// exceed a quarter of nat_sessions' slots.
-static int maybe_compact_locked(bng_ctx *c) {
-    u64 ev = 0;
-    CU(c, cudaMemcpyAsync(&ev, c->dev.stats + ST_LRU_EVICT, 8, cudaMemcpyDeviceToHost, c->L.stream));
-    CU(c, cudaStreamSynchronize(c->L.stream));
+// churns at capacity runs out of EMPTY slots (every lookup of an absent key then walks the whole table).  Rebuilds
+// the three flow tables once the evictions since the last rebuild exceed a quarter of nat_sessions' slots, given
+// the eviction count `ev` read at some point of the stream after the last rebuild.
+static int compact_if_due_locked(bng_ctx *c, u64 ev) {
     if (ev - c->evict_at_rebuild <= (c->dev.sessions.mask + 1) / 4) return 0;
     c->evict_at_rebuild = ev;
     int r;
     if ((r = table_rebuild_locked(c, &c->dev.sessions)) != 0) return r;
     if ((r = table_rebuild_locked(c, &c->dev.reverse)) != 0) return r;
     return table_rebuild_locked(c, &c->dev.eim);
+}
+
+// Where the stream is synchronised anyway (host-fed batches, bng_sync): the count as of now.
+static int maybe_compact_locked(bng_ctx *c) {
+    u64 ev = 0;
+    CU(c, cudaMemcpyAsync(&ev, c->dev.stats + ST_LRU_EVICT, 8, cudaMemcpyDeviceToHost, c->L.stream));
+    CU(c, cudaStreamSynchronize(c->L.stream));
+    c->evict_pending = false; // (a queued read is older than this one)
+    return compact_if_due_locked(c, ev);
+}
+
+// A BNG_MEM_DEVICE batch returns without synchronising: it queues a copy of the eviction count behind itself, and
+// the next bng_prog_run / bng_sweep applies the rule to it if the copy has landed by then (else a later call does).
+// The steady state costs one 8-byte copy per batch and no host wait; only a rebuild itself synchronises.
+static int queue_evict_read_locked(bng_ctx *c) {
+    if (!c->evict_word) CU(c, cudaHostAlloc((void **)&c->evict_word, 8, cudaHostAllocDefault));
+    if (!c->evict_ev) CU(c, cudaEventCreateWithFlags(&c->evict_ev, cudaEventDisableTiming));
+    CU(c, cudaMemcpyAsync(c->evict_word, c->dev.stats + ST_LRU_EVICT, 8, cudaMemcpyDeviceToHost, c->L.stream));
+    CU(c, cudaEventRecord(c->evict_ev, c->L.stream));
+    c->evict_pending = true;
+    return 0;
+}
+
+static int poll_compact_locked(bng_ctx *c) {
+    if (!c->evict_pending) return 0;
+    const cudaError_t e = cudaEventQuery(c->evict_ev);
+    if (e == cudaErrorNotReady) return 0;
+    c->evict_pending = false;
+    CU(c, e);
+    return compact_if_due_locked(c, *(volatile u64 *)c->evict_word);
 }
 
 // Session expiry sweep (sweep.cu): removes every nat_sessions entry idle for longer than the timeout of its
@@ -1378,8 +1417,9 @@ int bng_sweep(bng_ctx *c, uint64_t now_ns, uint64_t *expired_out) {
     if (!c) return -EINVAL;
     std::lock_guard<std::mutex> g(c->mu);
     cudaSetDevice(c->device);
-    int r = flush_staged_locked(c, -1);
+    int r = poll_compact_locked(c);
     if (r) return r;
+    if ((r = flush_staged_locked(c, -1)) != 0) return r;
     c->dev.batch_seq++;
     c->dev.epoch = c->dev.batch_seq % 65535u + 1;
     if (c->dev.epoch == 1 && c->dev.batch_seq > 1) CU(c, run_epoch_reset(c->L, c->dev.sessions));

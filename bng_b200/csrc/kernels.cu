@@ -651,20 +651,25 @@ static __device__ __noinline__ int nat_egress_seq(const DevCtx &c, BlockStats &b
 __device__ __forceinline__ bool resolve_nat_chunk(const DevCtx &c, const DevBatch &b, BlockStats &bs, u8 *sub, u32 idx, u32 len,
                                                       bool is_miss, bool fresh, u32 mm, u32 lane) {
     NatPend pend;
-    // one nat_log_rb reservation for all new flows of this chunk (every one of them
-    // logs at most one record; a slot left unused is tagged invalid for the drain)
+    // one nat_log_rb reservation for all new flows of this chunk that classify found (every one of them logs at most
+    // one record; a slot left unused is tagged invalid for the drain).  A deferred TC frame has not been looked up
+    // yet and is most often a session hit: it reserves its record when it writes one, so hits cost no staging space.
     const EvRing &r = c.natlog_ev;
-    u32 nrec = __popc(mm), basepos = 0;
-    if (lane == 0) basepos = atomicAdd(r.count, nrec);
-    basepos = __shfl_sync(0xffffffffu, basepos, 0);
-    if (lane == 0 && basepos + nrec > r.cap) { // staging ring full: the tail of the chunk has no slot
-        u32 over = basepos >= r.cap ? nrec : basepos + nrec - r.cap;
-        atomicSub(r.count, over);
-        atomicAdd(&c.stats[r.lost_stat], (u64)over);
+    const u32 pre = __ballot_sync(0xffffffffu, is_miss && !fresh);
+    u32 nrec = __popc(pre), basepos = 0;
+    if (nrec) {
+        if (lane == 0) basepos = atomicAdd(r.count, nrec);
+        basepos = __shfl_sync(0xffffffffu, basepos, 0);
+        if (lane == 0 && basepos + nrec > r.cap) { // staging ring full: the tail of the chunk has no slot
+            u32 over = basepos >= r.cap ? nrec : basepos + nrec - r.cap;
+            atomicSub(r.count, over);
+            atomicAdd(&c.stats[r.lost_stat], (u64)over);
+        }
     }
-    const u32 rpos = basepos + __popc(mm & ((1u << lane) - 1));
-    pend.log_rec = (is_miss && rpos < r.cap) ? r.buf + (size_t)rpos * r.rec_bytes : nullptr;
+    const u32 rpos = basepos + __popc(pre & ((1u << lane) - 1));
+    pend.log_rec = (is_miss && !fresh && rpos < r.cap) ? r.buf + (size_t)rpos * r.rec_bytes : nullptr;
     pend.logged = false;
+    pend.lazy = fresh;
     if (pend.log_rec) *(uint2 *)(pend.log_rec + r.rec_bytes - 8) = make_uint2(idx + b.base, c.batch_seq);
     bool dropped = false;
     u32 todo = mm;

@@ -296,13 +296,15 @@ __device__ __forceinline__ bool is_private_ip(u32 ip_le) { // bpf/nat44.c:340-36
 struct NatPend {
     u8 *log_rec; // staged nat_log_rb record reserved for this frame (nullptr: ring full)
     bool logged;
+    bool lazy;   // nothing reserved up front: the record is reserved when it is written (a deferred TC frame, which is
+                 // most often a session hit and logs nothing)
 };
 
 __device__ __forceinline__ void nat_log(const DevCtx &c, u32 idx, u64 now, u32 type, u32 sub_id, u32 priv_ip,
                                         u32 pub_ip, u16 priv_port, u16 pub_port, u32 dst_ip, u16 dst_port, u8 proto,
                                         u8 flags, NatPend *pd = nullptr) { // log_nat_event(), :531-562
     u8 *r;
-    if (pd) { // the resolve kernel reserved the record up front (one atomic per 32 frames)
+    if (pd && !pd->lazy) { // the resolve kernel reserved the record up front (one atomic per 32 frames)
         r = pd->log_rec;
         pd->logged = true;
     } else {

@@ -184,8 +184,13 @@ int bng_restore(bng_ctx *ctx, const void *buf, uint64_t len);
 uint64_t bng_launch_count(bng_ctx *ctx);  /* kernels launched by this context so far */
 uint64_t bng_lru_overflow(bng_ctx *ctx);  /* inserts that found no victim to evict in a full LRU map (should stay 0) */
 uint64_t bng_lru_evictions(bng_ctx *ctx); /* entries evicted from full LRU maps by the data path */
-uint64_t bng_table_rebuilds(bng_ctx *ctx); /* flow-table rebuilds: bng_sweep compacts nat_sessions / nat_reverse / eim_table once a
-                                            quarter of the session slots are tombstones */
+/* Flow-table rebuilds so far.  nat_sessions / nat_reverse / eim_table are rebuilt (tombstones dropped) together:
+ *  - by bng_sweep, once a quarter of nat_sessions' slots are tombstones after it;
+ *  - once LRU evictions since the last rebuild exceed a quarter of nat_sessions' slots.  Host-fed batches and
+ *    bng_sync check this with the count as of their end.  A BNG_MEM_DEVICE batch of nat44_egress / pipeline_up /
+ *    pipeline_tc does not wait: it queues a copy of the count behind itself, and the next bng_prog_run or bng_sweep
+ *    applies the rule to that copy if it has completed by then.  Only a rebuild synchronises the stream. */
+uint64_t bng_table_rebuilds(bng_ctx *ctx);
 uint64_t bng_events_lost(bng_ctx *ctx);   /* event records dropped because the staging buffer was full */
 /* per-kernel device timing (CUDA events around every launch); read returns "name launches total_ms\n" lines */
 int bng_prof_enable(bng_ctx *ctx, int on);

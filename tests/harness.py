@@ -74,6 +74,12 @@ class Script:
                            None if now_v is None else np.ascontiguousarray(now_v, dtype=np.uint64).copy()))
         return self
 
+    def repeat(self, prog, arena, lens, now_ns, count, stride=64):
+        """`count` runs of one small fixed-stride batch (e.g. to advance the batch counter); the results of the last
+        run are recorded."""
+        self.steps.append(("repeat", prog, arena.copy(), lens.astype(np.uint32).copy(), int(now_ns), int(stride), int(count)))
+        return self
+
     def drain(self):
         """Drain both event rings at this point (frees nat_log_rb space)."""
         self.steps.append(("drain",))
@@ -115,6 +121,17 @@ class OracleBackend:
         self.o.free_arenas()
         return v
 
+    def run_repeat(self, prog, arena, lens, now, stride, count):
+        oa = self.o.arena(len(arena) + 64)
+        for _ in range(count):
+            oa[:len(arena)] = arena
+            l = lens.copy()
+            v = self.o.run(prog, oa, l, now, stride=stride)
+        arena[:] = oa[:len(arena)]
+        lens[:] = l
+        self.o.free_arenas()
+        return v
+
     def stats(self, m):
         return self.o.lookup(m, np.zeros(4, np.uint8)).view("<u8").copy()
 
@@ -129,6 +146,13 @@ class OracleBackend:
 
 
 class GpuBackend:
+    """The dataplane through the C ABI.  `pinned` picks how a batch is fed:
+    False    pageable numpy arrays (BNG_MEM_HOST, whole-arena staging copies, synchronised by the library);
+    True     pinned torch tensors (BNG_MEM_HOST, zero-copy header gather / scatter in chunks);
+    "abi"    an arena from bng_host_alloc() (BNG_MEM_HOST, zero-copy);
+    "device" torch CUDA tensors (BNG_MEM_DEVICE), synchronised with torch.cuda.synchronize() only, so nothing runs
+             on the host that a caller of the device-resident path does not get."""
+
     def __init__(self, dp=None, pinned=False, **opts):
         self.pinned = pinned
         if dp is None:
@@ -157,9 +181,26 @@ class GpuBackend:
     def run(self, prog, arena, lens, now, off16, stride, prio, now_v=None):
         if not getattr(self, "pinned", False):
             return self.dp.run(prog, arena, lens, now, off16=off16, stride=stride, priority=prio, now_v=now_v)
-        # pinned host buffers: exercises the zero-copy gather/scatter path of BNG_MEM_HOST
         import torch
-        from bng_b200 import MEM_HOST
+        from bng_b200 import MEM_DEVICE, MEM_HOST
+        if self.pinned == "device":
+            dev = torch.device("cuda")
+            ta = torch.from_numpy(arena.copy()).to(dev)
+            tl = torch.from_numpy(lens.view(np.int32).copy()).to(dev)
+            to = None if off16 is None else torch.from_numpy(off16.view(np.int32).copy()).to(dev)
+            tp = None if prio is None else torch.from_numpy(prio.view(np.int32).copy()).to(dev)
+            tn = None if now_v is None else torch.from_numpy(now_v.view(np.int64).copy()).to(dev)
+            tv = torch.zeros(len(lens), dtype=torch.uint8, device=dev)
+            torch.cuda.synchronize()  # the library's stream does not wait for torch's
+            self.dp.run(prog, ta, tl, now, off16=to, stride=stride, priority=tp, verdict=tv, mem=MEM_DEVICE,
+                        arena_bytes=arena.nbytes, now_v=tn)
+            torch.cuda.synchronize()
+            arena[:] = ta.cpu().numpy()
+            lens[:] = tl.cpu().numpy().view(np.uint32)
+            if prio is not None:
+                prio[:] = tp.cpu().numpy().view(np.uint32)
+            return tv.cpu().numpy()
+        # pinned host buffers: exercises the zero-copy gather/scatter path of BNG_MEM_HOST
         if self.pinned == "abi":  # the arena comes from bng_host_alloc() (huge-page backed, registered)
             import ctypes
             from bng_b200.dataplane import load_library
@@ -196,6 +237,34 @@ class GpuBackend:
         if prio is not None:
             prio[:] = tp.numpy().view(np.uint32)
         return tv.numpy().copy()
+
+    def run_repeat(self, prog, arena, lens, now, stride, count):
+        if self.pinned != "device":
+            for _ in range(count):
+                a, l = arena.copy(), lens.copy()
+                v = self.run(prog, a, l, now, None, stride, None)
+            arena[:], lens[:] = a, l
+            return v
+        # device-resident: the inputs are staged once and restored on the library's own stream before every run,
+        # so the runs queue back to back with no host synchronisation in between
+        import torch
+        from bng_b200 import MEM_DEVICE
+        dev = torch.device("cuda")
+        a0 = torch.from_numpy(arena.copy()).to(dev)
+        l0 = torch.from_numpy(lens.view(np.int32).copy()).to(dev)
+        ta, tl = a0.clone(), l0.clone()
+        tv = torch.zeros(len(lens), dtype=torch.uint8, device=dev)
+        pid = self.dp.prog_id(prog)
+        torch.cuda.synchronize()
+        with torch.cuda.stream(torch.cuda.ExternalStream(self.dp.stream, device=dev)):
+            for _ in range(count):
+                ta.copy_(a0)
+                tl.copy_(l0)
+                self.dp.run(pid, ta, tl, now, stride=stride, verdict=tv, mem=MEM_DEVICE, arena_bytes=arena.nbytes)
+        torch.cuda.synchronize()
+        arena[:] = ta.cpu().numpy()
+        lens[:] = tl.cpu().numpy().view(np.uint32)
+        return tv.cpu().numpy()
 
     def stats(self, m):
         return self.dp.stats(m)
@@ -242,6 +311,12 @@ def run_script(be, script: Script, tables=TABLES) -> dict:
             res[tag + "_len"] = l
             if p is not None:
                 res[tag + "_prio"] = p
+        elif st[0] == "repeat":
+            _, prog, arena, lens, now, stride, count = st
+            a, l = arena.copy(), lens.copy()
+            res[tag + "_verdict"] = np.asarray(be.run_repeat(prog, a, l, now, stride, count)).copy()
+            res[tag + "_frames"] = a
+            res[tag + "_len"] = l
         elif st[0] == "drain":
             for m in EVENT_MAPS:
                 events[m].append(be.drain(m))

@@ -90,7 +90,7 @@ def _gpu_run(wl, arena, off16, stride, steps, mode, sizing=None):
                 tv = torch.zeros(wl.n, dtype=torch.uint8, device="cuda")
                 torch.cuda.synchronize()
                 dp.run(wl.prog, ta, tl, now, off16=to, stride=stride, verdict=tv, mem=MEM_DEVICE)
-                dp.sync()
+                torch.cuda.synchronize()  # not dp.sync(): that runs host-side work a device-path caller never gets
                 a, l, v = ta.cpu().numpy(), tl.cpu().numpy().view(np.uint32), tv.cpu().numpy()
             outs.append((np.asarray(v), a, l))
         stats = {m: dp.stats(m) for m in ("antispoof_stats", "qos_stats_map", "nat_stats_map", "stats_map")}
@@ -128,12 +128,15 @@ def _same(a, b, what):
 
 
 @pytest.mark.parametrize("name", ["pipeline_imix", "pipeline_64", "nat_cold_64", "nat_steady_64", "nat_ingress_64", "antispoof_64",
-                                  "qos_64", "qos_egress_64"])
+                                  "qos_64", "qos_egress_64", "pipeline_tc"])
 def test_million_frames_against_reference(name):
     """Every bench workload at BASELINE scale (10 k subscribers / 1 M flows of config #3, 2^20 frames) against the
-    reference oracle, bit for bit: verdicts, frame bytes, counters, event streams, table dumps."""
+    reference oracle, bit for bit: verdicts, frame bytes, counters, event streams, table dumps.  pipeline_tc is
+    pipeline_imix in the order of the reference's TC hooks (QoS before NAT)."""
     n = 1 << 20
-    wl = W.BUILDERS[name](n, 0, 1)
+    wl = W.BUILDERS["pipeline_imix" if name == "pipeline_tc" else name](n, 0, 1)
+    if name == "pipeline_tc":
+        wl.prog = "pipeline_tc"
     if wl.derive is not None:  # return traffic: derived from what the oracle's own prewarm translated
         from oracle.pyoracle import Oracle, available
         o = Oracle("reference" if available("reference") else "port")
@@ -176,6 +179,31 @@ def test_fat_subscribers_against_reference(case):
     ref = _oracle_run(wl, arena, off16, stride, steps)
     gpu = _gpu_run(wl, arena, off16, stride, steps, "device")
     _same(ref, gpu, f"fat subscribers / {case}: reference oracle vs gpu")
+
+
+def test_tc_staging_holds_only_records_written():
+    """pipeline_tc runs nat44_egress after the token bucket, in the ordered phase, for every frame the bucket passed
+    — session hits included.  Those hits log nothing and must not take nat_log_rb staging space: a staging buffer
+    of 2^15 records (more than the 21 845 of the reference's 1 MiB ring) has to hold one batch of 2^16 frames that
+    are nearly all hits, and the few hundred new flows near its end keep their SESSION_CREATE records."""
+    n = 1 << 16
+    wl = W.pipeline(n, 0, 1, n_subs=1000, flows_per_sub=8, imix=False)
+    wl.prog = "pipeline_tc"
+    for i, (m, k, v) in enumerate(wl.maps):
+        if m == "qos_ingress":  # every bucket rate-limited but deep: every frame waits for it, and passes
+            v = v.copy()
+            v["rate_bps"], v["burst_bytes"] = 10**12, 1 << 30
+            v["tokens"] = v["burst_bytes"]
+            wl.maps[i] = (m, k, v)
+    tail = np.arange(n - 512, n)
+    tail = tail[np.isin(wl.headers[tail, 23], (6, 17))]
+    wl.headers[tail, 35] ^= 0x5A  # new source ports: new flows, late in index order
+    arena, off16, stride = _arena(wl)
+    ref = _oracle_run(wl, arena, off16, stride, 1)
+    created = int(ref[1]["nat_stats_map"][5]) - len(wl.prewarm[0][2])
+    assert created >= 200, created
+    gpu = _gpu_run(wl, arena, off16, stride, 1, "device", sizing=dict(W.sizing(wl), event_capacity=1 << 15))
+    _same(ref, gpu, "pipeline_tc, 2^16 frames, 2^15 staging records: reference oracle vs gpu")
 
 
 @pytest.mark.parametrize("case", ["pipeline_up", "pipeline_tc", "qos"])

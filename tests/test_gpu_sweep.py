@@ -123,10 +123,34 @@ def test_sweep_matches_the_spec_on_the_oracle(flags, ora_kind):
 def test_full_lru_tables_evict_instead_of_failing():
     """nat_sessions / nat_reverse / eim_table are BPF_MAP_TYPE_LRU_HASH (bpf/nat44.c:218-244): an insert into a full
     map makes room.  200 subscribers x 8 new flows per batch into tables of 512 entries: nothing is ever refused,
-    the tables stay at their size, what survives is recent, and replies to surviving flows are still translated."""
-    from bng_b200 import Dataplane
+    the tables stay at their size, what survives is recent, and replies to surviving flows are still translated.
+    Every eviction leaves a tombstone, so the flow tables are rebuilt on the way."""
+    _lru_churn("pageable")
+
+
+def test_full_lru_tables_are_compacted_on_the_device_path():
+    """The same churn with device-resident batches that nothing but torch ever synchronises: the flow tables must
+    still be rebuilt (a table without EMPTY slots makes every lookup of an absent key walk all of it)."""
+    _lru_churn("device")
+
+
+def _lru_churn(feed):
+    import torch
+    from bng_b200 import MEM_DEVICE, Dataplane
     cap = 512
     dp = Dataplane(max_subscribers=1 << 10, max_nat_sessions=cap, max_eim_mappings=cap, max_batch=1 << 13)
+
+    def run(prog, a, lens, now):
+        if feed == "pageable":
+            return np.asarray(dp.run(prog, a, lens, now, stride=64))
+        ta, tl = torch.from_numpy(a).cuda(), torch.from_numpy(lens.view(np.int32)).cuda()
+        tv = torch.zeros(len(lens), dtype=torch.uint8, device="cuda")
+        torch.cuda.synchronize()
+        dp.run(prog, ta, tl, now, stride=64, verdict=tv, mem=MEM_DEVICE)
+        torch.cuda.synchronize()
+        a[:] = ta.cpu().numpy()
+        return tv.cpu().numpy()
+
     try:
         sc = harness.Script("maps")
         n_subs = 200
@@ -141,14 +165,15 @@ def test_full_lru_tables_evict_instead_of_failing():
             h = S.ipv4_headers(S.sub_mac_key(sub), np.uint64(scenarios.GW_MAC), S.sub_ip(sub), np.uint32(0x08080808), 17, sport, 53,
                                lens, l4_check=0x2222)
             a = h.reshape(-1).copy()
-            v = dp.run("nat44_egress", a, lens, (10 + b) * NS, stride=64)
-            assert (np.asarray(v) == 0).all()
+            v = run("nat44_egress", a, lens, (10 + b) * NS)
+            assert (v == 0).all()
             assert (a.reshape(-1, 64)[:, 26:30] != h[:, 26:30]).any(axis=1).all(), "a frame left untranslated"
             last = a.reshape(-1, 64).copy()
             for m in ("nat_sessions", "nat_reverse", "eim_table"):
                 assert dp.map_info(m)["count"] <= cap, m
         assert dp.lru_overflow == 0
         assert dp.lru_evictions >= 11 * n_subs * 8  # every batch after the first pushed something out
+        assert dp.table_rebuilds >= 3, f"{dp.lru_evictions} evictions, {dp.table_rebuilds} rebuilds of the flow tables"
         k, v = dp.dump("nat_sessions")
         ses = v.view(L.nat_session).reshape(-1)
         assert len(ses) >= cap - 64 and int(ses["last_seen"].min()) >= 19 * NS, "old sessions survived newer ones"
@@ -158,7 +183,7 @@ def test_full_lru_tables_evict_instead_of_failing():
         out[:, 34:36], out[:, 36:38] = last[:, 36:38], last[:, 34:36]
         before = dp.stats("nat_stats_map")[1]
         r = out.reshape(-1).copy()
-        dp.run("nat44_ingress", r, np.full(len(out), 64, np.uint32), 30 * NS, stride=64)
+        run("nat44_ingress", r, np.full(len(out), 64, np.uint32), 30 * NS)
         dnat = int(dp.stats("nat_stats_map")[1] - before)
         assert dnat >= cap // 8, f"only {dnat} replies translated"  # session AND reverse entry survived (independent evictions)
         back = r.reshape(-1, 64)
@@ -208,3 +233,93 @@ def test_session_churn_rebuilds_the_flow_tables():
         assert dp.lru_overflow == 0
     finally:
         dp.close()
+
+
+EPOCH_PERIOD = 65535  # bng_prog_run: epoch = batch_seq % 65535 + 1; every epoch is cleared when it comes round to 1
+
+
+def epoch_wrap_script():
+    """A session hit stores last_seen only when the session's 16-bit epoch differs from the batch's (common.cuh,
+    ses_touch), so the epochs are all cleared when the batch counter comes round to the same values again.  Two
+    sets of flows, each split four ways: hits of nat44_egress, replies through nat44_ingress, pipeline_up,
+    pipeline_tc (half the subscribers with a rate-limited bucket: TC runs NAT after it, in the ordered phase).
+      set 2 is touched in the four batches before the reset (batch 65 535) and in the four from it on;
+      set 1 is touched in batches 6-9 and then not again until batches 6-9 + 65 535, with the same epoch values.
+    Everything between is 1-frame ARP batches of antispoof_ingress.  Returns (script, batches)."""
+    n_subs, ns = 16, 10**9
+    sc = harness.Script("epoch_wrap")
+    keys, v = S.bindings(n_subs)
+    sc.update("subscriber_bindings", keys, v)
+    cfg = np.zeros(1, L.antispoof_config)
+    cfg["default_mode"] = 1
+    sc.update1("antispoof_config", np.uint32(0), cfg)
+    scenarios.nat_maps(sc, n_subs, 64, 0x0F)
+    qk, qv = S.qos_buckets(n_subs // 2)
+    qv["rate_bps"], qv["burst_bytes"] = 10**12, 1 << 30
+    qv["tokens"] = qv["burst_bytes"]
+    sc.update("qos_ingress", qk, qv)
+    sub = np.tile(np.arange(n_subs), 2)  # two frames of every flow per batch
+    lens = np.full(len(sub), 64, np.uint32)
+    sites = ("nat44_egress", "nat44_ingress", "pipeline_up", "pipeline_tc")
+
+    def frames(flow_set, site):
+        return S.ipv4_headers(S.sub_mac_key(sub), np.uint64(scenarios.GW_MAC), S.sub_ip(sub), np.uint32(0x08080808), 17,
+                              20000 + 100 * flow_set + 10 * site, 53, lens, l4_check=0x1234)
+
+    setup = len(sc.steps)
+    seq = 1
+    sc.run("nat44_egress", scenarios.fixed(np.concatenate([frames(s, i) for s in (1, 2) for i in range(4)])), np.tile(lens, 8), ns)
+    arp = scenarios.fixed(frames(0, 0)[:1])
+    arp[12:14] = [0x08, 0x06]
+
+    def replies(res, flow_set):
+        out = res[f"s{setup:03d}_frames"].reshape(8, len(sub), 64)[4 * (flow_set - 1) + 1].copy()
+        rep = out.copy()
+        rep[:, 26:30], rep[:, 30:34] = out[:, 30:34], out[:, 26:30]
+        rep[:, 34:36], rep[:, 36:38] = out[:, 36:38], out[:, 34:36]
+        return rep
+
+    def touch(flow_set, now):
+        nonlocal seq
+        for i, prog in enumerate(sites):
+            if prog == "nat44_ingress":
+                sc.run_from(prog, lambda res, fs=flow_set, t=now + i: {"arena": replies(res, fs).reshape(-1), "lens": lens,
+                                                                       "now_ns": t, "stride": 64})
+            else:
+                sc.run(prog, scenarios.fixed(frames(flow_set, i)), lens, now + i)
+        seq += 4
+
+    def filler(count, now):
+        nonlocal seq
+        sc.repeat("antispoof_ingress", arp, np.full(1, 64, np.uint32), now, count)
+        seq += count
+
+    filler(4, 2 * ns)
+    first = seq + 1
+    touch(1, 3 * ns)
+    filler(EPOCH_PERIOD - 5 - seq, 4 * ns)
+    touch(2, 5 * ns)
+    assert seq + 1 == EPOCH_PERIOD  # the next batch clears the epochs
+    touch(2, 6 * ns)
+    filler(first + EPOCH_PERIOD - 1 - seq, 7 * ns)
+    touch(1, 8 * ns)  # the same epoch values as batches first..first+3
+    assert seq == first + EPOCH_PERIOD + 3
+    return sc, seq
+
+
+def test_last_seen_across_the_epoch_wrap(ora_kind):
+    """The 16-bit epoch wrap, device-resident as the headline runs, against the oracle: nat_sessions (last_seen
+    above all), counters, verdicts and frames."""
+    if ora_kind == "none":
+        pytest.fail("no oracle library present on this box")
+    sc, batches = epoch_wrap_script()
+    assert batches > EPOCH_PERIOD
+    want = harness.run_script(harness.OracleBackend(ora_kind), sc)
+    last_seen = want["tv_nat_sessions"].view(L.nat_session)["last_seen"]
+    assert len(last_seen) == 128 and last_seen.min() >= 6 * NS  # every session's last touch is one of the late ones
+    gpu = harness.GpuBackend(pinned="device")
+    try:
+        got = harness.run_script(gpu, sc)
+    finally:
+        gpu.close()
+    harness.compare(want, got, f"epoch wrap: {ora_kind} oracle vs gpu (device-resident)")

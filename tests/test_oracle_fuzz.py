@@ -116,7 +116,7 @@ def test_mutated_frames_agree(prog, seed):
 # ctx.cu / hostio.cu (96-byte slots sized per frame from ihl, pinned-ness from cudaPointerGetAttributes); every
 # program is now a plain pass on every seed, pinned and pageable.
 @pytest.mark.gpu
-@pytest.mark.parametrize("pinned", [False, True], ids=["pageable", "pinned"])
+@pytest.mark.parametrize("pinned", [False, True, "device"], ids=["pageable", "pinned", "device"])
 @pytest.mark.parametrize("seed", [11, 13, 17, 23])
 @pytest.mark.parametrize("prog", sorted(TARGETS))
 def test_gpu_mutated_frames_agree(prog, seed, pinned, ora_kind):
@@ -128,4 +128,5 @@ def test_gpu_mutated_frames_agree(prog, seed, pinned, ora_kind):
         got = harness.run_script(be, fuzz_script(prog, seed))
     finally:
         be.close()
-    harness.compare(want, got, f"fuzz {prog} seed {seed} ({'pinned' if pinned else 'pageable'}): {ora_kind} oracle vs gpu")
+    feed = {False: "pageable", True: "pinned"}.get(pinned, pinned)
+    harness.compare(want, got, f"fuzz {prog} seed {seed} ({feed}): {ora_kind} oracle vs gpu")
