@@ -747,9 +747,10 @@ __device__ __forceinline__ void hdr_store_chunk(const Hdr64 &h, u8 *p, int c) {
 struct __align__(16) U256 {
     u32 w[8];
 };
-// L2 eviction priority of a 32-byte access (ld/st.global.L2::evict_{first,last}).  Frames stream through
-// once: evict-first keeps them from pushing the flow table's hot sectors (touched ~6 times per batch) out
-// of the 50 MB L2; the flow-table probe asks to stay (evict-last).
+// L2 eviction priority of a 32-byte access.  Frames stream through once: evict-first is meant to keep them
+// from pushing the flow table's hot sectors (touched ~6 times per batch) out of the 50 MB L2; the flow-table
+// probe asks to stay (evict-last).  Both are off by default: neither gain measured on H100 is clear of the
+// run-to-run spread (DESIGN.md §5).
 enum { L2_NORMAL = 0, L2_FIRST = 1, L2_LAST = 2 };
 #ifndef FRAME_POLICY
 #define FRAME_POLICY L2_NORMAL
@@ -757,44 +758,65 @@ enum { L2_NORMAL = 0, L2_FIRST = 1, L2_LAST = 2 };
 #ifndef SES_POLICY
 #define SES_POLICY L2_NORMAL
 #endif
-#define BNG_LDG128(HINT, r, q)                                                                                   \
-    asm volatile("ld.global" HINT ".v4.u32 {%0,%1,%2,%3}, [%4];"                                                 \
+// sm_90 has the .L2::evict_{first,last} qualifiers on 256-bit accesses only; a 128-bit access carries its
+// priority as an L2 cache policy (createpolicy) through .L2::cache_hint.
+template <int POLICY>
+__device__ __forceinline__ u64 l2_policy() {
+    u64 pol;
+    if (POLICY == L2_FIRST)
+        asm("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+    else
+        asm("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
+    return pol;
+}
+#define BNG_LDG128(r, q)                                                                                         \
+    asm volatile("ld.global.v4.u32 {%0,%1,%2,%3}, [%4];"                                                         \
                  : "=r"((r)[0]), "=r"((r)[1]), "=r"((r)[2]), "=r"((r)[3])                                        \
                  : "l"(q)                                                                                        \
                  : "memory")
-#define BNG_STG128(HINT, q, w)                                                                                   \
-    asm volatile("st.global" HINT ".v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(q), "r"((w)[0]), "r"((w)[1]), "r"((w)[2]), \
+#define BNG_LDG128_HINT(r, q, pol)                                                                               \
+    asm volatile("ld.global.L2::cache_hint.v4.u32 {%0,%1,%2,%3}, [%4], %5;"                                      \
+                 : "=r"((r)[0]), "=r"((r)[1]), "=r"((r)[2]), "=r"((r)[3])                                        \
+                 : "l"(q), "l"(pol)                                                                              \
+                 : "memory")
+#define BNG_STG128(q, w)                                                                                         \
+    asm volatile("st.global.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(q), "r"((w)[0]), "r"((w)[1]), "r"((w)[2]),         \
                  "r"((w)[3])                                                                                     \
+                 : "memory")
+#define BNG_STG128_HINT(q, w, pol)                                                                               \
+    asm volatile("st.global.L2::cache_hint.v4.u32 [%0], {%1,%2,%3,%4}, %5;" ::"l"(q), "r"((w)[0]), "r"((w)[1]),   \
+                 "r"((w)[2]), "r"((w)[3]), "l"(pol)                                                              \
                  : "memory")
 template <int POLICY = L2_NORMAL>
 __device__ __forceinline__ U256 ldg256(const void *p) {
     U256 r;
     const u8 *q = (const u8 *)p;
-    if (POLICY == L2_FIRST) {
-        BNG_LDG128(".L2::evict_first", &r.w[0], q);
-        BNG_LDG128(".L2::evict_first", &r.w[4], q + 16);
-    } else if (POLICY == L2_LAST) {
-        BNG_LDG128(".L2::evict_last", &r.w[0], q);
-        BNG_LDG128(".L2::evict_last", &r.w[4], q + 16);
+    if (POLICY == L2_NORMAL) {
+        BNG_LDG128(&r.w[0], q);
+        BNG_LDG128(&r.w[4], q + 16);
     } else {
-        BNG_LDG128("", &r.w[0], q);
-        BNG_LDG128("", &r.w[4], q + 16);
+        const u64 pol = l2_policy<POLICY>();
+        BNG_LDG128_HINT(&r.w[0], q, pol);
+        BNG_LDG128_HINT(&r.w[4], q + 16, pol);
     }
     return r;
 }
 template <int POLICY = L2_NORMAL>
 __device__ __forceinline__ void stg256(void *p, const u32 *w) {
     u8 *q = (u8 *)p;
-    if (POLICY == L2_FIRST) {
-        BNG_STG128(".L2::evict_first", q, &w[0]);
-        BNG_STG128(".L2::evict_first", q + 16, &w[4]);
+    if (POLICY == L2_NORMAL) {
+        BNG_STG128(q, &w[0]);
+        BNG_STG128(q + 16, &w[4]);
     } else {
-        BNG_STG128("", q, &w[0]);
-        BNG_STG128("", q + 16, &w[4]);
+        const u64 pol = l2_policy<POLICY>();
+        BNG_STG128_HINT(q, &w[0], pol);
+        BNG_STG128_HINT(q + 16, &w[4], pol);
     }
 }
 #undef BNG_LDG128
+#undef BNG_LDG128_HINT
 #undef BNG_STG128
+#undef BNG_STG128_HINT
 // Frame header load: two 32-byte loads when the whole warp's frames allow it (32-byte aligned and 64
 // bytes inside the arena), 16-byte chunks otherwise.  `wide` must be warp-uniform.
 __device__ __forceinline__ void hdr_load_wide(Hdr64 &h, const u8 *p, u32 len, bool wide) {
