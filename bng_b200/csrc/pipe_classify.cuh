@@ -15,14 +15,15 @@
 // gather-heavy kernel like this one.
 #pragma once
 
-// Resident blocks per SM each instantiation is compiled for (registers: 65536 / (256 x blocks)).  At 4 blocks the
-// pipeline instantiations get 64 registers and spill a few bytes; at 3 they get 85 and spill nothing.  Which is faster
-// on H100 has not been measured (-DCLASSIFY_BLOCKS=3 is the whole change).
+// Resident blocks per SM each instantiation is compiled for (registers: 65536 / (256 x blocks)).  Fewer warps that do
+// not spill beat more warps that do: at 4 blocks the pipeline instantiations get 64 registers and spill 48 bytes, at
+// 3 they use 72 and spill nothing; <false,false> spills 56 bytes at 5 blocks (48 registers) and nothing at 4 (62).
+// On H100 the smaller counts shorten classify by ~9 % on pipeline_imix and ~13 % on nat_steady_64 (DESIGN.md §9).
 #ifndef CLASSIFY_BLOCKS
-#define CLASSIFY_BLOCKS 4
+#define CLASSIFY_BLOCKS 3
 #endif
 #ifndef CLASSIFY_BLOCKS_NAT
-#define CLASSIFY_BLOCKS_NAT 5
+#define CLASSIFY_BLOCKS_NAT 4
 #endif
 #define CLASSIFY_BPS(AS) ((AS) ? CLASSIFY_BLOCKS : CLASSIFY_BLOCKS_NAT)
 // CLASSIFY_PAIR: fetch the home PAIR of slots of the bindings table / subscriber directory with the first probe
