@@ -1,0 +1,145 @@
+// bng_b200 — per-subscriber traffic accounting (bng_acct_*, include/bng_b200.h).
+//
+// One record of ACCT_WORDS u64 per subscriber directory slot (struct bng_acct: upstream pass / drop, downstream
+// pass / drop, packets and bytes each).  k_acct runs after a program, on the same stream, one thread per frame: it
+// finds the frame's directory slot (the word classify recorded, or the address in the outgoing header), reads the
+// verdict and skb->len, and adds the frame to the slot's pass or drop pair.  Frames of one warp that go to the same
+// pair are summed first (__match_any_sync): the leader of each group issues the two atomics, so a subscriber that
+// owns a whole batch costs one atomic pair per warp, not per frame.
+#include <errno.h>
+
+#include "kernels.h"
+#include "progs.cuh"
+
+#define ACCT_BLOCK 256
+
+__device__ __forceinline__ u32 dir_slot_of(const Tbl &dir, u32 addr) {
+    const u64 k = addr;
+    const u8 *s = tbl_find<1, false>(dir, &k);
+    return s ? (u32)((s - dir.slots) >> 4) : DIR_NONE;
+}
+
+template <int MODE>
+__global__ void __launch_bounds__(ACCT_BLOCK) k_acct(const __grid_constant__ Tbl dir, const __grid_constant__ DevBatch b, const u32 *attr,
+                                                      u64 *acct) {
+    const u32 lane = threadIdx.x & 31;
+    // warp-uniform trip count: __match_any_sync needs every lane
+    for (u32 base = blockIdx.x * ACCT_BLOCK + (threadIdx.x & ~31u); base < b.n; base += gridDim.x * ACCT_BLOCK) {
+        const u32 i = base + lane;
+        u32 slot = DIR_NONE, len = 0, drop = 0;
+        if (i < b.n) {
+            const u8 v = b.verdict[i];
+            if (v == TC_OK || v == TC_SHOT) {
+                len = b.len[i];
+                drop = v == TC_SHOT;
+                if (MODE == ACCT_ATTR) {
+                    slot = attr[i];
+                } else {
+                    // untagged IPv4 with the address's four bytes present: the source (26-29) as the frame entered,
+                    // or the destination (30-33) as it leaves
+                    const u32 off = MODE == ACCT_SRC ? 26 : 30;
+                    const u8 *p = frame_ptr(b, i);
+                    if (frame_dlen(b, len) >= off + 4 && rd16(p, 12) == ETH_P_IP_LE) slot = dir_slot_of(dir, rd32(p, off));
+                }
+            }
+        }
+        const bool has = slot != DIR_NONE;
+        const u32 grp = has ? (slot << 1 | drop) : (0xFFFFFFE0u | lane); // (directory slots < 2^31 - 16)
+        const u32 peers = __match_any_sync(0xffffffffu, grp);
+        u64 bytes = len;
+        if (!__all_sync(0xffffffffu, peers == (1u << lane))) { // some lanes share a record: sum each group
+            bytes = 0;
+#pragma unroll
+            for (int j = 0; j < 32; j++) {
+                const u32 lj = __shfl_sync(0xffffffffu, len, j);
+                if ((peers >> j) & 1) bytes += lj;
+            }
+        }
+        if (has && lane == (u32)__ffs(peers) - 1) {
+            u64 *r = acct + (size_t)slot * ACCT_WORDS + (MODE == ACCT_DST ? 4 : 0) + 2 * drop;
+            atomicAdd((unsigned long long *)r, (unsigned long long)__popc(peers));
+            atomicAdd((unsigned long long *)(r + 1), (unsigned long long)bytes);
+        }
+    }
+}
+
+__global__ void k_acct_read(const __grid_constant__ Tbl dir, const u64 *acct, const u32 *addrs, u64 n, u64 *out, int *results) {
+    for (u64 i = blockIdx.x * (u64)blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x) {
+        const u32 s = dir_slot_of(dir, addrs[i]);
+        u64 *o = out + i * ACCT_WORDS;
+#pragma unroll
+        for (int j = 0; j < ACCT_WORDS; j++) o[j] = (s != DIR_NONE && acct) ? acct[(size_t)s * ACCT_WORDS + j] : 0;
+        results[i] = s != DIR_NONE ? 0 : -ENOENT;
+    }
+}
+
+// one atomic per warp on the output count: the interim-update sweep reads 10^5 - 10^6 records at once
+__global__ void k_acct_dump(const __grid_constant__ Tbl dir, const u64 *acct, u32 *addrs_out, u64 *out, u32 *count, u64 cap) {
+    const u64 slots = (u64)dir.mask + 1;
+    const u32 lane = threadIdx.x & 31;
+    for (u64 base = blockIdx.x * (u64)blockDim.x + (threadIdx.x & ~31u); base < slots; base += (u64)gridDim.x * blockDim.x) {
+        const u64 i = base + lane;
+        const u64 k = i < slots ? *(const u64 *)(dir.slots + i * 16) : K_EMPTY;
+        const bool live = k < K_BUSY;
+        const u32 m = __ballot_sync(0xffffffffu, live);
+        if (!m) continue;
+        u32 pos = 0;
+        if (lane == 0) pos = atomicAdd(count, (u32)__popc(m));
+        pos = __shfl_sync(0xffffffffu, pos, 0) + __popc(m & ((1u << lane) - 1));
+        if (!live || pos >= cap) continue;
+        addrs_out[pos] = (u32)k;
+        u64 *o = out + (u64)pos * ACCT_WORDS;
+#pragma unroll
+        for (int j = 0; j < ACCT_WORDS; j++) o[j] = acct ? acct[i * ACCT_WORDS + j] : 0;
+    }
+}
+
+__global__ void k_acct_load(const __grid_constant__ Tbl dir, u64 *acct, const u32 *addrs, const u64 *recs, u64 n) {
+    for (u64 i = blockIdx.x * (u64)blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x) {
+        const u32 s = dir_slot_of(dir, addrs[i]);
+        if (s == DIR_NONE) continue;
+#pragma unroll
+        for (int j = 0; j < ACCT_WORDS; j++) acct[(size_t)s * ACCT_WORDS + j] = recs[i * ACCT_WORDS + j];
+    }
+}
+
+static inline int acct_grid(const Launcher &L, u64 n, int per_sm) {
+    const u64 want = (n + ACCT_BLOCK - 1) / ACCT_BLOCK, cap = (u64)L.num_sms * per_sm;
+    return (int)(want < 1 ? 1 : (want < cap ? want : cap));
+}
+
+cudaError_t run_acct(Launcher &L, const Tbl &dir, const DevBatch &b, int mode, u64 *acct) {
+    const int grid = acct_grid(L, b.n, 8);
+    prof_begin(L, "k_acct");
+    if (mode == ACCT_ATTR)
+        k_acct<ACCT_ATTR><<<grid, ACCT_BLOCK, 0, L.stream>>>(dir, b, L.acct_attr, acct);
+    else if (mode == ACCT_SRC)
+        k_acct<ACCT_SRC><<<grid, ACCT_BLOCK, 0, L.stream>>>(dir, b, nullptr, acct);
+    else
+        k_acct<ACCT_DST><<<grid, ACCT_BLOCK, 0, L.stream>>>(dir, b, nullptr, acct);
+    prof_end(L);
+    L.launches++;
+    return cudaGetLastError();
+}
+
+cudaError_t run_acct_read(Launcher &L, const Tbl &dir, const u64 *acct, const u32 *addrs, u64 n, u64 *out, int *results) {
+    if (n == 0) return cudaSuccess;
+    k_acct_read<<<acct_grid(L, n, 8), ACCT_BLOCK, 0, L.stream>>>(dir, acct, addrs, n, out, results);
+    L.launches++;
+    return cudaGetLastError();
+}
+
+cudaError_t run_acct_dump(Launcher &L, const Tbl &dir, const u64 *acct, u32 *addrs_out, u64 *out, u32 *count, u64 cap) {
+    prof_begin(L, "k_acct_dump");
+    k_acct_dump<<<acct_grid(L, (u64)dir.mask + 1, 8), ACCT_BLOCK, 0, L.stream>>>(dir, acct, addrs_out, out, count, cap);
+    prof_end(L);
+    L.launches++;
+    return cudaGetLastError();
+}
+
+cudaError_t run_acct_load(Launcher &L, const Tbl &dir, u64 *acct, const u32 *addrs, const u64 *recs, u64 n) {
+    if (n == 0) return cudaSuccess;
+    k_acct_load<<<acct_grid(L, n, 8), ACCT_BLOCK, 0, L.stream>>>(dir, acct, addrs, recs, n);
+    L.launches++;
+    return cudaGetLastError();
+}

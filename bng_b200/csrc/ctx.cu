@@ -105,6 +105,12 @@ struct bng_ctx {
     ncclComm_t comm = nullptr;
     u32 comm_rank = 0, comm_world = 1;
     u64 *stats_global = nullptr; // device: all-reduced counter vector
+    // per-subscriber traffic accounting (bng_acct_*): records index-aligned with the subscriber directory, allocated
+    // by the first bng_acct_enable (or a restore that carries records); acct_progs: bit p = program p is accounted
+    u64 *acct = nullptr;
+    u32 acct_progs = 0;
+    u8 *acct_dump_buf = nullptr; // grow-only scratch of bng_acct_dump: records, then addresses
+    u64 acct_dump_cap = 0;
 };
 
 namespace {
@@ -170,8 +176,9 @@ int ensure_scratch(bng_ctx *c, u32 n) {
     Scratch &s = c->L.s;
     if (n <= s.cap) return 0;
     u32 cap = std::max<u32>(n, 1024);
-    void **ptrs[] = {(void **)&s.key_a, (void **)&s.key_b, (void **)&s.val_a, (void **)&s.val_b, (void **)&s.qslot};
+    void **ptrs[] = {(void **)&s.key_a, (void **)&s.key_b, (void **)&s.val_a, (void **)&s.val_b, (void **)&s.qslot, (void **)&s.attr};
     for (void **pp : ptrs) {
+        if (pp == (void **)&s.attr && !c->acct) continue; // the attribution words exist once accounting does
         if (*pp) cudaFree(*pp);
         CU(c, cudaMalloc(pp, (size_t)cap * 4));
     }
@@ -265,7 +272,7 @@ int hash_cmd(bng_ctx *c, MapReg *m, int op, const void *keys, void *vals, u64 n,
         CU(c, cudaMemcpyAsync(c->io_dev, c->io_host, up, cudaMemcpyHostToDevice, c->L.stream));
         const int role = m->tbl == &c->dev.sub_nat ? 1 : (m->tbl == &c->dev.qos_in ? 2 : 0);
         CU(c, run_table_op(c->L, t, op, c->io_dev + koff, c->io_dev + voff, (int *)(c->io_dev + roff), k, flags, c->dev.subdir,
-                           role));
+                           role, c->acct));
         size_t dfrom = op == TOP_LOOKUP ? voff : roff;
         CU(c, cudaMemcpyAsync(c->io_host + dfrom, c->io_dev + dfrom, roff + rb - dfrom, cudaMemcpyDeviceToHost, c->L.stream));
         CU(c, cudaStreamSynchronize(c->L.stream));
@@ -485,7 +492,7 @@ int bng_close(bng_ctx *c) {
         }
         for (void *p : c->allocs) cudaFree(p);
         Scratch &s = c->L.s;
-        void *sp[] = {s.key_a, s.key_b, s.val_a, s.val_b, s.qslot, s.cub_tmp, s.counters,
+        void *sp[] = {s.key_a, s.key_b, s.val_a, s.val_b, s.qslot, s.attr, s.cub_tmp, s.counters, c->acct_dump_buf,
                       c->io_dev, c->hb_pkts, c->hb_off, c->hb_len, c->hb_prio, c->hb_verdict, c->hb_now, c->dump_k, c->dump_v, c->dump_c};
         for (void *p : sp)
             if (p) cudaFree(p);
@@ -994,8 +1001,13 @@ int bng_prog_id(bng_ctx *c, const char *name) {
     return -ENOENT;
 }
 
+// the accounting mode of each program: where its frames' subscriber is found (-1: not accountable)
+static const int k_acct_mode[] = {-1, ACCT_DST, ACCT_SRC, ACCT_ATTR, ACCT_DST, -1, -1, ACCT_ATTR, ACCT_ATTR};
+
 static int dispatch(bng_ctx *c, int prog, const DevBatch &b) {
     cudaError_t e;
+    const bool acct = c->acct && ((c->acct_progs >> prog) & 1);
+    c->L.acct_attr = acct ? c->L.s.attr : nullptr; // the upstream classify records attributions
     switch (prog) {
     case P_ANTISPOOF: e = run_antispoof(c->L, c->dev, b); break;
     case P_QOS_EG: e = run_qos(c->L, c->dev, b, true); break;
@@ -1008,6 +1020,8 @@ static int dispatch(bng_ctx *c, int prog, const DevBatch &b) {
     case P_PIPE_TC: e = run_pipeline_tc(c->L, c->dev, b); break;
     default: return -EINVAL;
     }
+    // after the program, before anything copies the frames out: the downstream modes read the rewritten headers
+    if (e == cudaSuccess && acct) e = run_acct(c->L, c->dev.subdir, b, k_acct_mode[prog], c->acct);
     if (e != cudaSuccess) return fail(c, -EIO, "launch %s: %s", k_prog_names[prog], cudaGetErrorString(e));
     return 0;
 }
@@ -1501,6 +1515,100 @@ int bng_events_drain(bng_ctx *c, int map, void *buf, uint64_t cap_records, uint6
 }
 
 // ---------------------------------------------------------------------------
+// per-subscriber traffic accounting (acct.cu)
+// ---------------------------------------------------------------------------
+static_assert(sizeof(bng_acct) == ACCT_WORDS * 8, "struct bng_acct is the device record");
+
+// The records (one per directory slot) and the per-frame attribution words, on first use.
+static int acct_alloc_locked(bng_ctx *c) {
+    if (c->acct) return 0;
+    Scratch &s = c->L.s;
+    if (!s.attr) CU(c, cudaMalloc((void **)&s.attr, (size_t)s.cap * 4));
+    u64 *a = nullptr;
+    const size_t bytes = ((size_t)c->dev.subdir.mask + 1) * sizeof(bng_acct);
+    if (cudaMalloc((void **)&a, bytes) != cudaSuccess) return fail(c, -ENOMEM, "accounting: %zu bytes of device memory", bytes);
+    c->allocs.push_back(a);
+    CU(c, cudaMemsetAsync(a, 0, bytes, c->L.stream));
+    c->acct = a;
+    return 0;
+}
+
+// the directory follows subscriber_nat and qos_ingress: their staged upserts come first
+static int acct_flush_locked(bng_ctx *c) {
+    for (const char *m : {"subscriber_nat", "qos_ingress"})
+        if (int fr = flush_staged_locked(c, bng_map_id(c, m))) return fr;
+    return 0;
+}
+
+static int64_t acct_dump_locked(bng_ctx *c, uint32_t *addrs_out, bng_acct *out, uint64_t cap) {
+    if (cap == 0) return 0;
+    const u64 ecap = std::min<u64>(cap, (u64)c->dev.subdir.mask + 1); // no more entries than slots
+    const size_t aoff = ecap * sizeof(bng_acct), coff = (aoff + ecap * 4 + 15) & ~(size_t)15, need = coff + 16;
+    if (need > c->acct_dump_cap) {
+        if (c->acct_dump_buf) cudaFree(c->acct_dump_buf);
+        c->acct_dump_buf = nullptr;
+        c->acct_dump_cap = 0;
+        if (cudaMalloc((void **)&c->acct_dump_buf, need) != cudaSuccess) return fail(c, -ENOMEM, "acct_dump: out of device memory");
+        c->acct_dump_cap = need;
+    }
+    u8 *buf = c->acct_dump_buf;
+    u32 *cnt = (u32 *)(buf + coff), n = 0;
+    CU(c, cudaMemsetAsync(cnt, 0, 4, c->L.stream));
+    CU(c, run_acct_dump(c->L, c->dev.subdir, c->acct, (u32 *)(buf + aoff), (u64 *)buf, cnt, ecap));
+    CU(c, cudaMemcpyAsync(&n, cnt, 4, cudaMemcpyDeviceToHost, c->L.stream));
+    CU(c, cudaStreamSynchronize(c->L.stream));
+    const u64 got = std::min<u64>(n, ecap);
+    if (got) {
+        CU(c, cudaMemcpy(out, buf, got * sizeof(bng_acct), cudaMemcpyDeviceToHost));
+        CU(c, cudaMemcpy(addrs_out, buf + aoff, got * 4, cudaMemcpyDeviceToHost));
+    }
+    return (int64_t)got;
+}
+
+int bng_acct_enable(bng_ctx *c, int prog, int on) {
+    if (!c || prog < 0 || prog >= P_COUNT) return -EINVAL;
+    if (k_acct_mode[prog] < 0) return -EOPNOTSUPP;
+    std::lock_guard<std::mutex> g(c->mu);
+    cudaSetDevice(c->device);
+    if (on) {
+        if (int r = acct_alloc_locked(c)) return r;
+        c->acct_progs |= 1u << prog;
+    } else {
+        c->acct_progs &= ~(1u << prog);
+    }
+    return 0;
+}
+
+int bng_acct_read(bng_ctx *c, const uint32_t *addrs, uint64_t n, bng_acct *out, int32_t *results) {
+    if (!c || (n && (!addrs || !out || !results))) return -EINVAL;
+    std::lock_guard<std::mutex> g(c->mu);
+    cudaSetDevice(c->device);
+    if (int fr = acct_flush_locked(c)) return fr;
+    const u64 chunk_max = 1u << 16;
+    for (u64 done = 0; done < n; done += chunk_max) {
+        const u64 k = std::min(chunk_max, n - done);
+        const size_t ooff = (k * 4 + 255) & ~(size_t)255, roff = ooff + k * sizeof(bng_acct);
+        if (int r = ensure_io(c, roff + k * 4)) return r;
+        memcpy(c->io_host, addrs + done, k * 4);
+        CU(c, cudaMemcpyAsync(c->io_dev, c->io_host, k * 4, cudaMemcpyHostToDevice, c->L.stream));
+        CU(c, run_acct_read(c->L, c->dev.subdir, c->acct, (const u32 *)c->io_dev, k, (u64 *)(c->io_dev + ooff), (int *)(c->io_dev + roff)));
+        CU(c, cudaMemcpyAsync(c->io_host + ooff, c->io_dev + ooff, roff + k * 4 - ooff, cudaMemcpyDeviceToHost, c->L.stream));
+        CU(c, cudaStreamSynchronize(c->L.stream));
+        memcpy(out + done, c->io_host + ooff, k * sizeof(bng_acct));
+        memcpy(results + done, c->io_host + roff, k * 4);
+    }
+    return 0;
+}
+
+int64_t bng_acct_dump(bng_ctx *c, uint32_t *addrs_out, bng_acct *out, uint64_t cap) {
+    if (!c || (cap && (!addrs_out || !out))) return -EINVAL;
+    std::lock_guard<std::mutex> g(c->mu);
+    cudaSetDevice(c->device);
+    if (int fr = acct_flush_locked(c)) return fr;
+    return acct_dump_locked(c, addrs_out, out, cap);
+}
+
+// ---------------------------------------------------------------------------
 // snapshot / restore (SURVEY.md §8f-4: device-table state for HA hand-over, reference pkg/ha)
 // A snapshot is a self-describing blob: header, then per map { name, kind, key size, value size, entry count,
 // keys, values } for every hash / array / LPM / statistics map (event rings are not state).  Restore clears
@@ -1515,6 +1623,10 @@ struct SnapMapHdr {
     u32 kind, key_size, value_size, pad;
     u64 count;
 };
+// Trailing section of the accounting records: (address, struct bng_acct) pairs.  No map has this name, so a library
+// without accounting steps over it; a context that never allocated records writes no such section.
+const char kSnapAcct[] = "subscriber_acct";
+const u32 kSnapAcctKind = 5;
 } // namespace
 
 int64_t bng_snapshot(bng_ctx *c, void *buf, uint64_t cap) {
@@ -1551,6 +1663,22 @@ int64_t bng_snapshot(bng_ctx *c, void *buf, uint64_t cap) {
         out.insert(out.end(), vals.begin(), vals.begin() + (size_t)got * m->value_size);
         nmaps++;
     }
+    if (c->acct) {
+        u32 n32 = 0;
+        CU(c, cudaMemcpy(&n32, c->dev.subdir.count, 4, cudaMemcpyDeviceToHost));
+        const u64 cnt = std::max<u32>(n32, 1);
+        std::vector<u32> addrs(cnt);
+        std::vector<bng_acct> recs(cnt);
+        int64_t got = acct_dump_locked(c, addrs.data(), recs.data(), cnt);
+        if (got < 0) return got;
+        SnapMapHdr h{};
+        snprintf(h.name, sizeof(h.name), "%s", kSnapAcct);
+        h.kind = kSnapAcctKind, h.key_size = 4, h.value_size = sizeof(bng_acct), h.count = (u64)got;
+        out.insert(out.end(), (u8 *)&h, (u8 *)&h + sizeof(h));
+        out.insert(out.end(), (u8 *)addrs.data(), (u8 *)(addrs.data() + got));
+        out.insert(out.end(), (u8 *)recs.data(), (u8 *)(recs.data() + got));
+        nmaps++;
+    }
     memcpy(&out[nmaps_at], &nmaps, 8);
     if (buf && cap >= out.size()) memcpy(buf, out.data(), out.size());
     return (int64_t)out.size(); // the size needed; nothing was copied when cap is smaller
@@ -1562,6 +1690,16 @@ int bng_restore(bng_ctx *c, const void *buf, uint64_t len) {
     u64 nmaps;
     memcpy(&nmaps, p + 8, 8);
     p += 16;
+    { // the blob's records replace these; a blob without them leaves every record at zero
+        std::lock_guard<std::mutex> g(c->mu);
+        cudaSetDevice(c->device);
+        if (c->acct) {
+            CU(c, cudaMemsetAsync(c->acct, 0, ((size_t)c->dev.subdir.mask + 1) * sizeof(bng_acct), c->L.stream));
+            CU(c, cudaStreamSynchronize(c->L.stream));
+        }
+    }
+    const u8 *acct_p = nullptr;
+    u64 acct_n = 0;
     for (u64 k = 0; k < nmaps; k++) {
         if (p + sizeof(SnapMapHdr) > end) return -EINVAL;
         SnapMapHdr h;
@@ -1570,6 +1708,13 @@ int bng_restore(bng_ctx *c, const void *buf, uint64_t len) {
         h.name[sizeof(h.name) - 1] = 0;
         const u64 kb = h.count * h.key_size, vb = h.count * h.value_size;
         if (p + kb + vb > end) return -EINVAL;
+        if (!strcmp(h.name, kSnapAcct)) { // applied below, once the maps (and so the directory) are in place
+            if (h.key_size != 4 || h.value_size != sizeof(bng_acct)) return fail(c, -EINVAL, "snapshot: %s has another layout", h.name);
+            acct_p = p;
+            acct_n = h.count;
+            p += kb + vb;
+            continue;
+        }
         int id = bng_map_id(c, h.name);
         if (id >= 0) {
             MapReg *m = get_map(c, id);
@@ -1590,6 +1735,22 @@ int bng_restore(bng_ctx *c, const void *buf, uint64_t len) {
             }
         }
         p += kb + vb;
+    }
+    if (acct_n) {
+        std::lock_guard<std::mutex> g(c->mu);
+        cudaSetDevice(c->device);
+        if (int r = acct_alloc_locked(c)) return r;
+        const u64 chunk_max = 1u << 16;
+        for (u64 done = 0; done < acct_n; done += chunk_max) {
+            const u64 k = std::min(chunk_max, acct_n - done);
+            const size_t roff = (k * 4 + 255) & ~(size_t)255;
+            if (int r = ensure_io(c, roff + k * sizeof(bng_acct))) return r;
+            memcpy(c->io_host, acct_p + done * 4, k * 4);
+            memcpy(c->io_host + roff, acct_p + acct_n * 4 + done * sizeof(bng_acct), k * sizeof(bng_acct));
+            CU(c, cudaMemcpyAsync(c->io_dev, c->io_host, roff + k * sizeof(bng_acct), cudaMemcpyHostToDevice, c->L.stream));
+            CU(c, run_acct_load(c->L, c->dev.subdir, c->acct, (const u32 *)c->io_dev, (const u64 *)(c->io_dev + roff), k));
+            CU(c, cudaStreamSynchronize(c->L.stream));
+        }
     }
     return 0;
 }

@@ -1063,7 +1063,10 @@ cudaError_t run_qos(Launcher &L, const DevCtx &c, const DevBatch &b0, bool egres
 cudaError_t run_nat_egress(Launcher &L, const DevCtx &c, const DevBatch &b0) {
     DevBatch b = b0;
     b.kshift = kshift_for((u64)c.subdir.mask + 1);
-    LAUNCH((k_pipe_classify<false, false>), b.n, CLASSIFY_BPS(false), c, b, L.s.key_a, L.s.val_a, L.s.counters, sort_T(L));
+    if (L.acct_attr)
+        LAUNCH((k_pipe_classify<false, false, false, true>), b.n, CLASSIFY_BPS(false), c, b, L.s.key_a, L.s.val_a, L.s.counters, sort_T(L), L.acct_attr);
+    else
+        LAUNCH((k_pipe_classify<false, false>), b.n, CLASSIFY_BPS(false), c, b, L.s.key_a, L.s.val_a, L.s.counters, sort_T(L), nullptr);
     Grouped g;
     cudaError_t e = group_by_key(L, b.n, (u64)c.subdir.mask + 1, b.kshift, &g);
     if (e != cudaSuccess) return e;
@@ -1084,7 +1087,10 @@ cudaError_t run_nat_hairpin_xdp(Launcher &L, const DevCtx &c, const DevBatch &b)
 cudaError_t run_pipeline_up(Launcher &L, const DevCtx &c, const DevBatch &b0) {
     DevBatch b = b0;
     b.kshift = kshift_for((u64)c.subdir.mask + 1);
-    LAUNCH((k_pipe_classify<true, true>), b.n, CLASSIFY_BPS(true), c, b, L.s.key_a, L.s.val_a, L.s.counters, sort_T(L));
+    if (L.acct_attr)
+        LAUNCH((k_pipe_classify<true, true, false, true>), b.n, CLASSIFY_BPS(true), c, b, L.s.key_a, L.s.val_a, L.s.counters, sort_T(L), L.acct_attr);
+    else
+        LAUNCH((k_pipe_classify<true, true>), b.n, CLASSIFY_BPS(true), c, b, L.s.key_a, L.s.val_a, L.s.counters, sort_T(L), nullptr);
     Grouped g;
     cudaError_t e = group_by_key(L, b.n, (u64)c.subdir.mask + 1, b.kshift, &g);
     if (e != cudaSuccess) return e;
@@ -1095,7 +1101,10 @@ cudaError_t run_pipeline_up(Launcher &L, const DevCtx &c, const DevBatch &b0) {
 cudaError_t run_pipeline_tc(Launcher &L, const DevCtx &c, const DevBatch &b0) {
     DevBatch b = b0;
     b.kshift = kshift_for((u64)c.subdir.mask + 1);
-    LAUNCH((k_pipe_classify<true, true, true>), b.n, CLASSIFY_BPS(true), c, b, L.s.key_a, L.s.val_a, L.s.counters, sort_T(L));
+    if (L.acct_attr)
+        LAUNCH((k_pipe_classify<true, true, true, true>), b.n, CLASSIFY_BPS(true), c, b, L.s.key_a, L.s.val_a, L.s.counters, sort_T(L), L.acct_attr);
+    else
+        LAUNCH((k_pipe_classify<true, true, true>), b.n, CLASSIFY_BPS(true), c, b, L.s.key_a, L.s.val_a, L.s.counters, sort_T(L), nullptr);
     Grouped g;
     cudaError_t e = group_by_key(L, b.n, (u64)c.subdir.mask + 1, b.kshift, &g);
     if (e != cudaSuccess) return e;

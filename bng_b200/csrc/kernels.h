@@ -10,6 +10,7 @@ struct Scratch {
     size_t cub_tmp_bytes;
     u32 *counters; // 16 x u32 of per-run device counters
     u32 cap;       // frames the arrays above can hold
+    u32 *attr;     // [cap] per-frame accounting attribution (directory slot or DIR_NONE); allocated with the counters
 };
 
 // optional per-kernel timing (bng_prof_enable): CUDA events around every launch
@@ -22,6 +23,7 @@ struct Launcher {
     cudaStream_t stream;
     int num_sms;
     Scratch s;
+    u32 *acct_attr; // non-null: the upstream classify of this run records each frame's attribution here (acct.cu)
     unsigned long long launches;
     // per-context (= per-device) launch configuration, filled on first use: nothing here may be process-wide,
     // one process can hold contexts on several GPUs
@@ -60,11 +62,25 @@ cudaError_t run_scatter_frames(cudaStream_t st, int blocks, u8 *arena, const u32
 // table maintenance (tableops.cu); keys/values/results are device pointers
 enum { TOP_UPDATE = 0, TOP_LOOKUP = 1, TOP_DELETE = 2 };
 // dir / dir_role: the subscriber directory and which half of it table t feeds (0 none, 1 subscriber_nat, 2 qos_ingress)
+// acct: the per-subscriber counter records (nullptr until accounting is first enabled); a directory slot that is
+// claimed for an address has its record zeroed
 cudaError_t run_table_op(Launcher &L, const Tbl &t, int op, const u8 *keys, u8 *vals, int *results, u64 n, u32 flags,
-                         const Tbl &dir, int dir_role);
+                         const Tbl &dir, int dir_role, u64 *acct);
 cudaError_t run_dir_clear_half(Launcher &L, const Tbl &dir, int role);
 cudaError_t run_epoch_reset(Launcher &L, const Tbl &sessions);
 cudaError_t run_table_rebuild(Launcher &L, const Tbl &old_table, const Tbl &empty_table);
 // session expiry sweep (sweep.cu); n_expired: device counter, incremented by the number of sessions removed
 cudaError_t run_nat_sweep(Launcher &L, const DevCtx &c, u64 now, u32 *n_expired /* [0] expired, [1] tombstones seen */);
 cudaError_t run_table_dump(Launcher &L, const Tbl &t, u8 *keys_out, u8 *vals_out, u32 *count_out, u64 cap);
+
+// per-subscriber traffic accounting (acct.cu).  A record is ACCT_WORDS u64 (struct bng_acct), index-aligned with the
+// subscriber directory.  Modes of run_acct: where a frame's subscriber comes from.
+#define ACCT_WORDS 8
+enum { ACCT_ATTR = 0, ACCT_SRC = 1, ACCT_DST = 2 }; // attribution words of classify / header source / header destination
+cudaError_t run_acct(Launcher &L, const Tbl &dir, const DevBatch &b, int mode, u64 *acct);
+// results[i] = 0 / -ENOENT, out[i] zeroed on a miss; acct may be nullptr (every record reads as zero)
+cudaError_t run_acct_read(Launcher &L, const Tbl &dir, const u64 *acct, const u32 *addrs, u64 n, u64 *out, int *results);
+// every directory address with its record, compacted at *count (grows past cap: only cap are written)
+cudaError_t run_acct_dump(Launcher &L, const Tbl &dir, const u64 *acct, u32 *addrs_out, u64 *out, u32 *count, u64 cap);
+// record of every address of the list that has a directory entry := the given one (snapshot restore)
+cudaError_t run_acct_load(Launcher &L, const Tbl &dir, u64 *acct, const u32 *addrs, const u64 *recs, u64 n);

@@ -38,9 +38,13 @@
 // reaches NAT, so whatever NAT would do to a frame with a rate-limited bucket — session counters, rewrite,
 // new flows, even the "no allocation" statistic — waits for the bucket's verdict: the frame goes to the ordered
 // phase with DEFER_FLAG and nat44_egress runs there, after token_bucket_check().
-template <bool AS, bool QOS, bool TC = false>
+// ACCT: traffic accounting is on for this run: attr[i] := the directory slot frame i is charged to (its source
+// address as it entered), or DIR_NONE when the frame is not attributable or antispoof dropped it (acct.cu).  A
+// template parameter, so that the instantiations without it are the code they were.
+template <bool AS, bool QOS, bool TC = false, bool ACCT = false>
 __global__ void __launch_bounds__(BLOCK, CLASSIFY_BPS(AS))
-    k_pipe_classify(const __grid_constant__ DevCtx c, const __grid_constant__ DevBatch b, u32 *skey, u32 *sval, u32 *cnt, u32 *T) {
+    k_pipe_classify(const __grid_constant__ DevCtx c, const __grid_constant__ DevBatch b, u32 *skey, u32 *sval, u32 *cnt, u32 *T,
+                    u32 *attr) {
     __shared__ SmallTabs st;
     scratch_reset(cnt, T);
     __shared__ BlockStats bs;
@@ -140,7 +144,7 @@ __global__ void __launch_bounds__(BLOCK, CLASSIFY_BPS(AS))
         const bool alive = act && v != TC_SHOT && ip4;
 
         // ---- phase 3: the subscriber directory: does this address own a NAT block / a bucket? ----
-        u32 nat_slot = DIR_NONE, qos_slot = DIR_NONE, dir_idx = 0;
+        u32 nat_slot = DIR_NONE, qos_slot = DIR_NONE, dir_idx = ACCT ? DIR_NONE : 0; // (ACCT: DIR_NONE = no entry)
         if (alive) {
             const u64 k0 = (u64)d0.w[0] | ((u64)d0.w[1] << 32), k1 = (u64)d0.w[4] | ((u64)d0.w[5] << 32);
             if (k0 == sk) {
@@ -254,6 +258,15 @@ __global__ void __launch_bounds__(BLOCK, CLASSIFY_BPS(AS))
             b.verdict[i] = (u8)v;
             skey[i] = okey;
             sval[i] = oval;
+        }
+        if (ACCT) {
+            // a frame too short for classify's IPv4 parse (bytes 26-29 present, 30-33 not) is still its source's
+            u32 aw = alive ? dir_idx : DIR_NONE;
+            if (act && !ip4 && dlen >= 30 && h.b16(12) == ETH_P_IP_LE && (!AS || v != TC_SHOT)) {
+                const u8 *de = tbl_find<1, false>(c.subdir, &sk);
+                if (de) aw = (u32)((de - c.subdir.slots) >> 4);
+            }
+            if (act) attr[i] = aw;
         }
         if (AS) ascnt_spill(bs, cn);
         if (QOS && __any_sync(0xffffffffu, n_qbytes >= 0x04000000u)) {

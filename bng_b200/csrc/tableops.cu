@@ -43,11 +43,18 @@ __device__ __forceinline__ void val_from_slot(const Tbl &t, u8 *abi, const u8 *s
 // role: which half of the directory entry the table being changed owns
 enum { DIR_ROLE_NONE = 0, DIR_ROLE_NAT = 1, DIR_ROLE_QOS = 2 };
 
-__device__ __forceinline__ void dir_set(const Tbl &dir, u64 key, int role, u32 val) {
+__device__ __forceinline__ void dir_set(const Tbl &dir, u64 key, int role, u32 val, u64 *acct) {
     bool created;
     u8 *d = tbl_find_or_claim<1>(dir, &key, &created);
     if (!d) return; // cannot happen: the directory is sized for both maps' max_entries
-    if (created) *(u64 *)(d + 8) = ~0ull; // DIR_NONE | DIR_NONE << 32
+    if (created) {
+        *(u64 *)(d + 8) = ~0ull; // DIR_NONE | DIR_NONE << 32
+        if (acct) { // the address's traffic record starts at zero, whoever held the slot before
+            u64 *r = acct + (size_t)((d - dir.slots) >> 4) * ACCT_WORDS;
+#pragma unroll
+            for (int j = 0; j < ACCT_WORDS; j++) r[j] = 0;
+        }
+    }
     *(u32 *)(d + (role == DIR_ROLE_NAT ? 8 : 12)) = val;
     if (created) tbl_publish(d, key);
 }
@@ -65,7 +72,7 @@ __device__ __forceinline__ u32 dir_value(const Tbl &t, const u8 *slot, int role)
 
 template <int KW>
 __global__ void k_table_op(const __grid_constant__ Tbl t, int op, const u8 *keys, u8 *vals, int *results, u64 n, u32 flags,
-                           const __grid_constant__ Tbl dir, int dir_role) {
+                           const __grid_constant__ Tbl dir, int dir_role, u64 *acct) {
     for (u64 i = blockIdx.x * (u64)blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x) {
         u64 kw[KW];
         load_key<KW>(t, keys + i * t.key_size, kw);
@@ -104,7 +111,7 @@ __global__ void k_table_op(const __grid_constant__ Tbl t, int op, const u8 *keys
                     if (created) tbl_publish(s, kw[0]);
                 }
             }
-            if (!r && dir_role) dir_set(dir, kw[0], dir_role, dir_value(t, s, dir_role));
+            if (!r && dir_role) dir_set(dir, kw[0], dir_role, dir_value(t, s, dir_role), acct);
         }
         results[i] = r;
     }
@@ -145,17 +152,17 @@ __global__ void k_table_dump(const __grid_constant__ Tbl t, u8 *keys_out, u8 *va
 }
 
 cudaError_t run_table_op(Launcher &L, const Tbl &t, int op, const u8 *keys, u8 *vals, int *results, u64 n, u32 flags,
-                         const Tbl &dir, int dir_role) {
+                         const Tbl &dir, int dir_role, u64 *acct) {
     if (n == 0) return cudaSuccess;
     int block = 128;
     u64 want = (n + block - 1) / block;
     int grid = (int)(want < (u64)L.num_sms * 8 ? want : (u64)L.num_sms * 8);
     if (t.key_size <= 8)
-        k_table_op<1><<<grid, block, 0, L.stream>>>(t, op, keys, vals, results, n, flags, dir, dir_role);
+        k_table_op<1><<<grid, block, 0, L.stream>>>(t, op, keys, vals, results, n, flags, dir, dir_role, acct);
     else if (t.key_size == 16)
-        k_table_op<2><<<grid, block, 0, L.stream>>>(t, op, keys, vals, results, n, flags, dir, 0);
+        k_table_op<2><<<grid, block, 0, L.stream>>>(t, op, keys, vals, results, n, flags, dir, 0, nullptr);
     else
-        k_table_op<4><<<grid, block, 0, L.stream>>>(t, op, keys, vals, results, n, flags, dir, 0);
+        k_table_op<4><<<grid, block, 0, L.stream>>>(t, op, keys, vals, results, n, flags, dir, 0, nullptr);
     L.launches++;
     return cudaGetLastError();
 }

@@ -12,7 +12,7 @@ import os
 
 import numpy as np
 
-from .layouts import as_bytes
+from .layouts import as_bytes, bng_acct
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("BNG_B200_LIB") or os.path.join(HERE, "libbng_b200.so")  # override: A/B builds
@@ -101,6 +101,9 @@ def load_library() -> C.CDLL:
         "bng_prof_read": ([vp, C.c_char_p, u64], C.c_int64),
         "bng_host_alloc": ([C.c_size_t], vp),
         "bng_host_free": ([vp], None),
+        "bng_acct_enable": ([vp, i32, i32], i32),
+        "bng_acct_read": ([vp, vp, u64, vp, vp], i32),
+        "bng_acct_dump": ([vp, vp, vp, u64], C.c_int64),
     }
     for name, (args, res) in protos.items():
         fn = getattr(lib, name)
@@ -118,6 +121,7 @@ EXPORTED_SYMBOLS = (
     "bng_stats_device_ptr", "bng_launch_count", "bng_lru_overflow", "bng_events_lost", "bng_prof_enable",
     "bng_prof_read", "bng_host_alloc", "bng_host_free", "bng_map_update_staged", "bng_staged_info",
     "bng_comm_unique_id", "bng_comm_init", "bng_sync_reduce", "bng_sweep", "bng_lru_evictions", "bng_snapshot", "bng_restore", "bng_table_rebuilds",
+    "bng_acct_enable", "bng_acct_read", "bng_acct_dump",
 )
 
 
@@ -314,6 +318,31 @@ class Dataplane:
     def restore(self, blob: bytes):
         buf = C.create_string_buffer(blob, len(blob))
         self._chk(self.lib.bng_restore(self.h, buf, len(blob)), "restore")
+
+    # ---- per-subscriber traffic accounting ----
+    def acct_enable(self, prog, on: bool = True):
+        """Count the octets and packets of `prog`'s runs per subscriber address (off by default)."""
+        pid = prog if isinstance(prog, int) else self.prog_id(prog)
+        self._chk(self.lib.bng_acct_enable(self.h, pid, 1 if on else 0), f"acct_enable({prog})")
+
+    def acct_read(self, addrs):
+        """addrs: u8[n, 4] (qos_ingress key bytes) or u32[n] -> (bng_acct records[n], found bool[n])."""
+        a = np.asarray(addrs)
+        a = np.ascontiguousarray(a).view("<u4").reshape(-1) if a.dtype == np.uint8 else np.ascontiguousarray(a, "<u4").reshape(-1)
+        out = np.zeros(len(a), dtype=bng_acct)
+        res = np.zeros(len(a), dtype=np.int32)
+        self._chk(self.lib.bng_acct_read(self.h, a.ctypes.data, len(a), out.ctypes.data, res.ctypes.data), "acct_read")
+        return out, res == 0
+
+    def acct_dump(self):
+        """(addresses u32[n], bng_acct records[n]) of every subscriber address, sorted by address bytes."""
+        cap = max(int(self.map_info("subscriber_nat")["count"]) + int(self.map_info("qos_ingress")["count"]), 1)
+        a = np.zeros(cap, dtype="<u4")
+        out = np.zeros(cap, dtype=bng_acct)
+        n = self._chk(self.lib.bng_acct_dump(self.h, a.ctypes.data, out.ctypes.data, cap), "acct_dump")
+        a, out = a[:n], out[:n]
+        order = np.argsort(a.byteswap(), kind="stable")
+        return a[order], out[order]
 
     def sweep(self, now_ns: int) -> int:
         """Session expiry sweep at now_ns; returns the number of sessions removed."""

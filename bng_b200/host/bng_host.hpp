@@ -24,6 +24,7 @@
 #include <chrono>
 #include <cstdint>
 #include <cstring>
+#include <functional>
 #include <map>
 #include <memory>
 #include <mutex>
@@ -91,6 +92,62 @@ inline Error MapErr(const char *what, int rc) {
     if (rc == 0) return Nil();
     return Error(std::string(what) + ": errno " + std::to_string(-rc));
 }
+
+// ===========================================================================
+// RADIUS accounting counters (reference pkg/radius/accounting.go:128-137: SessionCounters and the CounterFetcher
+// callback that SetCounterFetcher installs).  Acct-Input-* is traffic FROM the user: the upstream pass pair of the
+// subscriber's bng_acct record; Acct-Output-* the downstream pass pair.
+namespace radius {
+
+struct SessionCounters {
+    uint64_t InputOctets = 0, OutputOctets = 0, InputPackets = 0, OutputPackets = 0;
+};
+
+inline SessionCounters CountersOf(const bng_acct &a) {
+    SessionCounters s;
+    s.InputOctets = a.up_bytes;
+    s.InputPackets = a.up_packets;
+    s.OutputOctets = a.down_bytes;
+    s.OutputPackets = a.down_packets;
+    return s;
+}
+
+// func(sessionID string) (*SessionCounters, error)
+using CounterFetcher = std::function<Result<SessionCounters>(const std::string &session_id)>;
+// session id -> the subscriber's IPv4 address as the qos_ingress key holds it (the accounting manager knows the
+// Framed-IP-Address of every session it started)
+using SessionAddr = std::function<std::optional<uint32_t>(const std::string &session_id)>;
+// reads one subscriber's record: 0, -ENOENT or a negative errno
+using AcctReader = std::function<int(uint32_t addr_key, bng_acct *out)>;
+
+inline CounterFetcher MakeCounterFetcher(SessionAddr addr_of, AcctReader read) {
+    return [addr_of = std::move(addr_of), read = std::move(read)](const std::string &id) {
+        Result<SessionCounters> r;
+        auto a = addr_of(id);
+        if (!a) {
+            r.err = Error("session " + id + ": no address");
+            return r;
+        }
+        bng_acct rec{};
+        if (Error e = MapErr("bng_acct_read", read(*a, &rec))) {
+            r.err = e;
+            return r;
+        }
+        r.value = CountersOf(rec);
+        return r;
+    };
+}
+
+// the reader of one context
+inline AcctReader ContextReader(std::shared_ptr<Backend> b) {
+    return [b = std::move(b)](uint32_t addr, bng_acct *out) {
+        int32_t res = 0;
+        int rc = bng_acct_read(b->ctx, &addr, 1, out, &res);
+        return rc ? rc : res;
+    };
+}
+
+} // namespace radius
 
 // ===========================================================================
 namespace ebpf {

@@ -204,6 +204,23 @@ class Router {
         }
         return rc;
     }
+    // Per-subscriber traffic record (bng_acct_read) from the shard that owns the address: upstream frames follow
+    // the subscriber's MAC to it and downstream frames are steered to it by (public address, port block)
+    // (SteerDownstream), so its record is the whole record and no other shard holds one.
+    int AcctOwner(uint32_t addr_key) const {
+        auto s = dir_->ShardOfIP(addr_key);
+        return s ? (int)*s : -ENOENT;
+    }
+    int AcctRead(uint32_t addr_key, bng_acct *out) {
+        int o = AcctOwner(addr_key);
+        if (o < 0) return o;
+        int32_t res = 0;
+        int rc = bng_acct_read(shards_[(size_t)o]->ctx, &addr_key, 1, out, &res);
+        return rc ? rc : res;
+    }
+    radius::AcctReader Reader() {
+        return [this](uint32_t addr, bng_acct *out) { return AcctRead(addr, out); };
+    }
     // PERCPU-style totals: the packed counter vector summed over the shards (host-side sum; with a communicator
     // per context bng_sync_reduce() does the same on the devices)
     int Totals(uint64_t out[BNG_NUM_STATS]) {

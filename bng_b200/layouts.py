@@ -112,7 +112,12 @@ dhcp_stats = np.dtype([(n, "<u8") for n in (
 # bpf/maps.h:218-220 (32 B)
 circuit_id_key = np.dtype([("data", "u1", 32)])
 
-assert subscriber_binding.itemsize == 24 and token_bucket.itemsize == 32
+# include/bng_b200.h struct bng_acct (64 B): per-subscriber traffic totals, not a reference map
+bng_acct = np.dtype([(n, "<u8") for n in (
+    "up_packets", "up_bytes", "up_drop_packets", "up_drop_bytes",
+    "down_packets", "down_bytes", "down_drop_packets", "down_drop_bytes")])
+
+assert subscriber_binding.itemsize == 24 and token_bucket.itemsize == 32 and bng_acct.itemsize == 64
 assert nat_key.itemsize == 16 and eim_key.itemsize == 8 and eim_mapping.itemsize == 32
 assert nat_session.itemsize == 80 and port_block.itemsize == 32 and subscriber_nat.itemsize == 64
 assert nat_stats.itemsize == 104 and nat_log_entry.itemsize == 40 and nat_config.itemsize == 16

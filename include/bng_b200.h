@@ -180,6 +180,42 @@ int bng_sync_reduce(bng_ctx *ctx, uint64_t *totals_out /* [BNG_NUM_STATS] */);
 int64_t bng_snapshot(bng_ctx *ctx, void *buf, uint64_t cap);
 int bng_restore(bng_ctx *ctx, const void *buf, uint64_t len);
 
+/* ---- per-subscriber traffic accounting (what RADIUS Accounting Interim-Update / Stop report) ----
+ * One record per subscriber address: an address that keys a subscriber_nat or a qos_ingress entry (staged upserts
+ * included).  Counters are totals since the address got its entry; they never go backwards.
+ *   - Bytes are the frame's len as the batch passes it in (skb->len).
+ *   - Upstream programs (nat44_egress, qos_ingress_prog, pipeline_up, pipeline_tc) charge a frame to the IPv4 SOURCE
+ *     address it entered the program with (before SNAT): untagged Ethernet II, ethertype 0x0800, bytes 26-29 present.
+ *   - Downstream programs (nat44_ingress, qos_egress_prog) charge a frame to the IPv4 DESTINATION address it leaves
+ *     with (after DNAT), bytes 30-33: a frame nat44_ingress did not translate keeps its public address.
+ *   - Verdict TC_ACT_OK counts in the pass pair, TC_ACT_SHOT in the drop pair (NAT port exhaustion, token bucket).
+ *     In the two pipelines a frame that antispoof drops is not counted at all: it may have forged its address.
+ *   - A frame whose address has no entry when the batch runs is not counted anywhere.
+ *   - A record starts at zero when its address gets its entry; it survives updates of either map, the expiry
+ *     sweep, LRU eviction and flow-table rebuilds, and ends when the address loses both entries (delete or
+ *     bng_map_clear).  Snapshots carry the records (a trailing "subscriber_acct" section), so an HA hand-over keeps
+ *     them; bng_restore() of a blob without that section leaves every record at zero.
+ * Accounting is enabled per program and off by default.  The first bng_acct_enable() allocates the records:
+ * 64 bytes per subscriber-directory slot, i.e. 64 x (the power of two >= max(64, 2 x max_subscribers)) bytes —
+ * 128 MiB at the default 1e6 subscribers — plus 4 bytes per frame of max_batch.  A context that never enables
+ * accounting allocates neither. */
+typedef struct bng_acct {
+    uint64_t up_packets, up_bytes;            /* upstream, verdict TC_ACT_OK */
+    uint64_t up_drop_packets, up_drop_bytes;  /* upstream, verdict TC_ACT_SHOT */
+    uint64_t down_packets, down_bytes;        /* downstream, verdict TC_ACT_OK */
+    uint64_t down_drop_packets, down_drop_bytes;
+} bng_acct;
+/* on != 0 enables accounting of the program's runs from the next bng_prog_run on.  -EOPNOTSUPP for
+ * antispoof_ingress, nat44_hairpin_xdp and dhcp_fastpath_prog; -EINVAL for an unknown program id. */
+int bng_acct_enable(bng_ctx *ctx, int prog, int on);
+/* Records of n addresses (4 bytes each, in the byte order of the qos_ingress key).  results[i] = 0, or -ENOENT
+ * when the address has no entry (out[i] is then zeroed).  Staged upserts are applied first and the read sees
+ * everything queued on the context's stream, as bng_map_lookup() does.  Returns 0 or a negative errno. */
+int bng_acct_read(bng_ctx *ctx, const uint32_t *addrs, uint64_t n, bng_acct *out, int32_t *results);
+/* Up to cap (address, record) pairs of the addresses that have an entry, in no particular order (compacted on the
+ * GPU, then copied out).  Returns the number written or a negative errno, as bng_map_dump() does. */
+int64_t bng_acct_dump(bng_ctx *ctx, uint32_t *addrs_out, bng_acct *out, uint64_t cap);
+
 /* ---- diagnostics ---- */
 uint64_t bng_launch_count(bng_ctx *ctx);  /* kernels launched by this context so far */
 uint64_t bng_lru_overflow(bng_ctx *ctx);  /* inserts that found no victim to evict in a full LRU map (should stay 0) */
