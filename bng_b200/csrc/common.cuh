@@ -57,7 +57,7 @@ struct Tbl {
     u8 *slots;
     u32 *count;      // live entries
     u32 mask;        // capacity - 1 (capacity is a power of two)
-    u32 home_mask;   // hash -> home slot: mask, or mask & ~1 for tables whose lookups fetch the home PAIR of slots at once
+    u32 home_mask;   // hash -> home slot: mask, or mask & ~1 for even home slots (bng_open: bindings, subscriber directory)
     u32 slot_bytes;  // multiple of 32
     u32 voff;        // value offset inside the slot
     u32 max_entries; // the reference map's max_entries
@@ -401,10 +401,8 @@ __device__ __forceinline__ bool tbl_evict_near(const Tbl &t, u32 home, u64 *stat
 // The state words of PROBE_W consecutive slots are requested together: in a table that lives in DRAM every probe
 // step is a full memory round trip, and the longest chain among a warp's 32 lanes (3-4 steps at load 0.25) costs
 // that many round trips per lookup.  Every speculative slot is a 64-byte DRAM burst, though, and the cold-start
-// kernel is bound by the rate of scattered DRAM bursts, so the window stays narrow (-DPROBE_W=1|2|4 to compare).
-#ifndef PROBE_W
+// kernel is bound by the rate of scattered DRAM bursts, so the window stays narrow.
 #define PROBE_W 2
-#endif
 template <int KW>
 __device__ __forceinline__ u8 *tbl_find_ins(const Tbl &t, const u64 *k, u32 *ins) {
     *ins = 0xFFFFFFFFu;
@@ -747,76 +745,31 @@ __device__ __forceinline__ void hdr_store_chunk(const Hdr64 &h, u8 *p, int c) {
 struct __align__(16) U256 {
     u32 w[8];
 };
-// L2 eviction priority of a 32-byte access.  Frames stream through once: evict-first is meant to keep them
-// from pushing the flow table's hot sectors (touched ~6 times per batch) out of the 50 MB L2; the flow-table
-// probe asks to stay (evict-last).  Both are off by default: neither gain measured on H100 is clear of the
-// run-to-run spread (DESIGN.md §5).
-enum { L2_NORMAL = 0, L2_FIRST = 1, L2_LAST = 2 };
-#ifndef FRAME_POLICY
-#define FRAME_POLICY L2_NORMAL
-#endif
-#ifndef SES_POLICY
-#define SES_POLICY L2_NORMAL
-#endif
-// sm_90 has the .L2::evict_{first,last} qualifiers on 256-bit accesses only; a 128-bit access carries its
-// priority as an L2 cache policy (createpolicy) through .L2::cache_hint.
-template <int POLICY>
-__device__ __forceinline__ u64 l2_policy() {
-    u64 pol;
-    if (POLICY == L2_FIRST)
-        asm("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
-    else
-        asm("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
-    return pol;
-}
+// Each half is one inline-asm ld/st.global.v4.u32 with the default L2 policy (DESIGN.md §5 has the eviction
+// hints that were measured and not kept).
 #define BNG_LDG128(r, q)                                                                                         \
     asm volatile("ld.global.v4.u32 {%0,%1,%2,%3}, [%4];"                                                         \
                  : "=r"((r)[0]), "=r"((r)[1]), "=r"((r)[2]), "=r"((r)[3])                                        \
                  : "l"(q)                                                                                        \
                  : "memory")
-#define BNG_LDG128_HINT(r, q, pol)                                                                               \
-    asm volatile("ld.global.L2::cache_hint.v4.u32 {%0,%1,%2,%3}, [%4], %5;"                                      \
-                 : "=r"((r)[0]), "=r"((r)[1]), "=r"((r)[2]), "=r"((r)[3])                                        \
-                 : "l"(q), "l"(pol)                                                                              \
-                 : "memory")
 #define BNG_STG128(q, w)                                                                                         \
     asm volatile("st.global.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(q), "r"((w)[0]), "r"((w)[1]), "r"((w)[2]),         \
                  "r"((w)[3])                                                                                     \
                  : "memory")
-#define BNG_STG128_HINT(q, w, pol)                                                                               \
-    asm volatile("st.global.L2::cache_hint.v4.u32 [%0], {%1,%2,%3,%4}, %5;" ::"l"(q), "r"((w)[0]), "r"((w)[1]),   \
-                 "r"((w)[2]), "r"((w)[3]), "l"(pol)                                                              \
-                 : "memory")
-template <int POLICY = L2_NORMAL>
 __device__ __forceinline__ U256 ldg256(const void *p) {
     U256 r;
     const u8 *q = (const u8 *)p;
-    if (POLICY == L2_NORMAL) {
-        BNG_LDG128(&r.w[0], q);
-        BNG_LDG128(&r.w[4], q + 16);
-    } else {
-        const u64 pol = l2_policy<POLICY>();
-        BNG_LDG128_HINT(&r.w[0], q, pol);
-        BNG_LDG128_HINT(&r.w[4], q + 16, pol);
-    }
+    BNG_LDG128(&r.w[0], q);
+    BNG_LDG128(&r.w[4], q + 16);
     return r;
 }
-template <int POLICY = L2_NORMAL>
 __device__ __forceinline__ void stg256(void *p, const u32 *w) {
     u8 *q = (u8 *)p;
-    if (POLICY == L2_NORMAL) {
-        BNG_STG128(q, &w[0]);
-        BNG_STG128(q + 16, &w[4]);
-    } else {
-        const u64 pol = l2_policy<POLICY>();
-        BNG_STG128_HINT(q, &w[0], pol);
-        BNG_STG128_HINT(q + 16, &w[4], pol);
-    }
+    BNG_STG128(q, &w[0]);
+    BNG_STG128(q + 16, &w[4]);
 }
 #undef BNG_LDG128
-#undef BNG_LDG128_HINT
 #undef BNG_STG128
-#undef BNG_STG128_HINT
 // Frame header load: two 32-byte loads when the whole warp's frames allow it (32-byte aligned and 64
 // bytes inside the arena), 16-byte chunks otherwise.  `wide` must be warp-uniform.
 __device__ __forceinline__ void hdr_load_wide(Hdr64 &h, const u8 *p, u32 len, bool wide) {
@@ -824,8 +777,8 @@ __device__ __forceinline__ void hdr_load_wide(Hdr64 &h, const u8 *p, u32 len, bo
         U256 a, b;
 #pragma unroll
         for (int k = 0; k < 8; k++) a.w[k] = b.w[k] = 0;
-        if (len > 0) a = ldg256<FRAME_POLICY>(p);
-        if (len > 32) b = ldg256<FRAME_POLICY>(p + 32);
+        if (len > 0) a = ldg256(p);
+        if (len > 32) b = ldg256(p + 32);
 #pragma unroll
         for (int k = 0; k < 8; k++) {
             h.w[k] = a.w[k];

@@ -49,9 +49,7 @@ thread_local std::string g_open_err;
 } // namespace
 
 // buffers of the zero-copy pipeline: three stages (in, compute, out) in flight need three
-#ifndef ZC_BUFS
 #define ZC_BUFS 3
-#endif
 
 struct bng_ctx {
     std::mutex mu;
@@ -81,7 +79,6 @@ struct bng_ctx {
     u32 *zc_off[ZC_BUFS] = {}, *zc_len[ZC_BUFS] = {}, *zc_len0[ZC_BUFS] = {}, *zc_prio[ZC_BUFS] = {};
     u32 zc_hb = 0;
     u32 zc_chunk = 1u << 18; // frames per chunk of the zero-copy pipeline
-    u32 zc_bps = 1;          // blocks per SM of the header gather / scatter kernels (PCIe-bound: hostio.cu)
     // staged upserts (bng_map_update_staged): per map, keys/values in arrival order, applied at the next batch boundary
     struct Staged {
         std::vector<u8> keys, vals;
@@ -558,7 +555,6 @@ bng_ctx *bng_open(const bng_open_opts *o) {
     }
     c->L.num_sms = prop.multiProcessorCount;
     c->zc_chunk = zc_chunk_frames();
-    if (const char *e = getenv("BNG_ZC_BLOCKS_PER_SM")) c->zc_bps = (u32)std::min(16, std::max(1, atoi(e))); // tuning knob
     OPEN_CU(cudaStreamCreateWithFlags(&c->L.stream, cudaStreamNonBlocking));
 
     u32 max_subs = opts.max_subscribers ? opts.max_subscribers : 1000000u;
@@ -591,7 +587,7 @@ bng_ctx *bng_open(const bng_open_opts *o) {
     // subscriber directory: 16-byte slots, as many as the per-subscriber maps have, room for both maps' keys
     OPEN_R(make_table(c, &d.subdir, 4, 8, 8, max_subs, 0, 16));
     d.subdir.max_entries = std::min<u64>(2ull * max_subs, d.subdir.mask);
-    d.subdir.home_mask = d.subdir.mask & ~1u; // classify fetches the home pair (32 bytes) in one load
+    d.subdir.home_mask = d.subdir.mask & ~1u; // even home slots: part of the directory's slot layout
     OPEN_R(make_lpm(c, &d.ranges_v4, 256));
     OPEN_R(make_lpm(c, &d.priv_ranges, 64));
     OPEN_R(dev_alloc(c, (void **)&d.as_config, 16, 0));
@@ -1044,11 +1040,9 @@ static int run_host_zero_copy(bng_ctx *c, int prog, bng_batch *bb, u8 *arena_dev
     const u32 hb_need = tc ? 96u : 448u;
     const bool contiguous = !bb->off16 && bb->stride <= hb_need;
     const u32 hb = contiguous ? bb->stride : hb_need;         // compact slot stride
-    // The TC programs write below byte 16 only in flagged frames (ihl = 0), but the first 16 bytes are written back
-    // all the same: ONE 64-byte PCIe write per frame rather than a 16- and a 32-byte one (what the link counts is
-    // TLPs, not bytes).  BNG_ZC_SKIP_CH0=1 restores the 48-byte write-back for A/B runs.
-    static const bool skip_ch0 = getenv("BNG_ZC_SKIP_CH0") != nullptr;
-    const u32 first_chunk = (tc && skip_ch0) ? 1u : 0u;
+    // The TC programs write below byte 16 only in frames with ihl = 0, but the first 16 bytes are written back all
+    // the same: ONE 64-byte PCIe write per frame rather than a 16- and a 32-byte one (what the link counts is TLPs,
+    // not bytes).
     if (!c->s_in) {
         CU(c, cudaStreamCreateWithFlags(&c->s_in, cudaStreamNonBlocking));
         CU(c, cudaStreamCreateWithFlags(&c->s_out, cudaStreamNonBlocking));
@@ -1103,7 +1097,7 @@ static int run_host_zero_copy(bng_ctx *c, int prog, bng_batch *bb, u8 *arena_dev
             CU(c, cudaMemcpyAsync(c->zc_hdr[buf], (u8 *)bb->pkts + (size_t)base * hb, (size_t)cn * hb, cudaMemcpyHostToDevice,
                                   c->s_in));
         } else {
-            CU(c, run_gather_frames(c->s_in, c->L.num_sms * (int)c->zc_bps, chunk_arena, bb->off16 ? c->zc_off[buf] : nullptr, c->zc_len[buf],
+            CU(c, run_gather_frames(c->s_in, c->L.num_sms, chunk_arena, bb->off16 ? c->zc_off[buf] : nullptr, c->zc_len[buf],
                                     bb->stride, cn, hb, tc, c->zc_hdr[buf], c->zc_len0[buf]));
             c->L.launches++;
         }
@@ -1136,8 +1130,8 @@ static int run_host_zero_copy(bng_ctx *c, int prog, bng_batch *bb, u8 *arena_dev
             CU(c, cudaMemcpyAsync((u8 *)bb->pkts + (size_t)base * hb, c->zc_hdr[buf], (size_t)cn * hb, cudaMemcpyDeviceToHost,
                                   c->s_out));
         } else {
-            CU(c, run_scatter_frames(c->s_out, c->L.num_sms * (int)c->zc_bps, chunk_arena, bb->off16 ? c->zc_off[buf] : nullptr,
-                                     c->zc_len0[buf], bb->stride, cn, hb, c->zc_hdr[buf], first_chunk));
+            CU(c, run_scatter_frames(c->s_out, c->L.num_sms, chunk_arena, bb->off16 ? c->zc_off[buf] : nullptr, c->zc_len0[buf],
+                                     bb->stride, cn, hb, c->zc_hdr[buf]));
             c->L.launches++;
         }
         CU(c, cudaMemcpyAsync(bb->verdict + base, c->zc_verdict[buf], cn, cudaMemcpyDeviceToHost, c->s_out));

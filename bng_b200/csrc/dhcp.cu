@@ -285,13 +285,10 @@ __device__ __forceinline__ int dhcp_one(const DevCtx &c, BlockStats &bs, u8 *p, 
 // would put them on 1 or 2.  Frames whose options end beyond it (QinQ + IPv4 options) run in place.
 #define DH_SLOT 400
 
-// DHCP_TILE_TMA: in a fixed-stride arena (a receive ring: what a NIC fills) the 128 frames of a tile are one
+// Tile mode: in a fixed-stride arena (a receive ring: what a NIC fills) the 128 frames of a tile are one
 // contiguous run, so the whole tile moves with ONE bulk copy each way instead of one per frame — the per-frame
 // version issues 2 x 2^22 TMA operations per batch, a few dozen cycles apart on every SM, and that, not HBM,
-// bounds it.
-#ifndef DHCP_TILE_TMA
-#define DHCP_TILE_TMA 1
-#endif
+// bounds it.  Every other arena (an offset table, or slots that do not fit a staging slot) moves frame by frame.
 __global__ void __launch_bounds__(DH_TILE) k_dhcp_fastpath(const __grid_constant__ DevCtx c, const __grid_constant__ DevBatch b) {
     extern __shared__ __align__(128) u8 stage[]; // DH_TILE * DH_SLOT
     __shared__ BlockStats bs;
@@ -305,7 +302,7 @@ __global__ void __launch_bounds__(DH_TILE) k_dhcp_fastpath(const __grid_constant
     }
     __syncthreads();
     // tile mode: fixed stride no larger than a staging slot, every frame's bytes inside its slot
-    const bool tile_mode = DHCP_TILE_TMA && !b.off16 && b.stride <= DH_SLOT && b.cap == b.stride;
+    const bool tile_mode = !b.off16 && b.stride <= DH_SLOT && b.cap == b.stride;
     const u32 sstride = tile_mode ? b.stride : DH_SLOT; // slot stride in shared memory
     u8 *mine = stage + (size_t)threadIdx.x * sstride;
     const u32 mine_a = (u32)__cvta_generic_to_shared(mine), stage_a = (u32)__cvta_generic_to_shared(stage);

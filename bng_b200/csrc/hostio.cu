@@ -8,18 +8,15 @@
 // How many bytes can a program touch?  The TC programs (antispoof, QoS, NAT44, the pipeline) read at most
 // the Ethernet + IPv4 header and 20 bytes of L4 header at 14 + ihl*4: 54 bytes when ihl = 5 — one 64-byte
 // slot covers it — and up to 14 + 60 + 20 = 94 bytes when the header carries options (bpf/nat44.c:606-653,
-// 752-798).  Compact slots are therefore 96 bytes apart; the first 64 bytes are always moved (both ways: a single
-// 64-byte PCIe write per frame costs less than the 48 bytes that can change sent as two), the two
-// further 16-byte chunks only for frames whose ihl says the L4 header reaches them.  The TC programs never
-// write below byte 16 — except nat44_egress on a frame with ihl = 0, whose "TCP source port" is bytes
-// 14-15 (the L4 header then overlaps the IP header); such frames are flagged so the scatter writes their
-// first chunk back too.  dhcp_fastpath_prog touches up to 14 + 8 (QinQ) + 60 + 8 + 240 + 64 = 394 bytes and
-// rewrites the Ethernet header: 448-byte slots, everything scattered back.
+// 752-798).  Compact slots are therefore 96 bytes apart.  The first min(len, 64) bytes of every frame are moved
+// both ways, the two further 16-byte chunks only for frames whose ihl says the L4 header reaches them: the scatter
+// writes back every chunk the gather moved.  Chunk 0 included, although the TC programs write below byte 16 only
+// in nat44_egress on a frame with ihl = 0 (its "TCP source port" is bytes 14-15): a single 64-byte PCIe write per
+// frame costs less than the 48 bytes that can change sent as two.  dhcp_fastpath_prog touches up to 14 + 8 (QinQ)
+// + 60 + 8 + 240 + 64 = 394 bytes and rewrites the Ethernet header: 448-byte slots, everything scattered back.
 #include "kernels.h"
 
-#define ZC_CH0_DIRTY 0x80000000u // need[] flag: the program may have written bytes 0..15 of this frame
-
-// dst[f][0..need) <- arena[off(f) .. off(f)+need); need[f] = bytes moved (+ ZC_CH0_DIRTY)
+// dst[f][0..need) <- arena[off(f) .. off(f)+need); need[f] = bytes moved
 __global__ void __launch_bounds__(256) k_gather_frames(const u8 *__restrict__ arena, const u32 *__restrict__ off16,
                                                        const u32 *__restrict__ len, u32 stride, u32 n, u32 slot, u32 tc,
                                                        u8 *dst, u32 *need) {
@@ -49,23 +46,20 @@ __global__ void __launch_bounds__(256) k_gather_frames(const u8 *__restrict__ ar
                 for (u32 c = 4; c * 16 < want; c++) *(uint4 *)(d + c * 16) = *(const uint4 *)(src + c * 16);
                 nd = want;
             }
-            if (ip4 && ihl == 0) nd |= ZC_CH0_DIRTY;
         }
         need[f] = nd;
     }
 }
 
-// arena[off(f) .. ) <- dst[f][0..need) for the chunks the program may have written
+// arena[off(f) .. ) <- dst[f][0..need): every chunk the gather moved
 __global__ void __launch_bounds__(256) k_scatter_frames(u8 *__restrict__ arena, const u32 *__restrict__ off16,
                                                         const u32 *__restrict__ need, u32 stride, u32 n, u32 slot,
-                                                        const u8 *__restrict__ src, u32 first_chunk) {
+                                                        const u8 *__restrict__ src) {
     const u32 cpf = slot / 16;
     const u64 total = (u64)n * cpf;
     for (u64 t = blockIdx.x * (u64)blockDim.x + threadIdx.x; t < total; t += (u64)gridDim.x * blockDim.x) {
         const u32 f = (u32)(t / cpf), ch = (u32)(t % cpf);
-        const u32 nd = need[f];
-        if (ch < first_chunk && !(nd & ZC_CH0_DIRTY)) continue;
-        if (ch * 16 < (nd & ~ZC_CH0_DIRTY)) {
+        if (ch * 16 < need[f]) {
             u8 *d = arena + (off16 ? (size_t)off16[f] * 16 : (size_t)f * stride) + ch * 16;
             *(uint4 *)d = *(const uint4 *)(src + (size_t)f * slot + ch * 16);
         }
@@ -73,7 +67,7 @@ __global__ void __launch_bounds__(256) k_scatter_frames(u8 *__restrict__ arena, 
 }
 
 // Both kernels are bound by PCIe, not by the SMs: one 256-thread block per SM keeps hundreds of KB of 16-byte
-// accesses in flight (tools/e2e_chunk_sweep.sh sweeps the count), and leaves the SMs to the program kernels of the
+// accesses in flight, and leaves the SMs to the program kernels of the
 // chunk in between.  What limits the pipeline is the link itself (BNG_ZC_TRACE=1 times the stages): the gather's
 // read requests and the scatter's small write TLPs share the upstream direction.  Copy-engine traffic (a header-split ring, moved with cudaMemcpyAsync) overlaps cleanly.
 cudaError_t run_gather_frames(cudaStream_t st, int blocks, const u8 *arena, const u32 *off16, const u32 *len, u32 stride,
@@ -83,7 +77,7 @@ cudaError_t run_gather_frames(cudaStream_t st, int blocks, const u8 *arena, cons
 }
 
 cudaError_t run_scatter_frames(cudaStream_t st, int blocks, u8 *arena, const u32 *off16, const u32 *need, u32 stride, u32 n,
-                               u32 slot, const u8 *src, u32 first_chunk) {
-    k_scatter_frames<<<blocks, 256, 0, st>>>(arena, off16, need, stride, n, slot, src, first_chunk);
+                               u32 slot, const u8 *src) {
+    k_scatter_frames<<<blocks, 256, 0, st>>>(arena, off16, need, stride, n, slot, src);
     return cudaGetLastError();
 }

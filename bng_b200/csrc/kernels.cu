@@ -69,21 +69,11 @@ __device__ __forceinline__ void grouped_select(const Grouped &g, const u32 *cnt,
 // ---------------------------------------------------------------------------
 // antispoof_ingress
 // ---------------------------------------------------------------------------
-// AS_UNROLL frames per thread and trip: their headers are requested together, then their binding probes, then the
-// verdicts: two dependent round trips serve AS_UNROLL frames instead of one.
-#ifndef AS_UNROLL
-#define AS_UNROLL 1
-#endif
-#ifndef AS_FULL_HEADER
-#define AS_FULL_HEADER 0
-#endif
-#ifndef AS_MINB
 #define AS_MINB 5
-#endif
 __global__ void __launch_bounds__(BLOCK, AS_MINB) k_antispoof(const __grid_constant__ DevCtx c, const __grid_constant__ DevBatch b) {
     __shared__ BlockStats bs;
     __shared__ SpoofQ sqs[BLOCK / 32];
-    static_assert(32 * AS_UNROLL + 32 <= SPOOFQ_CAP, "a trip must fit in what a flush leaves free");
+    static_assert(64 <= SPOOFQ_CAP, "a trip's 32 frames must fit in what a flush at 32 leaves free");
     bstats_init(bs);
     spoofq_init(sqs);
     SpoofQ &sq = sqs[threadIdx.x >> 5];
@@ -91,66 +81,38 @@ __global__ void __launch_bounds__(BLOCK, AS_MINB) k_antispoof(const __grid_const
     AsCnt cn = {0, 0};
     const u32 lane = threadIdx.x & 31;
     // warp-uniform trip count: the warp decides together whether its frames allow 32-byte loads
-    for (u32 base = (blockIdx.x * BLOCK + (threadIdx.x & ~31u)) * AS_UNROLL; base < b.n; base += gridDim.x * BLOCK * AS_UNROLL) {
+    for (u32 base = blockIdx.x * BLOCK + (threadIdx.x & ~31u); base < b.n; base += gridDim.x * BLOCK) {
         if (*(volatile u32 *)&sq.n >= 32) spoof_flush(c, sq); // (warp-uniform: the queue is the warp's own)
-        Hdr64 h[AS_UNROLL];
-        u32 len[AS_UNROLL], idx[AS_UNROLL];
-        bool act[AS_UNROLL];
-#pragma unroll
-        for (int u = 0; u < AS_UNROLL; u++) {
-            idx[u] = base + u * 32 + lane;
-            act[u] = idx[u] < b.n;
-            len[u] = act[u] ? frame_dlen(b, b.len[idx[u]]) : 0; // antispoof only bounds-checks: the bytes present
-        }
+        const u32 i = base + lane;
+        const bool act = i < b.n;
+        const u32 len = act ? frame_dlen(b, b.len[i]) : 0; // antispoof only bounds-checks: the bytes present
         // antispoof_ingress reads the Ethernet header and the IPv4 source address (bytes 26-29): the first 32-byte
         // sector of the frame.  Only an IPv6 frame needs more (its source address ends at byte 37).
-        const u8 *fp[AS_UNROLL];
-#pragma unroll
-        for (int u = 0; u < AS_UNROLL; u++) {
-            fp[u] = act[u] ? frame_ptr(b, idx[u]) : b.pkts;
-            const bool wide = __all_sync(0xffffffffu, !act[u] || FRAME_WIDE_OK(b, fp[u]));
-#if AS_FULL_HEADER
-            hdr_load_wide(h[u], fp[u], len[u] < 38 ? len[u] : 38, wide);
-#else
-            hdr_load_wide(h[u], fp[u], len[u] < 32 ? len[u] : 32, wide);
-#endif
-        }
-#if !AS_FULL_HEADER
-#pragma unroll
-        for (int u = 0; u < AS_UNROLL; u++)
-            if (len[u] > 32 && h[u].b16(12) == ETH_P_IPV6_LE) hdr_load(h[u], fp[u], len[u] < 48 ? len[u] : 48);
-#endif
+        const u8 *p = act ? frame_ptr(b, i) : b.pkts;
+        Hdr64 h;
+        hdr_load_wide(h, p, len < 32 ? len : 32, __all_sync(0xffffffffu, !act || FRAME_WIDE_OK(b, p)));
+        if (len > 32 && h.b16(12) == ETH_P_IPV6_LE) hdr_load(h, p, len < 48 ? len : 48);
         // first probe = the home PAIR of 32-byte slots (key + binding each), both in flight at once; a third slot
         // is needed by ~0.1 % of the lookups (the table is sparse)
-        BindVal bv[AS_UNROLL];
-        U256 s1[AS_UNROLL];
-        u64 mk[AS_UNROLL];
-        u32 hi[AS_UNROLL];
-#pragma unroll
-        for (int u = 0; u < AS_UNROLL; u++) {
-            mk[u] = mac_key(h[u], 6);
-            bv[u].has = false;
-            hi[u] = tbl_hash<1>(&mk[u]) & c.bindings.home_mask;
-            if (len[u] >= 14) {
-                bv[u].s = ldg256(tbl_slot(c.bindings, hi[u]));
-                s1[u] = ldg256(tbl_slot(c.bindings, hi[u] + 1));
+        BindVal bv;
+        U256 s1;
+        u64 mk = mac_key(h, 6);
+        bv.has = false;
+        const u32 hi = tbl_hash<1>(&mk) & c.bindings.home_mask;
+        if (len >= 14) {
+            bv.s = ldg256(tbl_slot(c.bindings, hi));
+            s1 = ldg256(tbl_slot(c.bindings, hi + 1));
+            const u64 w0 = (u64)bv.s.w[0] | ((u64)bv.s.w[1] << 32), w1 = (u64)s1.w[0] | ((u64)s1.w[1] << 32);
+            if (w0 == mk) {
+                bv.has = true;
+            } else if (w0 != K_EMPTY && w1 == mk) {
+                bv.has = true;
+                bv.s = s1;
+            } else if (w0 != K_EMPTY && w1 != K_EMPTY) {
+                bv = bind_load(tbl_finish<1>(c.bindings, &mk, hi + 1, w1, true));
             }
         }
-#pragma unroll
-        for (int u = 0; u < AS_UNROLL; u++) {
-            if (len[u] >= 14) {
-                const u64 w0 = (u64)bv[u].s.w[0] | ((u64)bv[u].s.w[1] << 32), w1 = (u64)s1[u].w[0] | ((u64)s1[u].w[1] << 32);
-                if (w0 == mk[u]) {
-                    bv[u].has = true;
-                } else if (w0 != K_EMPTY && w1 == mk[u]) {
-                    bv[u].has = true;
-                    bv[u].s = s1[u];
-                } else if (w0 != K_EMPTY && w1 != K_EMPTY) {
-                    bv[u] = bind_load(tbl_finish<1>(c.bindings, &mk[u], hi[u] + 1, w1, true));
-                }
-            }
-            if (act[u]) b.verdict[idx[u]] = (u8)antispoof_eval(c, &sq, h[u], len[u], idx[u] + b.base, frame_now(b, idx[u]), bv[u], cfg, cn);
-        }
+        if (act) b.verdict[i] = (u8)antispoof_eval(c, &sq, h, len, i + b.base, frame_now(b, i), bv, cfg, cn);
         ascnt_spill(bs, cn);
     }
     spoof_flush(c, sq);
@@ -257,8 +219,8 @@ __global__ void __launch_bounds__(BLOCK) k_nat_ingress(const __grid_constant__ D
         for (int k = 0; k < 8; k++) s1.w[k] = 0;
         if (have && ok[0] < K_BUSY) {
             u8 *s0 = tbl_slot(c.sessions, tbl_hash<2>(ok) & c.sessions.mask);
-            const U256 s = ldg256<SES_POLICY>(s0);
-            s1 = ldg256<SES_POLICY>(s0 + 32);
+            const U256 s = ldg256(s0);
+            s1 = ldg256(s0 + 32);
             const u64 w0 = (u64)s.w[0] | ((u64)s.w[1] << 32), w1 = (u64)s.w[2] | ((u64)s.w[3] << 32);
             seen = s.w[5] >> 16;
             if (w0 == ok[0] && w1 == ok[1]) {
@@ -314,9 +276,9 @@ __global__ void __launch_bounds__(BLOCK) k_nat_ingress(const __grid_constant__ D
                 h.s16(36, csum_upd16(h.b16(36), dport, new_port));
             }
             if (wide) {
-                stg256<FRAME_POLICY>(p, &h.w[0]);
+                stg256(p, &h.w[0]);
                 if (proto == 6)
-                    stg256<FRAME_POLICY>(p + 32, &h.w[8]);
+                    stg256(p + 32, &h.w[8]);
                 else
                     hdr_store_chunk(h, p, 2);
             } else {
@@ -359,9 +321,7 @@ __global__ void __launch_bounds__(BLOCK) k_nat_hairpin_xdp(const __grid_constant
 // read *cnt[CNT_M] elements.  Every block owns one contiguous range of the
 // input, so (digit, block) order of the scanned histogram is index order.
 // ---------------------------------------------------------------------------
-#ifndef RS_BLOCKS_PER_SM
 #define RS_BLOCKS_PER_SM 3 // what the scatter's 71 registers x 256 threads lets an SM hold: one wave, whole tiles
-#endif
 
 __device__ __forceinline__ void rs_range(u32 total, u32 &lo, u32 &hi) {
     u32 per = (total + gridDim.x - 1) / gridDim.x;
@@ -616,8 +576,8 @@ __global__ void __launch_bounds__(BLOCK) k_heads(const __grid_constant__ Grouped
 }
 
 // ---------------------------------------------------------------------------
-// RESOLVE: one TEAM (a single warp in every program as built: concurrency across groups hides more latency
-// than parallelism inside one; the code is written for any multiple of 32) per group, frames in index order.
+// RESOLVE: one block of RS_TEAM threads per group, frames in index order.  The block is a single warp:
+// concurrency across groups hides more latency than parallelism inside one.
 //   stage   all threads copy the group's (value, length) pairs into shared memory, RS_STAGE frames per
 //           sweep, with coalesced loads: the length comes out of the key word (DevBatch.kshift), so nothing
 //           depends on the frame index just loaded (a fat group — 3 000 frames per subscriber when 10 k
@@ -630,12 +590,8 @@ __global__ void __launch_bounds__(BLOCK) k_heads(const __grid_constant__ Grouped
 // The group key is the subscriber-directory slot (programs with a NAT stage) or the bucket's own slot.
 // ---------------------------------------------------------------------------
 #define DROP_FLAG 0x40000000u // staged value: nat44_egress dropped the frame (port exhaustion): no QoS stage
-#ifndef RS_PER_THREAD
+#define RS_TEAM 32
 #define RS_PER_THREAD 8
-#endif
-#ifndef RS_PREFETCH
-#define RS_PREFETCH 1
-#endif
 
 // The NAT stage of one 32-frame chunk that holds new flows (mm: their lanes), kept out of line: the steady state
 // never calls it, and its registers (the frame header, three table probes, the translation) must not cost the
@@ -697,13 +653,10 @@ __device__ __forceinline__ bool resolve_nat_chunk(const DevCtx &c, const DevBatc
 
 // TC (pipeline_tc): the token bucket runs BEFORE the NAT stage: QoS walk first, then nat44_egress — hits and
 // new flows alike — for the frames it passed (DEFER_FLAG), with the parse-stage counters still to be counted.
-template <bool NAT, bool QOS, bool EGRESS, int TEAM, bool TC = false>
-#ifndef RESOLVE_MINB
-#define RESOLVE_MINB 16
-#endif
-__global__ void __launch_bounds__(TEAM, (TEAM == 128 ? 6 : RESOLVE_MINB)) k_resolve(const __grid_constant__ DevCtx c, const __grid_constant__ DevBatch b,
-                                                  const __grid_constant__ Grouped g, const u32 *seg, u32 *cnt) {
-    constexpr int STAGE = TEAM * RS_PER_THREAD;
+template <bool NAT, bool QOS, bool EGRESS, bool TC = false>
+__global__ void __launch_bounds__(RS_TEAM, 16) k_resolve(const __grid_constant__ DevCtx c, const __grid_constant__ DevBatch b,
+                                                      const __grid_constant__ Grouped g, const u32 *seg, u32 *cnt) {
+    constexpr int STAGE = RS_TEAM * RS_PER_THREAD;
     __shared__ BlockStats bs;
     __shared__ u32 s_sv[STAGE], s_len[STAGE];
     __shared__ u32 s_cnt, s_next;
@@ -745,7 +698,7 @@ __global__ void __launch_bounds__(TEAM, (TEAM == 128 ? 6 : RESOLVE_MINB)) k_reso
                 bool ok[RS_PER_THREAD];
 #pragma unroll
                 for (int t = 0; t < RS_PER_THREAD; t++) {
-                    const u32 q = pos + t * TEAM + tid;
+                    const u32 q = pos + t * RS_TEAM + tid;
                     kk[t] = q < m ? skey[q] : 0;
                     sv[t] = q < m ? sval[q] : 0;
                     ok[t] = q < m && (kk[t] & kmask) == key;
@@ -753,7 +706,7 @@ __global__ void __launch_bounds__(TEAM, (TEAM == 128 ? 6 : RESOLVE_MINB)) k_reso
                 u32 first_bad = STAGE;
 #pragma unroll
                 for (int t = 0; t < RS_PER_THREAD; t++) {
-                    const u32 j = t * TEAM + tid;
+                    const u32 j = t * RS_TEAM + tid;
                     if (ok[t]) {
                         // the length came with the key (DevBatch.kshift); a jumbo frame's, or any when the key space
                         // leaves no room, is looked up
@@ -770,7 +723,6 @@ __global__ void __launch_bounds__(TEAM, (TEAM == 128 ? 6 : RESOLVE_MINB)) k_reso
             __syncthreads();
             const u32 n_here = s_cnt;
             const u32 nchunk = (n_here + 31) / 32;
-#if RS_PREFETCH
             // a fat group: the next sweep's two cache-line runs are requested now (into L1, no registers held) and
             // arrive while this sweep is walked
             if (n_here == (u32)STAGE && tid < 2 * (STAGE * 4 / 128)) {
@@ -778,7 +730,6 @@ __global__ void __launch_bounds__(TEAM, (TEAM == 128 ? 6 : RESOLVE_MINB)) k_reso
                 const u32 q = pos + STAGE + (tid % (STAGE / 32)) * 32;
                 if (q < m) asm volatile("prefetch.global.L1 [%0];" ::"l"(base + q));
             }
-#endif
             // ---- NAT stage of this subscriber's frames, strictly in index order: new flows (MISS_FLAG) and, in TC
             //      order, every frame that waited for the token bucket (DEFER_FLAG) and was not dropped by it ----
             auto nat_phase = [&]() {
@@ -951,12 +902,8 @@ void prof_collect(Launcher &L) {
 // set up early and wait in pdl_wait() (griddepcontrol.wait: returns once the preceding grid has completed and its
 // memory operations are visible), which takes the launch latency out of the chain of eight dependent kernels that
 // a small batch consists of.  Every kernel launched this way calls pdl_wait() before its first global access.
-#ifndef BNG_PDL
-#define BNG_PDL 1
-#endif
 template <typename... KArgs, typename... Args>
 static inline void launch_dep(void (*kern)(KArgs...), dim3 grid, dim3 block, cudaStream_t st, Args &&...args) {
-#if BNG_PDL
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = grid;
     cfg.blockDim = block;
@@ -968,18 +915,17 @@ static inline void launch_dep(void (*kern)(KArgs...), dim3 grid, dim3 block, cud
     cfg.attrs = at;
     cfg.numAttrs = 1;
     cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
-#else
-    kern<<<grid, block, 0, st>>>(KArgs(args)...);
-#endif
 }
 
-#define LAUNCH(kern, n, bps, ...)                                      \
-    do {                                                               \
-        prof_begin(L, #kern);                                          \
+// name: what the launch is timed as (bng_prof_enable)
+#define LAUNCH_AS(name, kern, n, bps, ...)                              \
+    do {                                                                \
+        prof_begin(L, name);                                            \
         kern<<<grid_for(L, n, bps), BLOCK, 0, L.stream>>>(__VA_ARGS__); \
-        prof_end(L);                                                   \
-        L.launches++;                                                  \
+        prof_end(L);                                                    \
+        L.launches++;                                                   \
     } while (0)
+#define LAUNCH(kern, n, bps, ...) LAUNCH_AS(#kern, kern, n, bps, __VA_ARGS__)
 
 // Groups the (key, value) pairs in (key_a, val_a)[0..n) by key, stably, skipping NO_KEY.
 // On return *sk / *sv name the buffers holding the grouped pairs; counters[CNT_M] holds their
@@ -1025,17 +971,17 @@ static inline u32 kshift_for(u64 key_space) { return bits_for(key_space) <= KEY_
 
 // k_resolve walks one group per block and a batch of n frames can hold n groups: the grid is sized for n blocks,
 // capped at what the GPU holds at once (the blocks loop over the groups).
-template <bool NAT, bool QOS, bool EGRESS, int TEAM, bool TC = false>
+template <bool NAT, bool QOS, bool EGRESS, bool TC = false>
 static void launch_resolve(Launcher &L, const DevCtx &c, const DevBatch &b, const Grouped &g, const char *name) {
-    int &per_sm = L.resolve_bps[TC ? 4 : (NAT ? 2 : 0) + (QOS ? 0 : 1) + (EGRESS ? 1 : 0)]; // resident blocks per SM of this instantiation
+    int &per_sm = L.resolve_bps[NAT * 8 + QOS * 4 + EGRESS * 2 + TC]; // resident blocks per SM of this instantiation
     if (!per_sm) {
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_resolve<NAT, QOS, EGRESS, TEAM, TC>, TEAM, 0) != cudaSuccess || per_sm < 1)
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_resolve<NAT, QOS, EGRESS, TC>, RS_TEAM, 0) != cudaSuccess || per_sm < 1)
             per_sm = 8;
     }
     long cap = (long)L.num_sms * per_sm, want = b.n ? b.n : 1;
     int grid = (int)(want < cap ? want : cap);
     prof_begin(L, name);
-    launch_dep(k_resolve<NAT, QOS, EGRESS, TEAM, TC>, grid, TEAM, L.stream, c, b, g, L.s.qslot, L.s.counters);
+    launch_dep(k_resolve<NAT, QOS, EGRESS, TC>, grid, RS_TEAM, L.stream, c, b, g, L.s.qslot, L.s.counters);
     prof_end(L);
     L.launches++;
 }
@@ -1054,24 +1000,36 @@ cudaError_t run_qos(Launcher &L, const DevCtx &c, const DevBatch &b0, bool egres
     cudaError_t e = group_by_key(L, b.n, (u64)t.mask + 1, b.kshift, &g);
     if (e != cudaSuccess) return e;
     if (egress)
-        launch_resolve<false, true, true, 32>(L, c, b, g, "(k_resolve<false, true, true>)");
+        launch_resolve<false, true, true>(L, c, b, g, "(k_resolve<false, true, true>)");
     else
-        launch_resolve<false, true, false, 32>(L, c, b, g, "(k_resolve<false, true, false>)");
+        launch_resolve<false, true, false>(L, c, b, g, "(k_resolve<false, true, false>)");
     return cudaGetLastError();
 }
 
-cudaError_t run_nat_egress(Launcher &L, const DevCtx &c, const DevBatch &b0) {
+// The programs keyed on the subscriber directory (nat44_egress, pipeline_up, pipeline_tc): classify, group by
+// directory slot, resolve.  The names are what each launch is timed as; with accounting on, classify is the
+// ACCT instantiation and is timed under its own name.
+template <bool AS, bool QOS, bool TC>
+static cudaError_t run_dir_prog(Launcher &L, const DevCtx &c, const DevBatch &b0, const char *classify_name,
+                                const char *classify_acct_name, const char *resolve_name) {
     DevBatch b = b0;
     b.kshift = kshift_for((u64)c.subdir.mask + 1);
     if (L.acct_attr)
-        LAUNCH((k_pipe_classify<false, false, false, true>), b.n, CLASSIFY_BPS(false), c, b, L.s.key_a, L.s.val_a, L.s.counters, sort_T(L), L.acct_attr);
+        LAUNCH_AS(classify_acct_name, (k_pipe_classify<AS, QOS, TC, true>), b.n, CLASSIFY_BPS(AS), c, b, L.s.key_a, L.s.val_a,
+                  L.s.counters, sort_T(L), L.acct_attr);
     else
-        LAUNCH((k_pipe_classify<false, false>), b.n, CLASSIFY_BPS(false), c, b, L.s.key_a, L.s.val_a, L.s.counters, sort_T(L), nullptr);
+        LAUNCH_AS(classify_name, (k_pipe_classify<AS, QOS, TC>), b.n, CLASSIFY_BPS(AS), c, b, L.s.key_a, L.s.val_a, L.s.counters,
+                  sort_T(L), nullptr);
     Grouped g;
     cudaError_t e = group_by_key(L, b.n, (u64)c.subdir.mask + 1, b.kshift, &g);
     if (e != cudaSuccess) return e;
-    launch_resolve<true, false, false, 32>(L, c, b, g, "(k_resolve<true, false, false>)");
+    launch_resolve<true, QOS, false, TC>(L, c, b, g, resolve_name);
     return cudaGetLastError();
+}
+
+cudaError_t run_nat_egress(Launcher &L, const DevCtx &c, const DevBatch &b) {
+    return run_dir_prog<false, false, false>(L, c, b, "(k_pipe_classify<false, false>)", "(k_pipe_classify<false, false, false, true>)",
+                                             "(k_resolve<true, false, false>)");
 }
 
 cudaError_t run_nat_ingress(Launcher &L, const DevCtx &c, const DevBatch &b) {
@@ -1084,30 +1042,12 @@ cudaError_t run_nat_hairpin_xdp(Launcher &L, const DevCtx &c, const DevBatch &b)
     return cudaGetLastError();
 }
 
-cudaError_t run_pipeline_up(Launcher &L, const DevCtx &c, const DevBatch &b0) {
-    DevBatch b = b0;
-    b.kshift = kshift_for((u64)c.subdir.mask + 1);
-    if (L.acct_attr)
-        LAUNCH((k_pipe_classify<true, true, false, true>), b.n, CLASSIFY_BPS(true), c, b, L.s.key_a, L.s.val_a, L.s.counters, sort_T(L), L.acct_attr);
-    else
-        LAUNCH((k_pipe_classify<true, true>), b.n, CLASSIFY_BPS(true), c, b, L.s.key_a, L.s.val_a, L.s.counters, sort_T(L), nullptr);
-    Grouped g;
-    cudaError_t e = group_by_key(L, b.n, (u64)c.subdir.mask + 1, b.kshift, &g);
-    if (e != cudaSuccess) return e;
-    launch_resolve<true, true, false, 32>(L, c, b, g, "(k_resolve<true, true, false>)");
-    return cudaGetLastError();
+cudaError_t run_pipeline_up(Launcher &L, const DevCtx &c, const DevBatch &b) {
+    return run_dir_prog<true, true, false>(L, c, b, "(k_pipe_classify<true, true>)", "(k_pipe_classify<true, true, false, true>)",
+                                           "(k_resolve<true, true, false>)");
 }
 
-cudaError_t run_pipeline_tc(Launcher &L, const DevCtx &c, const DevBatch &b0) {
-    DevBatch b = b0;
-    b.kshift = kshift_for((u64)c.subdir.mask + 1);
-    if (L.acct_attr)
-        LAUNCH((k_pipe_classify<true, true, true, true>), b.n, CLASSIFY_BPS(true), c, b, L.s.key_a, L.s.val_a, L.s.counters, sort_T(L), L.acct_attr);
-    else
-        LAUNCH((k_pipe_classify<true, true, true>), b.n, CLASSIFY_BPS(true), c, b, L.s.key_a, L.s.val_a, L.s.counters, sort_T(L), nullptr);
-    Grouped g;
-    cudaError_t e = group_by_key(L, b.n, (u64)c.subdir.mask + 1, b.kshift, &g);
-    if (e != cudaSuccess) return e;
-    launch_resolve<true, true, false, 32, true>(L, c, b, g, "(k_resolve<true, true, false, tc>)");
-    return cudaGetLastError();
+cudaError_t run_pipeline_tc(Launcher &L, const DevCtx &c, const DevBatch &b) {
+    return run_dir_prog<true, true, true>(L, c, b, "(k_pipe_classify<true, true, true>)", "(k_pipe_classify<true, true, true, true>)",
+                                          "(k_resolve<true, true, false, tc>)");
 }

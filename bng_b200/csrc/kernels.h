@@ -28,7 +28,7 @@ struct Launcher {
     // per-context (= per-device) launch configuration, filled on first use: nothing here may be process-wide,
     // one process can hold contexts on several GPUs
     int dhcp_smem_set;  // cudaFuncAttributeMaxDynamicSharedMemorySize applied on this context's device
-    int resolve_bps[6]; // resident blocks per SM of the k_resolve instantiations
+    int resolve_bps[16]; // resident blocks per SM of the k_resolve instantiations, by <NAT, QOS, EGRESS, TC> bits
     int prof;
     ProfPending pend[32];
     int npend;
@@ -57,7 +57,7 @@ cudaError_t run_dhcp_fastpath(Launcher &L, const DevCtx &c, const DevBatch &b);
 cudaError_t run_gather_frames(cudaStream_t st, int blocks, const u8 *arena, const u32 *off16, const u32 *len, u32 stride,
                               u32 n, u32 slot, bool tc, u8 *dst, u32 *need);
 cudaError_t run_scatter_frames(cudaStream_t st, int blocks, u8 *arena, const u32 *off16, const u32 *need, u32 stride, u32 n,
-                               u32 slot, const u8 *src, u32 first_chunk);
+                               u32 slot, const u8 *src);
 
 // table maintenance (tableops.cu); keys/values/results are device pointers
 enum { TOP_UPDATE = 0, TOP_LOOKUP = 1, TOP_DELETE = 2 };

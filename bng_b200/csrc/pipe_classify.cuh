@@ -19,17 +19,9 @@
 // not spill beat more warps that do: at 4 blocks the pipeline instantiations get 64 registers and spill 48 bytes, at
 // 3 they use 72 and spill nothing; <false,false> spills 56 bytes at 5 blocks (48 registers) and nothing at 4 (62).
 // On H100 the smaller counts shorten classify by ~9 % on pipeline_imix and ~13 % on nat_steady_64 (DESIGN.md §9).
-#ifndef CLASSIFY_BLOCKS
 #define CLASSIFY_BLOCKS 3
-#endif
-#ifndef CLASSIFY_BLOCKS_NAT
 #define CLASSIFY_BLOCKS_NAT 4
-#endif
 #define CLASSIFY_BPS(AS) ((AS) ? CLASSIFY_BLOCKS : CLASSIFY_BLOCKS_NAT)
-// CLASSIFY_PAIR: fetch the home PAIR of slots of the bindings table / subscriber directory with the first probe
-#ifndef CLASSIFY_PAIR
-#define CLASSIFY_PAIR 0 // the 16 extra registers spill
-#endif
 
 // AS: run antispoof_ingress first; QOS: honour the qos_ingress bucket.  <false,false> is the
 // standalone nat44_egress classify.
@@ -76,7 +68,7 @@ __global__ void __launch_bounds__(BLOCK, CLASSIFY_BPS(AS))
         u64 mk = mac_key(h, 6);
         const u32 bi = tbl_hash<1>(&mk) & c.bindings.home_mask;
         u64 sk = saddr;
-        const u32 di = tbl_hash<1>(&sk) & c.subdir.home_mask; // even: the home pair is one aligned 32-byte load
+        const u32 di = tbl_hash<1>(&sk) & c.subdir.home_mask;
         u16 sport, dport;
         if (proto == 1) {
             sport = h.b16(38); // echo id stands in for the source port (bpf/nat44.c:647-649)
@@ -89,29 +81,19 @@ __global__ void __launch_bounds__(BLOCK, CLASSIFY_BPS(AS))
         key[0] = (u64)saddr | ((u64)daddr << 32);
         key[1] = (u64)sport | ((u64)dport << 16) | ((u64)proto << 32);
         const u32 hi = tbl_hash<2>(key) & c.sessions.mask;
-        // whole 32-byte sectors per probe: the binding slot, and the flow slot's key + translation + counters
-        // the L2-resident per-subscriber tables are probed a PAIR of slots at a time (a dependent second probe stalls
-        // the whole warp; with sparse tables a third slot is needed by ~0.1 % of the lookups)
+        // whole 32-byte sectors per probe: the binding slot, and the flow slot's key + translation + counters; the
+        // directory's home slot is one 16-byte load
         BindVal bv;
-        U256 s0, b1, d0;
-        bv.s.w[0] = bv.s.w[1] = b1.w[0] = b1.w[1] = s0.w[0] = s0.w[1] = 0xFFFFFFFFu; // K_EMPTY
+        U256 s0;
+        bv.s.w[0] = bv.s.w[1] = s0.w[0] = s0.w[1] = 0xFFFFFFFFu; // K_EMPTY
         s0.w[2] = s0.w[3] = 0;
-#pragma unroll
-        for (int k = 0; k < 8; k++) d0.w[k] = 0xFFFFFFFFu;
+        uint4 d0 = make_uint4(0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu);
         const u8 *bslot0 = tbl_slot(c.bindings, bi);
         u8 *sslot0 = tbl_slot(c.sessions, hi);
-        if (AS && dlen >= 14) {
-            bv.s = ldg256(bslot0);
-            if (CLASSIFY_PAIR) b1 = ldg256(bslot0 + 32);
-        }
+        if (AS && dlen >= 14) bv.s = ldg256(bslot0);
         if (ip4) {
-            if (CLASSIFY_PAIR) {
-                d0 = ldg256(tbl_slot(c.subdir, di));
-            } else {
-                const uint4 q = *(const uint4 *)tbl_slot(c.subdir, di);
-                d0.w[0] = q.x, d0.w[1] = q.y, d0.w[2] = q.z, d0.w[3] = q.w;
-            }
-            s0 = ldg256<SES_POLICY>(sslot0);
+            d0 = *(const uint4 *)tbl_slot(c.subdir, di);
+            s0 = ldg256(sslot0);
         }
         const u64 kw0 = (u64)s0.w[0] | ((u64)s0.w[1] << 32), kw1 = (u64)s0.w[2] | ((u64)s0.w[3] << 32);
 
@@ -120,20 +102,12 @@ __global__ void __launch_bounds__(BLOCK, CLASSIFY_BPS(AS))
         if (AS) {
             const u8 *bind = nullptr;
             if (dlen >= 14 && mk < K_BUSY) {
-                const u64 w0 = (u64)bv.s.w[0] | ((u64)bv.s.w[1] << 32), w1 = (u64)b1.w[0] | ((u64)b1.w[1] << 32);
+                const u64 w0 = (u64)bv.s.w[0] | ((u64)bv.s.w[1] << 32);
                 if (w0 == mk) {
                     bind = bslot0;
                 } else if (w0 != K_EMPTY) {
-                    if (!CLASSIFY_PAIR) {
-                        bind = tbl_finish<1>(c.bindings, &mk, bi, w0, true);
-                        if (bind) bv.s = ldg256(bind);
-                    } else if (w1 == mk) {
-                        bind = bslot0 + 32;
-                        bv.s = b1;
-                    } else if (w1 != K_EMPTY) {
-                        bind = tbl_finish<1>(c.bindings, &mk, bi + 1, w1, true); // third slot and beyond (rare)
-                        if (bind) bv.s = ldg256(bind);
-                    }
+                    bind = tbl_finish<1>(c.bindings, &mk, bi, w0, true);
+                    if (bind) bv.s = ldg256(bind);
                 }
             }
             __syncwarp();
@@ -146,20 +120,16 @@ __global__ void __launch_bounds__(BLOCK, CLASSIFY_BPS(AS))
         // ---- phase 3: the subscriber directory: does this address own a NAT block / a bucket? ----
         u32 nat_slot = DIR_NONE, qos_slot = DIR_NONE, dir_idx = ACCT ? DIR_NONE : 0; // (ACCT: DIR_NONE = no entry)
         if (alive) {
-            const u64 k0 = (u64)d0.w[0] | ((u64)d0.w[1] << 32), k1 = (u64)d0.w[4] | ((u64)d0.w[5] << 32);
+            const u64 k0 = (u64)d0.x | ((u64)d0.y << 32);
             if (k0 == sk) {
-                nat_slot = d0.w[2], qos_slot = d0.w[3], dir_idx = di;
+                nat_slot = d0.z, qos_slot = d0.w, dir_idx = di;
             } else if (k0 != K_EMPTY) {
-                if (CLASSIFY_PAIR && k1 == sk) {
-                    nat_slot = d0.w[6], qos_slot = d0.w[7], dir_idx = di + 1;
-                } else if (!CLASSIFY_PAIR || k1 != K_EMPTY) { // third slot and beyond (rare)
-                    const u8 *de = CLASSIFY_PAIR ? tbl_finish<1>(c.subdir, &sk, di + 1, k1, true) : tbl_finish<1>(c.subdir, &sk, di, k0, true);
-                    if (de) {
-                        const u64 w = *(const u64 *)(de + 8);
-                        nat_slot = (u32)w;
-                        qos_slot = (u32)(w >> 32);
-                        dir_idx = (u32)((de - c.subdir.slots) >> 4);
-                    }
+                const u8 *de = tbl_finish<1>(c.subdir, &sk, di, k0, true);
+                if (de) {
+                    const u64 w = *(const u64 *)(de + 8);
+                    nat_slot = (u32)w;
+                    qos_slot = (u32)(w >> 32);
+                    dir_idx = (u32)((de - c.subdir.slots) >> 4);
                 }
             }
         }
@@ -220,9 +190,9 @@ __global__ void __launch_bounds__(BLOCK, CLASSIFY_BPS(AS))
             // 32-47.  A partial sector is a read-modify-write at HBM once its line has left L2: storing the unchanged
             // 16 bytes too made classify ~8 % faster on pipeline_imix (DESIGN.md §9).
             if (wide) {
-                stg256<FRAME_POLICY>(p, &h.w[0]);
+                stg256(p, &h.w[0]);
                 if (proto == 6 || dlen >= 64)
-                    stg256<FRAME_POLICY>(p + 32, &h.w[8]);
+                    stg256(p + 32, &h.w[8]);
                 else
                     hdr_store_chunk(h, p, 2);
             } else {

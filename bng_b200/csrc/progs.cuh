@@ -62,9 +62,7 @@ __device__ __forceinline__ void ascnt_spill(BlockStats &bs, AsCnt &n) { // calle
 // what the record needs into a queue of their WARP in shared memory, and the warp writes a batch of records at a
 // time — one atomic for the batch, one lane per record, 64-byte records side by side (spoof_flush).  The order of the
 // records in the ring is immaterial: the drain sorts by (batch, frame).
-#ifndef SPOOFQ_CAP
-#define SPOOFQ_CAP 64
-#endif // // flushed from 32 up, at most 32 more per trip of the frame loop
+#define SPOOFQ_CAP 64 // flushed from 32 up, at most 32 more per trip of the frame loop
 struct SpoofQ {
     u32 n, pad[3];
     uint4 e[SPOOFQ_CAP][2]; // {now, source MAC, ip version} {spoofed, allowed, frame index}

@@ -60,7 +60,7 @@ def launch_shares(path):
 
 # what one pipeline_up batch launches (DESIGN.md section 3): kernel -> launches per batch
 STEP = (("k_pipe_classify<1, 1, 0>", 1), ("k_rs_hist", 2), ("k_rs_scan", 2), ("k_rs_scatter", 2), ("k_heads", 1),
-        ("k_resolve<1, 1, 0, 32, 0>", 1))
+        ("k_resolve<1, 1, 0, 0>", 1))
 
 
 def main():
@@ -185,7 +185,7 @@ def main():
             km = json.loads(open(pj).readline())["roofline"]["kernels_ms"]
             tt = sum(km.values())
             ev = {"k_pipe_classify<1, 1, 0>": km.get("(k_pipe_classify<true, true>)", 0) / tt,
-                  "k_resolve<1, 1, 0, 32, 0>": km.get("(k_resolve<true, true, false>)", 0) / tt, "group": km.get("group_by_key", 0) / tt}
+                  "k_resolve<1, 1, 0, 0>": km.get("(k_resolve<true, true, false>)", 0) / tt, "group": km.get("group_by_key", 0) / tt}
         for k, c in STEP:
             if k in tot:
                 L.append("| %s | %d | %.4f | %.4f | %.1f %% | %s |" % (k, c, med(tot[k]), per[k], 100 * per[k] / allt,

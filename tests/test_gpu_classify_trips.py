@@ -27,9 +27,8 @@ CLASSIFY_SRC = os.path.join(os.path.dirname(__file__), "..", "bng_b200", "csrc",
 
 def classify_grid(prog):
     """Blocks of the classify launch at a large batch: SMs x the blocks per SM the kernel is compiled for, which is
-    the default in pipe_classify.cuh.  The in-tree build takes the defaults; a library loaded through BNG_B200_LIB
-    may be an A/B build with other -DCLASSIFY_BLOCKS* values (tools/build_variants.sh), whose trip edges lie elsewhere,
-    so the test does not claim to check those edges there."""
+    read from pipe_classify.cuh.  A library loaded through BNG_B200_LIB may have been built from other sources, whose
+    trip edges lie elsewhere, so the test does not claim to check those edges there."""
     import torch
     from bng_b200 import dataplane
     if os.path.realpath(dataplane.LIB_PATH) != os.path.realpath(os.path.join(dataplane.HERE, "libbng_b200.so")):
