@@ -19,7 +19,10 @@
 // not spill beat more warps that do: at 4 blocks the pipeline instantiations get 64 registers and spill 48 bytes, at
 // 3 they use 72 and spill nothing; <false,false> spills 56 bytes at 5 blocks (48 registers) and nothing at 4 (62).
 // On H100 the smaller counts shorten classify by ~9 % on pipeline_imix and ~13 % on nat_steady_64 (DESIGN.md §9).
-#define CLASSIFY_BLOCKS 3
+// The pipelines run best at 2 blocks (16 warps, 75 registers): classify is bound by a memory resource its warps
+// share, not by the latency one warp waits out, and at 3 blocks each trip takes longer than the extra warps make up
+// for (about 8 % of classify on pipeline_imix, DESIGN.md §5).
+#define CLASSIFY_BLOCKS 2
 #define CLASSIFY_BLOCKS_NAT 4
 #define CLASSIFY_BPS(AS) ((AS) ? CLASSIFY_BLOCKS : CLASSIFY_BLOCKS_NAT)
 
