@@ -1418,6 +1418,28 @@ static int poll_compact_locked(bng_ctx *c) {
     return compact_if_due_locked(c, *(volatile u64 *)c->evict_word);
 }
 
+// After a pass that removes flow state (bng_sweep, bng_nat_flush), given the nat_sessions tombstones it counted:
+// once a quarter of nat_sessions' slots are tombstones, rebuild the three flow tables (they churn together).
+static int rebuild_if_tombstoned_locked(bng_ctx *c, u32 tombs) {
+    if (tombs <= (c->dev.sessions.mask + 1) / 4) return 0;
+    int r;
+    if ((r = table_rebuild_locked(c, &c->dev.sessions)) != 0) return r;
+    if ((r = table_rebuild_locked(c, &c->dev.reverse)) != 0) return r;
+    return table_rebuild_locked(c, &c->dev.eim);
+}
+
+// Start of a pass over the flow tables that is a batch of its own between program runs (bng_sweep, bng_nat_flush):
+// staged upserts first, then the batch sequence advances as a program run's does.
+static int flow_pass_begin_locked(bng_ctx *c) {
+    int r = poll_compact_locked(c);
+    if (r) return r;
+    if ((r = flush_staged_locked(c, -1)) != 0) return r;
+    c->dev.batch_seq++;
+    c->dev.epoch = c->dev.batch_seq % 65535u + 1;
+    if (c->dev.epoch == 1 && c->dev.batch_seq > 1) CU(c, run_epoch_reset(c->L, c->dev.sessions));
+    return 0;
+}
+
 // Session expiry sweep (sweep.cu): removes every nat_sessions entry idle for longer than the timeout of its
 // protocol / TCP state at now_ns, with its nat_reverse entry, its EIM reference, the subscriber's active-session
 // count; counts sessions_expired and logs NAT_LOG_SESSION_DELETE.  A batch of its own between program runs.
@@ -1425,12 +1447,8 @@ int bng_sweep(bng_ctx *c, uint64_t now_ns, uint64_t *expired_out) {
     if (!c) return -EINVAL;
     std::lock_guard<std::mutex> g(c->mu);
     cudaSetDevice(c->device);
-    int r = poll_compact_locked(c);
+    int r = flow_pass_begin_locked(c);
     if (r) return r;
-    if ((r = flush_staged_locked(c, -1)) != 0) return r;
-    c->dev.batch_seq++;
-    c->dev.epoch = c->dev.batch_seq % 65535u + 1;
-    if (c->dev.epoch == 1 && c->dev.batch_seq > 1) CU(c, run_epoch_reset(c->L, c->dev.sessions));
     u32 *cnt = c->L.s.counters + 8; // scratch words 8.. are free between program runs
     CU(c, cudaMemsetAsync(cnt, 0, 8, c->L.stream));
     CU(c, run_nat_sweep(c->L, c->dev, now_ns, cnt));
@@ -1439,13 +1457,42 @@ int bng_sweep(bng_ctx *c, uint64_t now_ns, uint64_t *expired_out) {
     CU(c, cudaStreamSynchronize(c->L.stream));
     prof_collect(c->L);
     if (expired_out) *expired_out = n[0];
-    // a quarter of nat_sessions' slots are tombstones: rebuild the three flow tables (they churn together)
-    if (n[1] > (c->dev.sessions.mask + 1) / 4) {
-        if ((r = table_rebuild_locked(c, &c->dev.sessions)) != 0) return r;
-        if ((r = table_rebuild_locked(c, &c->dev.reverse)) != 0) return r;
-        if ((r = table_rebuild_locked(c, &c->dev.eim)) != 0) return r;
+    return rebuild_if_tombstoned_locked(c, n[1]);
+}
+
+// NAT flow-state flush of a set of subscriber addresses (flush.cu).  The set is built here in the pinned staging
+// buffer and copied behind whatever the stream already holds.
+int bng_nat_flush(bng_ctx *c, const uint32_t *addrs, uint64_t n, uint64_t now_ns, uint64_t removed_out[3]) {
+    if (!c || (n && !addrs)) return -EINVAL;
+    if (removed_out) removed_out[0] = removed_out[1] = removed_out[2] = 0;
+    std::lock_guard<std::mutex> g(c->mu);
+    cudaSetDevice(c->device);
+    if (n == 0) return flush_staged_locked(c, -1);
+    u64 slots = 64;
+    while (slots < 2 * n) slots *= 2;
+    if (slots > (1ull << 32)) return fail(c, -EINVAL, "nat_flush: %llu addresses", (unsigned long long)n);
+    int r = flow_pass_begin_locked(c);
+    if (r) return r;
+    if ((r = ensure_io(c, slots * 8)) != 0) return r;
+    u64 *set = (u64 *)c->io_host;
+    memset(set, 0, slots * 8);
+    const u32 mask = (u32)(slots - 1);
+    for (u64 k = 0; k < n; k++) {
+        u32 i = aset_home(addrs[k], mask);
+        while (set[i] && (u32)set[i] != addrs[k]) i = (i + 1) & mask;
+        set[i] = ADDRSET_LIVE | addrs[k];
     }
-    return 0;
+    CU(c, cudaMemcpyAsync(c->io_dev, c->io_host, slots * 8, cudaMemcpyHostToDevice, c->L.stream));
+    u32 *cnt = c->L.s.counters + 8; // scratch words 8.. are free between program runs
+    CU(c, cudaMemsetAsync(cnt, 0, 16, c->L.stream));
+    CU(c, run_nat_flush(c->L, c->dev, AddrSet{(const u64 *)c->io_dev, mask}, now_ns, cnt));
+    u32 got[4] = {0, 0, 0, 0};
+    CU(c, cudaMemcpyAsync(got, cnt, 16, cudaMemcpyDeviceToHost, c->L.stream));
+    CU(c, cudaStreamSynchronize(c->L.stream));
+    prof_collect(c->L);
+    if (removed_out)
+        for (int k = 0; k < 3; k++) removed_out[k] = got[k];
+    return rebuild_if_tombstoned_locked(c, got[3]);
 }
 
 // ---------------------------------------------------------------------------

@@ -71,6 +71,23 @@ cudaError_t run_epoch_reset(Launcher &L, const Tbl &sessions);
 cudaError_t run_table_rebuild(Launcher &L, const Tbl &old_table, const Tbl &empty_table);
 // session expiry sweep (sweep.cu); n_expired: device counter, incremented by the number of sessions removed
 cudaError_t run_nat_sweep(Launcher &L, const DevCtx &c, u64 now, u32 *n_expired /* [0] expired, [1] tombstones seen */);
+// NAT flow-state flush (flush.cu).  The address set: mask + 1 (a power of two >= 2 x the distinct addresses) u64
+// words, 0 = empty, ADDRSET_LIVE | address = member; linear probing from aset_home().  Built on the host.
+#define ADDRSET_LIVE (1ull << 32)
+struct AddrSet {
+    const u64 *words;
+    u32 mask;
+};
+__host__ __device__ __forceinline__ u32 aset_home(u32 addr, u32 mask) {
+    u32 h = addr; // murmur3 finaliser: the last octet sits in the top byte of the word, so every bit must mix down
+    h ^= h >> 16;
+    h *= 0x85EBCA6Bu;
+    h ^= h >> 13;
+    h *= 0xC2B2AE35u;
+    h ^= h >> 16;
+    return h & mask;
+}
+cudaError_t run_nat_flush(Launcher &L, const DevCtx &c, const AddrSet &a, u64 now, u32 *cnt /* [4], see flush.cu */);
 cudaError_t run_table_dump(Launcher &L, const Tbl &t, u8 *keys_out, u8 *vals_out, u32 *count_out, u64 cap);
 
 // per-subscriber traffic accounting (acct.cu).  A record is ACCT_WORDS u64 (struct bng_acct), index-aligned with the

@@ -104,6 +104,7 @@ def load_library() -> C.CDLL:
         "bng_acct_enable": ([vp, i32, i32], i32),
         "bng_acct_read": ([vp, vp, u64, vp, vp], i32),
         "bng_acct_dump": ([vp, vp, vp, u64], C.c_int64),
+        "bng_nat_flush": ([vp, vp, u64, u64, C.POINTER(u64)], i32),
     }
     for name, (args, res) in protos.items():
         fn = getattr(lib, name)
@@ -121,12 +122,18 @@ EXPORTED_SYMBOLS = (
     "bng_stats_device_ptr", "bng_launch_count", "bng_lru_overflow", "bng_events_lost", "bng_prof_enable",
     "bng_prof_read", "bng_host_alloc", "bng_host_free", "bng_map_update_staged", "bng_staged_info",
     "bng_comm_unique_id", "bng_comm_init", "bng_sync_reduce", "bng_sweep", "bng_lru_evictions", "bng_snapshot", "bng_restore", "bng_table_rebuilds",
-    "bng_acct_enable", "bng_acct_read", "bng_acct_dump",
+    "bng_acct_enable", "bng_acct_read", "bng_acct_dump", "bng_nat_flush",
 )
 
 
 class BngError(OSError):
     pass
+
+
+def _addr_words(addrs) -> np.ndarray:
+    """Subscriber addresses as u32 words holding the 4 key bytes: from u8[n, 4] key bytes or u32[n]."""
+    a = np.asarray(addrs)
+    return np.ascontiguousarray(a).view("<u4").reshape(-1) if a.dtype == np.uint8 else np.ascontiguousarray(a, "<u4").reshape(-1)
 
 
 def _ptr(x):
@@ -327,8 +334,7 @@ class Dataplane:
 
     def acct_read(self, addrs):
         """addrs: u8[n, 4] (qos_ingress key bytes) or u32[n] -> (bng_acct records[n], found bool[n])."""
-        a = np.asarray(addrs)
-        a = np.ascontiguousarray(a).view("<u4").reshape(-1) if a.dtype == np.uint8 else np.ascontiguousarray(a, "<u4").reshape(-1)
+        a = _addr_words(addrs)
         out = np.zeros(len(a), dtype=bng_acct)
         res = np.zeros(len(a), dtype=np.int32)
         self._chk(self.lib.bng_acct_read(self.h, a.ctypes.data, len(a), out.ctypes.data, res.ctypes.data), "acct_read")
@@ -343,6 +349,15 @@ class Dataplane:
         a, out = a[:n], out[:n]
         order = np.argsort(a.byteswap(), kind="stable")
         return a[order], out[order]
+
+    def nat_flush(self, addrs, now_ns: int):
+        """Remove the NAT flow state of a set of subscriber addresses (u8[n, 4] subscriber_nat key bytes or u32[n]):
+        their sessions, the reverse entries that lead to them and their EIM mappings; their sessions_active becomes 0.
+        Returns (sessions, reverse entries, EIM mappings) removed."""
+        a = _addr_words(addrs)
+        out = (C.c_uint64 * 3)()
+        self._chk(self.lib.bng_nat_flush(self.h, a.ctypes.data if len(a) else None, len(a), now_ns, out), "nat_flush")
+        return tuple(int(x) for x in out)
 
     def sweep(self, now_ns: int) -> int:
         """Session expiry sweep at now_ns; returns the number of sessions removed."""

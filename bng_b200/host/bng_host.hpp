@@ -983,6 +983,20 @@ class Manager {
         if (a.PoolIndex < (int)pool_.size()) pool_[a.PoolIndex].Subscribers--;
         return Nil();
     }
+    // Not in the reference: DeallocateNAT leaves the subscribers' sessions, reverse entries and EIM mappings on the
+    // dataplane until they expire, and the next holder of the address inherits them.  One bng_nat_flush pass removes
+    // them.  Call it before DeallocateNAT, so that the NAT log records still carry the subscriber id.
+    // removed_out (may be null): sessions, reverse entries, EIM mappings removed.
+    Error FlushSessions(const std::vector<IP> &privateIPs, uint64_t now_ns, uint64_t removed_out[3] = nullptr) {
+        if (!be_ || !be_->ctx) return Error("dataplane not open");
+        std::vector<uint32_t> keys;
+        keys.reserve(privateIPs.size());
+        for (const IP &ip : privateIPs) {
+            if (!To4(ip)) return Error("IPv4 address required");
+            keys.push_back(be_->AddrKey(ebpf::IPToUint32(ip)));
+        }
+        return MapErr("bng_nat_flush", bng_nat_flush(be_->ctx, keys.data(), keys.size(), now_ns, removed_out));
+    }
     Error ConfigureALG(uint16_t port, uint8_t protocol, uint8_t algType, bool enabled) { // :542-560
         if (algPorts_ < 0) return Error("ALG map not loaded");
         uint32_t key = ((uint32_t)port << 16) | protocol;

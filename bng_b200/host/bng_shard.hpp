@@ -218,6 +218,35 @@ class Router {
         int rc = bng_acct_read(shards_[(size_t)o]->ctx, &addr_key, 1, out, &res);
         return rc ? rc : res;
     }
+    // NAT flow-state flush (bng_nat_flush) of addresses given as subscriber_nat key words.  A subscriber's sessions,
+    // reverse entries and EIM mappings are all created on its owner shard (downstream frames are steered there by
+    // public address and port block), so each address goes to its owner; one whose owner is not known goes to every
+    // shard, where a flush of an address without state is a no-op.  One call per shard that has addresses.
+    // removed_out (may be null): sessions, reverse entries, EIM mappings removed, summed over the shards.
+    std::vector<std::vector<uint32_t>> NatFlushGroups(const uint32_t *addrs, uint64_t n) const {
+        std::vector<std::vector<uint32_t>> g(shards_.size());
+        for (uint64_t i = 0; i < n; i++) {
+            auto s = dir_->ShardOfIP(addrs[i]);
+            for (size_t k = 0; k < shards_.size(); k++)
+                if (!s || *s == k) g[k].push_back(addrs[i]);
+        }
+        return g;
+    }
+    int NatFlush(const uint32_t *addrs, uint64_t n, uint64_t now_ns, uint64_t removed_out[3] = nullptr) {
+        if (removed_out) removed_out[0] = removed_out[1] = removed_out[2] = 0;
+        if (n && !addrs) return -EINVAL;
+        auto g = NatFlushGroups(addrs, n);
+        int rc = 0;
+        for (size_t k = 0; k < g.size(); k++) {
+            if (g[k].empty()) continue;
+            uint64_t rm[3] = {0, 0, 0};
+            int r = bng_nat_flush(shards_[k]->ctx, g[k].data(), g[k].size(), now_ns, rm);
+            if (r && !rc) rc = r;
+            if (removed_out)
+                for (int j = 0; j < 3; j++) removed_out[j] += rm[j];
+        }
+        return rc;
+    }
     radius::AcctReader Reader() {
         return [this](uint32_t addr, bng_acct *out) { return AcctRead(addr, out); };
     }

@@ -145,6 +145,34 @@ void *bng_stream(bng_ctx *ctx); /* the context's cudaStream_t */
  * recently used entry among the 16 slots next to the new key's home slot instead of failing. */
 int bng_sweep(bng_ctx *ctx, uint64_t now_ns, uint64_t *expired_out);
 
+/* ---- NAT flow-state flush (what a subscriber's release / RADIUS Disconnect needs) ----
+ * Removes the NAT flow state of a set of subscriber addresses.  Until it expires, a departed subscriber's flow state
+ * keeps translating: return traffic to its public ports is DNATed to the private address (nat44_ingress never
+ * consults subscriber_nat), and the address's next holder hits its sessions and EIM mappings upstream.
+ * addrs: n host-memory addresses, 4 bytes each, in the byte order of the subscriber_nat / qos_ingress key (as
+ * bng_acct_read takes them); duplicates are allowed and every value is an address, 0 and 0xFFFFFFFF included.
+ * With A the set of addresses, one call
+ *   - deletes every nat_sessions entry whose key src_ip is in A, and writes one NAT_LOG_SESSION_DELETE record per
+ *     deleted session to nat_log_rb: the sweep's record (subscriber_id from the address's subscriber_nat entry, 0
+ *     without one), with timestamp now_ns, drained ordered by content as the sweep's are; nat_log_rb's capacity and
+ *     bng_events_lost apply as usual;
+ *   - deletes every nat_reverse entry whose value (the original upstream nat_key) has src_ip in A, stale entries
+ *     whose session has already gone included;
+ *   - deletes every eim_table entry whose internal_ip is in A, whatever its ref_count;
+ *   - sets sessions_active of every subscriber_nat entry keyed by an address in A to 0 (block, next_port and
+ *     subscriber_id stay).
+ * Nothing else changes: not nat_stats (this is not an expiry), not the accounting records, not qos_* or any other
+ * map.  The caller deletes those by key.  Flush before deleting the subscriber_nat entry, so that the records still
+ * carry the subscriber_id.
+ * Ordering is bng_sweep's: staged upserts are applied first; the call is a batch of its own (it advances the batch
+ * sequence) queued on the context's stream behind everything before it, BNG_MEM_DEVICE batches that were not
+ * synchronised included; it returns synchronised, and rebuilds the flow tables under bng_sweep's rule.
+ * removed_out (may be NULL): sessions, nat_reverse entries and eim_table entries removed.  n == 0 applies the staged
+ * upserts and returns 0 with zero counts.  -EINVAL for a NULL ctx, or NULL addrs with n > 0.
+ * The pass streams the three flow tables once (about 0.67 GB at the reference's capacities); the set of addresses
+ * takes 8 bytes per slot of a power of two >= 2n in the context's staging buffers, which grow to hold it. */
+int bng_nat_flush(bng_ctx *ctx, const uint32_t *addrs, uint64_t n, uint64_t now_ns, uint64_t removed_out[3]);
+
 /* ---- events (spoof_events perf buffer, nat_log_rb ring buffer) ----
  * Records come out in the order the reference would have emitted them (batch
  * order, then frame index); nat_log_rb applies the kernel ring's capacity
@@ -221,7 +249,7 @@ uint64_t bng_launch_count(bng_ctx *ctx);  /* kernels launched by this context so
 uint64_t bng_lru_overflow(bng_ctx *ctx);  /* inserts that found no victim to evict in a full LRU map (should stay 0) */
 uint64_t bng_lru_evictions(bng_ctx *ctx); /* entries evicted from full LRU maps by the data path */
 /* Flow-table rebuilds so far.  nat_sessions / nat_reverse / eim_table are rebuilt (tombstones dropped) together:
- *  - by bng_sweep, once a quarter of nat_sessions' slots are tombstones after it;
+ *  - by bng_sweep and bng_nat_flush, once a quarter of nat_sessions' slots are tombstones after it;
  *  - once LRU evictions since the last rebuild exceed a quarter of nat_sessions' slots.  Host-fed batches and
  *    bng_sync check this with the count as of their end.  A BNG_MEM_DEVICE batch of nat44_egress / pipeline_up /
  *    pipeline_tc does not wait: it queues a copy of the count behind itself, and the next bng_prog_run or bng_sweep
