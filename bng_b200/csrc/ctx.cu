@@ -108,6 +108,19 @@ struct bng_ctx {
     u32 acct_progs = 0;
     u8 *acct_dump_buf = nullptr; // grow-only scratch of bng_acct_dump: records, then addresses
     u64 acct_dump_cap = 0;
+    u64 seq = 0; // the batch sequence in 64 bits (dev.batch_seq holds its low 32): bng_li_record.batch
+    // lawful intercept (bng_li_*, li.cu): allocated by the first bng_li_configure / bng_li_target_set (li_ctl != null)
+    u64 *li_ctl = nullptr;   // device: LiRing::ctl
+    u64 *li_words = nullptr; // device: the target set (AddrSet words, LI_TSLOTS), and its ids
+    u32 *li_ids = nullptr;
+    u32 li_mask = 0;
+    bool li_dirty = false;   // the host's targets changed since the device copy was made
+    std::unordered_map<u32, u32> li_targets; // authoritative: address -> target id
+    u8 *li_ring = nullptr;
+    u32 li_cap = 0, li_rec = 0, li_snap = 0;
+    uint2 *li_match = nullptr; // [L.s.cap]
+    std::vector<u8> li_pending; // records copied out of the ring, ordered, not yet drained
+    u64 li_lost_host = 0;       // records discarded by a reconfiguration
 };
 
 namespace {
@@ -175,9 +188,13 @@ int ensure_scratch(bng_ctx *c, u32 n) {
     u32 cap = std::max<u32>(n, 1024);
     void **ptrs[] = {(void **)&s.key_a, (void **)&s.key_b, (void **)&s.val_a, (void **)&s.val_b, (void **)&s.qslot, (void **)&s.attr};
     for (void **pp : ptrs) {
-        if (pp == (void **)&s.attr && !c->acct) continue; // the attribution words exist once accounting does
+        if (pp == (void **)&s.attr && !c->acct && !c->li_ctl) continue; // the attribution words exist once accounting or interception does
         if (*pp) cudaFree(*pp);
         CU(c, cudaMalloc(pp, (size_t)cap * 4));
+    }
+    if (c->li_ctl) {
+        if (c->li_match) cudaFree(c->li_match);
+        CU(c, cudaMalloc((void **)&c->li_match, (size_t)cap * sizeof(uint2)));
     }
     if (s.cub_tmp) cudaFree(s.cub_tmp);
     s.cub_tmp_bytes = sort_temp_bytes(cap);
@@ -489,7 +506,7 @@ int bng_close(bng_ctx *c) {
         }
         for (void *p : c->allocs) cudaFree(p);
         Scratch &s = c->L.s;
-        void *sp[] = {s.key_a, s.key_b, s.val_a, s.val_b, s.qslot, s.attr, s.cub_tmp, s.counters, c->acct_dump_buf,
+        void *sp[] = {s.key_a, s.key_b, s.val_a, s.val_b, s.qslot, s.attr, s.cub_tmp, s.counters, c->acct_dump_buf, c->li_ring, c->li_match,
                       c->io_dev, c->hb_pkts, c->hb_off, c->hb_len, c->hb_prio, c->hb_verdict, c->hb_now, c->dump_k, c->dump_v, c->dump_c};
         for (void *p : sp)
             if (p) cudaFree(p);
@@ -1000,10 +1017,27 @@ int bng_prog_id(bng_ctx *c, const char *name) {
 // the accounting mode of each program: where its frames' subscriber is found (-1: not accountable)
 static const int k_acct_mode[] = {-1, ACCT_DST, ACCT_SRC, ACCT_ATTR, ACCT_DST, -1, -1, ACCT_ATTR, ACCT_ATTR};
 
-static int dispatch(bng_ctx *c, int prog, const DevBatch &b) {
-    cudaError_t e;
+// the interception direction of each program: BNG_LI_UPLINK (0), BNG_LI_DOWNLINK (1), -1: never captures
+static const int k_li_dir[] = {-1, 1, 0, 0, 1, -1, -1, 0, 0};
+
+static int dispatch(bng_ctx *c, int prog, const DevBatch &b, const LiSrc &src = LiSrc{}) {
+    cudaError_t e = cudaSuccess;
     const bool acct = c->acct && ((c->acct_progs >> prog) & 1);
-    c->L.acct_attr = acct ? c->L.s.attr : nullptr; // the upstream classify records attributions
+    const int li = c->li_targets.empty() ? -1 : k_li_dir[prog]; // no target: not one kernel more
+    const bool pipe = prog == P_PIPE_UP || prog == P_PIPE_TC;
+    // the upstream classify records attributions: for accounting, and in the pipelines to tell antispoof's drops
+    c->L.acct_attr = (acct || (li == 0 && pipe)) ? c->L.s.attr : nullptr;
+    LiRing r{};
+    if (li >= 0) {
+        r.buf = c->li_ring, r.ctl = c->li_ctl, r.match = c->li_match;
+        r.cap = c->li_cap, r.rec_bytes = c->li_rec, r.snaplen = c->li_snap, r.prog = (u32)prog;
+        r.tgt = AddrSet{c->li_words, c->li_mask}, r.ids = c->li_ids, r.batch = c->seq;
+    }
+    if (li == 0) { // the frames as they entered, before the program rewrites them
+        e = cudaMemsetAsync(c->li_ctl + 2, 0, 4, c->L.stream);
+        if (e == cudaSuccess) e = run_li_capture(c->L, r, b, src, true);
+        if (e != cudaSuccess) return fail(c, -EIO, "launch k_li_capture: %s", cudaGetErrorString(e));
+    }
     switch (prog) {
     case P_ANTISPOOF: e = run_antispoof(c->L, c->dev, b); break;
     case P_QOS_EG: e = run_qos(c->L, c->dev, b, true); break;
@@ -1018,6 +1052,8 @@ static int dispatch(bng_ctx *c, int prog, const DevBatch &b) {
     }
     // after the program, before anything copies the frames out: the downstream modes read the rewritten headers
     if (e == cudaSuccess && acct) e = run_acct(c->L, c->dev.subdir, b, k_acct_mode[prog], c->acct);
+    if (e == cudaSuccess && li == 0) e = run_li_verdict(c->L, r, b, pipe ? c->L.s.attr : nullptr);
+    if (e == cudaSuccess && li == 1) e = run_li_capture(c->L, r, b, src, false);
     if (e != cudaSuccess) return fail(c, -EIO, "launch %s: %s", k_prog_names[prog], cudaGetErrorString(e));
     return 0;
 }
@@ -1032,6 +1068,7 @@ static int dispatch(bng_ctx *c, int prog, const DevBatch &b) {
 static int maybe_compact_locked(bng_ctx *c);
 static int poll_compact_locked(bng_ctx *c);
 static int queue_evict_read_locked(bng_ctx *c);
+static int li_upload_locked(bng_ctx *c);
 static int run_host_zero_copy(bng_ctx *c, int prog, bng_batch *bb, u8 *arena_dev) {
     // Bytes of a frame a program can touch (hostio.cu): 96 for the TC programs (Ethernet + IPv4 with options + 20
     // bytes of L4), 448 for dhcp_fastpath_prog.  Frames that ARE a fixed slot no larger than that (64-byte
@@ -1119,7 +1156,9 @@ static int run_host_zero_copy(bng_ctx *c, int prog, bng_batch *bb, u8 *arena_dev
         b.base = base;
         b.cap = hb; // bounds checks never look past a compact slot (a no-op for whole frames: hostio.cu)
         b.arena_len = (u64)cn * hb;
-        int r = dispatch(c, prog, b);
+        // interception copies the bytes past the compact copy straight from the host arena
+        const LiSrc src{chunk_arena, bb->off16 ? c->zc_off[buf] : nullptr, contiguous ? nullptr : c->zc_len0[buf], bb->stride};
+        int r = dispatch(c, prog, b, src);
         if (r) return r;
         CU(c, cudaEventRecord(c->ev_comp[buf], sc));
         mark(sc);
@@ -1168,6 +1207,8 @@ int bng_prog_run(bng_ctx *c, int prog, bng_batch *bb) {
     if ((r = poll_compact_locked(c)) != 0) return r;     // what an earlier device-resident batch left to compact
     if ((r = flush_staged_locked(c, -1)) != 0) return r; // the batch boundary: staged upserts become visible
     if (c->small_dirty && (r = small_refresh_p(c)) != 0) return r; // ... and the shared-memory image of the small maps is rebuilt
+    if (c->li_dirty && (r = li_upload_locked(c)) != 0) return r;   // ... and the interception targets in force now
+    c->seq++;
     c->dev.batch_seq++;
     c->dev.epoch = c->dev.batch_seq % 65535u + 1; // what a session hit stamps next to last_seen (common.cuh)
     if (c->dev.epoch == 1 && c->dev.batch_seq > 1) CU(c, run_epoch_reset(c->L, c->dev.sessions)); // the 16-bit stamp wraps
@@ -1434,6 +1475,7 @@ static int flow_pass_begin_locked(bng_ctx *c) {
     int r = poll_compact_locked(c);
     if (r) return r;
     if ((r = flush_staged_locked(c, -1)) != 0) return r;
+    c->seq++;
     c->dev.batch_seq++;
     c->dev.epoch = c->dev.batch_seq % 65535u + 1;
     if (c->dev.epoch == 1 && c->dev.batch_seq > 1) CU(c, run_epoch_reset(c->L, c->dev.sessions));
@@ -1650,6 +1692,161 @@ int64_t bng_acct_dump(bng_ctx *c, uint32_t *addrs_out, bng_acct *out, uint64_t c
 }
 
 // ---------------------------------------------------------------------------
+// lawful intercept (li.cu)
+// ---------------------------------------------------------------------------
+static_assert(sizeof(bng_li_record) == LI_HDR, "struct bng_li_record is the device record's header");
+#define LI_TSLOTS (2 * BNG_LI_MAX_TARGETS) // the target set at its fullest: load 1/2
+
+// A ring of cap records of 64 + snaplen (rounded up to 16) bytes.  The previous ring, if any, is discarded only once
+// the new one exists; its records (drained or not) are counted as lost.
+static int li_collect_locked(bng_ctx *c);
+static int li_ring_locked(bng_ctx *c, u32 snaplen, u32 cap) {
+    const u32 rec = LI_HDR + ((snaplen + 15u) & ~15u);
+    u8 *ring = nullptr;
+    if (cudaMalloc((void **)&ring, (size_t)cap * rec) != cudaSuccess) {
+        cudaGetLastError();
+        return fail(c, -ENOMEM, "li_configure: %zu bytes of device memory", (size_t)cap * rec);
+    }
+    if (c->li_ring) {
+        if (int r = li_collect_locked(c)) {
+            cudaFree(ring);
+            return r;
+        }
+        c->li_lost_host += c->li_pending.size() / c->li_rec;
+        c->li_pending.clear();
+        cudaFree(c->li_ring);
+    }
+    c->li_ring = ring, c->li_cap = cap, c->li_rec = rec, c->li_snap = snaplen;
+    CU(c, cudaMemsetAsync(c->li_ctl, 0, 8, c->L.stream)); // no slot handed out
+    return 0;
+}
+
+// Everything interception needs, on first use: control words, target set, match list, attribution words; the ring
+// with the given size unless one exists.
+static int li_alloc_locked(bng_ctx *c, u32 snaplen = 1518, u32 cap = 1u << 15) {
+    if (!c->li_ctl) {
+        Scratch &s = c->L.s;
+        if (!s.attr) CU(c, cudaMalloc((void **)&s.attr, (size_t)s.cap * 4));
+        CU(c, cudaMalloc((void **)&c->li_match, (size_t)s.cap * sizeof(uint2)));
+        if (int r = dev_alloc(c, (void **)&c->li_words, LI_TSLOTS * 8, 0)) return r;
+        if (int r = dev_alloc(c, (void **)&c->li_ids, LI_TSLOTS * 4, 0)) return r;
+        u64 *ctl = nullptr;
+        if (int r = dev_alloc(c, (void **)&ctl, 32, 0)) return r;
+        c->li_ctl = ctl;
+    }
+    return c->li_ring ? 0 : li_ring_locked(c, snaplen, cap);
+}
+
+// The device copy of the targets (bng_prog_run, when they changed): an AddrSet of a power of two >= 2n slots.
+static int li_upload_locked(bng_ctx *c) {
+    u32 slots = 64;
+    while (slots < 2 * c->li_targets.size()) slots *= 2;
+    std::vector<u64> words(slots, 0);
+    std::vector<u32> ids(slots, 0);
+    const u32 mask = slots - 1;
+    for (const auto &t : c->li_targets) {
+        u32 i = aset_home(t.first, mask);
+        while (words[i]) i = (i + 1) & mask;
+        words[i] = ADDRSET_LIVE | t.first;
+        ids[i] = t.second;
+    }
+    // pageable sources: the copies are staged before the calls return, so the vectors may go
+    CU(c, cudaMemcpyAsync(c->li_words, words.data(), (size_t)slots * 8, cudaMemcpyHostToDevice, c->L.stream));
+    CU(c, cudaMemcpyAsync(c->li_ids, ids.data(), (size_t)slots * 4, cudaMemcpyHostToDevice, c->L.stream));
+    c->li_mask = mask;
+    c->li_dirty = false;
+    return 0;
+}
+
+// Moves the ring's records to li_pending, ordered by (batch, frame), void ones left out; the ring is empty after.
+static int li_collect_locked(bng_ctx *c) {
+    u64 cnt = 0;
+    CU(c, cudaMemcpyAsync(&cnt, c->li_ctl, 8, cudaMemcpyDeviceToHost, c->L.stream));
+    CU(c, cudaStreamSynchronize(c->L.stream));
+    cnt = std::min<u64>(cnt, c->li_cap);
+    if (!cnt) return 0;
+    const size_t rb = c->li_rec;
+    std::vector<u8> raw(cnt * rb);
+    CU(c, cudaMemcpyAsync(raw.data(), c->li_ring, raw.size(), cudaMemcpyDeviceToHost, c->L.stream));
+    CU(c, cudaMemsetAsync(c->li_ctl, 0, 8, c->L.stream));
+    CU(c, cudaStreamSynchronize(c->L.stream));
+    std::vector<u32> order;
+    order.reserve(cnt);
+    for (u32 i = 0; i < cnt; i++)
+        if (((const bng_li_record *)(raw.data() + i * rb))->verdict != LI_VOID) order.push_back(i);
+    auto at = [&](u32 i) { return (const bng_li_record *)(raw.data() + i * rb); };
+    std::sort(order.begin(), order.end(), [&](u32 a, u32 b) {
+        return at(a)->batch != at(b)->batch ? at(a)->batch < at(b)->batch : at(a)->frame < at(b)->frame;
+    });
+    const size_t have = c->li_pending.size();
+    c->li_pending.resize(have + order.size() * rb);
+    for (size_t k = 0; k < order.size(); k++) memcpy(&c->li_pending[have + k * rb], at(order[k]), rb);
+    return 0;
+}
+
+int bng_li_configure(bng_ctx *c, uint32_t snaplen, uint32_t capacity) {
+    if (!c || snaplen > 65535 || capacity > (1u << 30)) return -EINVAL;
+    std::lock_guard<std::mutex> g(c->mu);
+    cudaSetDevice(c->device);
+    snaplen = snaplen ? snaplen : 1518;
+    capacity = capacity ? capacity : (1u << 15);
+    if (!c->li_ring) return li_alloc_locked(c, snaplen, capacity);
+    return li_ring_locked(c, snaplen, capacity);
+}
+
+uint32_t bng_li_record_size(bng_ctx *c) {
+    if (!c) return 0;
+    std::lock_guard<std::mutex> g(c->mu);
+    return c->li_ring ? c->li_rec : 0;
+}
+
+int bng_li_target_set(bng_ctx *c, uint32_t addr, uint32_t target_id) {
+    if (!c) return -EINVAL;
+    std::lock_guard<std::mutex> g(c->mu);
+    cudaSetDevice(c->device);
+    if (int r = li_alloc_locked(c)) return r;
+    if (c->li_targets.size() >= BNG_LI_MAX_TARGETS && !c->li_targets.count(addr)) return -E2BIG;
+    c->li_targets[addr] = target_id;
+    c->li_dirty = true;
+    return 0;
+}
+
+int bng_li_target_del(bng_ctx *c, uint32_t addr) {
+    if (!c) return -EINVAL;
+    std::lock_guard<std::mutex> g(c->mu);
+    if (!c->li_targets.erase(addr)) return -ENOENT;
+    c->li_dirty = true;
+    return 0;
+}
+
+int bng_li_drain(bng_ctx *c, void *buf, uint64_t cap_records, uint64_t *n_out) {
+    if (!c || !n_out || (cap_records && !buf)) return -EINVAL;
+    *n_out = 0;
+    std::lock_guard<std::mutex> g(c->mu);
+    cudaSetDevice(c->device);
+    if (!c->li_ring) return 0;
+    if (int r = li_collect_locked(c)) return r;
+    const u64 n = std::min<u64>(c->li_pending.size() / c->li_rec, cap_records);
+    if (n) {
+        memcpy(buf, c->li_pending.data(), n * c->li_rec);
+        c->li_pending.erase(c->li_pending.begin(), c->li_pending.begin() + n * c->li_rec);
+    }
+    *n_out = n;
+    return 0;
+}
+
+uint64_t bng_li_lost(bng_ctx *c) {
+    if (!c) return 0;
+    std::lock_guard<std::mutex> g(c->mu);
+    if (!c->li_ctl) return 0;
+    cudaSetDevice(c->device);
+    u64 v = 0;
+    if (cudaMemcpyAsync(&v, c->li_ctl + 1, 8, cudaMemcpyDeviceToHost, c->L.stream) != cudaSuccess) return 0;
+    cudaStreamSynchronize(c->L.stream);
+    return v + c->li_lost_host;
+}
+
+// ---------------------------------------------------------------------------
 // snapshot / restore (SURVEY.md §8f-4: device-table state for HA hand-over, reference pkg/ha)
 // A snapshot is a self-describing blob: header, then per map { name, kind, key size, value size, entry count,
 // keys, values } for every hash / array / LPM / statistics map (event rings are not state).  Restore clears
@@ -1668,6 +1865,10 @@ struct SnapMapHdr {
 // without accounting steps over it; a context that never allocated records writes no such section.
 const char kSnapAcct[] = "subscriber_acct";
 const u32 kSnapAcctKind = 5;
+// Trailing section of the interception targets: (address, target id) pairs, by address.  Written by a context that
+// has used interception; the records are not state and stay out.
+const char kSnapLi[] = "li_targets";
+const u32 kSnapLiKind = 6;
 } // namespace
 
 int64_t bng_snapshot(bng_ctx *c, void *buf, uint64_t cap) {
@@ -1720,6 +1921,17 @@ int64_t bng_snapshot(bng_ctx *c, void *buf, uint64_t cap) {
         out.insert(out.end(), (u8 *)recs.data(), (u8 *)(recs.data() + got));
         nmaps++;
     }
+    if (c->li_ctl) {
+        std::vector<std::pair<u32, u32>> t(c->li_targets.begin(), c->li_targets.end());
+        std::sort(t.begin(), t.end());
+        SnapMapHdr h{};
+        snprintf(h.name, sizeof(h.name), "%s", kSnapLi);
+        h.kind = kSnapLiKind, h.key_size = 4, h.value_size = 4, h.count = t.size();
+        out.insert(out.end(), (u8 *)&h, (u8 *)&h + sizeof(h));
+        for (auto &e : t) out.insert(out.end(), (u8 *)&e.first, (u8 *)&e.first + 4);
+        for (auto &e : t) out.insert(out.end(), (u8 *)&e.second, (u8 *)&e.second + 4);
+        nmaps++;
+    }
     memcpy(&out[nmaps_at], &nmaps, 8);
     if (buf && cap >= out.size()) memcpy(buf, out.data(), out.size());
     return (int64_t)out.size(); // the size needed; nothing was copied when cap is smaller
@@ -1738,9 +1950,13 @@ int bng_restore(bng_ctx *c, const void *buf, uint64_t len) {
             CU(c, cudaMemsetAsync(c->acct, 0, ((size_t)c->dev.subdir.mask + 1) * sizeof(bng_acct), c->L.stream));
             CU(c, cudaStreamSynchronize(c->L.stream));
         }
+        if (!c->li_targets.empty()) { // the same for the interception targets
+            c->li_targets.clear();
+            c->li_dirty = true;
+        }
     }
-    const u8 *acct_p = nullptr;
-    u64 acct_n = 0;
+    const u8 *acct_p = nullptr, *li_p = nullptr;
+    u64 acct_n = 0, li_n = 0;
     for (u64 k = 0; k < nmaps; k++) {
         if (p + sizeof(SnapMapHdr) > end) return -EINVAL;
         SnapMapHdr h;
@@ -1753,6 +1969,14 @@ int bng_restore(bng_ctx *c, const void *buf, uint64_t len) {
             if (h.key_size != 4 || h.value_size != sizeof(bng_acct)) return fail(c, -EINVAL, "snapshot: %s has another layout", h.name);
             acct_p = p;
             acct_n = h.count;
+            p += kb + vb;
+            continue;
+        }
+        if (!strcmp(h.name, kSnapLi)) {
+            if (h.key_size != 4 || h.value_size != 4 || h.count > BNG_LI_MAX_TARGETS)
+                return fail(c, -EINVAL, "snapshot: %s has another layout", h.name);
+            li_p = p;
+            li_n = h.count;
             p += kb + vb;
             continue;
         }
@@ -1792,6 +2016,18 @@ int bng_restore(bng_ctx *c, const void *buf, uint64_t len) {
             CU(c, run_acct_load(c->L, c->dev.subdir, c->acct, (const u32 *)c->io_dev, (const u64 *)(c->io_dev + roff), k));
             CU(c, cudaStreamSynchronize(c->L.stream));
         }
+    }
+    if (li_n) {
+        std::lock_guard<std::mutex> g(c->mu);
+        cudaSetDevice(c->device);
+        if (int r = li_alloc_locked(c)) return r;
+        for (u64 k = 0; k < li_n; k++) {
+            u32 a, id;
+            memcpy(&a, li_p + k * 4, 4);
+            memcpy(&id, li_p + li_n * 4 + k * 4, 4);
+            c->li_targets[a] = id;
+        }
+        c->li_dirty = true;
     }
     return 0;
 }

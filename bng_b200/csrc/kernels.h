@@ -101,3 +101,32 @@ cudaError_t run_acct_read(Launcher &L, const Tbl &dir, const u64 *acct, const u3
 cudaError_t run_acct_dump(Launcher &L, const Tbl &dir, const u64 *acct, u32 *addrs_out, u64 *out, u32 *count, u64 cap);
 // record of every address of the list that has a directory entry := the given one (snapshot restore)
 cudaError_t run_acct_load(Launcher &L, const Tbl &dir, u64 *acct, const u32 *addrs, const u64 *recs, u64 n);
+
+// lawful intercept (li.cu).  A record is LI_HDR bytes of header (struct bng_li_record) and the captured bytes, zero
+// padded to rec_bytes.  The targets are an AddrSet with target ids index-aligned to its words.
+#define LI_HDR 64
+#define LI_NOSLOT 0xFFFFFFFFu // match without a ring slot (the ring was full)
+#define LI_VOID 0xFFu         // verdict byte of a record the drain skips (a frame antispoof dropped)
+struct LiRing {
+    u8 *buf;   // cap records of rec_bytes
+    u64 *ctl;  // [0] slots handed out (may pass cap), [1] records lost, [2] (u32) uplink matches of the run
+    uint2 *match; // uplink: (frame, ring slot or LI_NOSLOT) of every match of the run, in no order
+    u32 cap, rec_bytes, snaplen, prog;
+    AddrSet tgt;
+    const u32 *ids;
+    u64 batch;
+};
+// Where the bytes of a chunk of a pinned host batch live (run_host_zero_copy): the program sees a compact copy of
+// the first need[i] bytes (rounded up to 16) of each frame; the rest stays in the mapped host arena, which the TC
+// programs never touch.  arena == nullptr: the DevBatch holds whole frames.
+struct LiSrc {
+    const u8 *arena;   // device view of the chunk's host arena
+    const u32 *off16;  // the chunk's offsets, or nullptr (fixed stride)
+    const u32 *need;   // bytes of each frame in the compact copy, or nullptr: the compact slot is the whole storage
+    u32 stride;        // the caller's stride
+};
+// UP: before the program (the frame as it entered), reserves the slots and lists the matches; then run_li_verdict
+// after the program.  !UP: after the program, complete records.  attr: classify's attribution words in the pipelines
+// (a SHOT frame without one was dropped by antispoof), else nullptr.
+cudaError_t run_li_capture(Launcher &L, const LiRing &r, const DevBatch &b, const LiSrc &src, bool up);
+cudaError_t run_li_verdict(Launcher &L, const LiRing &r, const DevBatch &b, const u32 *attr);

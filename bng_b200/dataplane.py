@@ -12,7 +12,7 @@ import os
 
 import numpy as np
 
-from .layouts import as_bytes, bng_acct
+from .layouts import as_bytes, bng_acct, bng_li_record
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("BNG_B200_LIB") or os.path.join(HERE, "libbng_b200.so")  # override: A/B builds
@@ -105,6 +105,12 @@ def load_library() -> C.CDLL:
         "bng_acct_read": ([vp, vp, u64, vp, vp], i32),
         "bng_acct_dump": ([vp, vp, vp, u64], C.c_int64),
         "bng_nat_flush": ([vp, vp, u64, u64, C.POINTER(u64)], i32),
+        "bng_li_configure": ([vp, u32, u32], i32),
+        "bng_li_record_size": ([vp], u32),
+        "bng_li_target_set": ([vp, u32, u32], i32),
+        "bng_li_target_del": ([vp, u32], i32),
+        "bng_li_drain": ([vp, vp, u64, C.POINTER(u64)], i32),
+        "bng_li_lost": ([vp], u64),
     }
     for name, (args, res) in protos.items():
         fn = getattr(lib, name)
@@ -123,6 +129,7 @@ EXPORTED_SYMBOLS = (
     "bng_prof_read", "bng_host_alloc", "bng_host_free", "bng_map_update_staged", "bng_staged_info",
     "bng_comm_unique_id", "bng_comm_init", "bng_sync_reduce", "bng_sweep", "bng_lru_evictions", "bng_snapshot", "bng_restore", "bng_table_rebuilds",
     "bng_acct_enable", "bng_acct_read", "bng_acct_dump", "bng_nat_flush",
+    "bng_li_configure", "bng_li_record_size", "bng_li_target_set", "bng_li_target_del", "bng_li_drain", "bng_li_lost",
 )
 
 
@@ -358,6 +365,48 @@ class Dataplane:
         out = (C.c_uint64 * 3)()
         self._chk(self.lib.bng_nat_flush(self.h, a.ctypes.data if len(a) else None, len(a), now_ns, out), "nat_flush")
         return tuple(int(x) for x in out)
+
+    # ---- lawful intercept: content of communication ----
+    def li_configure(self, snaplen: int = 0, capacity: int = 0):
+        """(Re)create the capture ring: `capacity` records of `snaplen` bytes (0: 1518 bytes, 2^15 records).  Records
+        not yet drained are discarded and counted in li_lost."""
+        self._chk(self.lib.bng_li_configure(self.h, snaplen, capacity), "li_configure")
+
+    @property
+    def li_record_size(self) -> int:
+        return self.lib.bng_li_record_size(self.h)
+
+    def li_target_set(self, addr: int, target_id: int):
+        """Capture the frames of `addr` (u32 holding the qos_ingress key bytes) as `target_id`."""
+        self._chk(self.lib.bng_li_target_set(self.h, int(addr), int(target_id)), "li_target_set")
+
+    def li_target_del(self, addr: int) -> int:
+        """Stop capturing `addr`; returns 0 or -ENOENT (no exception)."""
+        return self.lib.bng_li_target_del(self.h, int(addr))
+
+    def li_drain(self, cap: int | None = None):
+        """(bng_li_record headers[n], list of the captured bytes of each record) in (batch, frame) order; at most
+        `cap` records (None: all), the rest stay for the next call."""
+        rs = self.lib.bng_li_record_size(self.h)
+        if rs == 0:
+            return np.zeros(0, bng_li_record), []
+        out, got = [], 0
+        while cap is None or got < cap:
+            want = 1 << 14 if cap is None else min(cap - got, 1 << 14)
+            buf = np.zeros((want, rs), np.uint8)
+            n = C.c_uint64(0)
+            self._chk(self.lib.bng_li_drain(self.h, buf.ctypes.data, want, C.byref(n)), "li_drain")
+            out.append(buf[: n.value])
+            got += n.value
+            if n.value < want:
+                break
+        raw = np.concatenate(out) if out else np.zeros((0, rs), np.uint8)
+        hdr = raw[:, :64].copy().view(bng_li_record).reshape(-1)
+        return hdr, [raw[i, 64:64 + int(h["cap_len"])].copy() for i, h in enumerate(hdr)]
+
+    @property
+    def li_lost(self) -> int:
+        return self.lib.bng_li_lost(self.h)
 
     def sweep(self, now_ns: int) -> int:
         """Session expiry sweep at now_ns; returns the number of sessions removed."""

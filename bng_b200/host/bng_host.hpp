@@ -22,6 +22,7 @@
 #pragma once
 
 #include <chrono>
+#include <cstddef>
 #include <cstdint>
 #include <cstring>
 #include <functional>
@@ -148,6 +149,94 @@ inline AcctReader ContextReader(std::shared_ptr<Backend> b) {
 }
 
 } // namespace radius
+
+// ===========================================================================
+// Lawful intercept, content of communication (reference pkg/intercept/manager.go:337: Manager.RecordCC(warrant,
+// session, direction, srcIP, dstIP, srcPort, dstPort, protocol, payload)).  StartInterceptSession sets the session's
+// IPv4 address as a target (bng_li_target_set), StopInterceptSession deletes it; PumpCC drains the records and hands
+// each one, parsed into RecordCC's arguments, to the caller.
+namespace intercept {
+
+enum class Direction : uint8_t { Uplink = BNG_LI_UPLINK, Downlink = BNG_LI_DOWNLINK };
+
+struct CC {
+    bng_li_record rec;                // the record's header: target, frame, batch, verdict, timestamp
+    Direction direction = Direction::Uplink;
+    IP src, dst;                      // 4 bytes each, wire order; 0.0.0.0 when the capture is too short for it
+    uint16_t src_port = 0, dst_port = 0; // host order
+    uint8_t protocol = 0;
+    std::vector<uint8_t> payload;     // the IP packet as captured: bytes 14 .. cap_len of the frame
+};
+
+// The fields RecordCC takes, from one record (header + cap_len captured bytes).  Ports: TCP / UDP source and
+// destination port at 14 + 4 * ihl; ICMP echo request / reply: the echo id, which the NAT translates in place of a port,
+// as the subscriber-side port (src_port uplink, dst_port downlink); 0 for any other protocol or when the capture ends
+// before them.  Returns false when the capture does not hold the IPv4 header's first 20 bytes' addresses.
+inline bool ParseCC(const uint8_t *record, CC *out) {
+    memcpy(&out->rec, record, sizeof(bng_li_record));
+    const uint8_t *f = record + sizeof(bng_li_record);
+    const uint32_t n = out->rec.cap_len;
+    out->direction = out->rec.dir == BNG_LI_DOWNLINK ? Direction::Downlink : Direction::Uplink;
+    out->src = n >= 30 ? IP(f + 26, f + 30) : IPv4(0, 0, 0, 0);
+    out->dst = n >= 34 ? IP(f + 30, f + 34) : IPv4(0, 0, 0, 0);
+    out->protocol = n >= 24 ? f[23] : 0;
+    out->src_port = out->dst_port = 0;
+    out->payload.assign(f + (n > 14 ? 14 : n), f + n);
+    if (n < 34) return false;
+    const uint32_t l4 = 14 + 4u * (f[14] & 0x0f);
+    auto be16 = [&](uint32_t off) { return (uint16_t)(f[off] << 8 | f[off + 1]); };
+    if ((out->protocol == 6 || out->protocol == 17) && n >= l4 + 4) {
+        out->src_port = be16(l4);
+        out->dst_port = be16(l4 + 2);
+    } else if (out->protocol == 1 && n >= l4 + 6 && (f[l4] == 0 || f[l4] == 8)) {
+        (out->direction == Direction::Uplink ? out->src_port : out->dst_port) = be16(l4 + 4);
+    }
+    return true;
+}
+
+// The caller's warrant / session of a target id, or none: the record is skipped (an IRI-only warrant, a session that
+// ended while its records were queued), as RecordCC skips them.
+template <class W>
+using Resolver = std::function<std::optional<W>(uint32_t target_id)>;
+template <class W>
+using Sink = std::function<void(const W &warrant, const CC &cc)>;
+
+// records laid out as bng_li_drain() returns them; returns the number handed to the sink
+template <class W>
+inline uint64_t PumpRecords(const uint8_t *recs, uint64_t n, uint32_t rec_size, const Resolver<W> &resolve, const Sink<W> &sink) {
+    uint64_t done = 0;
+    CC cc;
+    for (uint64_t i = 0; i < n; i++) {
+        const uint8_t *r = recs + i * rec_size;
+        uint32_t id;
+        memcpy(&id, r + offsetof(bng_li_record, target_id), 4);
+        std::optional<W> w = resolve(id);
+        if (!w) continue;
+        ParseCC(r, &cc);
+        sink(*w, cc);
+        done++;
+    }
+    return done;
+}
+
+// Drains the context until it is empty, `batch` records per call.  Returns the records handed to the sink, or a
+// negative errno.
+template <class W>
+inline int64_t PumpCC(bng_ctx *ctx, const Resolver<W> &resolve, const Sink<W> &sink, uint64_t batch = 4096) {
+    const uint32_t rs = bng_li_record_size(ctx);
+    if (!rs) return 0;
+    std::vector<uint8_t> buf((size_t)batch * rs);
+    int64_t total = 0;
+    for (;;) {
+        uint64_t n = 0;
+        int rc = bng_li_drain(ctx, buf.data(), batch, &n);
+        if (rc) return rc;
+        total += (int64_t)PumpRecords<W>(buf.data(), n, rs, resolve, sink);
+        if (n < batch) return total;
+    }
+}
+
+} // namespace intercept
 
 // ===========================================================================
 namespace ebpf {

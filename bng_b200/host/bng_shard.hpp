@@ -247,6 +247,49 @@ class Router {
         }
         return rc;
     }
+    // Lawful-intercept targets (bng_li_target_set / _del) go to the shard that owns the address: its upstream frames
+    // follow the subscriber's MAC there, and downstream frames are steered there by (public address, port block).  An
+    // address whose owner is not known goes to every shard.  Del returns -ENOENT when no shard had the target.
+    std::vector<size_t> LiShards(uint32_t addr_key) const {
+        auto s = dir_->ShardOfIP(addr_key);
+        std::vector<size_t> out;
+        for (size_t k = 0; k < shards_.size(); k++)
+            if (!s || *s == k) out.push_back(k);
+        return out;
+    }
+    int LiTargetSet(uint32_t addr_key, uint32_t target_id) {
+        for (size_t k : LiShards(addr_key))
+            if (int r = bng_li_target_set(shards_[k]->ctx, addr_key, target_id)) return r;
+        return 0;
+    }
+    int LiTargetDel(uint32_t addr_key) {
+        int rc = -ENOENT;
+        for (size_t k : LiShards(addr_key)) {
+            int r = bng_li_target_del(shards_[k]->ctx, addr_key);
+            if (r == 0) rc = 0;
+            else if (r != -ENOENT) return r;
+        }
+        return rc;
+    }
+    // Drains every shard: fn(shard, record, record size) per record, in (batch, frame) order within a shard (batch
+    // numbers are per shard).  Returns the number of records or a negative errno.
+    template <class F>
+    int64_t LiDrain(F &&fn, uint64_t batch = 4096) {
+        int64_t total = 0;
+        for (size_t k = 0; k < shards_.size(); k++) {
+            const uint32_t rs = bng_li_record_size(shards_[k]->ctx);
+            if (!rs) continue;
+            std::vector<uint8_t> buf((size_t)batch * rs);
+            for (;;) {
+                uint64_t n = 0;
+                if (int r = bng_li_drain(shards_[k]->ctx, buf.data(), batch, &n)) return r;
+                for (uint64_t i = 0; i < n; i++) fn(k, buf.data() + i * rs, rs);
+                total += (int64_t)n;
+                if (n < batch) break;
+            }
+        }
+        return total;
+    }
     radius::AcctReader Reader() {
         return [this](uint32_t addr, bng_acct *out) { return AcctRead(addr, out); };
     }

@@ -117,7 +117,14 @@ bng_acct = np.dtype([(n, "<u8") for n in (
     "up_packets", "up_bytes", "up_drop_packets", "up_drop_bytes",
     "down_packets", "down_bytes", "down_drop_packets", "down_drop_bytes")])
 
+# lawful-intercept record header (include/bng_b200.h: struct bng_li_record, 64 B); the captured bytes follow it
+LI_UPLINK, LI_DOWNLINK = 0, 1
+bng_li_record = np.dtype([
+    ("ts_ns", "<u8"), ("batch", "<u8"), ("frame", "<u4"), ("target_id", "<u4"), ("addr", "<u4"), ("wire_len", "<u4"),
+    ("cap_len", "<u4"), ("dir", "u1"), ("verdict", "u1"), ("prog", "u1"), ("pad", "u1", 25)])
+
 assert subscriber_binding.itemsize == 24 and token_bucket.itemsize == 32 and bng_acct.itemsize == 64
+assert bng_li_record.itemsize == 64
 assert nat_key.itemsize == 16 and eim_key.itemsize == 8 and eim_mapping.itemsize == 32
 assert nat_session.itemsize == 80 and port_block.itemsize == 32 and subscriber_nat.itemsize == 64
 assert nat_stats.itemsize == 104 and nat_log_entry.itemsize == 40 and nat_config.itemsize == 16

@@ -244,6 +244,59 @@ int bng_acct_read(bng_ctx *ctx, const uint32_t *addrs, uint64_t n, bng_acct *out
  * GPU, then copied out).  Returns the number written or a negative errno, as bng_map_dump() does. */
 int64_t bng_acct_dump(bng_ctx *ctx, uint32_t *addrs_out, bng_acct *out, uint64_t cap);
 
+/* ---- lawful intercept: content of communication (what pkg/intercept's RecordCC takes) ----
+ * A frame of a target address is copied, as the subscriber's side of the BNG sees it, into a record on the GPU;
+ * bng_li_drain() hands the records out in frame order.
+ * Which frames are captured: exactly the frames accounting would charge, attributed by the same rule.
+ *   - Upstream programs (nat44_egress, qos_ingress_prog, pipeline_up, pipeline_tc): a frame whose IPv4 SOURCE, as the
+ *     frame entered the program, is a target: untagged Ethernet II, ethertype 0x0800, bytes 26-29 present.
+ *   - Downstream programs (nat44_ingress, qos_egress_prog): a frame whose IPv4 DESTINATION, as the frame leaves the
+ *     program (after DNAT), is a target: bytes 30-33 present.
+ *   - The verdict is TC_ACT_OK or TC_ACT_SHOT; both are captured.  In the two pipelines a frame that antispoof drops
+ *     is not captured: it may have forged its address.  Other programs never capture.
+ *   - A target is any address; it needs no subscriber_nat or qos_ingress entry.  The targets in force are those set
+ *     when bng_prog_run is called.
+ * What is captured: the first cap_len bytes of the frame as it entered the program (upstream, before SNAT) or as the
+ * program left it (downstream, after DNAT).  "Bytes present in the frame's storage" is len with an offset table and
+ * min(len, stride) in a fixed-stride arena.  The bytes of a record past cap_len are zero.
+ * Drain: records come out ordered by (batch, frame), each bng_li_record_size() bytes.  Records that do not fit in
+ * cap_records stay for the next call, as bng_events_drain leaves them; the call sees everything queued on the
+ * context's stream.  buf may be NULL when cap_records is 0.
+ * Overflow: when the ring is full, the records that do not fit are dropped and counted in bng_li_lost().  Which
+ * records of the overflowing batch survive is unspecified; every record that survives is complete and correct.
+ * Lifecycle: the first bng_li_configure() or bng_li_target_set() allocates the ring (capacity x record size bytes)
+ * and a table of up to BNG_LI_MAX_TARGETS targets; a context that never uses either allocates nothing, and with no
+ * target set bng_prog_run launches no kernel for interception.  bng_li_configure() again replaces the ring: records
+ * not yet drained are discarded and counted as lost.  bng_snapshot() carries the targets (a trailing "li_targets"
+ * section), not the records; bng_restore() of a blob without that section leaves no targets.
+ * The batch number is the context's batch sequence: 1 for its first bng_prog_run, advanced by every bng_prog_run,
+ * bng_sweep and bng_nat_flush. */
+#define BNG_LI_UPLINK 0
+#define BNG_LI_DOWNLINK 1
+#define BNG_LI_MAX_TARGETS 4096
+typedef struct bng_li_record { /* 64 bytes; followed by the captured bytes, up to the record size */
+    uint64_t ts_ns;     /* the frame's bpf_ktime_get_ns(): now_ns_v[i], or the batch's now_ns */
+    uint64_t batch;     /* the run's batch sequence number: strictly increasing from run to run on a context */
+    uint32_t frame;     /* index of the frame in its batch */
+    uint32_t target_id; /* as given to bng_li_target_set */
+    uint32_t addr;      /* the matched subscriber address, in the byte order of the qos_ingress key */
+    uint32_t wire_len;  /* the frame's len (the TC programs never change it) */
+    uint32_t cap_len;   /* captured bytes that follow: min(len, bytes present in the frame's storage, snaplen) */
+    uint8_t dir;        /* BNG_LI_UPLINK / BNG_LI_DOWNLINK */
+    uint8_t verdict;    /* TC_ACT_OK or TC_ACT_SHOT */
+    uint8_t prog;       /* bng_prog_id() of the run */
+    uint8_t pad[25];    /* zero */
+} bng_li_record;
+/* snaplen 0 = 1518 bytes, else 1..65535; capacity 0 = 2^15 records, else at most 2^30.  -EINVAL outside those,
+ * -ENOMEM when the ring does not fit in device memory (the previous ring is then kept). */
+int bng_li_configure(bng_ctx *ctx, uint32_t snaplen, uint32_t capacity);
+uint32_t bng_li_record_size(bng_ctx *ctx); /* 64 + snaplen rounded up to 16; 0 before the ring exists */
+int bng_li_target_set(bng_ctx *ctx, uint32_t addr, uint32_t target_id); /* insert or replace; -E2BIG when full */
+int bng_li_target_del(bng_ctx *ctx, uint32_t addr);                      /* -ENOENT when absent */
+/* *n_out = records copied to buf (n_out must not be NULL) */
+int bng_li_drain(bng_ctx *ctx, void *buf, uint64_t cap_records, uint64_t *n_out);
+uint64_t bng_li_lost(bng_ctx *ctx); /* records dropped because the ring was full, or discarded by a reconfiguration */
+
 /* ---- diagnostics ---- */
 uint64_t bng_launch_count(bng_ctx *ctx);  /* kernels launched by this context so far */
 uint64_t bng_lru_overflow(bng_ctx *ctx);  /* inserts that found no victim to evict in a full LRU map (should stay 0) */
