@@ -322,6 +322,7 @@ __global__ void __launch_bounds__(BLOCK) k_nat_hairpin_xdp(const __grid_constant
 // input, so (digit, block) order of the scanned histogram is index order.
 // ---------------------------------------------------------------------------
 #define RS_BLOCKS_PER_SM 3 // what the scatter's 71 registers x 256 threads lets an SM hold: one wave, whole tiles
+#define RS_HIST_VEC 4      // 16-byte key loads in flight per thread in k_rs_hist
 
 __device__ __forceinline__ void rs_range(u32 total, u32 &lo, u32 &hi) {
     u32 per = (total + gridDim.x - 1) / gridDim.x;
@@ -344,12 +345,31 @@ __global__ void __launch_bounds__(BLOCK) k_rs_hist(const u32 *keys, u32 n_host, 
     u32 total = first ? n_host : cnt[CNT_M];
     u32 lo, hi;
     rs_range(total, lo, hi);
-    for (u32 i = lo + threadIdx.x; i < hi; i += BLOCK) {
-        u32 k = keys[i];
-        if (k != NO_KEY) {
-            k &= kmask; // (the bits above the key carry the frame length: DevBatch.kshift)
-            atomicAdd(&h[(k >> shift) & 0xff], 1u);
-            mymax = k > mymax ? k : mymax;
+    // RS_HIST_VEC 16-byte loads per thread are issued before any of their keys is counted: one 4-byte load at a
+    // time leaves the pass latency-bound (lo is a multiple of BLOCK, so every vector is aligned)
+    for (u32 i0 = lo + threadIdx.x * 4; i0 < hi; i0 += BLOCK * 4 * RS_HIST_VEC) {
+        uint4 v[RS_HIST_VEC];
+#pragma unroll
+        for (int u = 0; u < RS_HIST_VEC; u++) {
+            const u32 i = i0 + u * BLOCK * 4;
+            if (i + 3 < hi) {
+                v[u] = *(const uint4 *)(keys + i);
+            } else {
+                v[u].x = i < hi ? keys[i] : NO_KEY;
+                v[u].y = i + 1 < hi ? keys[i + 1] : NO_KEY;
+                v[u].z = i + 2 < hi ? keys[i + 2] : NO_KEY;
+                v[u].w = NO_KEY;
+            }
+        }
+#pragma unroll
+        for (int u = 0; u < 4 * RS_HIST_VEC; u++) {
+            const uint4 &q = v[u / 4];
+            u32 k = (u & 3) == 0 ? q.x : (u & 3) == 1 ? q.y : (u & 3) == 2 ? q.z : q.w;
+            if (k != NO_KEY) {
+                k &= kmask; // (the bits above the key carry the frame length: DevBatch.kshift)
+                atomicAdd(&h[(k >> shift) & 0xff], 1u);
+                mymax = k > mymax ? k : mymax;
+            }
         }
     }
     __syncthreads();
@@ -410,7 +430,7 @@ __global__ void __launch_bounds__(1024) k_rs_scan(u32 *H, const u32 *T, u32 nblo
 
 // Stable scatter of one radix pass.  A tile is 8 warps x RS_ROWS x 32 elements; warp w owns the
 // contiguous elements [w * RS_ROWS * 32, (w + 1) * RS_ROWS * 32) of the tile and walks them row by row,
-// so index order is (warp, row, lane).  Ranks inside a row come from __match_any_sync, ranks across
+// so index order is (warp, row, lane).  Ranks inside a row come from one ballot per digit bit, ranks across
 // the rows of a warp from a warp-private running histogram in shared memory; thread d then turns the
 // 8 per-warp totals of digit d into tile-local offsets.  The tile is reordered by digit in shared
 // memory and written out from there, so that a warp's store covers runs of consecutive addresses
@@ -466,8 +486,15 @@ __global__ void __launch_bounds__(BLOCK) k_rs_scatter(const u32 *keys, const u32
 #pragma unroll
         for (int r = 0; r < RS_ROWS; r++) {
             const bool ok = k[r] != NO_KEY;
-            u32 d = ok ? (((k[r] & kmask) >> shift) & 0xff) : (256 + lane); // invalid lanes match nobody
-            u32 peers = __match_any_sync(0xffffffffu, d);
+            const u32 d = ok ? (((k[r] & kmask) >> shift) & 0xff) : 0;
+            // the valid lanes with the same digit: one ballot per digit bit (cheaper than match.any)
+            u32 peers = __ballot_sync(0xffffffffu, ok);
+#pragma unroll
+            for (int bit = 0; bit < 8; bit++) {
+                const bool one = (d >> bit) & 1;
+                const u32 ones = __ballot_sync(0xffffffffu, one);
+                peers &= one ? ones : ~ones;
+            }
             u32 before = ok ? wh[w][d] : 0; // elements of digit d in the earlier rows of this warp
             u32 rk = __popc(peers & ((1u << lane) - 1));
             __syncwarp();
