@@ -7,6 +7,7 @@
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
+#include <time.h>
 #include <dlfcn.h>
 #include <sys/mman.h>
 
@@ -121,6 +122,26 @@ struct bng_ctx {
     uint2 *li_match = nullptr; // [L.s.cap]
     std::vector<u8> li_pending; // records copied out of the ring, ordered, not yet drained
     u64 li_lost_host = 0;       // records discarded by a reconfiguration
+    // incremental replication (bng_delta_*, delta.cu).  Exporter: one shadow per hash map (map id), and one of the
+    // accounting records (map -1) once they exist; empty while tracking is off.
+    struct DeltaShadow {
+        int map;
+        u64 *words;
+        u64 nslots;
+        u32 sw;
+    };
+    std::vector<DeltaShadow> dshadow;
+    bool delta_full = true;                 // the next export is FULL
+    u64 delta_stream = 0, delta_seq = 0;    // exporter: stream id, sequence of the last export
+    std::vector<std::pair<u32, u32>> delta_li; // interception targets as last sent, by address
+    bool delta_li_sent = false;
+    u32 *dlist = nullptr;                   // diff lists of one table: deletions at [0, n), upserts at [n, 2n)
+    u64 dlist_slots = 0;
+    u32 *dsent = nullptr;                   // the lists of every table of an export, kept for the commit
+    u64 dsent_cap = 0;
+    u8 *demit = nullptr;                    // records of one table
+    u64 demit_cap = 0;
+    u64 dapply_stream = 0, dapply_seq = 0;  // applier: the last delta applied
 };
 
 namespace {
@@ -507,9 +528,11 @@ int bng_close(bng_ctx *c) {
         for (void *p : c->allocs) cudaFree(p);
         Scratch &s = c->L.s;
         void *sp[] = {s.key_a, s.key_b, s.val_a, s.val_b, s.qslot, s.attr, s.cub_tmp, s.counters, c->acct_dump_buf, c->li_ring, c->li_match,
-                      c->io_dev, c->hb_pkts, c->hb_off, c->hb_len, c->hb_prio, c->hb_verdict, c->hb_now, c->dump_k, c->dump_v, c->dump_c};
+                      c->io_dev, c->hb_pkts, c->hb_off, c->hb_len, c->hb_prio, c->hb_verdict, c->hb_now, c->dump_k, c->dump_v, c->dump_c,
+                      c->dlist, c->dsent, c->demit};
         for (void *p : sp)
             if (p) cudaFree(p);
+        for (auto &s : c->dshadow) cudaFree(s.words);
         if (c->io_host) cudaFreeHost(c->io_host);
         if (c->evict_word) cudaFreeHost(c->evict_word);
         if (c->evict_ev) cudaEventDestroy(c->evict_ev);
@@ -2029,6 +2052,366 @@ int bng_restore(bng_ctx *c, const void *buf, uint64_t len) {
         }
         c->li_dirty = true;
     }
+    return 0;
+}
+
+// ---------------------------------------------------------------------------
+// incremental replication (delta.cu; the blob is described in include/bng_b200.h)
+// ---------------------------------------------------------------------------
+namespace {
+const char kDeltaMagic[8] = {'B', 'N', 'G', 'D', 'E', 'L', 'T', '1'};
+struct DeltaHdr {
+    char magic[8];
+    u64 stream, seq_from, seq_to;
+    u32 flags, sections;
+};
+static_assert(sizeof(DeltaHdr) == 40 && sizeof(SnapMapHdr) == 64, "the delta framing of include/bng_b200.h");
+
+// A hash map's (or the accounting records') view for the diff: which words of a slot are compared, which is the
+// time word.  Volatile fields are left out of the mask unless exact.
+DeltaTbl delta_view(bng_ctx *c, const bng_ctx::DeltaShadow &s, u64 refresh, bool exact) {
+    DeltaTbl t{};
+    t.shadow = s.words;
+    t.nslots = s.nslots;
+    t.sw = s.sw;
+    t.tw = DELTA_NO_TIME;
+    t.refresh = refresh;
+    auto set = [&](u32 pos) { t.mask[pos / 8] |= 0xFFull << (8 * (pos % 8)); };
+    if (s.map < 0) { // accounting records: the directory's address, then the record
+        const Tbl &d = c->dev.subdir;
+        t.slots = d.slots, t.slot_bytes = d.slot_bytes, t.vals = (const u8 *)c->acct, t.vstride = sizeof(bng_acct);
+        t.kw = 1, t.key_size = 4, t.value_size = sizeof(bng_acct);
+        for (u32 b = 0; b < sizeof(bng_acct); b++) set(8 + b);
+        return t;
+    }
+    const MapReg &m = c->maps[s.map];
+    const Tbl &tb = *m.tbl;
+    t.slots = tb.slots, t.slot_bytes = tb.slot_bytes;
+    t.kw = tb.key_size <= 8 ? 1 : tb.key_size / 8;
+    t.key_size = tb.key_size, t.value_size = tb.value_size, t.voff = tb.voff, t.vlayout = tb.vlayout;
+    const bool ses = tb.vlayout == VL_SESSION, eim = !strcmp(m.name, "eim_table");
+    const bool qos = !strcmp(m.name, "qos_ingress") || !strcmp(m.name, "qos_egress");
+    for (u32 b = 0; b < tb.value_size; b++) {
+        const u32 pos = ses ? ses_abi_to_slot(b) : tb.voff + b;
+        if (ses && pos >= SES_PAD_A) continue; // the struct's padding: never compared
+        if (!exact) {
+            if (ses && b >= 24 && b < 32) continue;              // last_seen: the time rule
+            if (ses && b >= 40 && b < 72) continue;              // packets_* / bytes_*
+            if (eim && b >= 16 && b < 24) continue;              // last_used: the time rule
+            if (qos && b < 16) continue;                         // tokens; last_update: the time rule
+        }
+        set(pos);
+    }
+    if (!exact) {
+        if (ses) t.tw = SES_LAST_SEEN / 8;
+        if (eim || qos) t.tw = (tb.voff + (eim ? 16 : 8)) / 8;
+    }
+    return t;
+}
+
+int delta_words(const Tbl &t, bool ses) { // shadow words of a slot: through the last compared byte
+    return ses ? SES_PAD_A / 8 : (int)((t.voff + t.value_size + 7) / 8);
+}
+
+int delta_shadow_locked(bng_ctx *c, int map, const Tbl &t, u32 sw) {
+    bng_ctx::DeltaShadow s{map, nullptr, (u64)t.mask + 1, sw};
+    const size_t bytes = s.nslots * sw * 8;
+    if (cudaMalloc((void **)&s.words, bytes) != cudaSuccess) {
+        cudaGetLastError();
+        return fail(c, -ENOMEM, "delta_enable: %zu bytes of device memory for the shadow of %s", bytes, map < 0 ? kSnapAcct : c->maps[map].name);
+    }
+    c->dshadow.push_back(s);
+    CU(c, cudaMemsetAsync(s.words, 0xFF, bytes, c->L.stream)); // every slot empty: nothing sent yet
+    if (s.nslots > c->dlist_slots) {
+        if (c->dlist) cudaFree(c->dlist);
+        c->dlist = nullptr;
+        c->dlist_slots = 0;
+        if (cudaMalloc((void **)&c->dlist, s.nslots * 8) != cudaSuccess) {
+            cudaGetLastError();
+            return fail(c, -ENOMEM, "delta_enable: out of device memory");
+        }
+        c->dlist_slots = s.nslots;
+    }
+    return 0;
+}
+
+void delta_free_locked(bng_ctx *c) {
+    cudaStreamSynchronize(c->L.stream);
+    for (auto &s : c->dshadow) cudaFree(s.words);
+    c->dshadow.clear();
+}
+
+// a grow-only device buffer of at least `bytes`; keep: bytes at the start that survive the growth
+int delta_grow(bng_ctx *c, u8 **p, u64 *cap, u64 bytes, u64 keep = 0) {
+    if (bytes <= *cap) return 0;
+    const u64 nb = std::max<u64>(bytes + bytes / 2, 1 << 20);
+    u8 *q = nullptr;
+    if (cudaMalloc((void **)&q, nb) != cudaSuccess) {
+        cudaGetLastError();
+        return fail(c, -ENOMEM, "delta_export: %llu bytes of device memory", (unsigned long long)nb);
+    }
+    if (keep) CU(c, cudaMemcpyAsync(q, *p, keep, cudaMemcpyDeviceToDevice, c->L.stream));
+    CU(c, cudaStreamSynchronize(c->L.stream));
+    if (*p) cudaFree(*p);
+    *p = q;
+    *cap = nb;
+    return 0;
+}
+
+void put_section(std::vector<u8> &out, const char *name, u32 kind, u32 ks, u32 vs, u32 n_del, u64 n_up) {
+    SnapMapHdr h{};
+    snprintf(h.name, sizeof(h.name), "%s", name);
+    h.kind = kind, h.key_size = ks, h.value_size = vs, h.pad = n_del, h.count = n_up;
+    out.insert(out.end(), (u8 *)&h, (u8 *)&h + sizeof(h));
+}
+} // namespace
+
+int bng_delta_enable(bng_ctx *c, int on) {
+    if (!c) return -EINVAL;
+    std::lock_guard<std::mutex> g(c->mu);
+    cudaSetDevice(c->device);
+    delta_free_locked(c);
+    if (!on) return 0;
+    for (size_t mi = 0; mi < c->maps.size(); mi++) {
+        const MapReg &m = c->maps[mi];
+        if (m.kind != KIND_HASH) continue;
+        if (int r = delta_shadow_locked(c, (int)mi, *m.tbl, delta_words(*m.tbl, m.tbl->vlayout == VL_SESSION))) {
+            delta_free_locked(c);
+            return r;
+        }
+    }
+    if (c->acct) {
+        if (int r = delta_shadow_locked(c, -1, c->dev.subdir, 1 + ACCT_WORDS)) {
+            delta_free_locked(c);
+            return r;
+        }
+    }
+    CU(c, cudaStreamSynchronize(c->L.stream));
+    u64 id = 0;
+    FILE *f = fopen("/dev/urandom", "rb");
+    if (f) {
+        if (fread(&id, 8, 1, f) != 1) id = 0;
+        fclose(f);
+    }
+    id ^= splitmix64((u64)(uintptr_t)c ^ ((u64)clock() << 32) ^ (u64)time(nullptr));
+    c->delta_stream = id ? id : 1;
+    c->delta_seq = 0;
+    c->delta_full = true;
+    c->delta_li.clear();
+    c->delta_li_sent = false;
+    return 0;
+}
+
+int bng_delta_export(bng_ctx *c, uint64_t refresh_ns, uint32_t flags, void *buf, uint64_t cap, uint64_t *len_out) {
+    if (!c || !len_out || (cap && !buf) || (flags & ~(BNG_DELTA_FULL | BNG_DELTA_EXACT))) return -EINVAL;
+    *len_out = 0;
+    std::lock_guard<std::mutex> g(c->mu);
+    cudaSetDevice(c->device);
+    if (c->dshadow.empty()) return fail(c, -EINVAL, "delta_export: change tracking is not enabled");
+    int r = flow_pass_begin_locked(c);
+    if (r) return r;
+    if (c->acct && c->dshadow.back().map >= 0) { // accounting began after tracking did: its records start from "empty"
+        if ((r = delta_shadow_locked(c, -1, c->dev.subdir, 1 + ACCT_WORDS)) != 0) return r;
+    }
+    const bool full = (flags & BNG_DELTA_FULL) || c->delta_full, exact = flags & BNG_DELTA_EXACT;
+    std::vector<u8> out(sizeof(DeltaHdr));
+    u32 sections = 0;
+    struct Pending {
+        DeltaTbl t;
+        u64 at;
+        u32 n_del, n_up;
+    };
+    std::vector<Pending> commits;
+    u64 sent_used = 0;
+    u32 *cnt = c->L.s.counters + 8; // scratch words 8.. are free between program runs
+    for (const auto &s : c->dshadow) {
+        const DeltaTbl t = delta_view(c, s, refresh_ns, exact);
+        u32 *del = c->dlist, *up = c->dlist + s.nslots;
+        CU(c, cudaMemsetAsync(cnt, 0, 8, c->L.stream));
+        CU(c, run_delta_diff(c->L, t, del, up, cnt, full));
+        u32 n[2] = {0, 0};
+        CU(c, cudaMemcpyAsync(n, cnt, 8, cudaMemcpyDeviceToHost, c->L.stream));
+        CU(c, cudaStreamSynchronize(c->L.stream));
+        const u64 kb_del = (u64)n[0] * t.key_size, kb_up = (u64)n[1] * t.key_size, vb = (u64)n[1] * t.value_size;
+        if ((r = delta_grow(c, &c->demit, &c->demit_cap, kb_del + kb_up + vb)) != 0) return r;
+        if ((r = delta_grow(c, (u8 **)&c->dsent, &c->dsent_cap, (sent_used + n[0] + n[1]) * 4, sent_used * 4)) != 0) return r;
+        CU(c, run_delta_emit(c->L, t, del, n[0], up, n[1], c->demit, c->demit + kb_del, c->demit + kb_del + kb_up));
+        if (n[0]) CU(c, cudaMemcpyAsync(c->dsent + sent_used, del, (u64)n[0] * 4, cudaMemcpyDeviceToDevice, c->L.stream));
+        if (n[1]) CU(c, cudaMemcpyAsync(c->dsent + sent_used + n[0], up, (u64)n[1] * 4, cudaMemcpyDeviceToDevice, c->L.stream));
+        commits.push_back({t, sent_used, n[0], n[1]});
+        sent_used += n[0] + n[1];
+        if (s.map < 0)
+            put_section(out, kSnapAcct, kSnapAcctKind, 4, sizeof(bng_acct), n[0], n[1]);
+        else
+            put_section(out, c->maps[s.map].name, KIND_HASH, t.key_size, t.value_size, n[0], n[1]);
+        sections++;
+        const size_t at = out.size();
+        out.resize(at + kb_del + kb_up + vb);
+        if (out.size() > at) CU(c, cudaMemcpyAsync(out.data() + at, c->demit, kb_del + kb_up + vb, cudaMemcpyDeviceToHost, c->L.stream));
+        CU(c, cudaStreamSynchronize(c->L.stream));
+    }
+    for (auto &m : c->maps) { // the small maps, whole
+        if (m.kind == KIND_HASH || m.kind == KIND_EVENT) continue;
+        const u64 cnt_e = m.kind == KIND_LPM ? m.lpm_host.size() / 3 : (m.kind == KIND_STATS ? 1 : m.max_entries);
+        std::vector<u8> keys((size_t)std::max<u64>(cnt_e, 1) * m.key_size), vals((size_t)std::max<u64>(cnt_e, 1) * m.value_size);
+        const int64_t got = cnt_e ? map_dump_locked(c, &m, keys.data(), vals.data(), cnt_e) : 0;
+        if (got < 0) return (int)got;
+        put_section(out, m.name, (u32)m.kind, m.key_size, m.value_size, 0, (u64)got);
+        out.insert(out.end(), keys.begin(), keys.begin() + (size_t)got * m.key_size);
+        out.insert(out.end(), vals.begin(), vals.begin() + (size_t)got * m.value_size);
+        sections++;
+    }
+    std::vector<std::pair<u32, u32>> li(c->li_targets.begin(), c->li_targets.end());
+    std::sort(li.begin(), li.end());
+    const bool li_send = c->li_ctl && (full || !c->delta_li_sent || li != c->delta_li);
+    if (li_send) {
+        put_section(out, kSnapLi, kSnapLiKind, 4, 4, 0, li.size());
+        for (auto &e : li) out.insert(out.end(), (u8 *)&e.first, (u8 *)&e.first + 4);
+        for (auto &e : li) out.insert(out.end(), (u8 *)&e.second, (u8 *)&e.second + 4);
+        sections++;
+    }
+    DeltaHdr h{};
+    memcpy(h.magic, kDeltaMagic, 8);
+    h.stream = c->delta_stream, h.seq_from = c->delta_seq, h.seq_to = c->delta_seq + 1;
+    h.flags = (full ? BNG_DELTA_FULL : 0) | (exact ? BNG_DELTA_EXACT : 0), h.sections = sections;
+    memcpy(out.data(), &h, sizeof(h));
+    *len_out = out.size();
+    prof_collect(c->L);
+    if (cap < out.size()) return -ENOSPC; // the shadows are as they were: the next call covers the same changes
+    memcpy(buf, out.data(), out.size());
+    // the baseline moves to what this delta carries
+    if (full)
+        for (const auto &s : c->dshadow) CU(c, cudaMemsetAsync(s.words, 0xFF, s.nslots * s.sw * 8, c->L.stream));
+    for (const auto &p : commits)
+        CU(c, run_delta_commit(c->L, p.t, c->dsent + p.at, p.n_del, c->dsent + p.at + p.n_del, p.n_up));
+    CU(c, cudaStreamSynchronize(c->L.stream));
+    c->delta_seq++;
+    c->delta_full = false;
+    if (li_send) c->delta_li = li, c->delta_li_sent = true;
+    return 0;
+}
+
+int bng_delta_apply(bng_ctx *c, const void *buf, uint64_t len) {
+    if (!c || !buf || len < sizeof(DeltaHdr)) return -EINVAL;
+    DeltaHdr h;
+    memcpy(&h, buf, sizeof(h));
+    if (memcmp(h.magic, kDeltaMagic, 8)) return fail(c, -EINVAL, "delta_apply: not a delta");
+    const bool full = h.flags & BNG_DELTA_FULL;
+    // the whole blob is checked before anything changes
+    struct Sec {
+        SnapMapHdr h;
+        const u8 *p;
+        int id;
+    };
+    std::vector<Sec> secs;
+    const u8 *p = (const u8 *)buf + sizeof(h), *end = (const u8 *)buf + len;
+    for (u32 k = 0; k < h.sections; k++) {
+        Sec s{};
+        if ((u64)(end - p) < sizeof(SnapMapHdr)) return fail(c, -EINVAL, "delta_apply: truncated");
+        memcpy(&s.h, p, sizeof(s.h));
+        p += sizeof(s.h);
+        s.h.name[sizeof(s.h.name) - 1] = 0;
+        if (s.h.count > (1ull << 40) || s.h.key_size > 64 || s.h.value_size > 4096)
+            return fail(c, -EINVAL, "delta_apply: %s has a bad header", s.h.name);
+        const u64 need = (u64)s.h.pad * s.h.key_size + s.h.count * (s.h.key_size + s.h.value_size);
+        if ((u64)(end - p) < need) return fail(c, -EINVAL, "delta_apply: %s is truncated", s.h.name);
+        s.p = p;
+        p += need;
+        if (!strcmp(s.h.name, kSnapAcct)) {
+            if (s.h.key_size != 4 || s.h.value_size != sizeof(bng_acct)) return fail(c, -EINVAL, "delta_apply: %s has another layout", s.h.name);
+            s.id = -2;
+        } else if (!strcmp(s.h.name, kSnapLi)) {
+            if (s.h.key_size != 4 || s.h.value_size != 4 || s.h.count > BNG_LI_MAX_TARGETS)
+                return fail(c, -EINVAL, "delta_apply: %s has another layout", s.h.name);
+            s.id = -3;
+        } else {
+            s.id = bng_map_id(c, s.h.name);
+            if (s.id < 0) continue; // a map this library does not have
+            const MapReg *m = get_map(c, s.id);
+            if (m->key_size != s.h.key_size || m->value_size != s.h.value_size || (u32)m->kind != s.h.kind || (m->kind != KIND_HASH && s.h.pad))
+                return fail(c, -EINVAL, "delta_apply: %s has another layout", s.h.name);
+        }
+        secs.push_back(s);
+    }
+    {
+        std::lock_guard<std::mutex> g(c->mu);
+        cudaSetDevice(c->device);
+        if (!full && (h.stream != c->dapply_stream || h.seq_from != c->dapply_seq || !c->dapply_stream))
+            return fail(c, -ESTALE, "delta_apply: stream %llx seq %llu, expected stream %llx seq %llu", (unsigned long long)h.stream,
+                        (unsigned long long)h.seq_from, (unsigned long long)c->dapply_stream, (unsigned long long)c->dapply_seq);
+        c->dapply_stream = 0; // until this apply has completed, only a FULL delta is accepted
+        if (full) {
+            if (c->acct) CU(c, cudaMemsetAsync(c->acct, 0, ((size_t)c->dev.subdir.mask + 1) * sizeof(bng_acct), c->L.stream));
+            CU(c, cudaStreamSynchronize(c->L.stream));
+            if (!c->li_targets.empty()) c->li_targets.clear(), c->li_dirty = true;
+        }
+    }
+    for (const Sec &s : secs) {
+        if (s.id < 0) continue;
+        MapReg *m = get_map(c, s.id);
+        const u8 *dk = s.p, *uk = dk + (u64)s.h.pad * s.h.key_size, *uv = uk + s.h.count * s.h.key_size;
+        if (m->kind == KIND_HASH) {
+            if (full) {
+                if (int r = bng_map_clear(c, s.id)) return r;
+            }
+            if (s.h.pad) {
+                std::lock_guard<std::mutex> g(c->mu);
+                cudaSetDevice(c->device);
+                if (int r = flush_staged_locked(c, s.id)) return r;
+                int first = 0; // a key the standby no longer has is no error
+                if (int r = hash_cmd(c, m, TOP_DELETE, dk, nullptr, s.h.pad, 0, &first)) return r;
+                if (feeds_small_tabs(m)) c->small_dirty = true;
+            }
+        } else if (m->kind == KIND_LPM) {
+            std::lock_guard<std::mutex> g(c->mu);
+            cudaSetDevice(c->device);
+            m->lpm_host.clear();
+            if (int r = lpm_upload(c, m)) return r;
+        }
+        if (s.h.count) {
+            if (int r = bng_map_update_batch(c, s.id, uk, uv, s.h.count, BNG_ANY)) return fail(c, r, "delta_apply: loading %s failed", s.h.name);
+        }
+    }
+    std::lock_guard<std::mutex> g(c->mu);
+    cudaSetDevice(c->device);
+    for (const Sec &s : secs) {
+        const u8 *uk = s.p + (u64)s.h.pad * s.h.key_size, *uv = uk + s.h.count * s.h.key_size;
+        if (s.id == -2 && s.h.count) { // after the maps: the records go to the addresses' directory slots
+            if (int r = acct_alloc_locked(c)) return r;
+            const u64 chunk_max = 1u << 16;
+            for (u64 done = 0; done < s.h.count; done += chunk_max) {
+                const u64 k = std::min(chunk_max, s.h.count - done);
+                const size_t roff = (k * 4 + 255) & ~(size_t)255;
+                if (int r = ensure_io(c, roff + k * sizeof(bng_acct))) return r;
+                memcpy(c->io_host, uk + done * 4, k * 4);
+                memcpy(c->io_host + roff, uv + done * sizeof(bng_acct), k * sizeof(bng_acct));
+                CU(c, cudaMemcpyAsync(c->io_dev, c->io_host, roff + k * sizeof(bng_acct), cudaMemcpyHostToDevice, c->L.stream));
+                CU(c, run_acct_load(c->L, c->dev.subdir, c->acct, (const u32 *)c->io_dev, (const u64 *)(c->io_dev + roff), k));
+                CU(c, cudaStreamSynchronize(c->L.stream));
+            }
+        } else if (s.id == -3) {
+            if (int r = li_alloc_locked(c)) return r;
+            c->li_targets.clear();
+            for (u64 k = 0; k < s.h.count; k++) {
+                u32 a, id;
+                memcpy(&a, uk + k * 4, 4);
+                memcpy(&id, uv + k * 4, 4);
+                c->li_targets[a] = id;
+            }
+            c->li_dirty = true;
+        }
+    }
+    c->dapply_stream = h.stream;
+    c->dapply_seq = h.seq_to;
+    return 0;
+}
+
+int bng_delta_info(bng_ctx *c, uint64_t *stream_id, uint64_t *seq) {
+    if (!c) return -EINVAL;
+    std::lock_guard<std::mutex> g(c->mu);
+    const bool exporter = !c->dshadow.empty();
+    if (stream_id) *stream_id = exporter ? c->delta_stream : c->dapply_stream;
+    if (seq) *seq = exporter ? c->delta_seq : c->dapply_seq;
     return 0;
 }
 

@@ -130,3 +130,28 @@ struct LiSrc {
 // (a SHOT frame without one was dropped by antispoof), else nullptr.
 cudaError_t run_li_capture(Launcher &L, const LiRing &r, const DevBatch &b, const LiSrc &src, bool up);
 cudaError_t run_li_verdict(Launcher &L, const LiRing &r, const DevBatch &b, const u32 *attr);
+
+// incremental replication (delta.cu).  A table as the diff sees it: nslots slots whose first kw words are the key (word
+// 0 doubles as the slot state) and whose words [kw, sw) hold the compared bytes; the shadow keeps those sw words per
+// slot as last sent.  vals != nullptr: words [kw, sw) and the value come from vals + slot * vstride instead of the slot
+// (the accounting records beside the subscriber directory).
+#define DELTA_MAXW 16
+#define DELTA_NO_TIME 0xFFFFFFFFu
+struct DeltaTbl {
+    const u8 *slots;
+    const u8 *vals;
+    u64 *shadow;
+    u64 nslots;
+    u32 slot_bytes, vstride;
+    u32 kw, sw;
+    u32 tw;                     // word of the time field (DELTA_NO_TIME: none); sent again once it moves > refresh
+    u32 key_size, value_size, voff, vlayout;
+    u64 refresh;
+    u64 mask[DELTA_MAXW];       // per word: the bits compared exactly
+};
+// del / up: slot lists of the two classes (room for nslots each); cnt[0], cnt[1]: their lengths (zeroed by the caller).
+// full: the shadow is taken as empty (every live entry is an upsert, nothing is deleted)
+cudaError_t run_delta_diff(Launcher &L, const DeltaTbl &t, u32 *del, u32 *up, u32 *cnt, bool full);
+cudaError_t run_delta_emit(Launcher &L, const DeltaTbl &t, const u32 *del, u32 n_del, const u32 *up, u32 n_up, u8 *del_keys,
+                           u8 *up_keys, u8 *up_vals);
+cudaError_t run_delta_commit(Launcher &L, const DeltaTbl &t, const u32 *del, u32 n_del, const u32 *up, u32 n_up);

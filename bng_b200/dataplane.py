@@ -19,6 +19,7 @@ LIB_PATH = os.environ.get("BNG_B200_LIB") or os.path.join(HERE, "libbng_b200.so"
 
 MEM_DEVICE, MEM_HOST = 0, 1
 ANY, NOEXIST, EXIST = 0, 1, 2
+DELTA_FULL, DELTA_EXACT = 1, 2
 
 PROGRAMS = (
     "antispoof_ingress", "qos_egress_prog", "qos_ingress_prog", "nat44_egress", "nat44_ingress",
@@ -111,6 +112,10 @@ def load_library() -> C.CDLL:
         "bng_li_target_del": ([vp, u32], i32),
         "bng_li_drain": ([vp, vp, u64, C.POINTER(u64)], i32),
         "bng_li_lost": ([vp], u64),
+        "bng_delta_enable": ([vp, i32], i32),
+        "bng_delta_export": ([vp, u64, u32, vp, u64, C.POINTER(u64)], i32),
+        "bng_delta_apply": ([vp, vp, u64], i32),
+        "bng_delta_info": ([vp, C.POINTER(u64), C.POINTER(u64)], i32),
     }
     for name, (args, res) in protos.items():
         fn = getattr(lib, name)
@@ -130,6 +135,7 @@ EXPORTED_SYMBOLS = (
     "bng_comm_unique_id", "bng_comm_init", "bng_sync_reduce", "bng_sweep", "bng_lru_evictions", "bng_snapshot", "bng_restore", "bng_table_rebuilds",
     "bng_acct_enable", "bng_acct_read", "bng_acct_dump", "bng_nat_flush",
     "bng_li_configure", "bng_li_record_size", "bng_li_target_set", "bng_li_target_del", "bng_li_drain", "bng_li_lost",
+    "bng_delta_enable", "bng_delta_export", "bng_delta_apply", "bng_delta_info",
 )
 
 
@@ -407,6 +413,36 @@ class Dataplane:
     @property
     def li_lost(self) -> int:
         return self.lib.bng_li_lost(self.h)
+
+    # ---- incremental replication to a standby ----
+    def delta_enable(self, on: bool = True):
+        """Start (or stop) tracking changes for delta_export; starting sets the baseline to empty and a new stream id."""
+        self._chk(self.lib.bng_delta_enable(self.h, 1 if on else 0), "delta_enable")
+
+    def delta_export(self, refresh_ns: int = 0, full: bool = False, exact: bool = False) -> bytes:
+        """The changes since the previous export as one blob for delta_apply on the standby."""
+        flags = (DELTA_FULL if full else 0) | (DELTA_EXACT if exact else 0)
+        cap = 1 << 20  # most deltas are small; a larger one is sized by -ENOSPC, which leaves the baseline as it was
+        while True:
+            buf = np.empty(cap, np.uint8)  # not zero-filled: a FULL delta can be hundreds of MB
+            n = C.c_uint64(0)
+            r = self.lib.bng_delta_export(self.h, refresh_ns, flags, buf.ctypes.data, cap, C.byref(n))
+            if r != -errno.ENOSPC:
+                break
+            cap = n.value
+        self._chk(r, "delta_export")
+        return buf[: n.value].tobytes()
+
+    def delta_apply(self, blob: bytes) -> int:
+        """Apply a delta of the active context; returns 0 or -ESTALE (a gap or another stream: ask for a FULL one)."""
+        r = self.lib.bng_delta_apply(self.h, blob, len(blob))
+        return r if r == -errno.ESTALE else self._chk(r, "delta_apply")
+
+    def delta_info(self) -> tuple:
+        """(stream id, sequence): of the last export with tracking enabled, else of the last delta applied."""
+        s, q = C.c_uint64(), C.c_uint64()
+        self._chk(self.lib.bng_delta_info(self.h, C.byref(s), C.byref(q)), "delta_info")
+        return s.value, q.value
 
     def sweep(self, now_ns: int) -> int:
         """Session expiry sweep at now_ns; returns the number of sessions removed."""

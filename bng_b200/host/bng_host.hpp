@@ -21,6 +21,9 @@
 // real frames.
 #pragma once
 
+#include <errno.h>
+
+#include <algorithm>
 #include <chrono>
 #include <cstddef>
 #include <cstdint>
@@ -1236,4 +1239,131 @@ class Manager {
 };
 
 } // namespace nat
+
+// ===========================================================================
+// HA replication of the dataplane tables (reference pkg/ha: HASyncer sends a full sync every FullSyncInterval and
+// small sequenced messages in between).  The active node's DataplaneSync exports a delta (bng_delta_export) every
+// heartbeat and hands the bytes to the transport; the standby's DataplaneSync applies what arrives.  A delta that does
+// not follow the last one applied (lost, reordered, another stream) is refused with -ESTALE: the standby then asks the
+// peer for a FULL delta through request_full, and the active's next Export is FULL.
+namespace ha {
+
+struct DeltaHeader { // the first 40 bytes of a bng_delta_export blob
+    char magic[8];   // "BNGDELT1"
+    uint64_t stream_id, seq_from, seq_to;
+    uint32_t flags, sections;
+};
+static_assert(sizeof(DeltaHeader) == 40, "the delta header of include/bng_b200.h");
+
+struct DeltaSection { // one section: n_del keys, n_up keys, n_up values
+    std::string name;
+    uint32_t kind, key_size, value_size, n_del;
+    uint64_t n_up;
+    const uint8_t *del_keys, *up_keys, *up_values;
+};
+
+// Walks a blob: fn(const DeltaSection &) per section.  False when the blob is not a whole delta.
+template <class F>
+inline bool ParseDelta(const void *blob, size_t len, DeltaHeader *h, F &&fn) {
+    if (len < sizeof(DeltaHeader)) return false;
+    memcpy(h, blob, sizeof(*h));
+    if (memcmp(h->magic, "BNGDELT1", 8)) return false;
+    const uint8_t *p = (const uint8_t *)blob + sizeof(*h), *end = (const uint8_t *)blob + len;
+    for (uint32_t k = 0; k < h->sections; k++) {
+        if ((size_t)(end - p) < 64) return false;
+        char name[41] = {};
+        memcpy(name, p, 40);
+        DeltaSection s{name, 0, 0, 0, 0, 0, nullptr, nullptr, nullptr};
+        memcpy(&s.kind, p + 40, 4), memcpy(&s.key_size, p + 44, 4), memcpy(&s.value_size, p + 48, 4), memcpy(&s.n_del, p + 52, 4);
+        memcpy(&s.n_up, p + 56, 8);
+        p += 64;
+        if (s.n_up > (1ull << 40) || s.key_size > 64 || s.value_size > 4096) return false;
+        const uint64_t need = (uint64_t)s.n_del * s.key_size + s.n_up * (s.key_size + s.value_size);
+        if ((uint64_t)(end - p) < need) return false;
+        s.del_keys = p, s.up_keys = p + (uint64_t)s.n_del * s.key_size, s.up_values = s.up_keys + s.n_up * s.key_size;
+        fn(s);
+        p += need;
+    }
+    return p == end;
+}
+
+// The two library calls DataplaneSync makes (a test substitutes its own).
+struct DeltaOps {
+    std::function<int(uint64_t refresh_ns, uint32_t flags, void *buf, uint64_t cap, uint64_t *len_out)> Export;
+    std::function<int(const void *buf, uint64_t len)> Apply;
+    static DeltaOps Of(std::shared_ptr<Backend> b) {
+        DeltaOps o;
+        o.Export = [b](uint64_t r, uint32_t f, void *buf, uint64_t cap, uint64_t *len) { return bng_delta_export(b->ctx, r, f, buf, cap, len); };
+        o.Apply = [b](const void *buf, uint64_t len) { return bng_delta_apply(b->ctx, buf, len); };
+        return o;
+    }
+};
+
+class DataplaneSync {
+  public:
+    // request_full: how the standby asks its peer for a FULL delta (a message of the HA protocol)
+    explicit DataplaneSync(DeltaOps ops, std::function<void()> request_full = nullptr)
+        : ops_(std::move(ops)), request_full_(std::move(request_full)) {}
+
+    // Active node: the next delta.  FULL when `full` is set (FullSyncInterval elapsed), or when the peer asked for one
+    // since the last export that succeeded.  A buffer too small is grown to the size the library reports and the
+    // export repeated; the baseline only moves once a delta has been written.
+    Result<std::vector<uint8_t>> Export(uint64_t refresh_ns, bool full = false, bool exact = false) {
+        Result<std::vector<uint8_t>> r;
+        const bool want_full = full || full_pending_;
+        const uint32_t flags = (want_full ? BNG_DELTA_FULL : 0u) | (exact ? BNG_DELTA_EXACT : 0u);
+        std::vector<uint8_t> buf(cap_);
+        for (;;) {
+            uint64_t len = 0;
+            int rc = ops_.Export(refresh_ns, flags, buf.data(), buf.size(), &len);
+            if (rc == -ENOSPC && len > buf.size()) {
+                buf.resize(len);
+                continue;
+            }
+            if (rc) {
+                r.err = MapErr("bng_delta_export", rc);
+                return r;
+            }
+            buf.resize(len);
+            break;
+        }
+        cap_ = std::max<size_t>(cap_, buf.size());
+        if (want_full) full_pending_ = false;
+        r.value = std::move(buf);
+        return r;
+    }
+    // the peer's standby asked for a FULL delta
+    void RequestFull() { full_pending_ = true; }
+    bool FullPending() const { return full_pending_; }
+
+    // Standby: applies a delta.  -ESTALE (a gap, or another stream) asks the peer for a FULL delta once per gap: until a
+    // FULL delta has been applied every incremental one is refused, and asking again would only repeat the request.
+    Error Apply(const void *blob, size_t len) {
+        int rc = ops_.Apply(blob, len);
+        DeltaHeader h{};
+        if (rc == 0) {
+            if (ParseDelta(blob, len, &h, [](const DeltaSection &) {})) applied_ = h.seq_to;
+            awaiting_full_ = false;
+            return Nil();
+        }
+        if (rc == -ESTALE && !awaiting_full_) {
+            awaiting_full_ = true;
+            requests_++;
+            if (request_full_) request_full_();
+        }
+        return MapErr("bng_delta_apply", rc);
+    }
+    uint64_t Applied() const { return applied_; }     // seq_to of the last delta applied
+    uint64_t FullRequests() const { return requests_; } // FULL deltas asked for so far
+
+  private:
+    DeltaOps ops_;
+    std::function<void()> request_full_;
+    size_t cap_ = 1 << 16;
+    bool full_pending_ = false, awaiting_full_ = false;
+    uint64_t applied_ = 0, requests_ = 0;
+};
+
+} // namespace ha
+
 } // namespace bng

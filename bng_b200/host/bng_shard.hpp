@@ -17,6 +17,7 @@
 #include <errno.h>
 #include <string.h>
 
+#include <algorithm>
 #include <memory>
 #include <mutex>
 #include <optional>
@@ -289,6 +290,28 @@ class Router {
             }
         }
         return total;
+    }
+    // Incremental replication: shard k of the active node replicates to shard k of the standby node (the same
+    // subscribers steer to the same shard index on both), so each pair is independent and no collective is needed.
+    // DeltaExport writes shard k's delta into *out; DeltaApply applies, on shard k of the standby, the delta its peer
+    // exported.  Both return 0 or a negative errno (-ESTALE: the pair needs a FULL delta).
+    int DeltaExport(size_t k, uint64_t refresh_ns, uint32_t flags, std::vector<uint8_t> *out) {
+        if (k >= shards_.size() || !out) return -EINVAL;
+        out->resize(std::max<size_t>(out->capacity(), 1 << 16));
+        for (;;) {
+            uint64_t len = 0;
+            int r = bng_delta_export(shards_[k]->ctx, refresh_ns, flags, out->data(), out->size(), &len);
+            if (r == -ENOSPC && len > out->size()) {
+                out->resize(len);
+                continue;
+            }
+            out->resize(r ? 0 : len);
+            return r;
+        }
+    }
+    int DeltaApply(size_t k, const void *blob, uint64_t len) {
+        if (k >= shards_.size()) return -EINVAL;
+        return bng_delta_apply(shards_[k]->ctx, blob, len);
     }
     radius::AcctReader Reader() {
         return [this](uint32_t addr, bng_acct *out) { return AcctRead(addr, out); };

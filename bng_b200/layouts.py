@@ -172,3 +172,34 @@ def as_bytes(arr) -> np.ndarray:
     if a.ndim == 0:
         a = a.reshape(1)
     return a.view(np.uint8).reshape(a.shape[0], -1) if a.dtype.itemsize > 1 or a.ndim == 1 else a
+
+
+# bng_delta_export blobs (include/bng_b200.h): a 40-byte header, then sections in bng_snapshot's 64-byte framing
+delta_header = np.dtype([("magic", "S8"), ("stream_id", "<u8"), ("seq_from", "<u8"), ("seq_to", "<u8"),
+                         ("flags", "<u4"), ("sections", "<u4")])
+delta_section = np.dtype([("name", "S40"), ("kind", "<u4"), ("key_size", "<u4"), ("value_size", "<u4"),
+                          ("n_del", "<u4"), ("n_up", "<u8")])
+assert delta_header.itemsize == 40 and delta_section.itemsize == 64
+
+
+def parse_delta(blob: bytes) -> tuple:
+    """(header record, {section name: (kind, deleted keys u8[n_del, ks], upserted keys u8[n_up, ks], values u8[n_up, vs])})."""
+    b = np.frombuffer(blob, np.uint8)
+    hdr = b[:delta_header.itemsize].view(delta_header)[0]
+    if hdr["magic"] != b"BNGDELT1":
+        raise ValueError("not a delta blob")
+    out, p = {}, delta_header.itemsize
+    for _ in range(int(hdr["sections"])):
+        s = b[p:p + delta_section.itemsize].view(delta_section)[0]
+        p += delta_section.itemsize
+        ks, vs, nd, nu = int(s["key_size"]), int(s["value_size"]), int(s["n_del"]), int(s["n_up"])
+        dk = b[p:p + nd * ks].reshape(nd, ks)
+        p += nd * ks
+        uk = b[p:p + nu * ks].reshape(nu, ks)
+        p += nu * ks
+        uv = b[p:p + nu * vs].reshape(nu, vs)
+        p += nu * vs
+        out[s["name"].decode()] = (int(s["kind"]), dk, uk, uv)
+    if p != len(b):
+        raise ValueError(f"delta blob: {len(b) - p} trailing bytes")
+    return hdr, out

@@ -297,6 +297,47 @@ int bng_li_target_del(bng_ctx *ctx, uint32_t addr);                      /* -ENO
 int bng_li_drain(bng_ctx *ctx, void *buf, uint64_t cap_records, uint64_t *n_out);
 uint64_t bng_li_lost(bng_ctx *ctx); /* records dropped because the ring was full, or discarded by a reconfiguration */
 
+/* ---- incremental replication to an HA standby ----
+ * The active context exports deltas: what changed in its maps since its previous export; a standby context applies
+ * them in order and its maps follow the active's.  bng_snapshot / bng_restore remain the one-off hand-over.
+ * bng_delta_enable(on != 0) allocates change tracking (a shadow of every hash map's slots, and of the accounting
+ * records once they exist) and sets the baseline to "empty": a new random stream id, sequence 0, and the next export
+ * is FULL.  on == 0 frees it.  The shadows take, per slot of each table, its key and its compared bytes as last sent,
+ * rounded up to 8-byte words: 1.85 GiB at the default capacities (1e6 subscribers, 4e6 sessions, 2e6 EIM), 2.0 GiB
+ * with accounting records.
+ * bng_delta_export: a batch of its own, as bng_sweep is (staged upserts are applied first; it sees everything queued
+ * on the context's stream).  The blob it writes:
+ *   header   char magic[8] = "BNGDELT1"; uint64 stream_id, seq_from, seq_to; uint32 flags, sections  (40 bytes)
+ *   sections in bng_snapshot's framing: char name[40]; uint32 kind, key_size, value_size, n_del; uint64 n_up;
+ *            then n_del deleted keys, n_up upserted keys, n_up values (ABI layout).
+ *   - Hash maps: the change since the previous export.  A key is deleted when the copy last sent had it and the map
+ *     no longer has it in that slot; an entry is upserted when its key is new to its slot, when any byte outside the
+ *     map's volatile fields differs from the copy last sent, or when its time field is more than refresh_ns past the
+ *     copy last sent.  Volatile fields: nat_sessions packets_* / bytes_* (time field last_seen), eim_table (time field
+ *     last_used), qos_ingress / qos_egress tokens (time field last_update).  nat_sessions' struct padding is never
+ *     compared.  BNG_DELTA_EXACT compares every byte: the standby's maps become byte-identical to the active's.
+ *   - Array, LPM and statistics maps: every entry, every time (n_del = 0); they replace the standby's copy.
+ *   - "subscriber_acct" (kind 5, once accounting exists): the (address, struct bng_acct) records whose bytes changed.
+ *   - "li_targets" (kind 6): the whole interception target set (address, target id), when it changed.
+ *   - Event rings are not state and are never sent.
+ * seq_to = seq_from + 1.  A FULL delta (BNG_DELTA_FULL, or the first export after enabling) carries every live entry
+ * and no deletion.  When cap is smaller than the delta, nothing is written, *len_out is set to the size needed,
+ * -ENOSPC is returned and the baseline stays where it was: the next call covers everything since that same baseline.
+ * -EINVAL when tracking is not enabled.
+ * bng_delta_apply: a FULL delta is always accepted; another one only when its stream id is the one applied last and
+ * its seq_from is the seq_to applied last, else -ESTALE and nothing changes.  Per map, the deletions are applied
+ * before the upserts; a FULL delta first clears every map it carries, the accounting records and the interception
+ * targets, as bng_restore does.  Capacities may differ between the two contexts, layouts may not (-EINVAL).  When an
+ * apply fails part way, the standby accepts only a FULL delta next.
+ * bng_delta_info: with tracking enabled, the stream id and the sequence of the last export; otherwise those of the
+ * last delta applied (0, 0: none). */
+#define BNG_DELTA_FULL 1u  /* every live entry, and the applier first clears what the blob covers */
+#define BNG_DELTA_EXACT 2u /* compare every byte (no volatile fields, refresh_ns ignored) */
+int bng_delta_enable(bng_ctx *ctx, int on);
+int bng_delta_export(bng_ctx *ctx, uint64_t refresh_ns, uint32_t flags, void *buf, uint64_t cap, uint64_t *len_out);
+int bng_delta_apply(bng_ctx *ctx, const void *buf, uint64_t len);
+int bng_delta_info(bng_ctx *ctx, uint64_t *stream_id, uint64_t *seq);
+
 /* ---- diagnostics ---- */
 uint64_t bng_launch_count(bng_ctx *ctx);  /* kernels launched by this context so far */
 uint64_t bng_lru_overflow(bng_ctx *ctx);  /* inserts that found no victim to evict in a full LRU map (should stay 0) */
