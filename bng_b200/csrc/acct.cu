@@ -6,6 +6,10 @@
 // verdict and skb->len, and adds the frame to the slot's pass or drop pair.  Frames of one warp that go to the same
 // pair are summed first (__match_any_sync): the leader of each group issues the two atomics, so a subscriber that
 // owns a whole batch costs one atomic pair per warp, not per frame.
+//
+// The same pass stamps the idle records (idle.cu) when idle detection is on for the program: the leader of a group of
+// passed frames raises the record's stamp of the direction to the group's latest clock with one atomicMax.  With one
+// clock for the whole batch the leader reads the stamp first and skips the atomic when it is already there.
 #include <errno.h>
 
 #include "kernels.h"
@@ -13,15 +17,10 @@
 
 #define ACCT_BLOCK 256
 
-__device__ __forceinline__ u32 dir_slot_of(const Tbl &dir, u32 addr) {
-    const u64 k = addr;
-    const u8 *s = tbl_find<1, false>(dir, &k);
-    return s ? (u32)((s - dir.slots) >> 4) : DIR_NONE;
-}
-
-template <int MODE>
+// COUNT: add the frames to the counter records; STAMP: stamp the idle records.  <MODE, true, false> is accounting alone.
+template <int MODE, bool COUNT, bool STAMP>
 __global__ void __launch_bounds__(ACCT_BLOCK) k_acct(const __grid_constant__ Tbl dir, const __grid_constant__ DevBatch b, const u32 *attr,
-                                                      u64 *acct) {
+                                                      u64 *acct, u64 *idle) {
     const u32 lane = threadIdx.x & 31;
     // warp-uniform trip count: __match_any_sync needs every lane
     for (u32 base = blockIdx.x * ACCT_BLOCK + (threadIdx.x & ~31u); base < b.n; base += gridDim.x * ACCT_BLOCK) {
@@ -29,7 +28,7 @@ __global__ void __launch_bounds__(ACCT_BLOCK) k_acct(const __grid_constant__ Tbl
         u32 slot = DIR_NONE, len = 0, drop = 0;
         if (i < b.n) {
             const u8 v = b.verdict[i];
-            if (v == TC_OK || v == TC_SHOT) {
+            if (v == TC_OK || (COUNT && v == TC_SHOT)) { // stamping alone: dropped frames are nobody's
                 len = b.len[i];
                 drop = v == TC_SHOT;
                 if (MODE == ACCT_ATTR) {
@@ -47,18 +46,34 @@ __global__ void __launch_bounds__(ACCT_BLOCK) k_acct(const __grid_constant__ Tbl
         const u32 grp = has ? (slot << 1 | drop) : (0xFFFFFFE0u | lane); // (directory slots < 2^31 - 16)
         const u32 peers = __match_any_sync(0xffffffffu, grp);
         u64 bytes = len;
+        u64 last = 0; // STAMP: the latest clock of the lane's group of passed frames
+        if (STAMP && has && !drop) last = frame_now(b, i);
         if (!__all_sync(0xffffffffu, peers == (1u << lane))) { // some lanes share a record: sum each group
-            bytes = 0;
+            if (COUNT) bytes = 0;
 #pragma unroll
             for (int j = 0; j < 32; j++) {
-                const u32 lj = __shfl_sync(0xffffffffu, len, j);
-                if ((peers >> j) & 1) bytes += lj;
+                if (COUNT) {
+                    const u32 lj = __shfl_sync(0xffffffffu, len, j);
+                    if ((peers >> j) & 1) bytes += lj;
+                }
+                if (STAMP && b.nowv) { // (one clock per batch: every lane already holds it)
+                    const u64 tj = __shfl_sync(0xffffffffu, last, j);
+                    if (((peers >> j) & 1) && tj > last) last = tj;
+                }
             }
         }
         if (has && lane == (u32)__ffs(peers) - 1) {
-            u64 *r = acct + (size_t)slot * ACCT_WORDS + (MODE == ACCT_DST ? 4 : 0) + 2 * drop;
-            atomicAdd((unsigned long long *)r, (unsigned long long)__popc(peers));
-            atomicAdd((unsigned long long *)(r + 1), (unsigned long long)bytes);
+            if (COUNT) {
+                u64 *r = acct + (size_t)slot * ACCT_WORDS + (MODE == ACCT_DST ? 4 : 0) + 2 * drop;
+                atomicAdd((unsigned long long *)r, (unsigned long long)__popc(peers));
+                atomicAdd((unsigned long long *)(r + 1), (unsigned long long)bytes);
+            }
+            if (STAMP && !drop) {
+                u64 *w = idle + (size_t)slot * IDLE_WORDS + (MODE == ACCT_DST ? IDLE_DOWN : IDLE_UP);
+                const u64 v = (last < ~0ull ? last : ~0ull - 1) + 1; // clock + 1: 0 is "none"
+                // a stale read can only be lower than the stamp (stamps only rise within a launch): no atomic is lost
+                if (b.nowv || *w < v) atomicMax((unsigned long long *)w, (unsigned long long)v);
+            }
         }
     }
 }
@@ -108,15 +123,25 @@ static inline int acct_grid(const Launcher &L, u64 n, int per_sm) {
     return (int)(want < 1 ? 1 : (want < cap ? want : cap));
 }
 
-cudaError_t run_acct(Launcher &L, const Tbl &dir, const DevBatch &b, int mode, u64 *acct) {
+template <int MODE>
+static void launch_acct(Launcher &L, int grid, const Tbl &dir, const DevBatch &b, const u32 *attr, u64 *acct, u64 *idle) {
+    if (acct && idle)
+        k_acct<MODE, true, true><<<grid, ACCT_BLOCK, 0, L.stream>>>(dir, b, attr, acct, idle);
+    else if (acct)
+        k_acct<MODE, true, false><<<grid, ACCT_BLOCK, 0, L.stream>>>(dir, b, attr, acct, nullptr);
+    else
+        k_acct<MODE, false, true><<<grid, ACCT_BLOCK, 0, L.stream>>>(dir, b, attr, nullptr, idle);
+}
+
+cudaError_t run_acct(Launcher &L, const Tbl &dir, const DevBatch &b, int mode, u64 *acct, u64 *idle) {
     const int grid = acct_grid(L, b.n, 8);
     prof_begin(L, "k_acct");
     if (mode == ACCT_ATTR)
-        k_acct<ACCT_ATTR><<<grid, ACCT_BLOCK, 0, L.stream>>>(dir, b, L.acct_attr, acct);
+        launch_acct<ACCT_ATTR>(L, grid, dir, b, L.acct_attr, acct, idle);
     else if (mode == ACCT_SRC)
-        k_acct<ACCT_SRC><<<grid, ACCT_BLOCK, 0, L.stream>>>(dir, b, nullptr, acct);
+        launch_acct<ACCT_SRC>(L, grid, dir, b, nullptr, acct, idle);
     else
-        k_acct<ACCT_DST><<<grid, ACCT_BLOCK, 0, L.stream>>>(dir, b, nullptr, acct);
+        launch_acct<ACCT_DST>(L, grid, dir, b, nullptr, acct, idle);
     prof_end(L);
     L.launches++;
     return cudaGetLastError();

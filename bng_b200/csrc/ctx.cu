@@ -109,6 +109,13 @@ struct bng_ctx {
     u32 acct_progs = 0;
     u8 *acct_dump_buf = nullptr; // grow-only scratch of bng_acct_dump: records, then addresses
     u64 acct_dump_cap = 0;
+    // per-subscriber idle detection (bng_idle_*, idle.cu): records index-aligned with the subscriber directory, allocated
+    // by the first bng_idle_enable / bng_idle_timeout_set (or a restore / delta that carries timeouts); idle_progs: bit
+    // p = program p stamps
+    u64 *idle = nullptr;
+    u32 idle_progs = 0;
+    u8 *idle_scan_buf = nullptr; // grow-only scratch of bng_idle_scan: records, then addresses, then the count
+    u64 idle_scan_cap = 0;
     u64 seq = 0; // the batch sequence in 64 bits (dev.batch_seq holds its low 32): bng_li_record.batch
     // lawful intercept (bng_li_*, li.cu): allocated by the first bng_li_configure / bng_li_target_set (li_ctl != null)
     u64 *li_ctl = nullptr;   // device: LiRing::ctl
@@ -209,7 +216,7 @@ int ensure_scratch(bng_ctx *c, u32 n) {
     u32 cap = std::max<u32>(n, 1024);
     void **ptrs[] = {(void **)&s.key_a, (void **)&s.key_b, (void **)&s.val_a, (void **)&s.val_b, (void **)&s.qslot, (void **)&s.attr};
     for (void **pp : ptrs) {
-        if (pp == (void **)&s.attr && !c->acct && !c->li_ctl) continue; // the attribution words exist once accounting or interception does
+        if (pp == (void **)&s.attr && !c->acct && !c->idle && !c->li_ctl) continue; // the attribution words exist once accounting, idle detection or interception does
         if (*pp) cudaFree(*pp);
         CU(c, cudaMalloc(pp, (size_t)cap * 4));
     }
@@ -307,7 +314,7 @@ int hash_cmd(bng_ctx *c, MapReg *m, int op, const void *keys, void *vals, u64 n,
         CU(c, cudaMemcpyAsync(c->io_dev, c->io_host, up, cudaMemcpyHostToDevice, c->L.stream));
         const int role = m->tbl == &c->dev.sub_nat ? 1 : (m->tbl == &c->dev.qos_in ? 2 : 0);
         CU(c, run_table_op(c->L, t, op, c->io_dev + koff, c->io_dev + voff, (int *)(c->io_dev + roff), k, flags, c->dev.subdir,
-                           role, c->acct));
+                           role, c->acct, c->idle));
         size_t dfrom = op == TOP_LOOKUP ? voff : roff;
         CU(c, cudaMemcpyAsync(c->io_host + dfrom, c->io_dev + dfrom, roff + rb - dfrom, cudaMemcpyDeviceToHost, c->L.stream));
         CU(c, cudaStreamSynchronize(c->L.stream));
@@ -527,7 +534,7 @@ int bng_close(bng_ctx *c) {
         }
         for (void *p : c->allocs) cudaFree(p);
         Scratch &s = c->L.s;
-        void *sp[] = {s.key_a, s.key_b, s.val_a, s.val_b, s.qslot, s.attr, s.cub_tmp, s.counters, c->acct_dump_buf, c->li_ring, c->li_match,
+        void *sp[] = {s.key_a, s.key_b, s.val_a, s.val_b, s.qslot, s.attr, s.cub_tmp, s.counters, c->acct_dump_buf, c->idle_scan_buf, c->li_ring, c->li_match,
                       c->io_dev, c->hb_pkts, c->hb_off, c->hb_len, c->hb_prio, c->hb_verdict, c->hb_now, c->dump_k, c->dump_v, c->dump_c,
                       c->dlist, c->dsent, c->demit};
         for (void *p : sp)
@@ -1046,10 +1053,12 @@ static const int k_li_dir[] = {-1, 1, 0, 0, 1, -1, -1, 0, 0};
 static int dispatch(bng_ctx *c, int prog, const DevBatch &b, const LiSrc &src = LiSrc{}) {
     cudaError_t e = cudaSuccess;
     const bool acct = c->acct && ((c->acct_progs >> prog) & 1);
+    const bool idle = c->idle && ((c->idle_progs >> prog) & 1);
     const int li = c->li_targets.empty() ? -1 : k_li_dir[prog]; // no target: not one kernel more
     const bool pipe = prog == P_PIPE_UP || prog == P_PIPE_TC;
-    // the upstream classify records attributions: for accounting, and in the pipelines to tell antispoof's drops
-    c->L.acct_attr = (acct || (li == 0 && pipe)) ? c->L.s.attr : nullptr;
+    // the upstream classify records attributions: for accounting and idle detection, and in the pipelines to tell
+    // antispoof's drops
+    c->L.acct_attr = (acct || idle || (li == 0 && pipe)) ? c->L.s.attr : nullptr;
     LiRing r{};
     if (li >= 0) {
         r.buf = c->li_ring, r.ctl = c->li_ctl, r.match = c->li_match;
@@ -1074,7 +1083,7 @@ static int dispatch(bng_ctx *c, int prog, const DevBatch &b, const LiSrc &src = 
     default: return -EINVAL;
     }
     // after the program, before anything copies the frames out: the downstream modes read the rewritten headers
-    if (e == cudaSuccess && acct) e = run_acct(c->L, c->dev.subdir, b, k_acct_mode[prog], c->acct);
+    if (e == cudaSuccess && (acct || idle)) e = run_acct(c->L, c->dev.subdir, b, k_acct_mode[prog], acct ? c->acct : nullptr, idle ? c->idle : nullptr);
     if (e == cudaSuccess && li == 0) e = run_li_verdict(c->L, r, b, pipe ? c->L.s.attr : nullptr);
     if (e == cudaSuccess && li == 1) e = run_li_capture(c->L, r, b, src, false);
     if (e != cudaSuccess) return fail(c, -EIO, "launch %s: %s", k_prog_names[prog], cudaGetErrorString(e));
@@ -1715,6 +1724,157 @@ int64_t bng_acct_dump(bng_ctx *c, uint32_t *addrs_out, bng_acct *out, uint64_t c
 }
 
 // ---------------------------------------------------------------------------
+// per-subscriber idle detection (idle.cu; stamped by k_acct)
+// ---------------------------------------------------------------------------
+static_assert(sizeof(bng_idle) == IDLE_WORDS * 8, "struct bng_idle has the size of the device record");
+
+// The records (one per directory slot, every field none) and the per-frame attribution words, on first use.
+static int idle_alloc_locked(bng_ctx *c) {
+    if (c->idle) return 0;
+    Scratch &s = c->L.s;
+    if (!s.attr) CU(c, cudaMalloc((void **)&s.attr, (size_t)s.cap * 4));
+    u64 *a = nullptr;
+    const size_t bytes = ((size_t)c->dev.subdir.mask + 1) * sizeof(bng_idle);
+    if (cudaMalloc((void **)&a, bytes) != cudaSuccess) {
+        cudaGetLastError();
+        return fail(c, -ENOMEM, "idle detection: %zu bytes of device memory", bytes);
+    }
+    c->allocs.push_back(a);
+    CU(c, cudaMemsetAsync(a, 0, bytes, c->L.stream));
+    c->idle = a;
+    return 0;
+}
+
+// stamps and since of every record := none (restore, delta apply)
+static int idle_restart_locked(bng_ctx *c) {
+    if (c->idle) CU(c, run_idle_restart(c->L, c->dev.subdir, c->idle));
+    return 0;
+}
+
+// timeouts of n addresses from host memory, chunked through the staging buffers; results may be nullptr
+static int idle_timeouts_locked(bng_ctx *c, const uint32_t *addrs, const uint32_t *timeouts, uint64_t n, int32_t *results) {
+    if (int r = idle_alloc_locked(c)) return r;
+    const u64 chunk_max = 1u << 18;
+    for (u64 done = 0; done < n; done += chunk_max) {
+        const u64 k = std::min(chunk_max, n - done);
+        const size_t toff = (k * 4 + 255) & ~(size_t)255, roff = toff * 2;
+        if (int r = ensure_io(c, roff + k * 4)) return r;
+        memcpy(c->io_host, addrs + done, k * 4);
+        memcpy(c->io_host + toff, timeouts + done, k * 4);
+        CU(c, cudaMemcpyAsync(c->io_dev, c->io_host, toff + k * 4, cudaMemcpyHostToDevice, c->L.stream));
+        CU(c, run_idle_timeout_set(c->L, c->dev.subdir, c->idle, (const u32 *)c->io_dev, (const u32 *)(c->io_dev + toff), k,
+                                   (int *)(c->io_dev + roff)));
+        if (results) CU(c, cudaMemcpyAsync(c->io_host + roff, c->io_dev + roff, k * 4, cudaMemcpyDeviceToHost, c->L.stream));
+        CU(c, cudaStreamSynchronize(c->L.stream));
+        if (results) memcpy(results + done, c->io_host + roff, k * 4);
+    }
+    return 0;
+}
+
+// records of n addresses from host memory, chunked through the staging buffers
+static int idle_read_locked(bng_ctx *c, const uint32_t *addrs, uint64_t n, bng_idle *out, int32_t *results) {
+    const u64 chunk_max = 1u << 16;
+    for (u64 done = 0; done < n; done += chunk_max) {
+        const u64 k = std::min(chunk_max, n - done);
+        const size_t ooff = (k * 4 + 255) & ~(size_t)255, roff = ooff + k * sizeof(bng_idle);
+        if (int r = ensure_io(c, roff + k * 4)) return r;
+        memcpy(c->io_host, addrs + done, k * 4);
+        CU(c, cudaMemcpyAsync(c->io_dev, c->io_host, k * 4, cudaMemcpyHostToDevice, c->L.stream));
+        CU(c, run_idle_read(c->L, c->dev.subdir, c->idle, (const u32 *)c->io_dev, k, (u64 *)(c->io_dev + ooff), (int *)(c->io_dev + roff)));
+        CU(c, cudaMemcpyAsync(c->io_host + ooff, c->io_dev + ooff, roff + k * 4 - ooff, cudaMemcpyDeviceToHost, c->L.stream));
+        CU(c, cudaStreamSynchronize(c->L.stream));
+        memcpy(out + done, c->io_host + ooff, k * sizeof(bng_idle));
+        memcpy(results + done, c->io_host + roff, k * 4);
+    }
+    return 0;
+}
+
+// (address, timeout) of every record, by address, for the snapshot: the directory's addresses (k_acct_dump lists them
+// whether or not accounting records exist), then their records
+static int idle_timeouts_dump_locked(bng_ctx *c, std::vector<u32> *addrs, std::vector<u32> *timeouts) {
+    u32 n32 = 0;
+    CU(c, cudaMemcpy(&n32, c->dev.subdir.count, 4, cudaMemcpyDeviceToHost));
+    std::vector<u32> a(std::max<u32>(n32, 1));
+    std::vector<bng_acct> unused(a.size());
+    const int64_t got = acct_dump_locked(c, a.data(), unused.data(), a.size()); // the directory's addresses
+    if (got < 0) return (int)got;
+    a.resize((size_t)got);
+    std::vector<bng_idle> recs(a.size());
+    std::vector<int32_t> res(a.size());
+    if (int r = idle_read_locked(c, a.data(), a.size(), recs.data(), res.data())) return r;
+    addrs->clear();
+    timeouts->clear();
+    std::vector<size_t> order(a.size());
+    for (size_t i = 0; i < order.size(); i++) order[i] = i;
+    std::sort(order.begin(), order.end(), [&](size_t x, size_t y) { return a[x] < a[y]; });
+    for (size_t i : order) addrs->push_back(a[i]), timeouts->push_back(recs[i].timeout_s);
+    return 0;
+}
+
+int bng_idle_enable(bng_ctx *c, int prog, int on) {
+    if (!c || prog < 0 || prog >= P_COUNT) return -EINVAL;
+    if (k_acct_mode[prog] < 0) return -EOPNOTSUPP;
+    std::lock_guard<std::mutex> g(c->mu);
+    cudaSetDevice(c->device);
+    if (on) {
+        if (int r = idle_alloc_locked(c)) return r;
+        c->idle_progs |= 1u << prog;
+    } else {
+        c->idle_progs &= ~(1u << prog);
+    }
+    return 0;
+}
+
+int bng_idle_timeout_set(bng_ctx *c, const uint32_t *addrs, const uint32_t *timeouts_s, uint64_t n, int32_t *results) {
+    if (!c || (n && (!addrs || !timeouts_s || !results))) return -EINVAL;
+    std::lock_guard<std::mutex> g(c->mu);
+    cudaSetDevice(c->device);
+    if (int fr = acct_flush_locked(c)) return fr;
+    return idle_timeouts_locked(c, addrs, timeouts_s, n, results);
+}
+
+int bng_idle_read(bng_ctx *c, const uint32_t *addrs, uint64_t n, bng_idle *out, int32_t *results) {
+    if (!c || (n && (!addrs || !out || !results))) return -EINVAL;
+    std::lock_guard<std::mutex> g(c->mu);
+    cudaSetDevice(c->device);
+    if (int fr = acct_flush_locked(c)) return fr;
+    return idle_read_locked(c, addrs, n, out, results);
+}
+
+int64_t bng_idle_scan(bng_ctx *c, uint64_t now_ns, uint32_t default_s, uint32_t flags, uint32_t *addrs_out, bng_idle *out, uint64_t cap) {
+    if (!c || !(flags & (BNG_IDLE_UP | BNG_IDLE_DOWN)) || (flags & ~(BNG_IDLE_UP | BNG_IDLE_DOWN)) || (cap && (!addrs_out || !out)))
+        return -EINVAL;
+    std::lock_guard<std::mutex> g(c->mu);
+    cudaSetDevice(c->device);
+    if (int fr = acct_flush_locked(c)) return fr;
+    if (!c->idle) return 0; // no record exists yet: nobody can be idle
+    const u64 ecap = std::min<u64>(cap, (u64)c->dev.subdir.mask + 1); // no more entries than slots
+    const size_t aoff = ecap * sizeof(bng_idle), coff = (aoff + ecap * 4 + 15) & ~(size_t)15, need = coff + 16;
+    if (need > c->idle_scan_cap) {
+        if (c->idle_scan_buf) cudaFree(c->idle_scan_buf);
+        c->idle_scan_buf = nullptr;
+        c->idle_scan_cap = 0;
+        if (cudaMalloc((void **)&c->idle_scan_buf, need) != cudaSuccess) {
+            cudaGetLastError();
+            return fail(c, -ENOMEM, "idle_scan: out of device memory");
+        }
+        c->idle_scan_cap = need;
+    }
+    u8 *buf = c->idle_scan_buf;
+    u32 *cnt = (u32 *)(buf + coff), n = 0;
+    CU(c, cudaMemsetAsync(cnt, 0, 4, c->L.stream));
+    CU(c, run_idle_scan(c->L, c->dev.subdir, c->idle, now_ns, default_s, flags, (u32 *)(buf + aoff), (u64 *)buf, cnt, ecap));
+    CU(c, cudaMemcpyAsync(&n, cnt, 4, cudaMemcpyDeviceToHost, c->L.stream));
+    CU(c, cudaStreamSynchronize(c->L.stream));
+    const u64 got = std::min<u64>(n, ecap);
+    if (got) {
+        CU(c, cudaMemcpy(out, buf, got * sizeof(bng_idle), cudaMemcpyDeviceToHost));
+        CU(c, cudaMemcpy(addrs_out, buf + aoff, got * 4, cudaMemcpyDeviceToHost));
+    }
+    return (int64_t)n;
+}
+
+// ---------------------------------------------------------------------------
 // lawful intercept (li.cu)
 // ---------------------------------------------------------------------------
 static_assert(sizeof(bng_li_record) == LI_HDR, "struct bng_li_record is the device record's header");
@@ -1892,6 +2052,20 @@ const u32 kSnapAcctKind = 5;
 // has used interception; the records are not state and stay out.
 const char kSnapLi[] = "li_targets";
 const u32 kSnapLiKind = 6;
+// Trailing section of the idle timeouts: (address, uint32 timeout_s) pairs, by address.  Written once idle records
+// exist; the clocks are not state (another node's clock, or this one's minutes ago, says nothing about activity now).
+const char kSnapIdle[] = "subscriber_idle";
+const u32 kSnapIdleKind = 7;
+
+// one (address, u32) section
+void put_pairs(std::vector<u8> &out, const char *name, u32 kind, const std::vector<u32> &a, const std::vector<u32> &v) {
+    SnapMapHdr h{};
+    snprintf(h.name, sizeof(h.name), "%s", name);
+    h.kind = kind, h.key_size = 4, h.value_size = 4, h.count = a.size();
+    out.insert(out.end(), (u8 *)&h, (u8 *)&h + sizeof(h));
+    out.insert(out.end(), (const u8 *)a.data(), (const u8 *)(a.data() + a.size()));
+    out.insert(out.end(), (const u8 *)v.data(), (const u8 *)(v.data() + v.size()));
+}
 } // namespace
 
 int64_t bng_snapshot(bng_ctx *c, void *buf, uint64_t cap) {
@@ -1955,6 +2129,12 @@ int64_t bng_snapshot(bng_ctx *c, void *buf, uint64_t cap) {
         for (auto &e : t) out.insert(out.end(), (u8 *)&e.second, (u8 *)&e.second + 4);
         nmaps++;
     }
+    if (c->idle) {
+        std::vector<u32> a, t;
+        if (int r = idle_timeouts_dump_locked(c, &a, &t)) return r;
+        put_pairs(out, kSnapIdle, kSnapIdleKind, a, t);
+        nmaps++;
+    }
     memcpy(&out[nmaps_at], &nmaps, 8);
     if (buf && cap >= out.size()) memcpy(buf, out.data(), out.size());
     return (int64_t)out.size(); // the size needed; nothing was copied when cap is smaller
@@ -1977,9 +2157,13 @@ int bng_restore(bng_ctx *c, const void *buf, uint64_t len) {
             c->li_targets.clear();
             c->li_dirty = true;
         }
+        if (c->idle) { // and for the idle timeouts; every clock restarts
+            CU(c, cudaMemsetAsync(c->idle, 0, ((size_t)c->dev.subdir.mask + 1) * sizeof(bng_idle), c->L.stream));
+            CU(c, cudaStreamSynchronize(c->L.stream));
+        }
     }
-    const u8 *acct_p = nullptr, *li_p = nullptr;
-    u64 acct_n = 0, li_n = 0;
+    const u8 *acct_p = nullptr, *li_p = nullptr, *idle_p = nullptr;
+    u64 acct_n = 0, li_n = 0, idle_n = 0;
     for (u64 k = 0; k < nmaps; k++) {
         if (p + sizeof(SnapMapHdr) > end) return -EINVAL;
         SnapMapHdr h;
@@ -2000,6 +2184,13 @@ int bng_restore(bng_ctx *c, const void *buf, uint64_t len) {
                 return fail(c, -EINVAL, "snapshot: %s has another layout", h.name);
             li_p = p;
             li_n = h.count;
+            p += kb + vb;
+            continue;
+        }
+        if (!strcmp(h.name, kSnapIdle)) { // applied below, once the directory is in place
+            if (h.key_size != 4 || h.value_size != 4) return fail(c, -EINVAL, "snapshot: %s has another layout", h.name);
+            idle_p = p;
+            idle_n = h.count;
             p += kb + vb;
             continue;
         }
@@ -2052,6 +2243,14 @@ int bng_restore(bng_ctx *c, const void *buf, uint64_t len) {
         }
         c->li_dirty = true;
     }
+    if (idle_p) {
+        std::lock_guard<std::mutex> g(c->mu);
+        cudaSetDevice(c->device);
+        std::vector<u32> a(idle_n), t(idle_n);
+        if (idle_n) memcpy(a.data(), idle_p, idle_n * 4), memcpy(t.data(), idle_p + idle_n * 4, idle_n * 4);
+        if (int r = idle_timeouts_locked(c, a.data(), t.data(), idle_n, nullptr)) return r;
+        if (int r = idle_restart_locked(c)) return r;
+    }
     return 0;
 }
 
@@ -2067,7 +2266,10 @@ struct DeltaHdr {
 };
 static_assert(sizeof(DeltaHdr) == 40 && sizeof(SnapMapHdr) == 64, "the delta framing of include/bng_b200.h");
 
-// A hash map's (or the accounting records') view for the diff: which words of a slot are compared, which is the
+// shadow ids beside the hash maps' (map ids): the accounting records, the idle records
+const int kShadowAcct = -1, kShadowIdle = -2;
+
+// A hash map's (or the accounting or idle records') view for the diff: which words of a slot are compared, which is the
 // time word.  Volatile fields are left out of the mask unless exact.
 DeltaTbl delta_view(bng_ctx *c, const bng_ctx::DeltaShadow &s, u64 refresh, bool exact) {
     DeltaTbl t{};
@@ -2077,6 +2279,13 @@ DeltaTbl delta_view(bng_ctx *c, const bng_ctx::DeltaShadow &s, u64 refresh, bool
     t.tw = DELTA_NO_TIME;
     t.refresh = refresh;
     auto set = [&](u32 pos) { t.mask[pos / 8] |= 0xFFull << (8 * (pos % 8)); };
+    if (s.map == kShadowIdle) { // idle records: the directory's address, then the timeout (no time word; clocks are not sent)
+        const Tbl &d = c->dev.subdir;
+        t.slots = d.slots, t.slot_bytes = d.slot_bytes, t.vals = (const u8 *)c->idle, t.vstride = sizeof(bng_idle);
+        t.kw = 1, t.key_size = 4, t.value_size = 4;
+        for (u32 b = 0; b < 4; b++) set(8 + b);
+        return t;
+    }
     if (s.map < 0) { // accounting records: the directory's address, then the record
         const Tbl &d = c->dev.subdir;
         t.slots = d.slots, t.slot_bytes = d.slot_bytes, t.vals = (const u8 *)c->acct, t.vstride = sizeof(bng_acct);
@@ -2118,7 +2327,7 @@ int delta_shadow_locked(bng_ctx *c, int map, const Tbl &t, u32 sw) {
     const size_t bytes = s.nslots * sw * 8;
     if (cudaMalloc((void **)&s.words, bytes) != cudaSuccess) {
         cudaGetLastError();
-        return fail(c, -ENOMEM, "delta_enable: %zu bytes of device memory for the shadow of %s", bytes, map < 0 ? kSnapAcct : c->maps[map].name);
+        return fail(c, -ENOMEM, "delta_enable: %zu bytes of device memory for the shadow of %s", bytes, map == kShadowAcct ? kSnapAcct : (map == kShadowIdle ? kSnapIdle : c->maps[map].name));
     }
     c->dshadow.push_back(s);
     CU(c, cudaMemsetAsync(s.words, 0xFF, bytes, c->L.stream)); // every slot empty: nothing sent yet
@@ -2181,7 +2390,13 @@ int bng_delta_enable(bng_ctx *c, int on) {
         }
     }
     if (c->acct) {
-        if (int r = delta_shadow_locked(c, -1, c->dev.subdir, 1 + ACCT_WORDS)) {
+        if (int r = delta_shadow_locked(c, kShadowAcct, c->dev.subdir, 1 + ACCT_WORDS)) {
+            delta_free_locked(c);
+            return r;
+        }
+    }
+    if (c->idle) {
+        if (int r = delta_shadow_locked(c, kShadowIdle, c->dev.subdir, 2)) {
             delta_free_locked(c);
             return r;
         }
@@ -2210,8 +2425,17 @@ int bng_delta_export(bng_ctx *c, uint64_t refresh_ns, uint32_t flags, void *buf,
     if (c->dshadow.empty()) return fail(c, -EINVAL, "delta_export: change tracking is not enabled");
     int r = flow_pass_begin_locked(c);
     if (r) return r;
-    if (c->acct && c->dshadow.back().map >= 0) { // accounting began after tracking did: its records start from "empty"
-        if ((r = delta_shadow_locked(c, -1, c->dev.subdir, 1 + ACCT_WORDS)) != 0) return r;
+    // records that began after tracking did start from "empty"
+    auto has_shadow = [&](int id) {
+        for (const auto &s : c->dshadow)
+            if (s.map == id) return true;
+        return false;
+    };
+    if (c->acct && !has_shadow(kShadowAcct)) {
+        if ((r = delta_shadow_locked(c, kShadowAcct, c->dev.subdir, 1 + ACCT_WORDS)) != 0) return r;
+    }
+    if (c->idle && !has_shadow(kShadowIdle)) {
+        if ((r = delta_shadow_locked(c, kShadowIdle, c->dev.subdir, 2)) != 0) return r;
     }
     const bool full = (flags & BNG_DELTA_FULL) || c->delta_full, exact = flags & BNG_DELTA_EXACT;
     std::vector<u8> out(sizeof(DeltaHdr));
@@ -2240,8 +2464,10 @@ int bng_delta_export(bng_ctx *c, uint64_t refresh_ns, uint32_t flags, void *buf,
         if (n[1]) CU(c, cudaMemcpyAsync(c->dsent + sent_used + n[0], up, (u64)n[1] * 4, cudaMemcpyDeviceToDevice, c->L.stream));
         commits.push_back({t, sent_used, n[0], n[1]});
         sent_used += n[0] + n[1];
-        if (s.map < 0)
+        if (s.map == kShadowAcct)
             put_section(out, kSnapAcct, kSnapAcctKind, 4, sizeof(bng_acct), n[0], n[1]);
+        else if (s.map == kShadowIdle)
+            put_section(out, kSnapIdle, kSnapIdleKind, 4, 4, n[0], n[1]);
         else
             put_section(out, c->maps[s.map].name, KIND_HASH, t.key_size, t.value_size, n[0], n[1]);
         sections++;
@@ -2324,6 +2550,9 @@ int bng_delta_apply(bng_ctx *c, const void *buf, uint64_t len) {
             if (s.h.key_size != 4 || s.h.value_size != 4 || s.h.count > BNG_LI_MAX_TARGETS)
                 return fail(c, -EINVAL, "delta_apply: %s has another layout", s.h.name);
             s.id = -3;
+        } else if (!strcmp(s.h.name, kSnapIdle)) {
+            if (s.h.key_size != 4 || s.h.value_size != 4) return fail(c, -EINVAL, "delta_apply: %s has another layout", s.h.name);
+            s.id = -4;
         } else {
             s.id = bng_map_id(c, s.h.name);
             if (s.id < 0) continue; // a map this library does not have
@@ -2342,6 +2571,7 @@ int bng_delta_apply(bng_ctx *c, const void *buf, uint64_t len) {
         c->dapply_stream = 0; // until this apply has completed, only a FULL delta is accepted
         if (full) {
             if (c->acct) CU(c, cudaMemsetAsync(c->acct, 0, ((size_t)c->dev.subdir.mask + 1) * sizeof(bng_acct), c->L.stream));
+            if (c->idle) CU(c, cudaMemsetAsync(c->idle, 0, ((size_t)c->dev.subdir.mask + 1) * sizeof(bng_idle), c->L.stream));
             CU(c, cudaStreamSynchronize(c->L.stream));
             if (!c->li_targets.empty()) c->li_targets.clear(), c->li_dirty = true;
         }
@@ -2399,8 +2629,15 @@ int bng_delta_apply(bng_ctx *c, const void *buf, uint64_t len) {
                 c->li_targets[a] = id;
             }
             c->li_dirty = true;
+        } else if (s.id == -4) {
+            std::vector<u32> a(s.h.count), t(s.h.count);
+            if (s.h.count) memcpy(a.data(), uk, s.h.count * 4), memcpy(t.data(), uv, s.h.count * 4);
+            if (int r = idle_timeouts_locked(c, a.data(), t.data(), s.h.count, nullptr)) return r;
         }
     }
+    // every clock restarts: at a takeover no clock here started before the last delta applied
+    if (int r = idle_restart_locked(c)) return r;
+    CU(c, cudaStreamSynchronize(c->L.stream));
     c->dapply_stream = h.stream;
     c->dapply_seq = h.seq_to;
     return 0;

@@ -62,10 +62,10 @@ cudaError_t run_scatter_frames(cudaStream_t st, int blocks, u8 *arena, const u32
 // table maintenance (tableops.cu); keys/values/results are device pointers
 enum { TOP_UPDATE = 0, TOP_LOOKUP = 1, TOP_DELETE = 2 };
 // dir / dir_role: the subscriber directory and which half of it table t feeds (0 none, 1 subscriber_nat, 2 qos_ingress)
-// acct: the per-subscriber counter records (nullptr until accounting is first enabled); a directory slot that is
-// claimed for an address has its record zeroed
+// acct / idle: the per-subscriber counter and idle records (nullptr until first enabled); a directory slot that is
+// claimed for an address has both records zeroed
 cudaError_t run_table_op(Launcher &L, const Tbl &t, int op, const u8 *keys, u8 *vals, int *results, u64 n, u32 flags,
-                         const Tbl &dir, int dir_role, u64 *acct);
+                         const Tbl &dir, int dir_role, u64 *acct, u64 *idle);
 cudaError_t run_dir_clear_half(Launcher &L, const Tbl &dir, int role);
 cudaError_t run_epoch_reset(Launcher &L, const Tbl &sessions);
 cudaError_t run_table_rebuild(Launcher &L, const Tbl &old_table, const Tbl &empty_table);
@@ -94,13 +94,37 @@ cudaError_t run_table_dump(Launcher &L, const Tbl &t, u8 *keys_out, u8 *vals_out
 // subscriber directory.  Modes of run_acct: where a frame's subscriber comes from.
 #define ACCT_WORDS 8
 enum { ACCT_ATTR = 0, ACCT_SRC = 1, ACCT_DST = 2 }; // attribution words of classify / header source / header destination
-cudaError_t run_acct(Launcher &L, const Tbl &dir, const DevBatch &b, int mode, u64 *acct);
+// the directory slot of an address, or DIR_NONE
+__device__ __forceinline__ u32 dir_slot_of(const Tbl &dir, u32 addr) {
+    const u64 k = addr;
+    const u8 *s = tbl_find<1, false>(dir, &k);
+    return s ? (u32)((s - dir.slots) >> 4) : DIR_NONE;
+}
+// acct: count the frames into the counter records (nullptr: no counting); idle: stamp the idle records of the frames
+// that pass (nullptr: no stamping).  At least one of the two is given.
+cudaError_t run_acct(Launcher &L, const Tbl &dir, const DevBatch &b, int mode, u64 *acct, u64 *idle);
 // results[i] = 0 / -ENOENT, out[i] zeroed on a miss; acct may be nullptr (every record reads as zero)
 cudaError_t run_acct_read(Launcher &L, const Tbl &dir, const u64 *acct, const u32 *addrs, u64 n, u64 *out, int *results);
 // every directory address with its record, compacted at *count (grows past cap: only cap are written)
 cudaError_t run_acct_dump(Launcher &L, const Tbl &dir, const u64 *acct, u32 *addrs_out, u64 *out, u32 *count, u64 cap);
 // record of every address of the list that has a directory entry := the given one (snapshot restore)
 cudaError_t run_acct_load(Launcher &L, const Tbl &dir, u64 *acct, const u32 *addrs, const u64 *recs, u64 n);
+
+// per-subscriber idle detection (idle.cu).  A record is IDLE_WORDS u64, index-aligned with the subscriber directory:
+// word 0 the timeout (low half) and a scratch word of run_idle_timeout_set (high half, 0 between calls), then the
+// upstream stamp, the downstream stamp and since, each as clock + 1 (0: none).  run_acct stamps words 1 and 2.
+#define IDLE_WORDS 4
+enum { IDLE_UP = 1, IDLE_DOWN = 2, IDLE_SINCE = 3 };
+// every live directory slot: unstarted records start at now; the idle ones are compacted at *count (which grows past
+// cap: only cap are written) as (address, struct bng_idle)
+cudaError_t run_idle_scan(Launcher &L, const Tbl &dir, u64 *idle, u64 now, u32 default_s, u32 flags, u32 *addrs_out, u64 *out,
+                          u32 *count, u64 cap);
+// results[i] = 0 / -ENOENT, out[i] (struct bng_idle) zeroed on a miss; idle may be nullptr (every record reads as zero)
+cudaError_t run_idle_read(Launcher &L, const Tbl &dir, const u64 *idle, const u32 *addrs, u64 n, u64 *out, int *results);
+// timeout of every listed address that has a directory entry := timeouts[i], the last of a repeated address winning
+cudaError_t run_idle_timeout_set(Launcher &L, const Tbl &dir, u64 *idle, const u32 *addrs, const u32 *timeouts, u64 n, int *results);
+// every record's stamps and since := none (the timeouts stay)
+cudaError_t run_idle_restart(Launcher &L, const Tbl &dir, u64 *idle);
 
 // lawful intercept (li.cu).  A record is LI_HDR bytes of header (struct bng_li_record) and the captured bytes, zero
 // padded to rec_bytes.  The targets are an AddrSet with target ids index-aligned to its words.

@@ -43,7 +43,7 @@ __device__ __forceinline__ void val_from_slot(const Tbl &t, u8 *abi, const u8 *s
 // role: which half of the directory entry the table being changed owns
 enum { DIR_ROLE_NONE = 0, DIR_ROLE_NAT = 1, DIR_ROLE_QOS = 2 };
 
-__device__ __forceinline__ void dir_set(const Tbl &dir, u64 key, int role, u32 val, u64 *acct) {
+__device__ __forceinline__ void dir_set(const Tbl &dir, u64 key, int role, u32 val, u64 *acct, u64 *idle) {
     bool created;
     u8 *d = tbl_find_or_claim<1>(dir, &key, &created);
     if (!d) return; // cannot happen: the directory is sized for both maps' max_entries
@@ -53,6 +53,11 @@ __device__ __forceinline__ void dir_set(const Tbl &dir, u64 key, int role, u32 v
             u64 *r = acct + (size_t)((d - dir.slots) >> 4) * ACCT_WORDS;
 #pragma unroll
             for (int j = 0; j < ACCT_WORDS; j++) r[j] = 0;
+        }
+        if (idle) { // and its idle record: default timeout, no stamp, not started
+            u64 *r = idle + (size_t)((d - dir.slots) >> 4) * IDLE_WORDS;
+#pragma unroll
+            for (int j = 0; j < IDLE_WORDS; j++) r[j] = 0;
         }
     }
     *(u32 *)(d + (role == DIR_ROLE_NAT ? 8 : 12)) = val;
@@ -72,7 +77,7 @@ __device__ __forceinline__ u32 dir_value(const Tbl &t, const u8 *slot, int role)
 
 template <int KW>
 __global__ void k_table_op(const __grid_constant__ Tbl t, int op, const u8 *keys, u8 *vals, int *results, u64 n, u32 flags,
-                           const __grid_constant__ Tbl dir, int dir_role, u64 *acct) {
+                           const __grid_constant__ Tbl dir, int dir_role, u64 *acct, u64 *idle) {
     for (u64 i = blockIdx.x * (u64)blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x) {
         u64 kw[KW];
         load_key<KW>(t, keys + i * t.key_size, kw);
@@ -111,7 +116,7 @@ __global__ void k_table_op(const __grid_constant__ Tbl t, int op, const u8 *keys
                     if (created) tbl_publish(s, kw[0]);
                 }
             }
-            if (!r && dir_role) dir_set(dir, kw[0], dir_role, dir_value(t, s, dir_role), acct);
+            if (!r && dir_role) dir_set(dir, kw[0], dir_role, dir_value(t, s, dir_role), acct, idle);
         }
         results[i] = r;
     }
@@ -152,17 +157,17 @@ __global__ void k_table_dump(const __grid_constant__ Tbl t, u8 *keys_out, u8 *va
 }
 
 cudaError_t run_table_op(Launcher &L, const Tbl &t, int op, const u8 *keys, u8 *vals, int *results, u64 n, u32 flags,
-                         const Tbl &dir, int dir_role, u64 *acct) {
+                         const Tbl &dir, int dir_role, u64 *acct, u64 *idle) {
     if (n == 0) return cudaSuccess;
     int block = 128;
     u64 want = (n + block - 1) / block;
     int grid = (int)(want < (u64)L.num_sms * 8 ? want : (u64)L.num_sms * 8);
     if (t.key_size <= 8)
-        k_table_op<1><<<grid, block, 0, L.stream>>>(t, op, keys, vals, results, n, flags, dir, dir_role, acct);
+        k_table_op<1><<<grid, block, 0, L.stream>>>(t, op, keys, vals, results, n, flags, dir, dir_role, acct, idle);
     else if (t.key_size == 16)
-        k_table_op<2><<<grid, block, 0, L.stream>>>(t, op, keys, vals, results, n, flags, dir, 0, nullptr);
+        k_table_op<2><<<grid, block, 0, L.stream>>>(t, op, keys, vals, results, n, flags, dir, 0, nullptr, nullptr);
     else
-        k_table_op<4><<<grid, block, 0, L.stream>>>(t, op, keys, vals, results, n, flags, dir, 0, nullptr);
+        k_table_op<4><<<grid, block, 0, L.stream>>>(t, op, keys, vals, results, n, flags, dir, 0, nullptr, nullptr);
     L.launches++;
     return cudaGetLastError();
 }

@@ -12,7 +12,7 @@ import os
 
 import numpy as np
 
-from .layouts import as_bytes, bng_acct, bng_li_record
+from .layouts import as_bytes, bng_acct, bng_idle, bng_li_record
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("BNG_B200_LIB") or os.path.join(HERE, "libbng_b200.so")  # override: A/B builds
@@ -116,6 +116,10 @@ def load_library() -> C.CDLL:
         "bng_delta_export": ([vp, u64, u32, vp, u64, C.POINTER(u64)], i32),
         "bng_delta_apply": ([vp, vp, u64], i32),
         "bng_delta_info": ([vp, C.POINTER(u64), C.POINTER(u64)], i32),
+        "bng_idle_enable": ([vp, i32, i32], i32),
+        "bng_idle_timeout_set": ([vp, vp, vp, u64, vp], i32),
+        "bng_idle_read": ([vp, vp, u64, vp, vp], i32),
+        "bng_idle_scan": ([vp, u64, u32, u32, vp, vp, u64], C.c_int64),
     }
     for name, (args, res) in protos.items():
         fn = getattr(lib, name)
@@ -136,6 +140,7 @@ EXPORTED_SYMBOLS = (
     "bng_acct_enable", "bng_acct_read", "bng_acct_dump", "bng_nat_flush",
     "bng_li_configure", "bng_li_record_size", "bng_li_target_set", "bng_li_target_del", "bng_li_drain", "bng_li_lost",
     "bng_delta_enable", "bng_delta_export", "bng_delta_apply", "bng_delta_info",
+    "bng_idle_enable", "bng_idle_timeout_set", "bng_idle_read", "bng_idle_scan",
 )
 
 
@@ -362,6 +367,42 @@ class Dataplane:
         a, out = a[:n], out[:n]
         order = np.argsort(a.byteswap(), kind="stable")
         return a[order], out[order]
+
+    # ---- per-subscriber idle detection ----
+    def idle_enable(self, prog, on: bool = True):
+        """Stamp the last-activity clocks of `prog`'s subscribers (off by default; independent of accounting)."""
+        pid = prog if isinstance(prog, int) else self.prog_id(prog)
+        self._chk(self.lib.bng_idle_enable(self.h, pid, 1 if on else 0), f"idle_enable({prog})")
+
+    def idle_timeout_set(self, addrs, timeouts_s):
+        """Idle-Timeout of each address (u8[n, 4] key bytes or u32[n]) in seconds: 0 = the scan's default,
+        layouts.IDLE_NEVER = never idle.  Returns found bool[n] (False: the address has no entry)."""
+        a = _addr_words(addrs)
+        t = np.ascontiguousarray(np.broadcast_to(np.asarray(timeouts_s, "<u4"), a.shape))
+        res = np.zeros(len(a), dtype=np.int32)
+        self._chk(self.lib.bng_idle_timeout_set(self.h, a.ctypes.data, t.ctypes.data, len(a), res.ctypes.data), "idle_timeout_set")
+        return res == 0
+
+    def idle_read(self, addrs):
+        """addrs: u8[n, 4] (qos_ingress key bytes) or u32[n] -> (bng_idle records[n], found bool[n])."""
+        a = _addr_words(addrs)
+        out = np.zeros(len(a), dtype=bng_idle)
+        res = np.zeros(len(a), dtype=np.int32)
+        self._chk(self.lib.bng_idle_read(self.h, a.ctypes.data, len(a), out.ctypes.data, res.ctypes.data), "idle_read")
+        return out, res == 0
+
+    def idle_scan(self, now_ns: int, default_s: int = 0, flags: int = 3, cap: int | None = None):
+        """(addresses u32[k], bng_idle records[k], found) of the subscribers idle at now_ns, sorted by address bytes;
+        found is the number of idle records, k = min(found, cap) (cap None: room for every subscriber)."""
+        if cap is None:
+            cap = max(int(self.map_info("subscriber_nat")["count"]) + int(self.map_info("qos_ingress")["count"]), 1)
+        a = np.zeros(max(cap, 1), dtype="<u4")
+        out = np.zeros(max(cap, 1), dtype=bng_idle)
+        n = self._chk(self.lib.bng_idle_scan(self.h, now_ns, default_s, flags, a.ctypes.data, out.ctypes.data, cap), "idle_scan")
+        k = min(n, cap)
+        a, out = a[:k], out[:k]
+        order = np.argsort(a.byteswap(), kind="stable")
+        return a[order], out[order], n
 
     def nat_flush(self, addrs, now_ns: int):
         """Remove the NAT flow state of a set of subscriber addresses (u8[n, 4] subscriber_nat key bytes or u32[n]):

@@ -154,6 +154,141 @@ inline AcctReader ContextReader(std::shared_ptr<Backend> b) {
 } // namespace radius
 
 // ===========================================================================
+// Idle sessions (reference pkg/subscriber/manager.go:648-687, cleanupExpiredSessions: a session whose IdleTimeout > 0
+// is terminated with TerminateIdleTimeout once now - LastActivity > IdleTimeout).  LastActivity is the dataplane's
+// per-subscriber stamp (bng_idle_*): the Monitor arms each session's Idle-Timeout on its address when the session is
+// accepted or a CoA changes it, and on every tick asks the dataplane for the idle addresses and terminates their
+// sessions.  The session starts with the configured default unless Access-Accept carries Idle-Timeout (attribute 28,
+// pkg/subscriber/manager.go:138,238-240); a timeout of 0 disables the check, as `IdleTimeout > 0` does.
+namespace idle {
+
+inline constexpr const char *kReasonIdleTimeout = "idle_timeout"; // TerminateIdleTimeout, pkg/subscriber/types.go:230
+
+// bng_idle_timeout_set / bng_idle_scan of one context or of a shard::Router
+using TimeoutSetFn = std::function<int(const uint32_t *addrs, const uint32_t *timeouts_s, uint64_t n, int32_t *results)>;
+using ScanFn = std::function<int64_t(uint64_t now_ns, uint32_t default_s, uint32_t flags, uint32_t *addrs_out, bng_idle *out,
+                                     uint64_t cap)>;
+// TerminateSession(ctx, sessionID, reason)
+using TerminateFn = std::function<void(const std::string &session_id, const std::string &reason)>;
+// bpf_ktime_get_ns(): the clock the frames were stamped with (CLOCK_MONOTONIC)
+using ClockFn = std::function<uint64_t()>;
+
+inline uint64_t MonotonicNs() {
+    return (uint64_t)std::chrono::duration_cast<std::chrono::nanoseconds>(std::chrono::steady_clock::now().time_since_epoch()).count();
+}
+
+inline TimeoutSetFn ContextTimeoutSet(std::shared_ptr<Backend> b) {
+    return [b = std::move(b)](const uint32_t *a, const uint32_t *t, uint64_t n, int32_t *res) {
+        return bng_idle_timeout_set(b->ctx, a, t, n, res);
+    };
+}
+inline ScanFn ContextScan(std::shared_ptr<Backend> b) {
+    return [b = std::move(b)](uint64_t now, uint32_t def, uint32_t flags, uint32_t *a, bng_idle *o, uint64_t cap) {
+        return bng_idle_scan(b->ctx, now, def, flags, a, o, cap);
+    };
+}
+
+struct MonitorConfig {
+    uint32_t default_idle_timeout_s = 30 * 60;    // SubscriberConfig.DefaultIdleTimeout (types.go:268)
+    uint32_t flags = BNG_IDLE_UP | BNG_IDLE_DOWN; // which direction counts as activity
+};
+
+class Monitor {
+  public:
+    using Config = MonitorConfig;
+    Monitor(TimeoutSetFn set, ScanFn scan, TerminateFn terminate, ClockFn clock = MonotonicNs, Config cfg = Config())
+        : set_(std::move(set)), scan_(std::move(scan)), terminate_(std::move(terminate)), clock_(std::move(clock)), cfg_(cfg) {}
+
+    // Access-Accept: the session's address (as the qos_ingress key holds it) and its Idle-Timeout attribute, if any.
+    Error OnAccept(const std::string &session_id, uint32_t addr_key, std::optional<uint32_t> idle_timeout_s = std::nullopt) {
+        const uint32_t t = idle_timeout_s && *idle_timeout_s > 0 ? *idle_timeout_s : cfg_.default_idle_timeout_s;
+        if (Error e = Arm(addr_key, t)) return e; // (no entry for the address yet: the session is not watched)
+        std::lock_guard<std::mutex> g(mu_);
+        by_addr_[addr_key] = session_id;
+        addr_of_[session_id] = addr_key;
+        return Nil();
+    }
+    // CoA with Idle-Timeout (coa.go:364, coa_handler.go:411): 0 disables the check
+    Error OnCoA(const std::string &session_id, uint32_t idle_timeout_s) {
+        uint32_t a;
+        {
+            std::lock_guard<std::mutex> g(mu_);
+            auto it = addr_of_.find(session_id);
+            if (it == addr_of_.end()) return Error("session not found: " + session_id);
+            a = it->second;
+        }
+        return Arm(a, idle_timeout_s);
+    }
+    // the session ended for another reason: its address no longer belongs to it
+    void Forget(const std::string &session_id) {
+        std::lock_guard<std::mutex> g(mu_);
+        auto it = addr_of_.find(session_id);
+        if (it == addr_of_.end()) return;
+        by_addr_.erase(it->second);
+        addr_of_.erase(it);
+    }
+    size_t Sessions() const {
+        std::lock_guard<std::mutex> g(mu_);
+        return addr_of_.size();
+    }
+
+    // One cleanup tick: scans, then terminates the session of every idle address it knows, once (the session is
+    // forgotten and its address disarmed before the callback runs).  Returns the number of sessions terminated or a
+    // negative errno.
+    int64_t Tick() {
+        uint64_t cap = std::max<uint64_t>(Sessions(), 64);
+        std::vector<uint32_t> addrs;
+        std::vector<bng_idle> recs;
+        const uint64_t now = clock_();
+        int64_t found;
+        for (;;) {
+            addrs.resize(cap);
+            recs.resize(cap);
+            // default: never idle, so that only addresses armed by OnAccept / OnCoA can be reported
+            found = scan_(now, BNG_IDLE_NEVER, cfg_.flags, addrs.data(), recs.data(), cap);
+            if (found < 0) return found;
+            if ((uint64_t)found <= cap) break;
+            cap = (uint64_t)found; // the scan can be repeated: nothing has stamped in between that matters here
+        }
+        std::vector<std::pair<std::string, uint32_t>> gone;
+        {
+            std::lock_guard<std::mutex> g(mu_);
+            for (int64_t i = 0; i < found; i++) {
+                auto it = by_addr_.find(addrs[(size_t)i]);
+                if (it == by_addr_.end()) continue;
+                gone.emplace_back(it->second, it->first);
+                addr_of_.erase(it->second);
+                by_addr_.erase(it);
+            }
+        }
+        for (auto &s : gone) {
+            Arm(s.second, BNG_IDLE_NEVER); // until the entries go, the address is not reported again
+            terminate_(s.first, kReasonIdleTimeout);
+        }
+        return (int64_t)gone.size();
+    }
+
+  private:
+    Error Arm(uint32_t addr_key, uint32_t timeout_s) {
+        const uint32_t t = timeout_s ? timeout_s : BNG_IDLE_NEVER;
+        int32_t res = 0;
+        if (Error e = MapErr("bng_idle_timeout_set", set_(&addr_key, &t, 1, &res))) return e;
+        return MapErr("bng_idle_timeout_set", res);
+    }
+
+    TimeoutSetFn set_;
+    ScanFn scan_;
+    TerminateFn terminate_;
+    ClockFn clock_;
+    Config cfg_;
+    mutable std::mutex mu_;
+    std::map<uint32_t, std::string> by_addr_;
+    std::map<std::string, uint32_t> addr_of_;
+};
+
+} // namespace idle
+
+// ===========================================================================
 // Lawful intercept, content of communication (reference pkg/intercept/manager.go:337: Manager.RecordCC(warrant,
 // session, direction, srcIP, dstIP, srcPort, dstPort, protocol, payload)).  StartInterceptSession sets the session's
 // IPv4 address as a target (bng_li_target_set), StopInterceptSession deletes it; PumpCC drains the records and hands

@@ -313,6 +313,67 @@ class Router {
         if (k >= shards_.size()) return -EINVAL;
         return bng_delta_apply(shards_[k]->ctx, blob, len);
     }
+    // Idle detection (bng_idle_*).  A subscriber's record lives on its owner shard only: upstream frames follow its MAC
+    // there and downstream frames are steered there by (public address, port block), so the owner's record is the
+    // whole record and no collective is needed.  IdleTimeoutSet sends each address to its owner, or to every shard
+    // when the owner is not known; results[i] is 0 when some shard had an entry for it, else -ENOENT.
+    int IdleTimeoutSet(const uint32_t *addrs, const uint32_t *timeouts_s, uint64_t n, int32_t *results) {
+        if (n && (!addrs || !timeouts_s || !results)) return -EINVAL;
+        std::vector<std::vector<uint64_t>> idx(shards_.size());
+        for (uint64_t i = 0; i < n; i++) {
+            results[i] = -ENOENT;
+            for (size_t k : LiShards(addrs[i])) idx[k].push_back(i);
+        }
+        for (size_t k = 0; k < shards_.size(); k++) {
+            if (idx[k].empty()) continue;
+            std::vector<uint32_t> a, t;
+            for (uint64_t i : idx[k]) a.push_back(addrs[i]), t.push_back(timeouts_s[i]);
+            std::vector<int32_t> res(a.size());
+            if (int r = bng_idle_timeout_set(shards_[k]->ctx, a.data(), t.data(), a.size(), res.data())) return r;
+            for (size_t j = 0; j < a.size(); j++)
+                if (res[j] == 0) results[idx[k][j]] = 0;
+        }
+        return 0;
+    }
+    // Every shard's scan: returns the idle records found over all shards and writes the first cap of them.
+    int64_t IdleScan(uint64_t now_ns, uint32_t default_s, uint32_t flags, uint32_t *addrs_out, bng_idle *out, uint64_t cap) {
+        if (cap && (!addrs_out || !out)) return -EINVAL;
+        int64_t total = 0;
+        for (auto &s : shards_) {
+            const uint64_t at = std::min<uint64_t>((uint64_t)total, cap);
+            int64_t n = bng_idle_scan(s->ctx, now_ns, default_s, flags, cap > at ? addrs_out + at : nullptr,
+                                      cap > at ? out + at : nullptr, cap - at);
+            if (n < 0) return n;
+            total += n;
+        }
+        return total;
+    }
+    // Records of n addresses, each from its owner (or, when the owner is not known, from the shard that has it).
+    int IdleRead(const uint32_t *addrs, uint64_t n, bng_idle *out, int32_t *results) {
+        if (n && (!addrs || !out || !results)) return -EINVAL;
+        for (uint64_t i = 0; i < n; i++) {
+            out[i] = bng_idle{};
+            results[i] = -ENOENT;
+            for (size_t k : LiShards(addrs[i])) {
+                bng_idle rec{};
+                int32_t res = 0;
+                if (int r = bng_idle_read(shards_[k]->ctx, &addrs[i], 1, &rec, &res)) return r;
+                if (res == 0) {
+                    out[i] = rec, results[i] = 0;
+                    break;
+                }
+            }
+        }
+        return 0;
+    }
+    idle::TimeoutSetFn IdleTimeoutSetter() {
+        return [this](const uint32_t *a, const uint32_t *t, uint64_t n, int32_t *res) { return IdleTimeoutSet(a, t, n, res); };
+    }
+    idle::ScanFn IdleScanner() {
+        return [this](uint64_t now, uint32_t def, uint32_t flags, uint32_t *a, bng_idle *o, uint64_t cap) {
+            return IdleScan(now, def, flags, a, o, cap);
+        };
+    }
     radius::AcctReader Reader() {
         return [this](uint32_t addr, bng_acct *out) { return AcctRead(addr, out); };
     }

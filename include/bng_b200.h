@@ -304,7 +304,7 @@ uint64_t bng_li_lost(bng_ctx *ctx); /* records dropped because the ring was full
  * records once they exist) and sets the baseline to "empty": a new random stream id, sequence 0, and the next export
  * is FULL.  on == 0 frees it.  The shadows take, per slot of each table, its key and its compared bytes as last sent,
  * rounded up to 8-byte words: 1.85 GiB at the default capacities (1e6 subscribers, 4e6 sessions, 2e6 EIM), 2.0 GiB
- * with accounting records.
+ * with accounting records, 32 MiB more with idle records.
  * bng_delta_export: a batch of its own, as bng_sweep is (staged upserts are applied first; it sees everything queued
  * on the context's stream).  The blob it writes:
  *   header   char magic[8] = "BNGDELT1"; uint64 stream_id, seq_from, seq_to; uint32 flags, sections  (40 bytes)
@@ -319,6 +319,8 @@ uint64_t bng_li_lost(bng_ctx *ctx); /* records dropped because the ring was full
  *   - Array, LPM and statistics maps: every entry, every time (n_del = 0); they replace the standby's copy.
  *   - "subscriber_acct" (kind 5, once accounting exists): the (address, struct bng_acct) records whose bytes changed.
  *   - "li_targets" (kind 6): the whole interception target set (address, target id), when it changed.
+ *   - "subscriber_idle" (kind 7, once idle records exist): the (address, uint32 timeout_s) pairs whose timeout changed
+ *     (see bng_idle_* below).
  *   - Event rings are not state and are never sent.
  * seq_to = seq_from + 1.  A FULL delta (BNG_DELTA_FULL, or the first export after enabling) carries every live entry
  * and no deletion.  When cap is smaller than the delta, nothing is written, *len_out is set to the size needed,
@@ -337,6 +339,62 @@ int bng_delta_enable(bng_ctx *ctx, int on);
 int bng_delta_export(bng_ctx *ctx, uint64_t refresh_ns, uint32_t flags, void *buf, uint64_t cap, uint64_t *len_out);
 int bng_delta_apply(bng_ctx *ctx, const void *buf, uint64_t len);
 int bng_delta_info(bng_ctx *ctx, uint64_t *stream_id, uint64_t *seq);
+
+/* ---- per-subscriber idle detection (what RADIUS Idle-Timeout, attribute 28, needs) ----
+ * One record per subscriber address, with the population and lifecycle of the accounting record: an address that keys
+ * a subscriber_nat or qos_ingress entry (staged upserts included).  The record starts when the address gets its entry
+ * (every field none, timeout 0); it survives updates of either map, the expiry sweep, LRU eviction, flow-table
+ * rebuilds and bng_nat_flush, and ends when the address loses both entries.
+ *   - Stamps.  Frames are attributed to an address by accounting's rule: upstream programs (nat44_egress,
+ *     qos_ingress_prog, pipeline_up, pipeline_tc) by the IPv4 source the frame entered with, downstream programs
+ *     (nat44_ingress, qos_egress_prog) by the IPv4 destination it leaves with; in the two pipelines a frame antispoof
+ *     drops is attributed to nobody.  Only frames with verdict TC_ACT_OK stamp: a frame the token bucket or port
+ *     exhaustion drops was not carried.  The upstream stamp (up_ns) is the largest bpf_ktime_get_ns() of the stamping
+ *     frames of upstream programs (now_ns_v[i], or the batch's now_ns), the downstream stamp (down_ns) the same for
+ *     downstream programs.  A stamp never goes backwards.  (A clock of UINT64_MAX is stamped as UINT64_MAX - 1.)
+ *   - Timeout.  timeout_s 0 means "the scan's default", BNG_IDLE_NEVER "never idle".
+ *   - Scan.  bng_idle_scan(now_ns, default_s, flags) visits every record.  flags selects the stamps that count as
+ *     activity (BNG_IDLE_UP and / or BNG_IDLE_DOWN).  A record that has not been started (no since_ns) is started:
+ *     since_ns := now_ns, and it is not reported; so a subscriber that never sends anything is reported one timeout
+ *     after the first scan that saw it, never at once.  A started record's reference time ref is the largest of its
+ *     selected stamps and since_ns; it is idle when ref <= now_ns and now_ns - ref > timeout x 10^9 ns (timeout_s, or
+ *     default_s when timeout_s is 0; BNG_IDLE_NEVER in either place: never idle).
+ * Idle detection is enabled per program and off by default, independently of accounting.  The first
+ * bng_idle_enable() or bng_idle_timeout_set() allocates the records: 32 bytes per subscriber-directory slot (64 MiB at
+ * the default 1e6 subscribers), plus 4 bytes per frame of max_batch when accounting has not allocated those already.
+ * A context that never uses it allocates nothing and launches no kernel more.  Before the records exist a scan finds
+ * nothing and a read returns zeroed records.
+ * Only the timeouts are configuration.  bng_snapshot() carries them (a trailing "subscriber_idle" section of
+ * (address, uint32 timeout_s) pairs, written once records exist); bng_restore() sets them and restarts every clock
+ * (stamps and since_ns cleared); a blob without the section leaves every timeout at 0.  bng_delta_export() sends a
+ * "subscriber_idle" section (kind 7, once records exist) with the (address, timeout_s) pairs whose timeout changed,
+ * all of them in a FULL delta; every bng_delta_apply() restarts every clock of the standby, so that no clock on the
+ * standby started earlier than the last delta it applied and a takeover disconnects nobody early. */
+#define BNG_IDLE_UP 1u           /* flags: up_ns holds a value; scan: count upstream activity */
+#define BNG_IDLE_DOWN 2u         /* flags: down_ns holds a value; scan: count downstream activity */
+#define BNG_IDLE_STARTED 4u      /* flags: since_ns holds a value */
+#define BNG_IDLE_NEVER 0xFFFFFFFFu /* timeout_s: never idle */
+typedef struct bng_idle {       /* 32 bytes */
+    uint64_t up_ns, down_ns;    /* the stamps (0 unless the flag is set) */
+    uint64_t since_ns;          /* when the first scan saw the record (0 unless BNG_IDLE_STARTED) */
+    uint32_t timeout_s, flags;
+} bng_idle;
+/* on != 0 stamps the program's runs from the next bng_prog_run on.  -EOPNOTSUPP for antispoof_ingress,
+ * nat44_hairpin_xdp and dhcp_fastpath_prog; -EINVAL for an unknown program id. */
+int bng_idle_enable(bng_ctx *ctx, int prog, int on);
+/* timeouts_s[i] becomes the timeout of addrs[i] (4 bytes each, in the byte order of the qos_ingress key).  results[i]
+ * = 0, or -ENOENT when the address has no entry.  When an address repeats, the last of its values wins.  Staged
+ * upserts are applied first.  Returns 0 or a negative errno. */
+int bng_idle_timeout_set(bng_ctx *ctx, const uint32_t *addrs, const uint32_t *timeouts_s, uint64_t n, int32_t *results);
+/* Records of n addresses; results[i] = 0, or -ENOENT when the address has no entry (out[i] is then zeroed).  Staged
+ * upserts are applied first and the read sees everything queued on the context's stream, as bng_acct_read() does. */
+int bng_idle_read(bng_ctx *ctx, const uint32_t *addrs, uint64_t n, bng_idle *out, int32_t *results);
+/* The scan above.  Returns the number of idle records found and writes min(found, cap) of them, (address, record) in
+ * no particular order; calling it again gives the same answer while nothing stamps.  Staged upserts are applied first
+ * and the scan sees everything queued on the context's stream.  -EINVAL when flags selects neither direction or has
+ * other bits, or when cap > 0 and an output is NULL. */
+int64_t bng_idle_scan(bng_ctx *ctx, uint64_t now_ns, uint32_t default_s, uint32_t flags, uint32_t *addrs_out, bng_idle *out,
+                      uint64_t cap);
 
 /* ---- diagnostics ---- */
 uint64_t bng_launch_count(bng_ctx *ctx);  /* kernels launched by this context so far */
