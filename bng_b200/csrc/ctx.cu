@@ -116,6 +116,12 @@ struct bng_ctx {
     u32 idle_progs = 0;
     u8 *idle_scan_buf = nullptr; // grow-only scratch of bng_idle_scan: records, then addresses, then the count
     u64 idle_scan_cap = 0;
+    // NAT port-usage census (bng_nat_usage, natuse.cu): scratch allocated by the first call (nu_sum != null)
+    u64 *nu_set = nullptr, *nu_pub = nullptr, *nu_sum = nullptr;
+    u32 *nu_sub = nullptr;
+    u32 nu_set_mask = 0, nu_pub_mask = 0;
+    u8 *nu_out = nullptr; // grow-only: the qualifying records and their addresses
+    u64 nu_out_bytes = 0;
     u64 seq = 0; // the batch sequence in 64 bits (dev.batch_seq holds its low 32): bng_li_record.batch
     // lawful intercept (bng_li_*, li.cu): allocated by the first bng_li_configure / bng_li_target_set (li_ctl != null)
     u64 *li_ctl = nullptr;   // device: LiRing::ctl
@@ -536,7 +542,7 @@ int bng_close(bng_ctx *c) {
         Scratch &s = c->L.s;
         void *sp[] = {s.key_a, s.key_b, s.val_a, s.val_b, s.qslot, s.attr, s.cub_tmp, s.counters, c->acct_dump_buf, c->idle_scan_buf, c->li_ring, c->li_match,
                       c->io_dev, c->hb_pkts, c->hb_off, c->hb_len, c->hb_prio, c->hb_verdict, c->hb_now, c->dump_k, c->dump_v, c->dump_c,
-                      c->dlist, c->dsent, c->demit};
+                      c->dlist, c->dsent, c->demit, c->nu_set, c->nu_pub, c->nu_sum, c->nu_sub, c->nu_out};
         for (void *p : sp)
             if (p) cudaFree(p);
         for (auto &s : c->dshadow) cudaFree(s.words);
@@ -1872,6 +1878,121 @@ int64_t bng_idle_scan(bng_ctx *c, uint64_t now_ns, uint32_t default_s, uint32_t 
         CU(c, cudaMemcpy(addrs_out, buf + aoff, got * 4, cudaMemcpyDeviceToHost));
     }
     return (int64_t)n;
+}
+
+// ---------------------------------------------------------------------------
+// NAT port-usage census (natuse.cu)
+// ---------------------------------------------------------------------------
+static_assert(sizeof(bng_nat_sub_use) == 64 && sizeof(bng_nat_pub_use) == 64, "the census writes 16 u32 per record");
+static_assert(sizeof(bng_nat_usage_sum) == (NU_PUBS_FOUND + 1) * 8, "struct bng_nat_usage_sum is the head of the census's sum words");
+
+static int nu_malloc(bng_ctx *c, void **p, size_t bytes, const char *what) {
+    if (cudaMalloc(p, bytes) != cudaSuccess) {
+        cudaGetLastError();
+        *p = nullptr;
+        return fail(c, -ENOMEM, "nat_usage: %zu bytes of device memory for the %s", bytes, what);
+    }
+    return 0;
+}
+
+static u64 nu_pow2(u64 v) {
+    u64 p = 64;
+    while (p < v) p <<= 1;
+    return p;
+}
+
+// the public-address table: pub_mask + 1 slots
+static int nu_pub_alloc(bng_ctx *c, u64 slots) {
+    if (slots > (1ull << 32)) return fail(c, -ENOMEM, "nat_usage: %llu public-address slots", (unsigned long long)slots);
+    u64 *p = nullptr; // the old table stays when the new one does not fit
+    if (int r = nu_malloc(c, (void **)&p, slots * NU_PUB_WORDS * 8, "public-address table")) return r;
+    if (c->nu_pub) cudaFree(c->nu_pub);
+    c->nu_pub = p;
+    c->nu_pub_mask = (u32)(slots - 1);
+    return 0;
+}
+
+// The census's scratch, on first use (kernels.h: NatUse).  All of it or none.
+static int nu_alloc_locked(bng_ctx *c) {
+    if (c->nu_sum) return 0;
+    const u64 keys = 4ull * ((u64)c->dev.sessions.max_entries + c->dev.eim.max_entries);
+    const u64 set_slots = nu_pow2((keys * 4 + 2) / 3);
+    const u64 dir_slots = (u64)c->dev.subdir.mask + 1;
+    if (set_slots > (1ull << 30) || dir_slots > (1ull << 30))
+        return fail(c, -ENOMEM, "nat_usage: %llu set slots / %llu directory slots exceed 2^30", (unsigned long long)set_slots,
+                    (unsigned long long)dir_slots);
+    int r = nu_malloc(c, (void **)&c->nu_set, set_slots * 8, "triple set");
+    if (!r) r = nu_malloc(c, (void **)&c->nu_sub, dir_slots * NU_SUB_WORDS * 4, "subscriber counters");
+    if (!r) r = nu_pub_alloc(c, 1u << 16);
+    if (!r) r = nu_malloc(c, (void **)&c->nu_sum, NU_SUM_WORDS * 8, "summary");
+    if (r) {
+        for (void *p : {(void *)c->nu_set, (void *)c->nu_sub, (void *)c->nu_pub})
+            if (p) cudaFree(p);
+        c->nu_set = c->nu_pub = nullptr;
+        c->nu_sub = nullptr;
+        return r;
+    }
+    c->nu_set_mask = (u32)(set_slots - 1);
+    return 0;
+}
+
+int bng_nat_usage(bng_ctx *c, uint32_t min_permille, bng_nat_usage_sum *sum, uint32_t *sub_addrs, bng_nat_sub_use *sub_out,
+                  uint64_t sub_cap, uint32_t *pub_addrs, bng_nat_pub_use *pub_out, uint64_t pub_cap) {
+    if (!c || !sum || min_permille > 1000 || (sub_cap && (!sub_addrs || !sub_out)) || (pub_cap && (!pub_addrs || !pub_out)))
+        return -EINVAL;
+    std::lock_guard<std::mutex> g(c->mu);
+    cudaSetDevice(c->device);
+    int r = flush_staged_locked(c, -1);
+    if (r) return r;
+    if ((r = nu_alloc_locked(c)) != 0) return r;
+    const u64 scap = std::min<u64>(sub_cap, (u64)c->dev.subdir.mask + 1); // no more records than directory slots
+    u64 sum_w[NU_SUM_WORDS];
+    for (;;) {
+        const u64 pcap = std::min<u64>(pub_cap, (u64)c->nu_pub_mask + 1);
+        const u64 rec_b = (scap + pcap) * 64, need = rec_b + (scap + pcap) * 4;
+        if (need > c->nu_out_bytes) {
+            if (c->nu_out) cudaFree(c->nu_out);
+            c->nu_out_bytes = 0;
+            if ((r = nu_malloc(c, (void **)&c->nu_out, need, "records")) != 0) return r;
+            c->nu_out_bytes = need;
+        }
+        NatUse u{};
+        u.set = c->nu_set, u.set_mask = c->nu_set_mask, u.sub = c->nu_sub, u.pub = c->nu_pub, u.pub_mask = c->nu_pub_mask;
+        u.sum = c->nu_sum;
+        u.sub_out = (u32 *)c->nu_out, u.pub_out = (u32 *)(c->nu_out + scap * 64);
+        u.sub_addrs = (u32 *)(c->nu_out + rec_b), u.pub_addrs = u.sub_addrs + scap;
+        u.sub_cap = scap, u.pub_cap = pcap;
+        const u64 dir_slots = (u64)c->dev.subdir.mask + 1;
+        CU(c, cudaMemsetAsync(c->nu_set, 0, ((u64)c->nu_set_mask + 1) * 8, c->L.stream));
+        CU(c, cudaMemsetAsync(c->nu_sub, 0, dir_slots * NU_SUB_WORDS * 4, c->L.stream));
+        CU(c, cudaMemsetAsync(c->nu_pub, 0, ((u64)c->nu_pub_mask + 1) * NU_PUB_WORDS * 8, c->L.stream));
+        CU(c, cudaMemsetAsync(c->nu_sum, 0, NU_SUM_WORDS * 8, c->L.stream));
+        CU(c, run_nat_usage_flows(c->L, c->dev, u));
+        CU(c, cudaMemcpyAsync(sum_w, c->nu_sum, sizeof(sum_w), cudaMemcpyDeviceToHost, c->L.stream));
+        CU(c, cudaStreamSynchronize(c->L.stream));
+        if (sum_w[NU_SET_FULL]) return fail(c, -EIO, "nat_usage: the triple set is full");
+        if (sum_w[NU_OVERFLOW]) { // more public addresses than half the table: grow it past the reservations and count again
+            prof_collect(c->L);
+            if ((r = nu_pub_alloc(c, nu_pow2(2 * sum_w[NU_PUB_RESERVED]))) != 0) return r;
+            continue;
+        }
+        CU(c, run_nat_usage_emit(c->L, c->dev, u, min_permille));
+        CU(c, cudaMemcpyAsync(sum_w, c->nu_sum, sizeof(sum_w), cudaMemcpyDeviceToHost, c->L.stream));
+        CU(c, cudaStreamSynchronize(c->L.stream));
+        prof_collect(c->L);
+        const u64 ns = std::min<u64>(sum_w[NU_SUBS_FOUND], scap), np = std::min<u64>(sum_w[NU_PUBS_FOUND], pcap);
+        if (ns) {
+            CU(c, cudaMemcpy(sub_out, u.sub_out, ns * 64, cudaMemcpyDeviceToHost));
+            CU(c, cudaMemcpy(sub_addrs, u.sub_addrs, ns * 4, cudaMemcpyDeviceToHost));
+        }
+        if (np) {
+            CU(c, cudaMemcpy(pub_out, u.pub_out, np * 64, cudaMemcpyDeviceToHost));
+            CU(c, cudaMemcpy(pub_addrs, u.pub_addrs, np * 4, cudaMemcpyDeviceToHost));
+        }
+        break;
+    }
+    memcpy(sum, sum_w, sizeof(*sum));
+    return 0;
 }
 
 // ---------------------------------------------------------------------------

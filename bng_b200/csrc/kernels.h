@@ -126,6 +126,40 @@ cudaError_t run_idle_timeout_set(Launcher &L, const Tbl &dir, u64 *idle, const u
 // every record's stamps and since := none (the timeouts stay)
 cudaError_t run_idle_restart(Launcher &L, const Tbl &dir, u64 *idle);
 
+// NAT port-usage census (natuse.cu).  Scratch of its own, zeroed before every census:
+//   set        set_mask + 1 u64 words, 0 = empty: the distinct held triples and ports, overall and per subscriber.  A
+//              live session or EIM entry puts at most four keys in, so 4 x (max_nat_sessions + max_eim_mappings) keys
+//              fit in the power of two >= 4/3 of that (load <= 3/4).  Slot indices and directory slots are < 2^30.
+//   sub        NU_SUB_WORDS u32 per subscriber directory slot: sessions, eim, in_use[3], in_use_any, outside, unreachable
+//   pub        pub_mask + 1 records of NU_PUB_WORDS u64: ADDRSET_LIVE | address (0 = empty), the sum of block_ports, then
+//              u32 sessions, eim, blocks, in_use[3], in_use_any, unreachable
+//   sum        NU_SUM_WORDS u64: the struct bng_nat_usage_sum fields in order, then the census's own words
+#define NU_SUB_WORDS 8
+#define NU_PUB_WORDS 6
+#define NU_NONE 0xFFFFFFFFu
+enum {
+    NU_SUBSCRIBERS, NU_SESSIONS, NU_EIM, NU_TRIPLES, NU_UNREACHABLE, NU_STALE, NU_ORPHAN_SES, NU_ORPHAN_EIM, // summed per thread
+    NU_SUBS_FOUND, NU_PUBS_FOUND,
+    NU_PUB_RESERVED, // public-address slots reserved so far (reservations past half the table: overflow)
+    NU_OVERFLOW,     // the public-address table was too small: grow it and run again
+    NU_SET_FULL,     // the set was full (its sizing rules that out)
+    NU_SUM_WORDS
+};
+#define NU_LOCAL (NU_ORPHAN_EIM + 1)
+struct NatUse {
+    u64 *set;
+    u32 set_mask, pub_mask;
+    u32 *sub;
+    u64 *pub;
+    u64 *sum;
+    // qualifying records (struct bng_nat_sub_use / bng_nat_pub_use, 16 u32 each) and their addresses, up to the caps
+    u32 *sub_addrs, *sub_out, *pub_addrs, *pub_out;
+    u64 sub_cap, pub_cap;
+};
+cudaError_t run_nat_usage_flows(Launcher &L, const DevCtx &c, const NatUse &u);
+// qualifying subscriber records (permille >= min_permille) and every public-address record, compacted
+cudaError_t run_nat_usage_emit(Launcher &L, const DevCtx &c, const NatUse &u, u32 min_permille);
+
 // lawful intercept (li.cu).  A record is LI_HDR bytes of header (struct bng_li_record) and the captured bytes, zero
 // padded to rec_bytes.  The targets are an AddrSet with target ids index-aligned to its words.
 #define LI_HDR 64

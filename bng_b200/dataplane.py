@@ -12,7 +12,7 @@ import os
 
 import numpy as np
 
-from .layouts import as_bytes, bng_acct, bng_idle, bng_li_record
+from .layouts import as_bytes, bng_acct, bng_idle, bng_li_record, bng_nat_pub_use, bng_nat_sub_use, bng_nat_usage_sum
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("BNG_B200_LIB") or os.path.join(HERE, "libbng_b200.so")  # override: A/B builds
@@ -120,6 +120,7 @@ def load_library() -> C.CDLL:
         "bng_idle_timeout_set": ([vp, vp, vp, u64, vp], i32),
         "bng_idle_read": ([vp, vp, u64, vp, vp], i32),
         "bng_idle_scan": ([vp, u64, u32, u32, vp, vp, u64], C.c_int64),
+        "bng_nat_usage": ([vp, u32, vp, vp, vp, u64, vp, vp, u64], i32),
     }
     for name, (args, res) in protos.items():
         fn = getattr(lib, name)
@@ -140,7 +141,7 @@ EXPORTED_SYMBOLS = (
     "bng_acct_enable", "bng_acct_read", "bng_acct_dump", "bng_nat_flush",
     "bng_li_configure", "bng_li_record_size", "bng_li_target_set", "bng_li_target_del", "bng_li_drain", "bng_li_lost",
     "bng_delta_enable", "bng_delta_export", "bng_delta_apply", "bng_delta_info",
-    "bng_idle_enable", "bng_idle_timeout_set", "bng_idle_read", "bng_idle_scan",
+    "bng_idle_enable", "bng_idle_timeout_set", "bng_idle_read", "bng_idle_scan", "bng_nat_usage",
 )
 
 
@@ -412,6 +413,29 @@ class Dataplane:
         out = (C.c_uint64 * 3)()
         self._chk(self.lib.bng_nat_flush(self.h, a.ctypes.data if len(a) else None, len(a), now_ns, out), "nat_flush")
         return tuple(int(x) for x in out)
+
+    # ---- NAT port-usage census ----
+    def nat_usage(self, min_permille: int = 0, cap: int | None = None):
+        """Port utilisation per subscriber and per public address (include/bng_b200.h, bng_nat_usage).  Returns
+        (summary dict, subscriber addresses u32[k], bng_nat_sub_use[k], public addresses u32[m], bng_nat_pub_use[m]),
+        each kind sorted by address bytes: the subscribers whose permille >= min_permille and every public address,
+        at most `cap` of each (None: all of them)."""
+        sub_cap = cap if cap is not None else max(int(self.map_info("subscriber_nat")["count"]), 1)
+        pub_cap = cap if cap is not None else sub_cap + 64
+        while True:
+            s = np.zeros(1, dtype=bng_nat_usage_sum)
+            sa, so = np.zeros(max(sub_cap, 1), "<u4"), np.zeros(max(sub_cap, 1), bng_nat_sub_use)
+            pa, po = np.zeros(max(pub_cap, 1), "<u4"), np.zeros(max(pub_cap, 1), bng_nat_pub_use)
+            self._chk(self.lib.bng_nat_usage(self.h, min_permille, s.ctypes.data, sa.ctypes.data, so.ctypes.data, sub_cap,
+                                             pa.ctypes.data, po.ctypes.data, pub_cap), "nat_usage")
+            summary = {k: int(s[0][k]) for k in bng_nat_usage_sum.names}
+            if cap is not None or summary["pubs_found"] <= pub_cap:
+                break
+            pub_cap = summary["pubs_found"]  # more public addresses than the first guess: ask again with room for all
+        ks, kp = min(summary["subs_found"], sub_cap), min(summary["pubs_found"], pub_cap)
+        sa, so, pa, po = sa[:ks], so[:ks], pa[:kp], po[:kp]
+        os_, op = np.argsort(sa.byteswap(), kind="stable"), np.argsort(pa.byteswap(), kind="stable")
+        return summary, sa[os_], so[os_], pa[op], po[op]
 
     # ---- lawful intercept: content of communication ----
     def li_configure(self, snaplen: int = 0, capacity: int = 0):

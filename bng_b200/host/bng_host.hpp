@@ -1062,6 +1062,120 @@ struct Allocation { // :161-169
     int PoolIndex = 0;
     uint32_t SubscriberID = 0;
     uint64_t AllocatedAtNs = 0;
+    uint32_t PortsInUse = 0; // PortBlock.PortsInUse: in_use_any of the last PortUsage census that reported the subscriber
+};
+
+// NAT port-usage census (bng_nat_usage): the summary and the records of one context, or merged over a shard::Router.
+struct PortUsageReport {
+    bng_nat_usage_sum Summary{};
+    std::vector<uint32_t> SubAddrs; // subscriber addresses (key byte order), index-aligned with Subs
+    std::vector<bng_nat_sub_use> Subs;
+    std::vector<uint32_t> PubAddrs; // public addresses (key byte order), index-aligned with Pubs
+    std::vector<bng_nat_pub_use> Pubs;
+};
+// the census of every subscriber at or above min_permille and of every public address
+using UsageFn = std::function<int(uint32_t min_permille, PortUsageReport *out)>;
+
+// bng_nat_usage on one context, with room for every record (the call is repeated with larger buffers while it finds more)
+inline int ContextPortUsage(bng_ctx *c, uint32_t min_permille, PortUsageReport *out) {
+    uint64_t sub_cap = std::max<uint64_t>(out->SubAddrs.capacity(), 64), pub_cap = std::max<uint64_t>(out->PubAddrs.capacity(), 64);
+    for (;;) {
+        out->SubAddrs.resize(sub_cap);
+        out->Subs.resize(sub_cap);
+        out->PubAddrs.resize(pub_cap);
+        out->Pubs.resize(pub_cap);
+        int rc = bng_nat_usage(c, min_permille, &out->Summary, out->SubAddrs.data(), out->Subs.data(), sub_cap, out->PubAddrs.data(),
+                               out->Pubs.data(), pub_cap);
+        if (rc) return rc;
+        if (out->Summary.subs_found <= sub_cap && out->Summary.pubs_found <= pub_cap) break;
+        sub_cap = std::max(sub_cap, out->Summary.subs_found);
+        pub_cap = std::max(pub_cap, out->Summary.pubs_found);
+    }
+    out->SubAddrs.resize(out->Summary.subs_found);
+    out->Subs.resize(out->Summary.subs_found);
+    out->PubAddrs.resize(out->Summary.pubs_found);
+    out->Pubs.resize(out->Summary.pubs_found);
+    return 0;
+}
+
+// The larger of the per-protocol in_use counts over block_ports, in 1/1000 (0 without ports): bng_nat_sub_use.permille,
+// and the same rule for a public address.
+inline uint32_t Permille(const uint32_t in_use[3], uint64_t block_ports) {
+    const uint64_t mx = std::max(in_use[0], std::max(in_use[1], in_use[2]));
+    return block_ports ? (uint32_t)(mx * 1000 / block_ports) : 0;
+}
+
+// Port-utilisation monitoring on the metrics ticker (FEATURES.md §5 and §9; the reference declares the gauges
+// bng_nat_ports_used{public_ip} and bng_nat_bindings_active, metrics.SetNATPortsUsed / SetNATBindings, and never sets
+// them).  Each Tick runs one census and
+//   - sets PortsUsed(public address, in_use_any) for every public address and Bindings(live sessions);
+//   - raises an alert for a subscriber or a public address each time its permille crosses warn_permille or
+//     crit_permille upwards: once per crossing, not on every tick it stays above (a fall below re-arms the level).
+struct UsageMonitorConfig {
+    uint32_t warn_permille = 800; // FEATURES.md §9: alert at > 80 % ...
+    uint32_t crit_permille = 900; // ... and > 90 %
+};
+enum class UsageLevel { Ok = 0, Warning = 1, Critical = 2 };
+struct UsageAlert {
+    bool Public = false; // a public address (else a subscriber)
+    uint32_t Addr = 0;   // key byte order
+    UsageLevel Level = UsageLevel::Ok;
+    uint32_t Permille = 0;
+    uint32_t Unreachable = 0; // the subscriber's / address's unreachable sessions at the time
+};
+using PortsUsedFn = std::function<void(uint32_t public_addr, uint32_t ports_used)>; // SetNATPortsUsed
+using BindingsFn = std::function<void(uint64_t bindings)>;                          // SetNATBindings
+using AlertFn = std::function<void(const UsageAlert &)>;
+
+class UsageMonitor {
+  public:
+    using Config = UsageMonitorConfig;
+    UsageMonitor(UsageFn usage, PortsUsedFn ports_used, BindingsFn bindings, AlertFn alert, Config cfg = Config())
+        : usage_(std::move(usage)), ports_used_(std::move(ports_used)), bindings_(std::move(bindings)), alert_(std::move(alert)),
+          cfg_(cfg) {}
+
+    // One tick.  Only the subscribers at or above the warning level are copied out of the census.
+    Result<PortUsageReport> Tick() {
+        Result<PortUsageReport> r;
+        PortUsageReport u;
+        if ((r.err = MapErr("bng_nat_usage", usage_(cfg_.warn_permille, &u)))) return r;
+        for (size_t i = 0; i < u.PubAddrs.size(); i++) ports_used_(u.PubAddrs[i], u.Pubs[i].in_use_any);
+        bindings_(u.Summary.sessions);
+        std::map<uint32_t, UsageLevel> subs, pubs;
+        for (size_t i = 0; i < u.SubAddrs.size(); i++)
+            Step(false, u.SubAddrs[i], u.Subs[i].permille, u.Subs[i].unreachable, sub_level_, &subs);
+        for (size_t i = 0; i < u.PubAddrs.size(); i++)
+            Step(true, u.PubAddrs[i], Permille(u.Pubs[i].in_use, u.Pubs[i].block_ports), u.Pubs[i].unreachable, pub_level_, &pubs);
+        sub_level_.swap(subs); // an address missing from this census is below the warning level again
+        pub_level_.swap(pubs);
+        r.value = std::move(u);
+        return r;
+    }
+    UsageLevel SubscriberLevel(uint32_t addr) const { return Get(sub_level_, addr); }
+    UsageLevel PublicLevel(uint32_t addr) const { return Get(pub_level_, addr); }
+
+  private:
+    UsageLevel LevelOf(uint32_t permille) const {
+        return permille >= cfg_.crit_permille ? UsageLevel::Critical : permille >= cfg_.warn_permille ? UsageLevel::Warning : UsageLevel::Ok;
+    }
+    static UsageLevel Get(const std::map<uint32_t, UsageLevel> &m, uint32_t a) {
+        auto it = m.find(a);
+        return it == m.end() ? UsageLevel::Ok : it->second;
+    }
+    void Step(bool pub, uint32_t addr, uint32_t permille, uint32_t unreachable, const std::map<uint32_t, UsageLevel> &before,
+              std::map<uint32_t, UsageLevel> *now) {
+        const UsageLevel l = LevelOf(permille);
+        if (l == UsageLevel::Ok) return;
+        (*now)[addr] = l;
+        if (l > Get(before, addr)) alert_(UsageAlert{pub, addr, l, permille, unreachable});
+    }
+
+    UsageFn usage_;
+    PortsUsedFn ports_used_;
+    BindingsFn bindings_;
+    AlertFn alert_;
+    Config cfg_;
+    std::map<uint32_t, UsageLevel> sub_level_, pub_level_;
 };
 struct ManagerConfig { // :172-200
     std::string Interface, BPFPath;
@@ -1224,6 +1338,33 @@ class Manager {
         }
         return MapErr("bng_nat_flush", bng_nat_flush(be_->ctx, keys.data(), keys.size(), now_ns, removed_out));
     }
+    // Not in the reference: the port-usage census of this manager's dataplane (bng_nat_usage).  It also keeps each
+    // reported subscriber's in_use_any for GetAllocation's PortsInUse (with min_permille 0 every subscriber's).
+    Result<PortUsageReport> PortUsage(uint32_t min_permille = 0) {
+        Result<PortUsageReport> r;
+        if (!be_ || !be_->ctx) {
+            r.err = Error("dataplane not open");
+            return r;
+        }
+        PortUsageReport u;
+        if ((r.err = MapErr("bng_nat_usage", ContextPortUsage(be_->ctx, min_permille, &u)))) return r;
+        {
+            std::lock_guard<std::mutex> g(allocMu_);
+            if (min_permille == 0) portsInUse_.clear();
+            for (size_t i = 0; i < u.SubAddrs.size(); i++) portsInUse_[u.SubAddrs[i]] = u.Subs[i].in_use_any;
+        }
+        r.value = std::move(u);
+        return r;
+    }
+    // PortUsage as a UsageMonitor's census (the monitor then keeps GetAllocation's PortsInUse of the subscribers it sees)
+    UsageFn UsageSource() {
+        return [this](uint32_t min_permille, PortUsageReport *out) {
+            Result<PortUsageReport> r = PortUsage(min_permille);
+            if (r.err) return -EIO;
+            *out = std::move(*r.value);
+            return 0;
+        };
+    }
     Error ConfigureALG(uint16_t port, uint8_t protocol, uint8_t algType, bool enabled) { // :542-560
         if (algPorts_ < 0) return Error("ALG map not loaded");
         uint32_t key = ((uint32_t)port << 16) | protocol;
@@ -1299,7 +1440,12 @@ class Manager {
         std::lock_guard<std::mutex> g(allocMu_);
         auto it = allocations_.find(ebpf::IPToUint32(privateIP));
         if (it == allocations_.end()) return std::nullopt;
-        return it->second;
+        Allocation a = it->second;
+        if (be_) {
+            auto u = portsInUse_.find(be_->AddrKey(it->first));
+            if (u != portsInUse_.end()) a.PortsInUse = u->second;
+        }
+        return a;
     }
     Result<EIMMapping> GetEIMMapping(const IP &internalIP, uint16_t internalPort, uint8_t protocol) { // :767-784
         Result<EIMMapping> r;
@@ -1369,6 +1515,7 @@ class Manager {
     std::mutex poolMu_, allocMu_, idMu_;
     std::vector<PoolEntry> pool_;
     std::map<uint32_t, Allocation> allocations_;
+    std::map<uint32_t, uint32_t> portsInUse_; // subscriber address (key byte order) -> in_use_any of the last census
     uint32_t nextSubscriberID_ = 1;
     std::map<uint32_t, uint32_t> subscriberIDs_;
 };

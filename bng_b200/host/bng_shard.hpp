@@ -366,6 +366,44 @@ class Router {
         }
         return 0;
     }
+    // NAT port-usage census (bng_nat_usage) over every shard.  Each shard counts its own tables: a subscriber's record
+    // comes from the shard that holds its subscriber_nat entry (its owner), public-address records are merged by address
+    // with every field summed, and the summaries are summed.  A triple held on two shards (overlapping blocks, DESIGN.md
+    // §8) counts once per shard.
+    int NatUsage(uint32_t min_permille, nat::PortUsageReport *out) {
+        if (!out) return -EINVAL;
+        std::vector<nat::PortUsageReport> parts(shards_.size());
+        for (size_t k = 0; k < shards_.size(); k++)
+            if (int r = nat::ContextPortUsage(shards_[k]->ctx, min_permille, &parts[k])) return r;
+        *out = MergeNatUsage(parts);
+        return 0;
+    }
+    static nat::PortUsageReport MergeNatUsage(const std::vector<nat::PortUsageReport> &parts) {
+        nat::PortUsageReport m;
+        std::map<uint32_t, bng_nat_pub_use> pubs;
+        for (const auto &p : parts) {
+            const uint64_t *a = (const uint64_t *)&p.Summary;
+            uint64_t *s = (uint64_t *)&m.Summary;
+            for (size_t i = 0; i < sizeof(bng_nat_usage_sum) / 8; i++) s[i] += a[i];
+            m.SubAddrs.insert(m.SubAddrs.end(), p.SubAddrs.begin(), p.SubAddrs.end());
+            m.Subs.insert(m.Subs.end(), p.Subs.begin(), p.Subs.end());
+            for (size_t i = 0; i < p.PubAddrs.size(); i++) {
+                auto ins = pubs.emplace(p.PubAddrs[i], p.Pubs[i]);
+                if (ins.second) continue;
+                bng_nat_pub_use &t = ins.first->second;
+                const bng_nat_pub_use &u = p.Pubs[i];
+                t.sessions += u.sessions, t.eim += u.eim, t.block_ports += u.block_ports, t.blocks += u.blocks;
+                for (int c = 0; c < 3; c++) t.in_use[c] += u.in_use[c];
+                t.in_use_any += u.in_use_any, t.unreachable += u.unreachable;
+            }
+        }
+        for (auto &kv : pubs) m.PubAddrs.push_back(kv.first), m.Pubs.push_back(kv.second);
+        m.Summary.pubs_found = pubs.size();
+        return m;
+    }
+    nat::UsageFn NatUsageSource() {
+        return [this](uint32_t min_permille, nat::PortUsageReport *out) { return NatUsage(min_permille, out); };
+    }
     idle::TimeoutSetFn IdleTimeoutSetter() {
         return [this](const uint32_t *a, const uint32_t *t, uint64_t n, int32_t *res) { return IdleTimeoutSet(a, t, n, res); };
     }

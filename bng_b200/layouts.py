@@ -127,6 +127,18 @@ bng_li_record = np.dtype([
     ("ts_ns", "<u8"), ("batch", "<u8"), ("frame", "<u4"), ("target_id", "<u4"), ("addr", "<u4"), ("wire_len", "<u4"),
     ("cap_len", "<u4"), ("dir", "u1"), ("verdict", "u1"), ("prog", "u1"), ("pad", "u1", 25)])
 
+# include/bng_b200.h NAT port-usage census (bng_nat_usage): per-subscriber record, per-public-address record, summary
+bng_nat_sub_use = np.dtype([
+    ("sessions", "<u8"), ("eim", "<u8"), ("public_ip", "<u4"), ("block_ports", "<u4"), ("in_use", "<u4", 3),
+    ("in_use_any", "<u4"), ("outside", "<u4"), ("unreachable", "<u4"), ("permille", "<u4"), ("pad", "<u4", 3)])
+bng_nat_pub_use = np.dtype([
+    ("sessions", "<u8"), ("eim", "<u8"), ("block_ports", "<u8"), ("blocks", "<u4"), ("in_use", "<u4", 3),
+    ("in_use_any", "<u4"), ("unreachable", "<u4"), ("pad", "<u4", 4)])
+bng_nat_usage_sum = np.dtype([(n, "<u8") for n in (
+    "subscribers", "sessions", "eim", "triples", "unreachable", "stale_reverse", "orphan_sessions", "orphan_eim",
+    "subs_found", "pubs_found")])
+
+assert bng_nat_sub_use.itemsize == 64 and bng_nat_pub_use.itemsize == 64 and bng_nat_usage_sum.itemsize == 80
 assert subscriber_binding.itemsize == 24 and token_bucket.itemsize == 32 and bng_acct.itemsize == 64
 assert bng_li_record.itemsize == 64
 assert bng_idle.itemsize == 32

@@ -396,6 +396,67 @@ int bng_idle_read(bng_ctx *ctx, const uint32_t *addrs, uint64_t n, bng_idle *out
 int64_t bng_idle_scan(bng_ctx *ctx, uint64_t now_ns, uint32_t default_s, uint32_t flags, uint32_t *addrs_out, bng_idle *out,
                       uint64_t cap);
 
+/* ---- NAT port-usage census (port utilisation per subscriber and per public address; FEATURES.md §5, §9) ----
+ * One read-only GPU pass over the NAT tables, read in ABI layout as bng_map_dump returns them.
+ *   - Held triple.  Every live nat_sessions entry holds (nat_ip, ntohs(nat_port), protocol): the session's nat_port is
+ *     in network order.  Every live eim_table entry holds (external_ip, external_port, key.protocol): external_port is
+ *     in host order, the order of port_start / port_end.
+ *   - Attributed address: a session's key src_ip, an EIM entry's key internal_ip (bng_nat_flush's attribution).
+ *   - Protocol columns: [0] TCP (6), [1] UDP (17), [2] ICMP (1).  Other protocol bytes count in the totals and in
+ *     *_any, in no column.
+ *   - Unreachable session: a live session whose reverse key (src_ip = key.dst_ip, dst_ip = nat_ip, src_port =
+ *     key.dst_port, dst_port = nat_port, protocol = the session's protocol, pad 0), as nat44_egress builds it, has no
+ *     nat_reverse entry, or one whose value is not this session's key.  The reference allocator can hand out a
+ *     (port, remote endpoint) pair that a live session of another internal endpoint still holds once a block wraps;
+ *     the newer session then owns the reverse entry and the older one's return traffic goes to the wrong host.
+ *   - Stale reverse entry: a live nat_reverse entry whose value is not the key of a live session.
+ * Per-subscriber record: one per subscriber_nat entry; its block B = (public_ip, [port_start, port_end]) and
+ * block_ports = port_end >= port_start ? port_end - port_start + 1 : 0.
+ * Per-public-address record: one per address that is some subscriber_nat entry's block.public_ip or the public IP of
+ * some held triple.  Addresses are 4 bytes in key byte order (as bng_acct_read takes them).
+ * A subscriber record qualifies when permille >= min_permille (0 reports every subscriber); every public-address record
+ * qualifies.  The call writes min(found, cap) records of each kind, in no particular order; calling it again with
+ * nothing run in between gives the same answer.  Staged upserts are applied first and the census sees everything
+ * queued on the context's stream; it returns synchronised.  It writes no map byte, counter, event, accounting, idle or
+ * interception state, does not advance the batch sequence, and gives a following bng_delta_export nothing to send.
+ * -EINVAL for a NULL ctx or sum, min_permille > 1000, or a cap > 0 with NULL outputs.
+ * Memory: the first call allocates the census's scratch, kept until bng_close: a set of 8-byte words, the power of two
+ * >= 16/3 x (max_nat_sessions + max_eim_mappings) (256 MiB at the default capacities), 32 bytes per subscriber-directory
+ * slot (64 MiB at the default 1e6 subscribers), a public-address table of 48 bytes per slot (3 MiB; it grows when more
+ * than 32768 public addresses are seen), and room for the records the caps ask for.  A context that never calls
+ * bng_nat_usage allocates none of it and launches nothing more.
+ * In a sharded deployment each shard counts its own tables: a triple held on two shards (overlapping blocks) counts
+ * once per shard. */
+typedef struct bng_nat_sub_use {  /* 64 bytes */
+    uint64_t sessions;            /* live sessions attributed to the address */
+    uint64_t eim;                 /* live EIM entries attributed to the address */
+    uint32_t public_ip;           /* block.public_ip */
+    uint32_t block_ports;
+    uint32_t in_use[3];           /* distinct ports p in the block such that the address holds (public_ip, p, proto) */
+    uint32_t in_use_any;          /* distinct ports p in the block held by the address with any protocol */
+    uint32_t outside;             /* distinct triples the address holds outside B (other public IP, or port out of range) */
+    uint32_t unreachable;         /* its unreachable sessions */
+    uint32_t permille;            /* floor(max(in_use[0..2]) * 1000 / block_ports); 0 when block_ports == 0 */
+    uint32_t pad[3];              /* zero */
+} bng_nat_sub_use;
+typedef struct bng_nat_pub_use {  /* 64 bytes */
+    uint64_t sessions, eim;       /* live entries holding a triple on it */
+    uint64_t block_ports;         /* sum of block_ports of the subscriber_nat entries whose block is on it */
+    uint32_t blocks;              /* those entries */
+    uint32_t in_use[3], in_use_any; /* distinct ports held on it, per protocol / any protocol */
+    uint32_t unreachable;         /* unreachable sessions whose nat_ip is it */
+    uint32_t pad[4];              /* zero */
+} bng_nat_pub_use;
+typedef struct bng_nat_usage_sum {
+    uint64_t subscribers;                 /* subscriber_nat entries */
+    uint64_t sessions, eim, triples;      /* live entries; distinct held triples */
+    uint64_t unreachable, stale_reverse;
+    uint64_t orphan_sessions, orphan_eim; /* attributed to an address without a subscriber_nat entry (released, not flushed) */
+    uint64_t subs_found, pubs_found;      /* records that qualified (may exceed the caps) */
+} bng_nat_usage_sum;
+int bng_nat_usage(bng_ctx *ctx, uint32_t min_permille, bng_nat_usage_sum *sum, uint32_t *sub_addrs, bng_nat_sub_use *sub_out,
+                  uint64_t sub_cap, uint32_t *pub_addrs, bng_nat_pub_use *pub_out, uint64_t pub_cap);
+
 /* ---- diagnostics ---- */
 uint64_t bng_launch_count(bng_ctx *ctx);  /* kernels launched by this context so far */
 uint64_t bng_lru_overflow(bng_ctx *ctx);  /* inserts that found no victim to evict in a full LRU map (should stay 0) */
