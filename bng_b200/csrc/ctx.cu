@@ -122,6 +122,15 @@ struct bng_ctx {
     u32 nu_set_mask = 0, nu_pub_mask = 0;
     u8 *nu_out = nullptr; // grow-only: the qualifying records and their addresses
     u64 nu_out_bytes = 0;
+    // DHCP lease census and sweep (leases.cu): scratch allocated by the first call that needs it
+    u64 *ls_set = nullptr, *ls_pools = nullptr, *ls_sum = nullptr; // the census's (ls_sum != null), kernels.h: LeaseUse
+    u32 ls_set_mask = 0, ls_unk_mask = 0;
+    u8 *ls_out = nullptr; // grow-only: the records of either call, then the census's pool ids
+    u64 ls_out_bytes = 0;
+    u64 *ls_macs = nullptr; // grow-only: the sweep's words (LS_W_WORDS), then its MAC set
+    u64 ls_mac_slots = 0;
+    u32 ls_wire = 0; // bng_dhcp_lease_addr_order
+    u64 lease_rebuilds = 0; // rebuilds of the lease maps and circuit_id_map (not part of `rebuilds`)
     u64 seq = 0; // the batch sequence in 64 bits (dev.batch_seq holds its low 32): bng_li_record.batch
     // lawful intercept (bng_li_*, li.cu): allocated by the first bng_li_configure / bng_li_target_set (li_ctl != null)
     u64 *li_ctl = nullptr;   // device: LiRing::ctl
@@ -542,7 +551,8 @@ int bng_close(bng_ctx *c) {
         Scratch &s = c->L.s;
         void *sp[] = {s.key_a, s.key_b, s.val_a, s.val_b, s.qslot, s.attr, s.cub_tmp, s.counters, c->acct_dump_buf, c->idle_scan_buf, c->li_ring, c->li_match,
                       c->io_dev, c->hb_pkts, c->hb_off, c->hb_len, c->hb_prio, c->hb_verdict, c->hb_now, c->dump_k, c->dump_v, c->dump_c,
-                      c->dlist, c->dsent, c->demit, c->nu_set, c->nu_pub, c->nu_sum, c->nu_sub, c->nu_out};
+                      c->dlist, c->dsent, c->demit, c->nu_set, c->nu_pub, c->nu_sum, c->nu_sub, c->nu_out,
+                      c->ls_set, c->ls_pools, c->ls_sum, c->ls_out, c->ls_macs};
         for (void *p : sp)
             if (p) cudaFree(p);
         for (auto &s : c->dshadow) cudaFree(s.words);
@@ -1424,7 +1434,7 @@ void *bng_stream(bng_ctx *c) { return c ? (void *)c->L.stream : nullptr; }
 // Rebuilds a hash table in place (same capacity): what deletes, expiry and eviction left as tombstones is gone and
 // every probe chain is as short as the load factor allows.  Only for tables nothing else indexes by slot number
 // (the NAT flow tables; subscriber_nat / qos_ingress slots are referenced by the subscriber directory).
-static int table_rebuild_locked(bng_ctx *c, Tbl *t) {
+static int table_rebuild_locked(bng_ctx *c, Tbl *t, bool flow = true) {
     Tbl nw = *t;
     nw.lru = LRU_NONE;
     nw.max_entries = nw.mask; // the copy must never refuse or evict
@@ -1450,7 +1460,7 @@ static int table_rebuild_locked(bng_ctx *c, Tbl *t) {
         if (p == t->slots) p = nw.slots;
     cudaFree(t->slots);
     t->slots = nw.slots;
-    c->rebuilds++;
+    (flow ? c->rebuilds : c->lease_rebuilds)++;
     return 0;
 }
 
@@ -1994,6 +2004,164 @@ int bng_nat_usage(bng_ctx *c, uint32_t min_permille, bng_nat_usage_sum *sum, uin
     memcpy(sum, sum_w, sizeof(*sum));
     return 0;
 }
+
+// ---------------------------------------------------------------------------
+// DHCP lease census and expiry sweep (leases.cu)
+// ---------------------------------------------------------------------------
+static_assert(sizeof(bng_lease_pool_use) == 64 && sizeof(bng_lease_removed) == 64, "the lease kernels write 16 u32 per record");
+static_assert(sizeof(bng_lease_sum) == (LS_POOLS_FOUND + 1) * 8, "struct bng_lease_sum is the head of the census's sum words");
+
+static int ls_malloc(bng_ctx *c, void **p, size_t bytes, const char *what) {
+    if (cudaMalloc(p, bytes) != cudaSuccess) {
+        cudaGetLastError();
+        *p = nullptr;
+        return fail(c, -ENOMEM, "dhcp leases: %zu bytes of device memory for the %s", bytes, what);
+    }
+    return 0;
+}
+
+// the output records of either call (and the census's pool ids behind them): grow-only
+static int ls_out_locked(bng_ctx *c, u64 bytes) {
+    if (bytes <= c->ls_out_bytes) return 0;
+    if (c->ls_out) cudaFree(c->ls_out);
+    c->ls_out_bytes = 0;
+    if (int r = ls_malloc(c, (void **)&c->ls_out, bytes, "records")) return r;
+    c->ls_out_bytes = bytes;
+    return 0;
+}
+
+// leases.cu reads the lease slots by fixed offsets
+static int ls_layout_locked(bng_ctx *c) {
+    const DevCtx &d = c->dev;
+    if (d.sub_pools.slot_bytes != 64 || d.vlan_pools.slot_bytes != 64 || d.cid_subs.slot_bytes != 64 || d.sub_pools.voff != 8 ||
+        d.vlan_pools.voff != 8 || d.cid_subs.voff != 32)
+        return fail(c, -EINVAL, "dhcp leases: unexpected slot layout of the lease maps");
+    return 0;
+}
+
+// pool records: one per ip_pools slot, then the hash of unknown pool_ids (unk_slots of them)
+static int ls_pools_alloc(bng_ctx *c, u64 unk_slots) {
+    const u64 n = (u64)c->dev.ip_pools.mask + 1 + unk_slots;
+    if (n > (1ull << 26)) return fail(c, -ENOMEM, "lease_census: %llu pool records", (unsigned long long)n);
+    u64 *p = nullptr; // the old records stay when the new ones do not fit
+    if (int r = ls_malloc(c, (void **)&p, n * LS_POOL_WORDS * 8, "pool records")) return r;
+    if (c->ls_pools) cudaFree(c->ls_pools);
+    c->ls_pools = p;
+    c->ls_unk_mask = (u32)(unk_slots - 1);
+    return 0;
+}
+
+// The census's scratch, on first use (kernels.h: LeaseUse).  All of it or none.
+static int ls_alloc_locked(bng_ctx *c) {
+    if (c->ls_sum) return 0;
+    const u64 keys = 3ull * ((u64)c->dev.sub_pools.max_entries + c->dev.vlan_pools.max_entries + c->dev.cid_subs.max_entries);
+    const u64 set_slots = nu_pow2((keys * 4 + 2) / 3);
+    if (set_slots > (1ull << 32)) return fail(c, -ENOMEM, "lease_census: %llu set slots", (unsigned long long)set_slots);
+    int r = ls_malloc(c, (void **)&c->ls_set, set_slots * 8, "address set");
+    if (!r) r = ls_pools_alloc(c, 1u << 14);
+    if (!r) r = ls_malloc(c, (void **)&c->ls_sum, LS_SUM_WORDS * 8, "summary");
+    if (r) {
+        for (void *p : {(void *)c->ls_set, (void *)c->ls_pools})
+            if (p) cudaFree(p);
+        c->ls_set = c->ls_pools = nullptr;
+        return r;
+    }
+    c->ls_set_mask = (u32)(set_slots - 1);
+    return 0;
+}
+
+int bng_dhcp_lease_census(bng_ctx *c, uint64_t now_ns, bng_lease_sum *sum, uint32_t *pool_ids, bng_lease_pool_use *out, uint64_t cap) {
+    if (!c || !sum || (cap && (!pool_ids || !out))) return -EINVAL;
+    std::lock_guard<std::mutex> g(c->mu);
+    cudaSetDevice(c->device);
+    int r = flush_staged_locked(c, -1);
+    if (r) return r;
+    if ((r = ls_layout_locked(c)) != 0 || (r = ls_alloc_locked(c)) != 0) return r;
+    u64 sum_w[LS_SUM_WORDS];
+    for (;;) {
+        LeaseUse u{};
+        u.set = c->ls_set, u.set_mask = c->ls_set_mask, u.unk_mask = c->ls_unk_mask, u.n_known = c->dev.ip_pools.mask + 1;
+        u.pools = c->ls_pools, u.sum = c->ls_sum, u.wire = c->ls_wire;
+        const u64 recs = (u64)u.n_known + u.unk_mask + 1;
+        u.cap = std::min<u64>(cap, recs); // no more records than record slots
+        if ((r = ls_out_locked(c, u.cap * 68)) != 0) return r;
+        u.out = (u32 *)c->ls_out, u.ids_out = (u32 *)(c->ls_out + u.cap * 64);
+        CU(c, cudaMemsetAsync(c->ls_set, 0, ((u64)c->ls_set_mask + 1) * 8, c->L.stream));
+        CU(c, cudaMemsetAsync(c->ls_pools, 0, recs * LS_POOL_WORDS * 8, c->L.stream));
+        CU(c, cudaMemsetAsync(c->ls_sum, 0, LS_SUM_WORDS * 8, c->L.stream));
+        CU(c, run_lease_census(c->L, c->dev, u, now_ns / 1000000000ull));
+        CU(c, cudaMemcpyAsync(sum_w, c->ls_sum, sizeof(sum_w), cudaMemcpyDeviceToHost, c->L.stream));
+        CU(c, cudaStreamSynchronize(c->L.stream));
+        if (sum_w[LS_SET_FULL]) return fail(c, -EIO, "lease_census: the address set is full");
+        if (sum_w[LS_OVERFLOW]) { // more unknown pool_ids than half the hash: grow it past the claims and count again
+            prof_collect(c->L);
+            if ((r = ls_pools_alloc(c, nu_pow2(4 * sum_w[LS_UNK_CLAIMED]))) != 0) return r;
+            continue;
+        }
+        CU(c, run_lease_pools(c->L, c->dev, u));
+        CU(c, cudaMemcpyAsync(sum_w, c->ls_sum, sizeof(sum_w), cudaMemcpyDeviceToHost, c->L.stream));
+        CU(c, cudaStreamSynchronize(c->L.stream));
+        prof_collect(c->L);
+        if (const u64 n = std::min<u64>(sum_w[LS_POOLS_FOUND], u.cap)) {
+            CU(c, cudaMemcpy(out, u.out, n * 64, cudaMemcpyDeviceToHost));
+            CU(c, cudaMemcpy(pool_ids, u.ids_out, n * 4, cudaMemcpyDeviceToHost));
+        }
+        break;
+    }
+    memcpy(sum, sum_w, sizeof(*sum));
+    return 0;
+}
+
+int64_t bng_dhcp_lease_sweep(bng_ctx *c, uint64_t now_ns, uint32_t grace_s, bng_lease_removed *out, uint64_t cap, uint64_t removed_out[4]) {
+    if (!c || (cap && !out)) return -EINVAL;
+    if (removed_out) removed_out[0] = removed_out[1] = removed_out[2] = removed_out[3] = 0;
+    std::lock_guard<std::mutex> g(c->mu);
+    cudaSetDevice(c->device);
+    int r = flow_pass_begin_locked(c);
+    if (r) return r;
+    if ((r = ls_layout_locked(c)) != 0) return r;
+    DevCtx &d = c->dev;
+    // no more entries can be due than the three maps hold
+    const u64 ecap = std::min<u64>(cap, (u64)d.sub_pools.max_entries + d.vlan_pools.max_entries + d.cid_subs.max_entries);
+    const u64 mac_slots = nu_pow2(2 * std::min<u64>(ecap, d.sub_pools.max_entries));
+    if (mac_slots > (1ull << 32)) return fail(c, -ENOMEM, "lease_sweep: %llu MAC set slots", (unsigned long long)mac_slots);
+    if ((r = ls_out_locked(c, ecap * 64)) != 0) return r;
+    if (mac_slots > c->ls_mac_slots) {
+        if (c->ls_macs) cudaFree(c->ls_macs);
+        c->ls_mac_slots = 0;
+        if ((r = ls_malloc(c, (void **)&c->ls_macs, (LS_W_WORDS + mac_slots) * 8, "MAC set")) != 0) return r;
+        c->ls_mac_slots = mac_slots;
+    }
+    LeaseSweep w{};
+    w.now_s = now_ns / 1000000000ull, w.grace_s = grace_s, w.cap = ecap;
+    w.out = (u32 *)c->ls_out, w.cnt = c->ls_macs, w.macs = c->ls_macs + LS_W_WORDS, w.mac_mask = (u32)(mac_slots - 1);
+    CU(c, cudaMemsetAsync(c->ls_macs, 0, (LS_W_WORDS + mac_slots) * 8, c->L.stream));
+    CU(c, run_lease_sweep(c->L, d, w));
+    u64 cnt[LS_W_WORDS];
+    CU(c, cudaMemcpyAsync(cnt, w.cnt, sizeof(cnt), cudaMemcpyDeviceToHost, c->L.stream));
+    CU(c, cudaStreamSynchronize(c->L.stream));
+    prof_collect(c->L);
+    if (cnt[LS_W_SET_FULL]) return fail(c, -EIO, "lease_sweep: the MAC set is full");
+    if (cnt[LS_W_LOST]) return fail(c, -EIO, "lease_sweep: a due entry changed under the sweep");
+    if (const u64 n = std::min<u64>(cnt[LS_W_FOUND], ecap)) CU(c, cudaMemcpy(out, w.out, n * 64, cudaMemcpyDeviceToHost));
+    if (removed_out) memcpy(removed_out, cnt + LS_W_REMOVED, 4 * 8);
+    // A mass expiry tombstones most of a table, and the fast path's probes walk the tombstones.  A dry run changes
+    // nothing, so it rebuilds nothing.  The removals stand and are reported even when a rebuild finds no memory: the
+    // table it could not rebuild stays as it was and the next sweep tries again (bng_last_error has the text).
+    Tbl *tb[4] = {&d.sub_pools, &d.vlan_pools, &d.cid_subs, &d.cid_map};
+    for (int k = 0; k < 4 && ecap; k++)
+        if (cnt[LS_W_TOMBS + k] > ((u64)tb[k]->mask + 1) / 4 && table_rebuild_locked(c, tb[k], false) != 0) break;
+    return (int64_t)cnt[LS_W_FOUND];
+}
+
+int bng_dhcp_lease_addr_order(bng_ctx *c, uint32_t order) {
+    if (!c || order > BNG_LEASE_ADDR_WIRE) return -EINVAL;
+    std::lock_guard<std::mutex> g(c->mu);
+    c->ls_wire = order;
+    return 0;
+}
+
+uint64_t bng_lease_table_rebuilds(bng_ctx *c) { return c ? c->lease_rebuilds : 0; }
 
 // ---------------------------------------------------------------------------
 // lawful intercept (li.cu)

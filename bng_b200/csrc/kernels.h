@@ -160,6 +160,49 @@ cudaError_t run_nat_usage_flows(Launcher &L, const DevCtx &c, const NatUse &u);
 // qualifying subscriber records (permille >= min_permille) and every public-address record, compacted
 cudaError_t run_nat_usage_emit(Launcher &L, const DevCtx &c, const NatUse &u, u32 min_permille);
 
+// DHCP lease census and expiry sweep (leases.cu).  Scratch of the census, zeroed before every census:
+//   set        set_mask + 1 u64 words, 0 = empty.  An unexpired lease entry creates at most three keys (leases.cu), so
+//              3 x (the three lease maps' max_entries) keys fit in the power of two >= 4/3 of that (load <= 3/4).
+//   pools      LS_POOL_WORDS u64 per pool record: n_known records index-aligned with ip_pools' slots, then unk_mask + 1
+//              records of a hash keyed by the pool_ids that have no ip_pools entry (LS_P_KEY: ADDRSET_LIVE | pool_id,
+//              0 = empty).  Record indices are < 2^26.
+//   sum        LS_SUM_WORDS u64: the struct bng_lease_sum fields in order, then the census's own words
+#define LS_POOL_WORDS 8
+enum { LS_P_ENTRIES = 0, LS_P_EXPIRED = 3, LS_P_ADDRS, LS_P_OUTSIDE, LS_P_CONFLICTS, LS_P_KEY };
+#define LS_NONE 0xFFFFFFFFu
+enum {
+    LS_ENT0, LS_ENT1, LS_ENT2, LS_EXP0, LS_EXP1, LS_EXP2, LS_ADDRS, LS_CONFLICTS, LS_UNKNOWN_POOL, LS_CID_DANGLING, // summed per thread
+    LS_POOLS_FOUND,
+    LS_UNK_CLAIMED,  // unknown-pool slots claimed so far (half the hash claimed: overflow)
+    LS_OVERFLOW,     // the unknown-pool hash was too small: grow it and run again
+    LS_SET_FULL,     // the set was full (its sizing rules that out)
+    LS_SUM_WORDS
+};
+#define LS_LOCAL (LS_CID_DANGLING + 1)
+struct LeaseUse {
+    u64 *set;
+    u32 set_mask, unk_mask, n_known;
+    u32 wire; // the prefix test's byte order (bng_dhcp_lease_addr_order)
+    u64 *pools, *sum;
+    u32 *ids_out, *out; // pool ids and records (struct bng_lease_pool_use, 16 u32 each), up to cap
+    u64 cap;
+};
+cudaError_t run_lease_census(Launcher &L, const DevCtx &c, const LeaseUse &u, u64 now_s);
+cudaError_t run_lease_pools(Launcher &L, const DevCtx &c, const LeaseUse &u);
+// The sweep's words (zeroed by the caller): due entries found, entries removed from the three lease maps and from
+// circuit_id_map, tombstones seen in the four tables (its own included), "the MAC set was full" (sized against it) and
+// "a due entry was gone before its erase" (nothing runs beside the sweep); either of the two fails the call.
+enum { LS_W_FOUND = 0, LS_W_REMOVED = 1, LS_W_TOMBS = 5, LS_W_SET_FULL = 9, LS_W_LOST = 10, LS_W_WORDS = 11 };
+struct LeaseSweep {
+    u64 now_s, grace_s, cap;
+    u32 *out;  // struct bng_lease_removed, 16 u32 each, cap of them
+    u64 *cnt;
+    u64 *macs; // mac_mask + 1 words, zeroed: the MACs of the subscriber_pools entries removed (>= 2 x cap slots)
+    u32 mac_mask;
+};
+// removes the due entries whose output slot is below cap, then the circuit_id_map entries that name a removed MAC
+cudaError_t run_lease_sweep(Launcher &L, const DevCtx &c, const LeaseSweep &w);
+
 // lawful intercept (li.cu).  A record is LI_HDR bytes of header (struct bng_li_record) and the captured bytes, zero
 // padded to rec_bytes.  The targets are an AddrSet with target ids index-aligned to its words.
 #define LI_HDR 64

@@ -13,6 +13,7 @@ import os
 import numpy as np
 
 from .layouts import as_bytes, bng_acct, bng_idle, bng_li_record, bng_nat_pub_use, bng_nat_sub_use, bng_nat_usage_sum
+from .layouts import bng_lease_pool_use, bng_lease_removed, bng_lease_sum
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("BNG_B200_LIB") or os.path.join(HERE, "libbng_b200.so")  # override: A/B builds
@@ -121,6 +122,10 @@ def load_library() -> C.CDLL:
         "bng_idle_read": ([vp, vp, u64, vp, vp], i32),
         "bng_idle_scan": ([vp, u64, u32, u32, vp, vp, u64], C.c_int64),
         "bng_nat_usage": ([vp, u32, vp, vp, vp, u64, vp, vp, u64], i32),
+        "bng_dhcp_lease_census": ([vp, u64, vp, vp, vp, u64], i32),
+        "bng_dhcp_lease_sweep": ([vp, u64, u32, vp, u64, vp], C.c_int64),
+        "bng_lease_table_rebuilds": ([vp], u64),
+        "bng_dhcp_lease_addr_order": ([vp, u32], i32),
     }
     for name, (args, res) in protos.items():
         fn = getattr(lib, name)
@@ -142,6 +147,7 @@ EXPORTED_SYMBOLS = (
     "bng_li_configure", "bng_li_record_size", "bng_li_target_set", "bng_li_target_del", "bng_li_drain", "bng_li_lost",
     "bng_delta_enable", "bng_delta_export", "bng_delta_apply", "bng_delta_info",
     "bng_idle_enable", "bng_idle_timeout_set", "bng_idle_read", "bng_idle_scan", "bng_nat_usage",
+    "bng_dhcp_lease_census", "bng_dhcp_lease_sweep", "bng_lease_table_rebuilds", "bng_dhcp_lease_addr_order",
 )
 
 
@@ -436,6 +442,48 @@ class Dataplane:
         sa, so, pa, po = sa[:ks], so[:ks], pa[:kp], po[:kp]
         os_, op = np.argsort(sa.byteswap(), kind="stable"), np.argsort(pa.byteswap(), kind="stable")
         return summary, sa[os_], so[os_], pa[op], po[op]
+
+    # ---- DHCP lease census and expiry sweep ----
+    def lease_census(self, now_ns: int, cap: int | None = None):
+        """Per-pool utilisation of the DHCP lease maps at now_ns (include/bng_b200.h, bng_dhcp_lease_census).  Returns
+        (summary dict, pool ids u32[k], bng_lease_pool_use[k]) sorted by pool id: every pool, or at most `cap` of them."""
+        room = cap if cap is not None else 64
+        while True:
+            s = np.zeros(1, dtype=bng_lease_sum)
+            ids, out = np.zeros(max(room, 1), "<u4"), np.zeros(max(room, 1), bng_lease_pool_use)
+            self._chk(self.lib.bng_dhcp_lease_census(self.h, now_ns, s.ctypes.data, ids.ctypes.data, out.ctypes.data, room),
+                      "lease_census")
+            summary = {k: (int(s[0][k]) if s[0][k].ndim == 0 else [int(x) for x in s[0][k]]) for k in bng_lease_sum.names}
+            if cap is not None or summary["pools_found"] <= room:
+                break
+            room = summary["pools_found"]  # more pools than the first guess: ask again with room for all
+        k = min(summary["pools_found"], room)
+        o = np.argsort(ids[:k], kind="stable")
+        return summary, ids[:k][o], out[:k][o]
+
+    def lease_sweep(self, now_ns: int, grace_s: int = 0, cap: int | None = None):
+        """Remove the lease entries past lease_expiry + grace_s at now_ns (include/bng_b200.h, bng_dhcp_lease_sweep).
+        Returns (found, bng_lease_removed[k] sorted by (map, key bytes), removed per map [4]).  cap None: one call with
+        room for every entry the three maps hold; else at most `cap` are removed and found may exceed k."""
+        if cap is None:
+            cap = max(sum(int(self.map_info(m)["count"]) for m in
+                          ("subscriber_pools", "vlan_subscriber_pools", "circuit_id_subscribers")), 1)
+        out = np.zeros(max(cap, 1), bng_lease_removed)
+        removed = (C.c_uint64 * 4)()
+        found = self._chk(self.lib.bng_dhcp_lease_sweep(self.h, now_ns, grace_s, out.ctypes.data if cap else None, cap, removed),
+                          "lease_sweep")
+        out = out[:min(found, cap)]
+        o = np.lexsort([out["key"][:, j] for j in range(31, -1, -1)] + [out["map"]])
+        return found, out[o], [int(x) for x in removed]
+
+    def lease_addr_order(self, wire: bool):
+        """How this context's control plane stores allocated_ip and ip_pool.network: the numeric value in a native word
+        (False, the default: the Go loader and the C++ mirror) or the four bytes in wire order (True: synth.py, the
+        test scripts).  The census's prefix test follows it."""
+        self._chk(self.lib.bng_dhcp_lease_addr_order(self.h, 1 if wire else 0), "lease_addr_order")
+
+    def lease_table_rebuilds(self) -> int:
+        return self.lib.bng_lease_table_rebuilds(self.h)
 
     # ---- lawful intercept: content of communication ----
     def li_configure(self, snaplen: int = 0, capacity: int = 0):

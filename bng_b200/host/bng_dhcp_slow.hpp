@@ -229,6 +229,16 @@ class Pool {
                 return;
             }
     }
+    // The allocation of `mac`, if it is `ip`, back to the end of the list; false: the address is not (or no longer) this
+    // client's, and whoever holds it now keeps it.
+    bool ReleaseFor(uint64_t mac, uint32_t ip) {
+        std::lock_guard<std::mutex> g(mu_);
+        auto it = allocated_.find(mac);
+        if (it == allocated_.end() || it->second != ip) return false;
+        allocated_.erase(it);
+        available_.push_back(ip);
+        return true;
+    }
     bool Contains(uint32_t ip) const { return (ip & SubnetMask) == Network; } // :187-189
     PoolStats Stats() { // :205-214
         std::lock_guard<std::mutex> g(mu_);
@@ -441,6 +451,36 @@ class Server {
         std::lock_guard<std::mutex> g(mu_);
         return leases_.size();
     }
+    // cleanupExpiredLeases, :1115-1163, with the expired set taken from the dataplane instead of a walk over the lease
+    // map: the sweep removes the expired fast-path entries of all three lease maps (the reference's RemoveSubscriber
+    // leaves the VLAN and circuit-id entries behind, where they shadow a fresh lease) and reports them; each address
+    // of a removed subscriber_pools entry goes back to its pool and its lease is dropped, unless it was renewed meanwhile.
+    // Loops while the sweep reports more than one call returned.  Returns the entries removed, or a negative errno.
+    int64_t CleanupExpiredLeases(uint64_t now_ns, const ebpf::LeaseSweepFn &sweep, uint64_t batch = 65536) {
+        int64_t total = 0;
+        std::vector<bng_lease_removed> recs;
+        for (;;) {
+            const int64_t found = sweep(now_ns, 0, batch, &recs);
+            if (found < 0) return found;
+            for (const auto &r : recs) {
+                if (r.map != 0) continue; // a VLAN or circuit-id entry: the address stays with the subscriber's lease
+                uint64_t mac;
+                memcpy(&mac, r.key, 8);
+                {
+                    std::lock_guard<std::mutex> g(mu_);
+                    auto it = leases_.find(mac);
+                    if (it != leases_.end()) {
+                        if ((uint64_t)it->second.ExpiresAt > r.lease_expiry) continue; // renewed since: the address is in use
+                        leases_.erase(it);
+                    }
+                }
+                // allocated_ip is the numeric value updateFastPathCache stored (BNG_LEASE_ADDR_NUMERIC)
+                if (auto pool = poolMgr_->GetPool(r.pool_id)) pool->ReleaseFor(mac, r.allocated_ip);
+            }
+            total += (int64_t)recs.size();
+            if ((uint64_t)found <= batch || recs.empty()) return total;
+        }
+    }
     const Error &LastFastPathError() const { return fastPathError_; }
     uint64_t requestsTotal = 0, offersTotal = 0, acksTotal = 0, naksTotal = 0;
 
@@ -496,6 +536,65 @@ class Server {
     std::map<uint64_t, Lease> leases_;
     std::mutex mu_;
     Error fastPathError_;
+};
+
+// Pool-utilisation monitoring on the metrics ticker (FEATURES.md §9: alerts at > 80 % and > 90 % pool utilisation; the
+// gauges bng_pool_utilization_ratio{pool} and bng_dhcp_active_leases of pkg/metrics).  Each Tick runs one lease census and
+//   - sets Utilization(pool id, permille) for every pool ip_pools knows and ActiveLeases(unexpired subscriber_pools
+//     entries);
+//   - raises an alert each time a pool's permille crosses warn_permille or crit_permille upwards: once per crossing,
+//     not on every tick it stays above (a fall below re-arms the level); and one per tick for a pool with conflicts.
+struct PoolMonitorConfig {
+    uint32_t warn_permille = 800, crit_permille = 900;
+};
+enum class PoolLevel { Ok = 0, Warning = 1, Critical = 2 };
+struct PoolAlert {
+    uint32_t PoolID = 0;
+    PoolLevel Level = PoolLevel::Ok; // Ok with Conflicts > 0: an address-conflict alert
+    uint32_t Permille = 0, Conflicts = 0;
+};
+class PoolMonitor {
+  public:
+    using Config = PoolMonitorConfig;
+    using UtilizationFn = std::function<void(uint32_t pool_id, uint32_t permille)>;
+    using ActiveLeasesFn = std::function<void(uint64_t leases)>;
+    using AlertFn = std::function<void(const PoolAlert &)>;
+    PoolMonitor(ebpf::LeaseCensusFn census, UtilizationFn util, ActiveLeasesFn active, AlertFn alert, Config cfg = Config())
+        : census_(std::move(census)), util_(std::move(util)), active_(std::move(active)), alert_(std::move(alert)), cfg_(cfg) {}
+
+    Result<ebpf::LeaseCensusReport> Tick(uint64_t now_ns) {
+        Result<ebpf::LeaseCensusReport> r;
+        ebpf::LeaseCensusReport u;
+        if ((r.err = MapErr("bng_dhcp_lease_census", census_(now_ns, &u)))) return r;
+        active_(u.Summary.entries[0]);
+        std::map<uint32_t, PoolLevel> now;
+        for (size_t i = 0; i < u.PoolIDs.size(); i++) {
+            const bng_lease_pool_use &p = u.Pools[i];
+            if (p.conflicts) alert_(PoolAlert{u.PoolIDs[i], PoolLevel::Ok, p.permille, p.conflicts});
+            if (!p.known) continue;
+            util_(u.PoolIDs[i], p.permille);
+            const PoolLevel l = p.permille >= cfg_.crit_permille ? PoolLevel::Critical
+                                : p.permille >= cfg_.warn_permille ? PoolLevel::Warning : PoolLevel::Ok;
+            if (l == PoolLevel::Ok) continue;
+            now[u.PoolIDs[i]] = l;
+            if (l > Level(u.PoolIDs[i])) alert_(PoolAlert{u.PoolIDs[i], l, p.permille, p.conflicts});
+        }
+        level_.swap(now); // a pool missing from this census is below the warning level again
+        r.value = std::move(u);
+        return r;
+    }
+    PoolLevel Level(uint32_t pool_id) const {
+        auto it = level_.find(pool_id);
+        return it == level_.end() ? PoolLevel::Ok : it->second;
+    }
+
+  private:
+    ebpf::LeaseCensusFn census_;
+    UtilizationFn util_;
+    ActiveLeasesFn active_;
+    AlertFn alert_;
+    Config cfg_;
+    std::map<uint32_t, PoolLevel> level_;
 };
 
 // A client's DISCOVER / REQUEST as the load generator of the reference builds it (test/load/dhcp_benchmark.go:

@@ -455,6 +455,38 @@ inline uint64_t LeaseExpiryFromDuration(std::chrono::seconds d) {
         .count();
 }
 
+// DHCP lease census (bng_dhcp_lease_census): the summary and one record per pool, of one context or merged over a
+// shard::Router.
+struct LeaseCensusReport {
+    bng_lease_sum Summary{};
+    std::vector<uint32_t> PoolIDs; // index-aligned with Pools
+    std::vector<bng_lease_pool_use> Pools;
+};
+using LeaseCensusFn = std::function<int(uint64_t now_ns, LeaseCensusReport *out)>;
+// One sweep call: removes at most `cap` due entries into *out (replaced) and returns the number found, or a negative errno.
+using LeaseSweepFn = std::function<int64_t(uint64_t now_ns, uint32_t grace_s, uint64_t cap, std::vector<bng_lease_removed> *out)>;
+
+// bng_dhcp_lease_census on one context, with room for every pool (repeated with a larger buffer while it finds more)
+inline int ContextLeaseCensus(bng_ctx *c, uint64_t now_ns, LeaseCensusReport *out) {
+    uint64_t cap = std::max<uint64_t>(out->PoolIDs.capacity(), 64);
+    for (;;) {
+        out->PoolIDs.resize(cap);
+        out->Pools.resize(cap);
+        if (int rc = bng_dhcp_lease_census(c, now_ns, &out->Summary, out->PoolIDs.data(), out->Pools.data(), cap)) return rc;
+        if (out->Summary.pools_found <= cap) break;
+        cap = out->Summary.pools_found;
+    }
+    out->PoolIDs.resize(out->Summary.pools_found);
+    out->Pools.resize(out->Summary.pools_found);
+    return 0;
+}
+inline int64_t ContextLeaseSweep(bng_ctx *c, uint64_t now_ns, uint32_t grace_s, uint64_t cap, std::vector<bng_lease_removed> *out) {
+    out->resize(cap);
+    int64_t found = bng_dhcp_lease_sweep(c, now_ns, grace_s, cap ? out->data() : nullptr, cap, nullptr);
+    out->resize(found < 0 ? 0 : std::min<uint64_t>((uint64_t)found, cap));
+    return found;
+}
+
 class Loader {
   public:
     // NewLoader, :110-127.  `bpfPath` is kept for interface compatibility; it selects nothing here.
@@ -598,6 +630,25 @@ class Loader {
         return lookup<PoolAssignment>(circuitIDSubscribers_, "circuit_id_subscribers map not loaded", &k);
     }
     bool HasCircuitIDSubscriberSupport() const { return circuitIDSubscribers_ >= 0; }
+
+    // Not in the reference (its cleanup walks a Go map and deletes by MAC only): the lease census and the expiry sweep
+    // of this loader's dataplane (include/bng_b200.h).  SweepExpired removes at most `cap` due entries per call.
+    Result<LeaseCensusReport> LeaseCensus(uint64_t now_ns) {
+        Result<LeaseCensusReport> r;
+        LeaseCensusReport u;
+        if (!be_ || !be_->ctx) r.err = Error("dataplane not loaded");
+        else if (!(r.err = MapErr("bng_dhcp_lease_census", ContextLeaseCensus(be_->ctx, now_ns, &u)))) r.value = std::move(u);
+        return r;
+    }
+    int64_t SweepExpired(uint64_t now_ns, uint32_t grace_s, uint64_t cap, std::vector<bng_lease_removed> *out) {
+        if (!be_ || !be_->ctx || !out) return -EINVAL;
+        return ContextLeaseSweep(be_->ctx, now_ns, grace_s, cap, out);
+    }
+    LeaseSweepFn SweepSource() {
+        return [this](uint64_t now_ns, uint32_t grace_s, uint64_t cap, std::vector<bng_lease_removed> *out) {
+            return SweepExpired(now_ns, grace_s, cap, out);
+        };
+    }
 
   private:
     Loader() = default;

@@ -401,6 +401,58 @@ class Router {
         m.Summary.pubs_found = pubs.size();
         return m;
     }
+    // DHCP lease census over every shard.  Each shard counts its own tables: pool records are merged by pool_id with the
+    // counts summed (prefix_hosts and known taken from any shard that has them, permille recomputed), and the summaries
+    // are summed.  An address leased on two shards counts once per shard in addrs, and a conflict between two shards'
+    // subscribers is not seen: subscribers are sharded by MAC, so a pool's addresses are spread over the shards.
+    int LeaseCensus(uint64_t now_ns, ebpf::LeaseCensusReport *out) {
+        if (!out) return -EINVAL;
+        std::vector<ebpf::LeaseCensusReport> parts(shards_.size());
+        for (size_t k = 0; k < shards_.size(); k++)
+            if (int r = ebpf::ContextLeaseCensus(shards_[k]->ctx, now_ns, &parts[k])) return r;
+        *out = MergeLeaseCensus(parts);
+        return 0;
+    }
+    static ebpf::LeaseCensusReport MergeLeaseCensus(const std::vector<ebpf::LeaseCensusReport> &parts) {
+        ebpf::LeaseCensusReport m;
+        std::map<uint32_t, bng_lease_pool_use> pools;
+        for (const auto &p : parts) {
+            const uint64_t *a = (const uint64_t *)&p.Summary;
+            uint64_t *s = (uint64_t *)&m.Summary;
+            for (size_t i = 0; i < sizeof(bng_lease_sum) / 8; i++) s[i] += a[i];
+            for (size_t i = 0; i < p.PoolIDs.size(); i++) {
+                auto ins = pools.emplace(p.PoolIDs[i], p.Pools[i]);
+                if (ins.second) continue;
+                bng_lease_pool_use &t = ins.first->second;
+                const bng_lease_pool_use &u = p.Pools[i];
+                for (int c = 0; c < 3; c++) t.entries[c] += u.entries[c];
+                t.expired += u.expired, t.addrs += u.addrs, t.addrs_outside += u.addrs_outside, t.conflicts += u.conflicts;
+                if (u.known) t.known = 1, t.prefix_hosts = u.prefix_hosts;
+            }
+        }
+        for (auto &kv : pools) {
+            bng_lease_pool_use &t = kv.second;
+            t.permille = t.prefix_hosts ? (uint32_t)((uint64_t)(t.addrs - t.addrs_outside) * 1000 / t.prefix_hosts) : 0;
+            m.PoolIDs.push_back(kv.first), m.Pools.push_back(t);
+        }
+        m.Summary.pools_found = pools.size();
+        return m;
+    }
+    // Every shard's sweep, concatenated: at most `cap` entries removed per shard; returns the due entries found over
+    // all shards (repeat while it exceeds what came back).
+    int64_t LeaseSweep(uint64_t now_ns, uint32_t grace_s, uint64_t cap, std::vector<bng_lease_removed> *out) {
+        if (!out) return -EINVAL;
+        out->clear();
+        int64_t total = 0;
+        std::vector<bng_lease_removed> part;
+        for (auto &s : shards_) {
+            int64_t n = ebpf::ContextLeaseSweep(s->ctx, now_ns, grace_s, cap, &part);
+            if (n < 0) return n;
+            total += n;
+            out->insert(out->end(), part.begin(), part.end());
+        }
+        return total;
+    }
     nat::UsageFn NatUsageSource() {
         return [this](uint32_t min_permille, nat::PortUsageReport *out) { return NatUsage(min_permille, out); };
     }

@@ -138,6 +138,19 @@ bng_nat_usage_sum = np.dtype([(n, "<u8") for n in (
     "subscribers", "sessions", "eim", "triples", "unreachable", "stale_reverse", "orphan_sessions", "orphan_eim",
     "subs_found", "pubs_found")])
 
+# include/bng_b200.h DHCP lease census and sweep: per-pool record, summary, removed-entry record
+bng_lease_pool_use = np.dtype([
+    ("entries", "<u8", 3), ("expired", "<u8"), ("addrs", "<u4"), ("addrs_outside", "<u4"), ("conflicts", "<u4"),
+    ("prefix_hosts", "<u4"), ("permille", "<u4"), ("known", "u1"), ("pad", "u1", 11)])
+bng_lease_sum = np.dtype([
+    ("entries", "<u8", 3), ("expired", "<u8", 3), ("addrs", "<u8"), ("conflicts", "<u8"), ("unknown_pool", "<u8"),
+    ("cid_dangling", "<u8"), ("pools_found", "<u8")])
+bng_lease_removed = np.dtype([
+    ("key", "u1", 32), ("lease_expiry", "<u8"), ("pool_id", "<u4"), ("allocated_ip", "u1", 4), ("vlan_id", "<u4"),
+    ("map", "u1"), ("client_class", "u1"), ("flags", "u1"), ("pad", "u1", 9)])
+LEASE_MAPS = ("subscriber_pools", "vlan_subscriber_pools", "circuit_id_subscribers")  # bng_lease_removed.map
+
+assert bng_lease_pool_use.itemsize == 64 and bng_lease_removed.itemsize == 64 and bng_lease_sum.itemsize == 88
 assert bng_nat_sub_use.itemsize == 64 and bng_nat_pub_use.itemsize == 64 and bng_nat_usage_sum.itemsize == 80
 assert subscriber_binding.itemsize == 24 and token_bucket.itemsize == 32 and bng_acct.itemsize == 64
 assert bng_li_record.itemsize == 64

@@ -457,6 +457,97 @@ typedef struct bng_nat_usage_sum {
 int bng_nat_usage(bng_ctx *ctx, uint32_t min_permille, bng_nat_usage_sum *sum, uint32_t *sub_addrs, bng_nat_sub_use *sub_out,
                   uint64_t sub_cap, uint32_t *pub_addrs, bng_nat_pub_use *pub_out, uint64_t pub_cap);
 
+/* ---- DHCP lease census and expiry sweep ----
+ * dhcp_fastpath_prog finds a subscriber's pool_assignment by VLAN pair, then circuit-id, then chaddr, takes the first
+ * entry it finds and sends the frame to the slow path when that entry has expired, even if a fresh one exists further
+ * down the chain.  The three lease maps (map index 0 subscriber_pools, 1 vlan_subscriber_pools, 2
+ * circuit_id_subscribers) live only on the GPU, so finding and removing their expired entries, and counting what the
+ * pools hold, are GPU passes.
+ *   - Expired at now_ns is exactly the program's test: now_ns / 1000000000 > lease_expiry.  An entry the program would
+ *     still serve at now_ns is unexpired.
+ *   - Byte order.  Two conventions fill these maps.  The control plane (the reference's Go loader, whose IPToUint32 is
+ *     BigEndian.Uint32 stored in a native word, and its C++ mirror in bng_host.hpp / bng_dhcp_slow.hpp) stores the
+ *     address's numeric value: BNG_LEASE_ADDR_NUMERIC, the default, and the order in which dhcp::Pool takes an address
+ *     back.  The program itself copies allocated_ip into yiaddr and builds the subnet mask with htonl, so tables whose
+ *     replies must be right on the wire (the synthetic workloads and the test scripts) hold the four bytes in wire
+ *     order: BNG_LEASE_ADDR_WIRE.  bng_dhcp_lease_addr_order tells the context which one its control plane uses; the
+ *     census compares the leading prefix_len bits of allocated_ip and ip_pool.network in that order.  Only
+ *     addrs_outside and permille depend on it: the two fields always share one convention, and distinct counts and
+ *     conflicts compare words.  prefix_len 0 contains every address, 32 only `network`, a prefix_len > 32 none.
+ *     Records of removed entries carry allocated_ip as stored.
+ *
+ * bng_dhcp_lease_census: read-only.  One record for every pool_id that keys an ip_pools entry or is named by any lease
+ * entry, expired or not.
+ *   - Conflict: an address counts once in `conflicts` of pool P when, within one of the three maps, two or more
+ *     unexpired entries naming P hold it (the keys of a map are distinct, so those are two subscribers).  The same
+ *     subscriber appearing in different maps is not a conflict, and expired entries never conflict: their address may
+ *     have been leased again.
+ *   - The call writes min(pools_found, cap) records in no particular order; calling it again with nothing run in
+ *     between gives the same answer.  Staged upserts are applied first and the census sees everything queued on the
+ *     context's stream; it returns synchronised.  It writes no map byte, counter, event, accounting, idle or
+ *     interception state, does not advance the batch sequence, and gives a following bng_delta_export nothing to send.
+ *   - -EINVAL for a NULL ctx or sum, or a cap > 0 with NULL outputs.
+ *   - Memory: the first call allocates the census's scratch, kept until bng_close: a set of 8-byte words, the power of
+ *     two >= 4 x the summed max_entries of the three lease maps (128 MiB at the default capacities), 64 bytes per ip_pools
+ *     slot and per slot of the hash of unknown pool_ids (3 MiB; the hash grows, and the census counts again, once
+ *     8192 distinct unknown pool_ids have records), and room for the records.  A context that calls neither function allocates none of it.
+ *   - In a sharded deployment each shard counts its own tables: an address leased on two shards counts once per shard.
+ *
+ * bng_dhcp_lease_sweep: removes.  An entry of the three lease maps is due when
+ * now_ns / 1000000000 > lease_expiry + grace_s (the sum saturates); with grace_s == 0 that is every entry the program
+ * refuses.
+ *   - Returns the number of due entries found (or a negative errno).  It removes, and reports in `out`, at most `cap` of
+ *     them; which ones when there are more is unspecified, but every removed entry is reported exactly once and every
+ *     reported entry is removed.  cap == 0 removes nothing (a dry run; `out` may be NULL).  Repeat the call until the
+ *     return value is <= cap.
+ *   - circuit_id_map (fnv hash of the circuit-id -> MAC): an entry whose value MAC keys a subscriber_pools entry that
+ *     this call removes is removed with it, and no other.
+ *   - removed_out (may be NULL): entries removed from map 0, 1, 2 and from circuit_id_map.
+ *   - Nothing else changes: not stats_map (cache_expired is the program's counter), not ip_pools, no NAT / QoS map.
+ *     bng_map_get_info().count of the four maps drops by what was removed and a later insert finds the room.
+ *   - Staged upserts are applied first; the sweep is a batch of its own (it advances the batch sequence) and returns
+ *     synchronised.  The removed keys are deletions of the next bng_delta_export.
+ *   - Afterwards each of the four tables of which more than a quarter of the slots are tombstones is rebuilt.  These
+ *     rebuilds are counted by bng_lease_table_rebuilds, not by bng_table_rebuilds.  A dry run rebuilds nothing.  A
+ *     rebuild that finds no memory leaves its table as it was; the call still returns what it removed
+ *     (bng_last_error has the text) and the next sweep tries again.
+ *   - -EINVAL for a NULL ctx, or cap > 0 with a NULL out. */
+typedef struct bng_lease_pool_use { /* 64 bytes; one per pool_id seen */
+    uint64_t entries[3];     /* unexpired entries naming the pool, per map */
+    uint64_t expired;        /* expired entries naming the pool, the three maps together */
+    uint32_t addrs;          /* distinct allocated_ip among its unexpired entries */
+    uint32_t addrs_outside;  /* of those, the ones not inside network/prefix_len (all of them when no ip_pools entry) */
+    uint32_t conflicts;
+    uint32_t prefix_hosts;   /* 2^(32 - prefix_len), saturated at 2^32-1; 0 when prefix_len > 32 or no ip_pools entry */
+    uint32_t permille;       /* floor((addrs - addrs_outside) * 1000 / prefix_hosts), 0 when prefix_hosts == 0 */
+    uint8_t known;           /* 1 when ip_pools has the pool_id */
+    uint8_t pad[11];         /* zero */
+} bng_lease_pool_use;
+typedef struct bng_lease_sum {
+    uint64_t entries[3], expired[3]; /* per map, unexpired / expired */
+    uint64_t addrs;                  /* distinct allocated_ip over all unexpired entries */
+    uint64_t conflicts;              /* summed over pools */
+    uint64_t unknown_pool;           /* unexpired entries whose pool_id has no ip_pools entry (the program counts these as errors) */
+    uint64_t cid_dangling;           /* circuit_id_map entries whose value MAC keys no subscriber_pools entry */
+    uint64_t pools_found;            /* records that exist (may exceed cap) */
+} bng_lease_sum;
+int bng_dhcp_lease_census(bng_ctx *ctx, uint64_t now_ns, bng_lease_sum *sum, uint32_t *pool_ids, bng_lease_pool_use *out,
+                          uint64_t cap);
+typedef struct bng_lease_removed { /* 64 bytes */
+    uint8_t key[32];         /* the entry's key, zero-padded: 8-byte MAC word, 4-byte vlan_key, or 32-byte circuit-id */
+    uint64_t lease_expiry;
+    uint32_t pool_id, allocated_ip, vlan_id;
+    uint8_t map;             /* 0 subscriber_pools, 1 vlan_subscriber_pools, 2 circuit_id_subscribers */
+    uint8_t client_class, flags;
+    uint8_t pad[9];          /* zero */
+} bng_lease_removed;
+int64_t bng_dhcp_lease_sweep(bng_ctx *ctx, uint64_t now_ns, uint32_t grace_s, bng_lease_removed *out, uint64_t cap,
+                             uint64_t removed_out[4]);
+#define BNG_LEASE_ADDR_NUMERIC 0u
+#define BNG_LEASE_ADDR_WIRE 1u
+int bng_dhcp_lease_addr_order(bng_ctx *ctx, uint32_t order); /* -EINVAL for a NULL ctx or another value */
+uint64_t bng_lease_table_rebuilds(bng_ctx *ctx); /* rebuilds of the three lease maps and circuit_id_map by the sweep */
+
 /* ---- diagnostics ---- */
 uint64_t bng_launch_count(bng_ctx *ctx);  /* kernels launched by this context so far */
 uint64_t bng_lru_overflow(bng_ctx *ctx);  /* inserts that found no victim to evict in a full LRU map (should stay 0) */
