@@ -164,6 +164,11 @@ struct bng_ctx {
     u8 *demit = nullptr;                    // records of one table
     u64 demit_cap = 0;
     u64 dapply_stream = 0, dapply_seq = 0;  // applier: the last delta applied
+    // subscriber hand-over (bng_sub_export, move.cu): the flow tables' slot lists, allocated by the first export, and
+    // a grow-only staging buffer (address set and keys in, gathered entries and lookups out)
+    u32 *mv_lists = nullptr;
+    u8 *mv_buf = nullptr;
+    u64 mv_cap = 0;
 };
 
 namespace {
@@ -552,7 +557,7 @@ int bng_close(bng_ctx *c) {
         void *sp[] = {s.key_a, s.key_b, s.val_a, s.val_b, s.qslot, s.attr, s.cub_tmp, s.counters, c->acct_dump_buf, c->idle_scan_buf, c->li_ring, c->li_match,
                       c->io_dev, c->hb_pkts, c->hb_off, c->hb_len, c->hb_prio, c->hb_verdict, c->hb_now, c->dump_k, c->dump_v, c->dump_c,
                       c->dlist, c->dsent, c->demit, c->nu_set, c->nu_pub, c->nu_sum, c->nu_sub, c->nu_out,
-                      c->ls_set, c->ls_pools, c->ls_sum, c->ls_out, c->ls_macs};
+                      c->ls_set, c->ls_pools, c->ls_sum, c->ls_out, c->ls_macs, c->mv_lists, c->mv_buf};
         for (void *p : sp)
             if (p) cudaFree(p);
         for (auto &s : c->dshadow) cudaFree(s.words);
@@ -2938,6 +2943,333 @@ int bng_delta_info(bng_ctx *c, uint64_t *stream_id, uint64_t *seq) {
     const bool exporter = !c->dshadow.empty();
     if (stream_id) *stream_id = exporter ? c->delta_stream : c->dapply_stream;
     if (seq) *seq = exporter ? c->delta_seq : c->dapply_seq;
+    return 0;
+}
+
+// ---------------------------------------------------------------------------
+// subscriber hand-over between contexts (move.cu; the blob is described in include/bng_b200.h)
+// ---------------------------------------------------------------------------
+namespace {
+const char kMoveMagic[8] = {'B', 'N', 'G', 'M', 'O', 'V', 'E', '1'};
+// Whole idle records, (address, struct bng_idle): a name of its own, so that bng_restore and bng_delta_apply, which
+// take only timeouts under kSnapIdle, step over it.
+const char kMoveIdle[] = "subscriber_idle_rec";
+const u32 kMoveIdleKind = 8;
+// what a subscriber owns: maps keyed by its address, by its MAC, and the flow tables (selected by k_move_select)
+const char *const kMoveAddrMaps[] = {"subscriber_nat", "qos_ingress", "qos_egress"};
+const char *const kMoveMacMaps[] = {"subscriber_bindings", "subscriber_pools"};
+const char *const kMoveFlowMaps[] = {"nat_sessions", "nat_reverse", "eim_table"};
+
+size_t al256(size_t v) { return (v + 255) & ~(size_t)255; }
+
+// the staging buffer of bng_sub_export, grown to `bytes` with its first `keep` bytes kept
+int mv_grow(bng_ctx *c, u64 bytes, u64 keep) {
+    if (bytes <= c->mv_cap) return 0;
+    const u64 nb = std::max<u64>(bytes + bytes / 4, 1 << 20);
+    u8 *q = nullptr;
+    if (cudaMalloc((void **)&q, nb) != cudaSuccess) {
+        cudaGetLastError();
+        return fail(c, -ENOMEM, "sub_export: %llu bytes of device memory", (unsigned long long)nb);
+    }
+    if (keep) CU(c, cudaMemcpyAsync(q, c->mv_buf, keep, cudaMemcpyDeviceToDevice, c->L.stream));
+    CU(c, cudaStreamSynchronize(c->L.stream));
+    if (c->mv_buf) cudaFree(c->mv_buf);
+    c->mv_buf = q;
+    c->mv_cap = nb;
+    return 0;
+}
+
+// n (address, record) pairs into the addresses' directory slots, chunked through the staging buffers: accounting
+// records (rs = sizeof(bng_acct)) or whole idle records (rs = sizeof(bng_idle))
+int mv_load_records_locked(bng_ctx *c, const u8 *addrs, const u8 *recs, u64 n, size_t rs) {
+    const u64 chunk_max = 1u << 16;
+    for (u64 done = 0; done < n; done += chunk_max) {
+        const u64 k = std::min(chunk_max, n - done);
+        const size_t roff = al256(k * 4);
+        if (int r = ensure_io(c, roff + k * rs)) return r;
+        memcpy(c->io_host, addrs + done * 4, k * 4);
+        memcpy(c->io_host + roff, recs + done * rs, k * rs);
+        CU(c, cudaMemcpyAsync(c->io_dev, c->io_host, roff + k * rs, cudaMemcpyHostToDevice, c->L.stream));
+        if (rs == sizeof(bng_acct))
+            CU(c, run_acct_load(c->L, c->dev.subdir, c->acct, (const u32 *)c->io_dev, (const u64 *)(c->io_dev + roff), k));
+        else
+            CU(c, run_idle_load(c->L, c->dev.subdir, c->idle, (const u32 *)c->io_dev, (const u64 *)(c->io_dev + roff), k));
+        CU(c, cudaStreamSynchronize(c->L.stream));
+    }
+    return 0;
+}
+} // namespace
+
+int bng_sub_export(bng_ctx *c, const uint32_t *addrs, uint64_t n_addrs, const uint64_t *macs, uint64_t n_macs, uint32_t flags,
+                   void *buf, uint64_t cap, uint64_t *len_out) {
+    if (!c || !len_out || (n_addrs && !addrs) || (n_macs && !macs) || (cap && !buf) || (flags & ~BNG_SUB_DETACH)) return -EINVAL;
+    *len_out = 0;
+    std::lock_guard<std::mutex> g(c->mu);
+    cudaSetDevice(c->device);
+    if (int fr = flush_staged_locked(c, -1)) return fr;
+    // distinct addresses and MACs, in the order given
+    std::vector<u32> A;
+    std::vector<u64> M;
+    {
+        std::unordered_set<u32> seen;
+        for (u64 i = 0; i < n_addrs; i++)
+            if (seen.insert(addrs[i]).second) A.push_back(addrs[i]);
+    }
+    {
+        std::unordered_set<u64> seen;
+        for (u64 i = 0; i < n_macs; i++)
+            if (seen.insert(macs[i]).second) M.push_back(macs[i]);
+    }
+    const u64 na = A.size(), nm = M.size();
+    u64 slots = 64;
+    while (slots < 2 * na) slots *= 2;
+    if (slots > (1ull << 32)) return fail(c, -EINVAL, "sub_export: %llu addresses", (unsigned long long)na);
+    const DevCtx &d = c->dev;
+    const u64 ns = (u64)d.sessions.mask + 1, nr = (u64)d.reverse.mask + 1, ne = (u64)d.eim.mask + 1;
+    // the slot lists (4 bytes per slot of the three flow tables), allocated by the first export that has addresses
+    if (na && !c->mv_lists && cudaMalloc((void **)&c->mv_lists, (ns + nr + ne) * 4) != cudaSuccess) {
+        cudaGetLastError();
+        c->mv_lists = nullptr;
+        return fail(c, -ENOMEM, "sub_export: %llu bytes of device memory", (unsigned long long)((ns + nr + ne) * 4));
+    }
+    // staging: [in] address set, addresses, MACs, counters; [out] lookups by key, then the gathered flow entries
+    MapReg *am[3], *mm[2], *fm[3];
+    for (int k = 0; k < 3; k++) am[k] = get_map(c, bng_map_id(c, kMoveAddrMaps[k])), fm[k] = get_map(c, bng_map_id(c, kMoveFlowMaps[k]));
+    for (int k = 0; k < 2; k++) mm[k] = get_map(c, bng_map_id(c, kMoveMacMaps[k]));
+    const size_t aoff = al256(slots * 8), moff = al256(aoff + na * 4), coff = al256(moff + nm * 8), out0 = al256(coff + 16);
+    size_t at = out0, am_v[3], am_r[3], mm_v[2], mm_r[2], acct_v = 0, acct_r = 0, idle_v = 0, idle_r = 0;
+    for (int k = 0; k < 3; k++) am_v[k] = at, am_r[k] = al256(at + na * am[k]->value_size), at = al256(am_r[k] + na * 4);
+    for (int k = 0; k < 2; k++) mm_v[k] = at, mm_r[k] = al256(at + nm * mm[k]->value_size), at = al256(mm_r[k] + nm * 4);
+    if (c->acct) acct_v = at, acct_r = al256(at + na * sizeof(bng_acct)), at = al256(acct_r + na * 4);
+    if (c->idle) idle_v = at, idle_r = al256(at + na * sizeof(bng_idle)), at = al256(idle_r + na * 4);
+    const size_t flow0 = at;
+    if (int r = mv_grow(c, flow0, 0)) return r;
+    // the inputs are built in the pinned staging buffer and copied on the context's stream, ahead of the kernels that
+    // read them (as bng_nat_flush does)
+    if (int r = ensure_io(c, out0)) return r;
+    u8 *in = c->io_host;
+    memset(in, 0, out0);
+    u64 *set = (u64 *)in;
+    const u32 mask = (u32)(slots - 1);
+    for (u32 a : A) {
+        u32 i = aset_home(a, mask);
+        while (set[i]) i = (i + 1) & mask;
+        set[i] = ADDRSET_LIVE | a;
+    }
+    if (na) memcpy(in + aoff, A.data(), na * 4);
+    if (nm) memcpy(in + moff, M.data(), nm * 8);
+    u8 *dv = c->mv_buf;
+    CU(c, cudaMemcpyAsync(dv, in, out0, cudaMemcpyHostToDevice, c->L.stream));
+    for (int k = 0; k < 3; k++)
+        CU(c, run_table_op(c->L, *am[k]->tbl, TOP_LOOKUP, dv + aoff, dv + am_v[k], (int *)(dv + am_r[k]), na, 0, d.subdir, 0, nullptr, nullptr));
+    for (int k = 0; k < 2; k++)
+        CU(c, run_table_op(c->L, *mm[k]->tbl, TOP_LOOKUP, dv + moff, dv + mm_v[k], (int *)(dv + mm_r[k]), nm, 0, d.subdir, 0, nullptr, nullptr));
+    if (c->acct) CU(c, run_acct_read(c->L, d.subdir, c->acct, (const u32 *)(dv + aoff), na, (u64 *)(dv + acct_v), (int *)(dv + acct_r)));
+    if (c->idle) CU(c, run_idle_read(c->L, d.subdir, c->idle, (const u32 *)(dv + aoff), na, (u64 *)(dv + idle_v), (int *)(dv + idle_r)));
+    u32 *cnt = (u32 *)(dv + coff);
+    CU(c, cudaMemsetAsync(cnt, 0, 16, c->L.stream));
+    if (na) CU(c, run_move_select(c->L, d, AddrSet{(const u64 *)dv, mask}, c->mv_lists, cnt));
+    u32 n4[4] = {0, 0, 0, 0};
+    CU(c, cudaMemcpyAsync(n4, cnt, 16, cudaMemcpyDeviceToHost, c->L.stream));
+    CU(c, cudaStreamSynchronize(c->L.stream));
+    // the delta exporter's gather turns the slot lists into ABI keys and values
+    size_t fk[3], fv[3];
+    at = flow0;
+    for (int k = 0; k < 3; k++) {
+        const Tbl &t = *fm[k]->tbl;
+        fk[k] = at, fv[k] = at + (size_t)n4[k] * t.key_size, at = al256(fv[k] + (size_t)n4[k] * t.value_size);
+    }
+    if (int r = mv_grow(c, at, flow0)) return r;
+    dv = c->mv_buf;
+    for (int k = 0; k < 3 && c->mv_lists; k++) {
+        const u32 *lists[3] = {c->mv_lists, c->mv_lists + ns, c->mv_lists + ns + nr};
+        const Tbl &t = *fm[k]->tbl;
+        DeltaTbl v{};
+        v.slots = t.slots, v.slot_bytes = t.slot_bytes, v.nslots = (u64)t.mask + 1;
+        v.key_size = t.key_size, v.value_size = t.value_size, v.voff = t.voff, v.vlayout = t.vlayout;
+        CU(c, run_delta_emit(c->L, v, nullptr, 0, lists[k], n4[k], nullptr, dv + fk[k], dv + fv[k]));
+    }
+    std::vector<u8> got(at - out0);
+    CU(c, cudaMemcpyAsync(got.data(), dv + out0, got.size(), cudaMemcpyDeviceToHost, c->L.stream)); // the one copy out
+    CU(c, cudaStreamSynchronize(c->L.stream));
+    prof_collect(c->L);
+    auto host = [&](size_t off) { return got.data() + (off - out0); };
+    // the blob: snapshot framing, one section per map, then the records and the interception targets
+    std::vector<u8> out(kMoveMagic, kMoveMagic + 8);
+    out.resize(16);
+    u64 nsec = 0;
+    auto by_key = [&](MapReg *m, const u8 *keys, u64 n, size_t voff, size_t roff) {
+        const int *res = (const int *)host(roff);
+        const u8 *vals = host(voff);
+        std::vector<u8> kv, vv;
+        for (u64 i = 0; i < n; i++)
+            if (res[i] == 0) {
+                kv.insert(kv.end(), keys + i * m->key_size, keys + (i + 1) * m->key_size);
+                vv.insert(vv.end(), vals + i * m->value_size, vals + (i + 1) * m->value_size);
+            }
+        const u64 k = kv.size() / m->key_size;
+        put_section(out, m->name, KIND_HASH, m->key_size, m->value_size, 0, k);
+        out.insert(out.end(), kv.begin(), kv.end());
+        out.insert(out.end(), vv.begin(), vv.end());
+        nsec++;
+    };
+    for (int k = 0; k < 3; k++) by_key(am[k], (const u8 *)A.data(), na, am_v[k], am_r[k]);
+    for (int k = 0; k < 2; k++) by_key(mm[k], (const u8 *)M.data(), nm, mm_v[k], mm_r[k]);
+    for (int k = 0; k < 3; k++) {
+        const MapReg *m = fm[k];
+        put_section(out, m->name, KIND_HASH, m->key_size, m->value_size, 0, n4[k]);
+        out.insert(out.end(), host(fk[k]), host(fk[k]) + (size_t)n4[k] * m->key_size);
+        out.insert(out.end(), host(fv[k]), host(fv[k]) + (size_t)n4[k] * m->value_size);
+        nsec++;
+    }
+    auto records = [&](const char *name, u32 kind, size_t rs, size_t voff, size_t roff) {
+        const int *res = (const int *)host(roff);
+        std::vector<u32> a;
+        std::vector<u8> v;
+        for (u64 i = 0; i < na; i++)
+            if (res[i] == 0) a.push_back(A[i]), v.insert(v.end(), host(voff) + i * rs, host(voff) + (i + 1) * rs);
+        put_section(out, name, kind, 4, (u32)rs, 0, a.size());
+        out.insert(out.end(), (const u8 *)a.data(), (const u8 *)(a.data() + a.size()));
+        out.insert(out.end(), v.begin(), v.end());
+        nsec++;
+    };
+    if (c->acct) records(kSnapAcct, kSnapAcctKind, sizeof(bng_acct), acct_v, acct_r);
+    if (c->idle) records(kMoveIdle, kMoveIdleKind, sizeof(bng_idle), idle_v, idle_r);
+    std::vector<u32> li_a;
+    if (c->li_ctl) {
+        std::vector<u32> ids;
+        for (u32 a : A) {
+            auto it = c->li_targets.find(a);
+            if (it != c->li_targets.end()) li_a.push_back(a), ids.push_back(it->second);
+        }
+        put_pairs(out, kSnapLi, kSnapLiKind, li_a, ids);
+        nsec++;
+    }
+    memcpy(&out[8], &nsec, 8);
+    *len_out = out.size();
+    if (cap < out.size()) return -ENOSPC; // nothing written, nothing removed
+    memcpy(buf, out.data(), out.size());
+    if (!(flags & BNG_SUB_DETACH)) return 0;
+    // Detach exactly what was exported: the listed flow slots, then the keyed entries through the table-op path (the
+    // subscriber directory follows subscriber_nat and qos_ingress, and with it the records' lifetime).  Every input is
+    // already on the device and nothing below allocates, so once the blob is written the removal cannot fail part way
+    // for want of memory.  Deleting every given key deletes exactly the entries found: nothing ran in between, and a
+    // key without an entry is a miss that changes nothing.
+    if (c->mv_lists) CU(c, run_move_detach(c->L, d, c->mv_lists, n4));
+    for (int k = 0; k < 5; k++) {
+        MapReg *m = k < 3 ? am[k] : mm[k - 3];
+        const int role = m->tbl == &d.sub_nat ? 1 : (m->tbl == &d.qos_in ? 2 : 0);
+        CU(c, run_table_op(c->L, *m->tbl, TOP_DELETE, dv + (k < 3 ? aoff : moff), nullptr, (int *)(dv + (k < 3 ? am_r[k] : mm_r[k - 3])),
+                           k < 3 ? na : nm, 0, d.subdir, role, c->acct, c->idle));
+    }
+    if (!li_a.empty()) {
+        for (u32 a : li_a) c->li_targets.erase(a);
+        c->li_dirty = true;
+    }
+    CU(c, cudaStreamSynchronize(c->L.stream));
+    prof_collect(c->L);
+    // the flush's rebuild rule; a rebuild that finds no memory leaves the tables as they were, and the detach stands
+    if (rebuild_if_tombstoned_locked(c, n4[3] + n4[0])) cudaGetLastError();
+    return 0;
+}
+
+int bng_sub_import(bng_ctx *c, const void *buf, uint64_t len) {
+    if (!c) return -EINVAL;
+    if (!buf || len < 16 || memcmp(buf, kMoveMagic, 8)) return fail(c, -EINVAL, "sub_import: not a hand-over blob");
+    // the whole blob is checked before anything changes
+    struct Sec {
+        SnapMapHdr h;
+        const u8 *p;
+        int id; // map id, or -1 accounting records, -2 idle records, -3 interception targets
+    };
+    std::vector<Sec> secs;
+    u64 nsec;
+    memcpy(&nsec, (const u8 *)buf + 8, 8);
+    const u8 *p = (const u8 *)buf + 16, *end = (const u8 *)buf + len;
+    for (u64 k = 0; k < nsec; k++) {
+        Sec s{};
+        if ((u64)(end - p) < sizeof(SnapMapHdr)) return fail(c, -EINVAL, "sub_import: truncated");
+        memcpy(&s.h, p, sizeof(s.h));
+        p += sizeof(s.h);
+        s.h.name[sizeof(s.h.name) - 1] = 0;
+        const u64 per = (u64)s.h.key_size + s.h.value_size;
+        if (per == 0 || s.h.count > (u64)(end - p) / per) return fail(c, -EINVAL, "sub_import: %s is truncated", s.h.name);
+        s.p = p;
+        p += s.h.count * per;
+        if (!strcmp(s.h.name, kSnapAcct)) {
+            if (s.h.kind != kSnapAcctKind || s.h.key_size != 4 || s.h.value_size != sizeof(bng_acct)) s.id = -100;
+            else s.id = -1;
+        } else if (!strcmp(s.h.name, kMoveIdle)) {
+            if (s.h.kind != kMoveIdleKind || s.h.key_size != 4 || s.h.value_size != sizeof(bng_idle)) s.id = -100;
+            else s.id = -2;
+        } else if (!strcmp(s.h.name, kSnapLi)) {
+            if (s.h.kind != kSnapLiKind || s.h.key_size != 4 || s.h.value_size != 4 || s.h.count > BNG_LI_MAX_TARGETS) s.id = -100;
+            else s.id = -3;
+        } else {
+            s.id = bng_map_id(c, s.h.name);
+            const MapReg *m = s.id >= 0 ? get_map(c, s.id) : nullptr;
+            if (!m || m->kind != KIND_HASH || s.h.kind != KIND_HASH || m->key_size != s.h.key_size || m->value_size != s.h.value_size)
+                s.id = -100;
+        }
+        if (s.id == -100) return fail(c, -EINVAL, "sub_import: %s is not a section of this library's layout", s.h.name);
+        secs.push_back(s);
+    }
+    if (p != end) return fail(c, -EINVAL, "sub_import: %llu bytes after the last section", (unsigned long long)(end - p));
+    {   // room: nothing may be refused or evicted part way
+        std::lock_guard<std::mutex> g(c->mu);
+        cudaSetDevice(c->device);
+        if (int fr = flush_staged_locked(c, -1)) return fr;
+        std::unordered_map<int, u64> want;
+        std::unordered_set<u32> li_new;
+        for (const Sec &s : secs) {
+            if (s.id >= 0) want[s.id] += s.h.count;
+            if (s.id == -3)
+                for (u64 k = 0; k < s.h.count; k++) {
+                    u32 a;
+                    memcpy(&a, s.p + k * 4, 4);
+                    if (!c->li_targets.count(a)) li_new.insert(a);
+                }
+        }
+        for (const auto &w : want) {
+            const MapReg *m = get_map(c, w.first);
+            u32 live = 0;
+            CU(c, cudaMemcpyAsync(&live, m->tbl->count, 4, cudaMemcpyDeviceToHost, c->L.stream));
+            CU(c, cudaStreamSynchronize(c->L.stream));
+            if ((u64)live + w.second > m->max_entries)
+                return fail(c, -E2BIG, "sub_import: %s holds %u of %u entries, the blob brings %llu", m->name, live, m->max_entries,
+                            (unsigned long long)w.second);
+        }
+        if (c->li_targets.size() + li_new.size() > BNG_LI_MAX_TARGETS)
+            return fail(c, -E2BIG, "sub_import: more than %d interception targets", BNG_LI_MAX_TARGETS);
+    }
+    for (const Sec &s : secs) {
+        if (s.id < 0 || !s.h.count) continue;
+        const u8 *keys = s.p, *vals = s.p + s.h.count * s.h.key_size;
+        if (int r = bng_map_update_batch(c, s.id, keys, vals, s.h.count, BNG_ANY)) return fail(c, r, "sub_import: loading %s failed", s.h.name);
+    }
+    // after the maps: the records go to the addresses' (new) directory slots
+    std::lock_guard<std::mutex> g(c->mu);
+    cudaSetDevice(c->device);
+    for (const Sec &s : secs) {
+        const u8 *keys = s.p, *vals = s.p + s.h.count * s.h.key_size;
+        if (!s.h.count) continue;
+        if (s.id == -1) {
+            if (int r = acct_alloc_locked(c)) return r;
+            if (int r = mv_load_records_locked(c, keys, vals, s.h.count, sizeof(bng_acct))) return r;
+        } else if (s.id == -2) {
+            if (int r = idle_alloc_locked(c)) return r;
+            if (int r = mv_load_records_locked(c, keys, vals, s.h.count, sizeof(bng_idle))) return r;
+        } else if (s.id == -3) {
+            if (int r = li_alloc_locked(c)) return r;
+            for (u64 k = 0; k < s.h.count; k++) {
+                u32 a, id;
+                memcpy(&a, keys + k * 4, 4);
+                memcpy(&id, vals + k * 4, 4);
+                c->li_targets[a] = id;
+            }
+            c->li_dirty = true;
+        }
+    }
     return 0;
 }
 

@@ -14,14 +14,6 @@
 #include "kernels.h"
 #include "progs.cuh"
 
-__device__ __forceinline__ bool aset_has(const AddrSet &a, u32 addr) {
-    for (u32 i = aset_home(addr, a.mask);; i = (i + 1) & a.mask) {
-        const u64 w = a.words[i];
-        if (w == 0) return false;
-        if ((u32)w == addr) return true;
-    }
-}
-
 // cnt: [0] sessions, [1] reverse entries, [2] EIM mappings removed, [3] nat_sessions tombstones after the pass.
 // Index space of the grid-stride loop: nat_sessions slots, then nat_reverse slots, eim_table slots, set slots.
 __global__ void __launch_bounds__(256) k_nat_flush(const __grid_constant__ DevCtx c, const AddrSet a, u64 now, u32 *cnt) {

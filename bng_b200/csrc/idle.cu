@@ -5,6 +5,7 @@
 //   - k_idle_scan streams the directory's slots and the records once: it starts the records no scan has seen and
 //     compacts the idle ones with one atomic per warp on the output count, as k_acct_dump does;
 //   - k_idle_read, k_idle_timeout_set: by address;
+//   - k_idle_load: whole records by address (a subscriber handed over from another context, bng_sub_import);
 //   - k_idle_restart clears every clock (restore, delta apply): the stamps of another node or of another time are not
 //     evidence of activity here.
 #include <errno.h>
@@ -89,6 +90,22 @@ __global__ void k_idle_timeout_set(const __grid_constant__ Tbl dir, u64 *idle, c
     }
 }
 
+// struct bng_idle -> device record (idle_out's inverse); the scratch half-word is 0, as between calls
+__global__ void k_idle_load(const __grid_constant__ Tbl dir, u64 *idle, const u32 *addrs, const u64 *recs, u64 n) {
+    for (u64 i = blockIdx.x * (u64)blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x) {
+        const u32 s = dir_slot_of(dir, addrs[i]);
+        if (s == DIR_NONE) continue;
+        const u64 *o = recs + i * IDLE_WORDS;
+        const u32 f = (u32)(o[3] >> 32);
+        ulonglong4 w;
+        w.x = o[3] & 0xFFFFFFFFull;
+        w.y = (f & BNG_IDLE_UP) ? o[0] + 1 : 0;
+        w.z = (f & BNG_IDLE_DOWN) ? o[1] + 1 : 0;
+        w.w = (f & BNG_IDLE_STARTED) ? o[2] + 1 : 0;
+        *(ulonglong4 *)(idle + (size_t)s * IDLE_WORDS) = w;
+    }
+}
+
 __global__ void k_idle_restart(const __grid_constant__ Tbl dir, u64 *idle) {
     const u64 slots = (u64)dir.mask + 1;
     for (u64 i = blockIdx.x * (u64)blockDim.x + threadIdx.x; i < slots; i += (u64)gridDim.x * blockDim.x) {
@@ -123,6 +140,13 @@ cudaError_t run_idle_timeout_set(Launcher &L, const Tbl &dir, u64 *idle, const u
     k_idle_timeout_set<true><<<idle_grid(L, n), IDLE_BLOCK, 0, L.stream>>>(dir, idle, addrs, timeouts, n, results);
     k_idle_timeout_set<false><<<idle_grid(L, n), IDLE_BLOCK, 0, L.stream>>>(dir, idle, addrs, timeouts, n, results);
     L.launches += 2;
+    return cudaGetLastError();
+}
+
+cudaError_t run_idle_load(Launcher &L, const Tbl &dir, u64 *idle, const u32 *addrs, const u64 *recs, u64 n) {
+    if (n == 0) return cudaSuccess;
+    k_idle_load<<<idle_grid(L, n), IDLE_BLOCK, 0, L.stream>>>(dir, idle, addrs, recs, n);
+    L.launches++;
     return cudaGetLastError();
 }
 

@@ -87,6 +87,15 @@ __host__ __device__ __forceinline__ u32 aset_home(u32 addr, u32 mask) {
     h ^= h >> 16;
     return h & mask;
 }
+#ifdef __CUDACC__
+__device__ __forceinline__ bool aset_has(const AddrSet &a, u32 addr) {
+    for (u32 i = aset_home(addr, a.mask);; i = (i + 1) & a.mask) {
+        const u64 w = a.words[i];
+        if (w == 0) return false;
+        if ((u32)w == addr) return true;
+    }
+}
+#endif
 cudaError_t run_nat_flush(Launcher &L, const DevCtx &c, const AddrSet &a, u64 now, u32 *cnt /* [4], see flush.cu */);
 cudaError_t run_table_dump(Launcher &L, const Tbl &t, u8 *keys_out, u8 *vals_out, u32 *count_out, u64 cap);
 
@@ -125,6 +134,16 @@ cudaError_t run_idle_read(Launcher &L, const Tbl &dir, const u64 *idle, const u3
 cudaError_t run_idle_timeout_set(Launcher &L, const Tbl &dir, u64 *idle, const u32 *addrs, const u32 *timeouts, u64 n, int *results);
 // every record's stamps and since := none (the timeouts stay)
 cudaError_t run_idle_restart(Launcher &L, const Tbl &dir, u64 *idle);
+// whole record of every listed address that has a directory entry := recs[i] (struct bng_idle, as run_idle_read gives
+// it); the addresses are distinct (subscriber hand-over, bng_sub_import)
+cudaError_t run_idle_load(Launcher &L, const Tbl &dir, u64 *idle, const u32 *addrs, const u64 *recs, u64 n);
+
+// subscriber hand-over between contexts (move.cu).  The slot lists of the three flow tables live in one array:
+// nat_sessions' at [0, ns), nat_reverse's at [ns, ns + nr), eim_table's at [ns + nr, ns + nr + ne) (table slot counts).
+// cnt: [0..2] entries listed per table, [3] nat_sessions tombstones seen (zeroed by the caller).
+cudaError_t run_move_select(Launcher &L, const DevCtx &c, const AddrSet &a, u32 *lists, u32 *cnt);
+// tombstones the listed slots (no log record, no statistic); n[k] entries of table k's list
+cudaError_t run_move_detach(Launcher &L, const DevCtx &c, const u32 *lists, const u32 n[3]);
 
 // NAT port-usage census (natuse.cu).  Scratch of its own, zeroed before every census:
 //   set        set_mask + 1 u64 words, 0 = empty: the distinct held triples and ports, overall and per subscriber.  A

@@ -21,6 +21,7 @@ LIB_PATH = os.environ.get("BNG_B200_LIB") or os.path.join(HERE, "libbng_b200.so"
 MEM_DEVICE, MEM_HOST = 0, 1
 ANY, NOEXIST, EXIST = 0, 1, 2
 DELTA_FULL, DELTA_EXACT = 1, 2
+SUB_DETACH = 1
 
 PROGRAMS = (
     "antispoof_ingress", "qos_egress_prog", "qos_ingress_prog", "nat44_egress", "nat44_ingress",
@@ -126,6 +127,8 @@ def load_library() -> C.CDLL:
         "bng_dhcp_lease_sweep": ([vp, u64, u32, vp, u64, vp], C.c_int64),
         "bng_lease_table_rebuilds": ([vp], u64),
         "bng_dhcp_lease_addr_order": ([vp, u32], i32),
+        "bng_sub_export": ([vp, vp, u64, vp, u64, u32, vp, u64, C.POINTER(u64)], i32),
+        "bng_sub_import": ([vp, vp, u64], i32),
     }
     for name, (args, res) in protos.items():
         fn = getattr(lib, name)
@@ -148,6 +151,7 @@ EXPORTED_SYMBOLS = (
     "bng_delta_enable", "bng_delta_export", "bng_delta_apply", "bng_delta_info",
     "bng_idle_enable", "bng_idle_timeout_set", "bng_idle_read", "bng_idle_scan", "bng_nat_usage",
     "bng_dhcp_lease_census", "bng_dhcp_lease_sweep", "bng_lease_table_rebuilds", "bng_dhcp_lease_addr_order",
+    "bng_sub_export", "bng_sub_import",
 )
 
 
@@ -556,6 +560,29 @@ class Dataplane:
         s, q = C.c_uint64(), C.c_uint64()
         self._chk(self.lib.bng_delta_info(self.h, C.byref(s), C.byref(q)), "delta_info")
         return s.value, q.value
+
+    # ---- subscriber hand-over between contexts ----
+    def sub_export(self, addrs, macs=(), detach: bool = False) -> bytes:
+        """The state of a set of subscribers (addresses as u8[n, 4] key bytes or u32[n]; MACs as the u64 key words of
+        subscriber_bindings / subscriber_pools) as one blob for sub_import on another context; detach removes it here."""
+        a = _addr_words(addrs) if len(addrs) else np.zeros(0, "<u4")
+        m = np.ascontiguousarray(np.asarray(macs, dtype="<u8").reshape(-1))
+        flags = SUB_DETACH if detach else 0
+        cap = 1 << 16  # a larger blob is sized by -ENOSPC, which writes and removes nothing
+        while True:
+            buf = np.empty(cap, np.uint8)
+            n = C.c_uint64(0)
+            r = self.lib.bng_sub_export(self.h, a.ctypes.data if len(a) else None, len(a), m.ctypes.data if len(m) else None,
+                                        len(m), flags, buf.ctypes.data, cap, C.byref(n))
+            if r != -errno.ENOSPC:
+                break
+            cap = n.value
+        self._chk(r, "sub_export")
+        return buf[: n.value].tobytes()
+
+    def sub_import(self, blob: bytes) -> int:
+        """Take the subscribers of a sub_export blob into this context; returns 0 (errors raise BngError)."""
+        return self._chk(self.lib.bng_sub_import(self.h, blob, len(blob)), "sub_import")
 
     def sweep(self, now_ns: int) -> int:
         """Session expiry sweep at now_ns; returns the number of sessions removed."""

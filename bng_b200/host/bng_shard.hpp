@@ -49,7 +49,30 @@ class Directory {
     explicit Directory(uint32_t world, uint16_t range_start = 1024, uint16_t ports_per_sub = 1024)
         : world_(world ? world : 1), range_start_(range_start), pps_(ports_per_sub ? ports_per_sub : 1024) {}
     uint32_t World() const { return world_; }
-    uint32_t ShardOfMAC(uint64_t mac) const { return bng_shard_of_mac(mac, world_); }
+    // The owner of a MAC: its pin (Router::Move), else bng_shard_of_mac.  Every other route derives from this one.
+    uint32_t ShardOfMAC(uint64_t mac) const {
+        std::lock_guard<std::mutex> g(mu_);
+        return ShardOfMACLocked(mac);
+    }
+    // A pin overrides the hash for one MAC: a subscriber whose state was moved to another shard stays there.  It lasts
+    // until Unpin or Forget.
+    void Pin(uint64_t mac, uint32_t shard) {
+        std::lock_guard<std::mutex> g(mu_);
+        pins_[mac] = shard;
+    }
+    void Unpin(uint64_t mac) {
+        std::lock_guard<std::mutex> g(mu_);
+        pins_.erase(mac);
+    }
+    // (MAC, address) of every learned subscriber whose owner is shard k
+    std::vector<std::pair<uint64_t, uint32_t>> SubscribersOn(uint32_t k) const {
+        std::lock_guard<std::mutex> g(mu_);
+        std::vector<std::pair<uint64_t, uint32_t>> out;
+        for (const auto &e : mac_ip_)
+            if (ShardOfMACLocked(e.first) == k) out.push_back(e);
+        std::sort(out.begin(), out.end());
+        return out;
+    }
     void Learn(uint64_t mac, uint32_t ip_key) { // lease granted: pkg/dhcp/server.go:1062-1075
         std::lock_guard<std::mutex> g(mu_);
         auto old = mac_ip_.find(mac);
@@ -57,18 +80,22 @@ class Directory {
         mac_ip_[mac] = ip_key;
         ip_mac_[ip_key] = mac;
     }
+    // The subscriber is gone: its address mapping (unless the address has been learned for another MAC since) and its
+    // pin go with it, so a returning MAC is placed by bng_shard_of_mac again.
     void Forget(uint64_t mac) {
         std::lock_guard<std::mutex> g(mu_);
+        pins_.erase(mac);
         auto it = mac_ip_.find(mac);
         if (it == mac_ip_.end()) return;
-        ip_mac_.erase(it->second);
+        auto ip = ip_mac_.find(it->second);
+        if (ip != ip_mac_.end() && ip->second == mac) ip_mac_.erase(ip);
         mac_ip_.erase(it);
     }
     std::optional<uint32_t> ShardOfIP(uint32_t ip_key) const {
         std::lock_guard<std::mutex> g(mu_);
         auto it = ip_mac_.find(ip_key);
         if (it == ip_mac_.end()) return std::nullopt;
-        return bng_shard_of_mac(it->second, world_);
+        return ShardOfMACLocked(it->second);
     }
     // AllocateNAT gave `private_ip_key` the block [port_start, port_end] of public_ip_key
     void AddBlock(uint32_t public_ip_key, uint16_t port_start, uint32_t private_ip_key) {
@@ -126,8 +153,16 @@ class Directory {
     }
 
   private:
+    uint32_t ShardOfMACLocked(uint64_t mac) const {
+        if (!pins_.empty()) {
+            auto p = pins_.find(mac);
+            if (p != pins_.end()) return p->second;
+        }
+        return bng_shard_of_mac(mac, world_);
+    }
     static constexpr uint32_t kNone = 0xFFFFFFFFu;
     uint32_t world_;
+    std::unordered_map<uint64_t, uint32_t> pins_; // MAC -> shard, set by Router::Move
     uint16_t range_start_, pps_;
     mutable std::mutex mu_;
     std::unordered_map<uint64_t, uint32_t> mac_ip_;
@@ -312,6 +347,60 @@ class Router {
     int DeltaApply(size_t k, const void *blob, uint64_t len) {
         if (k >= shards_.size()) return -EINVAL;
         return bng_delta_apply(shards_[k]->ctx, blob, len);
+    }
+    // Subscriber hand-over (bng_sub_export / bng_sub_import): the state of `addrs` (subscriber_nat key words) and
+    // `macs` leaves shard `from` and is taken by shard `to`; on success the MACs are pinned to `to`, so every route
+    // (ShardOfMAC, ShardOfIP, ShardOfPublic, Steer*, Owner and the per-address calls above) follows them there.
+    // When `to` refuses the blob, it goes back into `from` (the import restores a context exactly), the pins stay as
+    // they were and the import's error is returned.  Should `from` refuse it too, the state is on neither shard:
+    // Move returns -ENOTRECOVERABLE and hands the blob to `stranded` (when given) for a later bng_sub_import.  The
+    // blob passes through host memory.
+    int Move(size_t from, size_t to, const std::vector<uint32_t> &addrs, const std::vector<uint64_t> &macs,
+             std::vector<uint8_t> *stranded = nullptr) {
+        if (from >= shards_.size() || to >= shards_.size() || from == to) return -EINVAL;
+        std::vector<uint8_t> blob(1 << 16);
+        for (;;) {
+            uint64_t len = 0;
+            int r = bng_sub_export(shards_[from]->ctx, addrs.data(), addrs.size(), macs.data(), macs.size(), BNG_SUB_DETACH,
+                                   blob.data(), blob.size(), &len);
+            if (r == -ENOSPC && len > blob.size()) {
+                blob.resize(len);
+                continue;
+            }
+            if (r) return r;
+            blob.resize(len);
+            break;
+        }
+        int r = bng_sub_import(shards_[to]->ctx, blob.data(), blob.size());
+        if (r) {
+            if (bng_sub_import(shards_[from]->ctx, blob.data(), blob.size()) == 0) return r;
+            if (stranded) *stranded = std::move(blob);
+            return -ENOTRECOVERABLE;
+        }
+        for (uint64_t m : macs) dir_->Pin(m, (uint32_t)to);
+        return 0;
+    }
+    // Destination of a subscriber drained off shard k: the bng_shard_of_mac(mac, N - 1)-th of the other shards.
+    size_t DrainTarget(size_t k, uint64_t mac) const {
+        const size_t j = bng_shard_of_mac(mac, (uint32_t)shards_.size() - 1);
+        return j < k ? j : j + 1;
+    }
+    // Takes shard k out of service: every subscriber the directory places there moves, MAC and address, to
+    // DrainTarget; one Move per destination.  Returns 0 or the first error (the subscribers of the destinations
+    // before it have moved).
+    int Drain(size_t k) {
+        if (k >= shards_.size() || shards_.size() < 2) return -EINVAL;
+        std::vector<std::vector<uint32_t>> a(shards_.size());
+        std::vector<std::vector<uint64_t>> m(shards_.size());
+        for (const auto &e : dir_->SubscribersOn((uint32_t)k)) {
+            const size_t t = DrainTarget(k, e.first);
+            m[t].push_back(e.first);
+            a[t].push_back(e.second);
+        }
+        for (size_t t = 0; t < shards_.size(); t++)
+            if (!m[t].empty())
+                if (int r = Move(k, t, a[t], m[t])) return r;
+        return 0;
     }
     // Idle detection (bng_idle_*).  A subscriber's record lives on its owner shard only: upstream frames follow its MAC
     // there and downstream frames are steered there by (public address, port block), so the owner's record is the

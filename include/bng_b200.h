@@ -340,6 +340,50 @@ int bng_delta_export(bng_ctx *ctx, uint64_t refresh_ns, uint32_t flags, void *bu
 int bng_delta_apply(bng_ctx *ctx, const void *buf, uint64_t len);
 int bng_delta_info(bng_ctx *ctx, uint64_t *stream_id, uint64_t *seq);
 
+/* ---- subscriber hand-over between contexts (taking a GPU out of service, a CPE swap, rebalancing) ----
+ * A subscriber's state lives on one context only (its shard).  bng_sub_export copies a set of subscribers' state out
+ * of one context, bng_sub_import takes it into another, bit for bit; bng::shard::Router::Move (bng_shard.hpp) does
+ * both and moves the routing with them.  Addresses are the 4 key bytes as subscriber_nat / qos_ingress hold them,
+ * MACs the 8-byte key word of subscriber_bindings / subscriber_pools.
+ * What the export selects (A: the addresses, M: the MACs):
+ *   - subscriber_nat, qos_ingress, qos_egress: the entry keyed by an address in A;
+ *   - nat_sessions: key src_ip in A; nat_reverse: value (the upstream nat_key) src_ip in A, stale entries included;
+ *     eim_table: internal_ip in A (bng_nat_flush's predicates);
+ *   - subscriber_bindings, subscriber_pools: the entry keyed by a MAC in M;
+ *   - the accounting record and the whole idle record (timeout, both stamps, since_ns, flags) of every address in A
+ *     that has one, and the interception target of every address in A that is one.
+ * Replicated maps, statistics and event rings are not part of a subscriber and are never exported.
+ * The blob: char magic[8] = "BNGMOVE1"; uint64 sections; then sections in bng_snapshot's framing: char name[40];
+ * uint32 kind, key_size, value_size, pad (0); uint64 count; count keys; count values.  One section per map above (kind
+ * 0, the map's ABI key / value layout); "subscriber_acct" (kind 5) once accounting records exist and "li_targets"
+ * (kind 6) once interception is in use, as the snapshot defines them; "subscriber_idle_rec" (kind 8: address, struct
+ * bng_idle) once idle records exist.  Entries within a section are in no particular order.
+ * bng_sub_export: staged upserts are applied first and the export sees everything queued on the context's stream, as
+ * bng_snapshot does.  It does not advance the batch sequence.  With BNG_SUB_DETACH, exactly the exported entries are
+ * removed in the same call: no NAT log record is written and no statistic changes (nothing expired or was deleted);
+ * the address maps' entries go through the ordinary delete path, so an address that loses both its subscriber_nat and
+ * qos_ingress entries loses its records as a delete does.  The removal follows bng_nat_flush's flow-table rebuild rule.
+ * Everything that can fail (memory, copies) happens before the blob is written, so a call that returns an error has
+ * removed nothing; once the blob is written the detach completes.  Memory: the first export with addresses allocates
+ * the slot lists, 4 bytes per slot of nat_sessions, nat_reverse and eim_table (80 MiB at the reference's capacities),
+ * and a staging buffer that grows to the largest blob exported; both are kept until bng_close.
+ * When cap is smaller than the blob, nothing is written or removed, *len_out is set to the size needed and -ENOSPC is
+ * returned.  Repeated addresses or MACs, and addresses without state, are harmless.  -EINVAL for a NULL ctx or
+ * len_out, a NULL array with a count > 0, a NULL buf with cap > 0, or unknown flag bits.
+ * bng_sub_import: the whole blob is checked before anything changes: magic, framing and layouts (-EINVAL); room, that
+ * is, for each map, its live entries plus the section's entries <= max_entries, and the interception target limit
+ * (-E2BIG; deliberately conservative: an import never evicts from an LRU map).  Then every entry is inserted or
+ * replaced (BNG_ANY) through bng_map_update_batch's path, after which the records go to the addresses' directory
+ * slots and the targets are set (records are allocated if the context had none, as bng_restore does).  Importing a
+ * blob into the context it came from restores that context exactly: the rollback of a failed hand-over.  Within one
+ * host the clocks agree, so a moved subscriber keeps its idle clock (bng_restore / bng_delta_apply restart clocks).
+ * Cost: the export streams the three flow tables once, one sector per slot (about 0.67 GB at the reference's
+ * capacities); everything else is by key.  No batch runs anything for this. */
+#define BNG_SUB_DETACH 1u /* remove what was exported, in the same call */
+int bng_sub_export(bng_ctx *ctx, const uint32_t *addrs, uint64_t n_addrs, const uint64_t *macs, uint64_t n_macs,
+                   uint32_t flags, void *buf, uint64_t cap, uint64_t *len_out);
+int bng_sub_import(bng_ctx *ctx, const void *buf, uint64_t len);
+
 /* ---- per-subscriber idle detection (what RADIUS Idle-Timeout, attribute 28, needs) ----
  * One record per subscriber address, with the population and lifecycle of the accounting record: an address that keys
  * a subscriber_nat or qos_ingress entry (staged upserts included).  The record starts when the address gets its entry
