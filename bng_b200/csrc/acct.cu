@@ -10,6 +10,10 @@
 // The same pass stamps the idle records (idle.cu) when idle detection is on for the program: the leader of a group of
 // passed frames raises the record's stamp of the direction to the group's latest clock with one atomicMax.  With one
 // clock for the whole batch the leader reads the stamp first and skips the atomic when it is already there.
+//
+// V6 (launched only while subscriber_ipv6 has live entries): an untagged IPv6 frame with verdict TC_ACT_OK belongs to
+// the owner of its source (bytes 22-37, upstream) or destination (38-53, downstream) address, v6_owner, and from there
+// to that IPv4 address's directory slot.  In ACCT_ATTR mode only frames classify left unattributed read the frame.
 #include <errno.h>
 
 #include "kernels.h"
@@ -18,10 +22,12 @@
 #define ACCT_BLOCK 256
 
 // COUNT: add the frames to the counter records; STAMP: stamp the idle records.  <MODE, true, false> is accounting alone.
-template <int MODE, bool COUNT, bool STAMP>
+template <int MODE, bool COUNT, bool STAMP, bool V6>
 __global__ void __launch_bounds__(ACCT_BLOCK) k_acct(const __grid_constant__ Tbl dir, const __grid_constant__ DevBatch b, const u32 *attr,
-                                                      u64 *acct, u64 *idle) {
+                                                      u64 *acct, u64 *idle, const __grid_constant__ Tbl v6) {
     const u32 lane = threadIdx.x & 31;
+    __shared__ V6Lens lens;
+    if (V6) v6_lens_load(lens, v6.plens);
     // warp-uniform trip count: __match_any_sync needs every lane
     for (u32 base = blockIdx.x * ACCT_BLOCK + (threadIdx.x & ~31u); base < b.n; base += gridDim.x * ACCT_BLOCK) {
         const u32 i = base + lane;
@@ -39,6 +45,15 @@ __global__ void __launch_bounds__(ACCT_BLOCK) k_acct(const __grid_constant__ Tbl
                     const u32 off = MODE == ACCT_SRC ? 26 : 30;
                     const u8 *p = frame_ptr(b, i);
                     if (frame_dlen(b, len) >= off + 4 && rd16(p, 12) == ETH_P_IP_LE) slot = dir_slot_of(dir, rd32(p, off));
+                }
+                if (V6 && slot == DIR_NONE && v == TC_OK) { // untagged IPv6 with the address's sixteen bytes present
+                    const u32 off = MODE == ACCT_DST ? 38 : 22;
+                    const u8 *p = frame_ptr(b, i);
+                    u32 a[4], owner;
+                    if (frame_dlen(b, len) >= off + 16 && rd16(p, 12) == ETH_P_IPV6_LE) {
+                        v6_addr(p, off, a);
+                        if (v6_owner(v6, lens, a, &owner)) slot = dir_slot_of(dir, owner);
+                    }
                 }
             }
         }
@@ -123,25 +138,35 @@ static inline int acct_grid(const Launcher &L, u64 n, int per_sm) {
     return (int)(want < 1 ? 1 : (want < cap ? want : cap));
 }
 
-template <int MODE>
-static void launch_acct(Launcher &L, int grid, const Tbl &dir, const DevBatch &b, const u32 *attr, u64 *acct, u64 *idle) {
+template <int MODE, bool V6>
+static void launch_acct(Launcher &L, int grid, const Tbl &dir, const DevBatch &b, const u32 *attr, u64 *acct, u64 *idle, const Tbl &v6) {
     if (acct && idle)
-        k_acct<MODE, true, true><<<grid, ACCT_BLOCK, 0, L.stream>>>(dir, b, attr, acct, idle);
+        k_acct<MODE, true, true, V6><<<grid, ACCT_BLOCK, 0, L.stream>>>(dir, b, attr, acct, idle, v6);
     else if (acct)
-        k_acct<MODE, true, false><<<grid, ACCT_BLOCK, 0, L.stream>>>(dir, b, attr, acct, nullptr);
+        k_acct<MODE, true, false, V6><<<grid, ACCT_BLOCK, 0, L.stream>>>(dir, b, attr, acct, nullptr, v6);
     else
-        k_acct<MODE, false, true><<<grid, ACCT_BLOCK, 0, L.stream>>>(dir, b, attr, nullptr, idle);
+        k_acct<MODE, false, true, V6><<<grid, ACCT_BLOCK, 0, L.stream>>>(dir, b, attr, nullptr, idle, v6);
 }
 
-cudaError_t run_acct(Launcher &L, const Tbl &dir, const DevBatch &b, int mode, u64 *acct, u64 *idle) {
-    const int grid = acct_grid(L, b.n, 8);
-    prof_begin(L, "k_acct");
+template <bool V6>
+static void launch_acct_mode(Launcher &L, int grid, const Tbl &dir, const DevBatch &b, int mode, u64 *acct, u64 *idle, const Tbl &v6) {
     if (mode == ACCT_ATTR)
-        launch_acct<ACCT_ATTR>(L, grid, dir, b, L.acct_attr, acct, idle);
+        launch_acct<ACCT_ATTR, V6>(L, grid, dir, b, L.acct_attr, acct, idle, v6);
     else if (mode == ACCT_SRC)
-        launch_acct<ACCT_SRC>(L, grid, dir, b, nullptr, acct, idle);
+        launch_acct<ACCT_SRC, V6>(L, grid, dir, b, nullptr, acct, idle, v6);
     else
-        launch_acct<ACCT_DST>(L, grid, dir, b, nullptr, acct, idle);
+        launch_acct<ACCT_DST, V6>(L, grid, dir, b, nullptr, acct, idle, v6);
+}
+
+cudaError_t run_acct(Launcher &L, const Tbl &dir, const DevBatch &b, int mode, u64 *acct, u64 *idle, const Tbl *v6) {
+    const int grid = acct_grid(L, b.n, 8);
+    if (v6) {
+        prof_begin(L, "k_acct<v6>");
+        launch_acct_mode<true>(L, grid, dir, b, mode, acct, idle, *v6);
+    } else {
+        prof_begin(L, "k_acct");
+        launch_acct_mode<false>(L, grid, dir, b, mode, acct, idle, Tbl{});
+    }
     prof_end(L);
     L.launches++;
     return cudaGetLastError();

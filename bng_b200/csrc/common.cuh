@@ -68,6 +68,9 @@ struct Tbl {
     // LRU_TS | offset << 8: evict the entry with the oldest u64 timestamp at that slot offset among the
     // slots next to the new key's home; LRU_ANY: no timestamp in the value (nat_reverse): the first live one.
     u32 lru;
+    // LPM-keyed tables only (subscriber_ipv6, below), else nullptr: LPM6_LENS live-entry counts, one per prefix length,
+    // kept by the table-op kernels beside `count`
+    u32 *plens;
 };
 #define LRU_NONE 0u
 #define LRU_TS 1u
@@ -625,6 +628,32 @@ __device__ __forceinline__ bool lpm_match(const LpmTbl &t, u32 addr, u32 maxlen)
         if (((a ^ e) & m) == 0) return true;
     }
     return false;
+}
+
+// ---------------------------------------------------------------------------
+// subscriber_ipv6: IPv6 prefix -> subscriber IPv4 address, an exact-match hash of (prefixlen, masked prefix) keys
+// probed once per prefix length in use, longest first.  The 20-byte key {u32 prefixlen; u8 addr[16]} (the layout of
+// a BPF_MAP_TYPE_LPM_TRIE key) is stored in three key words, the last one's high half zero; the u32 value sits at 24.
+// A 32-byte slot: one probe is one sector.  An address is handled as four little-endian words of its bytes in memory
+// order (a[0] holds bytes 0-3, as rd32 loads them).
+// ---------------------------------------------------------------------------
+#define LPM6_KEY 20u
+#define LPM6_KW 3
+#define LPM6_LENS 129u
+// the first `keep` bits (network order) of a little-endian word of address bytes
+__host__ __device__ __forceinline__ u32 lpm6_keep(u32 w, int keep) {
+    if (keep <= 0) return 0;
+    if (keep >= 32) return w;
+    const u32 m = 0xFFFFFFFFu << (32 - keep); // in numeric (big-endian) order; byte-swapped to memory order below
+    const u32 ml = (m >> 24) | ((m >> 8) & 0xFF00u) | ((m << 8) & 0xFF0000u) | (m << 24);
+    return w & ml;
+}
+// key words of (len, the address's first len bits)
+__host__ __device__ __forceinline__ void lpm6_key(u64 *kw, u32 len, const u32 *a) {
+    const int l = (int)len;
+    kw[0] = (u64)len | (u64)lpm6_keep(a[0], l) << 32;
+    kw[1] = (u64)lpm6_keep(a[1], l - 32) | (u64)lpm6_keep(a[2], l - 64) << 32;
+    kw[2] = (u64)lpm6_keep(a[3], l - 96);
 }
 
 // ---------------------------------------------------------------------------

@@ -169,6 +169,10 @@ struct bng_ctx {
     u32 *mv_lists = nullptr;
     u8 *mv_buf = nullptr;
     u64 mv_cap = 0;
+    // subscriber_ipv6 (not a map of the reference): IPv6 prefix -> subscriber IPv4 address, the attribution of IPv6
+    // frames; v6_live is its live-entry count as of the last command that changed it (0: the IPv6 kernels stay off)
+    Tbl v6{};
+    u32 v6_live = 0;
 };
 
 namespace {
@@ -317,6 +321,25 @@ int make_lpm(bng_ctx *c, LpmTbl *l, u32 max) {
     return dev_alloc(c, (void **)&l->count, 16, 0);
 }
 
+// ---- subscriber_ipv6 ----
+// the host's copy of the live-entry count, which selects the IPv6 instantiations of the attribution kernels
+int v6_refresh_locked(bng_ctx *c) {
+    CU(c, cudaMemcpyAsync(&c->v6_live, c->v6.count, 4, cudaMemcpyDeviceToHost, c->L.stream));
+    CU(c, cudaStreamSynchronize(c->L.stream));
+    return 0;
+}
+// The key as the table holds it: bits past prefixlen cleared (the device masks too; the host does it where keys are
+// compared as bytes, so that two spellings of one prefix count as one key)
+void v6_mask_key(u8 *key) {
+    u32 w[5];
+    memcpy(w, key, 20);
+    if (w[0] >= LPM6_LENS) return; // refused by the device
+    u64 kw[LPM6_KW];
+    lpm6_key(kw, w[0], w + 1);
+    w[1] = (u32)(kw[0] >> 32), w[2] = (u32)kw[1], w[3] = (u32)(kw[1] >> 32), w[4] = (u32)kw[2];
+    memcpy(key, w, 20);
+}
+
 // ---- control-plane commands on hash maps ----
 int hash_cmd(bng_ctx *c, MapReg *m, int op, const void *keys, void *vals, u64 n, u32 flags, int *first_err, u64 *n_err = nullptr) {
     const Tbl &t = *m->tbl;
@@ -350,6 +373,7 @@ int hash_cmd(bng_ctx *c, MapReg *m, int op, const void *keys, void *vals, u64 n,
                     memcpy((u8 *)vals + (done + i) * t.value_size, c->io_host + voff + i * t.value_size, t.value_size);
         }
     }
+    if (m->tbl == &c->v6 && op != TOP_LOOKUP) return v6_refresh_locked(c);
     return 0;
 }
 
@@ -652,6 +676,9 @@ bng_ctx *bng_open(const bng_open_opts *o) {
     OPEN_R(make_table(c, &d.cid_subs, 32, 25, 32, max_subs));
     OPEN_R(make_table(c, &d.ip_pools, 4, 28, 8, 10000));
     OPEN_R(make_table(c, &d.cid_map, 8, 8, 8, max_subs));
+    // subscriber_ipv6: a WAN /64 or /128 and a delegated prefix per subscriber; 32-byte slots (key words, value at 24)
+    OPEN_R(make_table(c, &c->v6, LPM6_KEY, 4, 24, 2 * max_subs));
+    OPEN_R(dev_alloc(c, (void **)&c->v6.plens, LPM6_LENS * 4, 0));
     // subscriber directory: 16-byte slots, as many as the per-subscriber maps have, room for both maps' keys
     OPEN_R(make_table(c, &d.subdir, 4, 8, 8, max_subs, 0, 16));
     d.subdir.max_entries = std::min<u64>(2ull * max_subs, d.subdir.mask);
@@ -698,6 +725,8 @@ bng_ctx *bng_open(const bng_open_opts *o) {
     add_stats(c, "stats_map", T_ARRAY, 80, ST_DHCP);
     add_hash(c, "circuit_id_map", T_HASH, 8, 8, max_subs, &d.cid_map);
     add_hash(c, "circuit_id_subscribers", T_HASH, 32, 25, max_subs, &d.cid_subs);
+    // not a map of the reference: IPv6 prefix -> subscriber IPv4 address (include/bng_b200.h), reported as an LPM trie
+    add_hash(c, "subscriber_ipv6", T_LPM, LPM6_KEY, 4, 2 * max_subs, &c->v6);
     c->staged.resize(c->maps.size());
     OPEN_R(small_refresh(c));
     cudaError_t se = cudaStreamSynchronize(c->L.stream);
@@ -763,6 +792,12 @@ int bng_map_update_batch(bng_ctx *c, int map, const void *keys, const void *valu
         // wherever a key repeats (usually nowhere) and the pieces run in order.
         int first = 0, r = 0;
         const u32 ks = m->key_size;
+        std::vector<u8> masked;
+        if (m->tbl == &c->v6) { // two spellings of one prefix are one key
+            masked.assign((const u8 *)keys, (const u8 *)keys + n * ks);
+            for (u64 i = 0; i < n; i++) v6_mask_key(masked.data() + i * ks);
+            keys = masked.data();
+        }
         u64 seg = 0;
         if (n > 1) {
             std::unordered_set<std::string_view> seen;
@@ -910,6 +945,8 @@ int bng_map_clear(bng_ctx *c, int map) {
     const Tbl &t = *m->tbl;
     CU(c, cudaMemsetAsync(t.slots, 0xFF, ((size_t)t.mask + 1) * t.slot_bytes, c->L.stream));
     CU(c, cudaMemsetAsync(t.count, 0, 4, c->L.stream));
+    if (t.plens) CU(c, cudaMemsetAsync(t.plens, 0, LPM6_LENS * 4, c->L.stream));
+    if (m->tbl == &c->v6) c->v6_live = 0;
     if (m->tbl == &c->dev.sub_nat || m->tbl == &c->dev.qos_in)
         CU(c, run_dir_clear_half(c->L, c->dev.subdir, m->tbl == &c->dev.sub_nat ? 1 : 2));
     CU(c, cudaStreamSynchronize(c->L.stream));
@@ -1077,6 +1114,7 @@ static int dispatch(bng_ctx *c, int prog, const DevBatch &b, const LiSrc &src = 
     const bool idle = c->idle && ((c->idle_progs >> prog) & 1);
     const int li = c->li_targets.empty() ? -1 : k_li_dir[prog]; // no target: not one kernel more
     const bool pipe = prog == P_PIPE_UP || prog == P_PIPE_TC;
+    const Tbl *v6 = c->v6_live ? &c->v6 : nullptr; // an empty table launches exactly what it did before it existed
     // the upstream classify records attributions: for accounting and idle detection, and in the pipelines to tell
     // antispoof's drops
     c->L.acct_attr = (acct || idle || (li == 0 && pipe)) ? c->L.s.attr : nullptr;
@@ -1088,7 +1126,7 @@ static int dispatch(bng_ctx *c, int prog, const DevBatch &b, const LiSrc &src = 
     }
     if (li == 0) { // the frames as they entered, before the program rewrites them
         e = cudaMemsetAsync(c->li_ctl + 2, 0, 4, c->L.stream);
-        if (e == cudaSuccess) e = run_li_capture(c->L, r, b, src, true);
+        if (e == cudaSuccess) e = run_li_capture(c->L, r, b, src, true, v6);
         if (e != cudaSuccess) return fail(c, -EIO, "launch k_li_capture: %s", cudaGetErrorString(e));
     }
     switch (prog) {
@@ -1104,9 +1142,9 @@ static int dispatch(bng_ctx *c, int prog, const DevBatch &b, const LiSrc &src = 
     default: return -EINVAL;
     }
     // after the program, before anything copies the frames out: the downstream modes read the rewritten headers
-    if (e == cudaSuccess && (acct || idle)) e = run_acct(c->L, c->dev.subdir, b, k_acct_mode[prog], acct ? c->acct : nullptr, idle ? c->idle : nullptr);
+    if (e == cudaSuccess && (acct || idle)) e = run_acct(c->L, c->dev.subdir, b, k_acct_mode[prog], acct ? c->acct : nullptr, idle ? c->idle : nullptr, v6);
     if (e == cudaSuccess && li == 0) e = run_li_verdict(c->L, r, b, pipe ? c->L.s.attr : nullptr);
-    if (e == cudaSuccess && li == 1) e = run_li_capture(c->L, r, b, src, false);
+    if (e == cudaSuccess && li == 1) e = run_li_capture(c->L, r, b, src, false, v6);
     if (e != cudaSuccess) return fail(c, -EIO, "launch %s: %s", k_prog_names[prog], cudaGetErrorString(e));
     return 0;
 }
@@ -1363,6 +1401,16 @@ int bng_map_update_staged(bng_ctx *c, int map, const void *key, const void *valu
     std::lock_guard<std::mutex> g(c->mu);
     bng_ctx::Staged &q = c->staged[map];
     q.keys.insert(q.keys.end(), (const u8 *)key, (const u8 *)key + m->key_size);
+    if (m->tbl == &c->v6) { // the last staged value of a prefix wins, however its key was spelled
+        u8 *k = q.keys.data() + q.keys.size() - m->key_size;
+        u32 pl;
+        memcpy(&pl, k, 4);
+        if (pl >= LPM6_LENS) {
+            q.keys.resize(q.keys.size() - m->key_size);
+            return -EINVAL;
+        }
+        v6_mask_key(k);
+    }
     q.vals.insert(q.vals.end(), (const u8 *)value, (const u8 *)value + m->value_size);
     q.n++;
     c->staged_total++;
@@ -2590,7 +2638,7 @@ DeltaTbl delta_view(bng_ctx *c, const bng_ctx::DeltaShadow &s, u64 refresh, bool
     const MapReg &m = c->maps[s.map];
     const Tbl &tb = *m.tbl;
     t.slots = tb.slots, t.slot_bytes = tb.slot_bytes;
-    t.kw = tb.key_size <= 8 ? 1 : tb.key_size / 8;
+    t.kw = tb.key_size <= 8 ? 1 : (tb.key_size + 7) / 8;
     t.key_size = tb.key_size, t.value_size = tb.value_size, t.voff = tb.voff, t.vlayout = tb.vlayout;
     const bool ses = tb.vlayout == VL_SESSION, eim = !strcmp(m.name, "eim_table");
     const bool qos = !strcmp(m.name, "qos_ingress") || !strcmp(m.name, "qos_egress");
@@ -3025,18 +3073,20 @@ int bng_sub_export(bng_ctx *c, const uint32_t *addrs, uint64_t n_addrs, const ui
     while (slots < 2 * na) slots *= 2;
     if (slots > (1ull << 32)) return fail(c, -EINVAL, "sub_export: %llu addresses", (unsigned long long)na);
     const DevCtx &d = c->dev;
-    const u64 ns = (u64)d.sessions.mask + 1, nr = (u64)d.reverse.mask + 1, ne = (u64)d.eim.mask + 1;
-    // the slot lists (4 bytes per slot of the three flow tables), allocated by the first export that has addresses
-    if (na && !c->mv_lists && cudaMalloc((void **)&c->mv_lists, (ns + nr + ne) * 4) != cudaSuccess) {
+    const u64 ns = (u64)d.sessions.mask + 1, nr = (u64)d.reverse.mask + 1, ne = (u64)d.eim.mask + 1, n6s = (u64)c->v6.mask + 1;
+    // the slot lists (4 bytes per slot of the three flow tables and subscriber_ipv6), allocated by the first export that
+    // has addresses
+    if (na && !c->mv_lists && cudaMalloc((void **)&c->mv_lists, (ns + nr + ne + n6s) * 4) != cudaSuccess) {
         cudaGetLastError();
         c->mv_lists = nullptr;
-        return fail(c, -ENOMEM, "sub_export: %llu bytes of device memory", (unsigned long long)((ns + nr + ne) * 4));
+        return fail(c, -ENOMEM, "sub_export: %llu bytes of device memory", (unsigned long long)((ns + nr + ne + n6s) * 4));
     }
+    u32 *v6_list = c->mv_lists ? c->mv_lists + ns + nr + ne : nullptr;
     // staging: [in] address set, addresses, MACs, counters; [out] lookups by key, then the gathered flow entries
     MapReg *am[3], *mm[2], *fm[3];
     for (int k = 0; k < 3; k++) am[k] = get_map(c, bng_map_id(c, kMoveAddrMaps[k])), fm[k] = get_map(c, bng_map_id(c, kMoveFlowMaps[k]));
     for (int k = 0; k < 2; k++) mm[k] = get_map(c, bng_map_id(c, kMoveMacMaps[k]));
-    const size_t aoff = al256(slots * 8), moff = al256(aoff + na * 4), coff = al256(moff + nm * 8), out0 = al256(coff + 16);
+    const size_t aoff = al256(slots * 8), moff = al256(aoff + na * 4), coff = al256(moff + nm * 8), out0 = al256(coff + 32);
     size_t at = out0, am_v[3], am_r[3], mm_v[2], mm_r[2], acct_v = 0, acct_r = 0, idle_v = 0, idle_r = 0;
     for (int k = 0; k < 3; k++) am_v[k] = at, am_r[k] = al256(at + na * am[k]->value_size), at = al256(am_r[k] + na * 4);
     for (int k = 0; k < 2; k++) mm_v[k] = at, mm_r[k] = al256(at + nm * mm[k]->value_size), at = al256(mm_r[k] + nm * 4);
@@ -3067,10 +3117,12 @@ int bng_sub_export(bng_ctx *c, const uint32_t *addrs, uint64_t n_addrs, const ui
     if (c->acct) CU(c, run_acct_read(c->L, d.subdir, c->acct, (const u32 *)(dv + aoff), na, (u64 *)(dv + acct_v), (int *)(dv + acct_r)));
     if (c->idle) CU(c, run_idle_read(c->L, d.subdir, c->idle, (const u32 *)(dv + aoff), na, (u64 *)(dv + idle_v), (int *)(dv + idle_r)));
     u32 *cnt = (u32 *)(dv + coff);
-    CU(c, cudaMemsetAsync(cnt, 0, 16, c->L.stream));
+    CU(c, cudaMemsetAsync(cnt, 0, 32, c->L.stream));
     if (na) CU(c, run_move_select(c->L, d, AddrSet{(const u64 *)dv, mask}, c->mv_lists, cnt));
-    u32 n4[4] = {0, 0, 0, 0};
-    CU(c, cudaMemcpyAsync(n4, cnt, 16, cudaMemcpyDeviceToHost, c->L.stream));
+    // subscriber_ipv6 by value, only while it has entries: an export from a context that never used it launches nothing more
+    if (na && c->v6_live) CU(c, run_move_select_v6(c->L, c->v6, AddrSet{(const u64 *)dv, mask}, v6_list, cnt + 4));
+    u32 n4[5] = {0, 0, 0, 0, 0}; // entries listed in nat_sessions, nat_reverse, eim_table; tombstones; subscriber_ipv6
+    CU(c, cudaMemcpyAsync(n4, cnt, 20, cudaMemcpyDeviceToHost, c->L.stream));
     CU(c, cudaStreamSynchronize(c->L.stream));
     // the delta exporter's gather turns the slot lists into ABI keys and values
     size_t fk[3], fv[3];
@@ -3079,6 +3131,9 @@ int bng_sub_export(bng_ctx *c, const uint32_t *addrs, uint64_t n_addrs, const ui
         const Tbl &t = *fm[k]->tbl;
         fk[k] = at, fv[k] = at + (size_t)n4[k] * t.key_size, at = al256(fv[k] + (size_t)n4[k] * t.value_size);
     }
+    const u32 n6 = n4[4];
+    const size_t v6k = at, v6v = al256(v6k + (size_t)n6 * LPM6_KEY), v6r = al256(v6v + (size_t)n6 * 4); // v6r: the detach's results
+    if (n6) at = al256(v6r + (size_t)n6 * 4);
     if (int r = mv_grow(c, at, flow0)) return r;
     dv = c->mv_buf;
     for (int k = 0; k < 3 && c->mv_lists; k++) {
@@ -3088,6 +3143,12 @@ int bng_sub_export(bng_ctx *c, const uint32_t *addrs, uint64_t n_addrs, const ui
         v.slots = t.slots, v.slot_bytes = t.slot_bytes, v.nslots = (u64)t.mask + 1;
         v.key_size = t.key_size, v.value_size = t.value_size, v.voff = t.voff, v.vlayout = t.vlayout;
         CU(c, run_delta_emit(c->L, v, nullptr, 0, lists[k], n4[k], nullptr, dv + fk[k], dv + fv[k]));
+    }
+    if (n6) {
+        DeltaTbl v{};
+        v.slots = c->v6.slots, v.slot_bytes = c->v6.slot_bytes, v.nslots = n6s;
+        v.key_size = c->v6.key_size, v.value_size = c->v6.value_size, v.voff = c->v6.voff;
+        CU(c, run_delta_emit(c->L, v, nullptr, 0, v6_list, n6, nullptr, dv + v6k, dv + v6v));
     }
     std::vector<u8> got(at - out0);
     CU(c, cudaMemcpyAsync(got.data(), dv + out0, got.size(), cudaMemcpyDeviceToHost, c->L.stream)); // the one copy out
@@ -3120,6 +3181,13 @@ int bng_sub_export(bng_ctx *c, const uint32_t *addrs, uint64_t n_addrs, const ui
         put_section(out, m->name, KIND_HASH, m->key_size, m->value_size, 0, n4[k]);
         out.insert(out.end(), host(fk[k]), host(fk[k]) + (size_t)n4[k] * m->key_size);
         out.insert(out.end(), host(fv[k]), host(fv[k]) + (size_t)n4[k] * m->value_size);
+        nsec++;
+    }
+    const MapReg *m6 = get_map(c, bng_map_id(c, "subscriber_ipv6"));
+    if (n6) { // only when there is one, so that blobs without IPv6 prefixes stay as they were
+        put_section(out, m6->name, KIND_HASH, m6->key_size, m6->value_size, 0, n6);
+        out.insert(out.end(), host(v6k), host(v6k) + (size_t)n6 * LPM6_KEY);
+        out.insert(out.end(), host(v6v), host(v6v) + (size_t)n6 * 4);
         nsec++;
     }
     auto records = [&](const char *name, u32 kind, size_t rs, size_t voff, size_t roff) {
@@ -3162,12 +3230,16 @@ int bng_sub_export(bng_ctx *c, const uint32_t *addrs, uint64_t n_addrs, const ui
         CU(c, run_table_op(c->L, *m->tbl, TOP_DELETE, dv + (k < 3 ? aoff : moff), nullptr, (int *)(dv + (k < 3 ? am_r[k] : mm_r[k - 3])),
                            k < 3 ? na : nm, 0, d.subdir, role, c->acct, c->idle));
     }
+    if (n6) CU(c, run_table_op(c->L, c->v6, TOP_DELETE, dv + v6k, nullptr, (int *)(dv + v6r), n6, 0, d.subdir, 0, nullptr, nullptr));
     if (!li_a.empty()) {
         for (u32 a : li_a) c->li_targets.erase(a);
         c->li_dirty = true;
     }
     CU(c, cudaStreamSynchronize(c->L.stream));
     prof_collect(c->L);
+    if (n6) {
+        if (int r = v6_refresh_locked(c)) return r;
+    }
     // the flush's rebuild rule; a rebuild that finds no memory leaves the tables as they were, and the detach stands
     if (rebuild_if_tombstoned_locked(c, n4[3] + n4[0])) cudaGetLastError();
     return 0;
@@ -3284,6 +3356,16 @@ int bng_stats_device_ptr(bng_ctx *c, void **dptr, uint32_t *n_u64) {
 }
 
 uint64_t bng_launch_count(bng_ctx *c) { return c ? c->L.launches : 0; }
+
+int bng_ipv6_prefix_lengths(bng_ctx *c, uint32_t *counts) {
+    if (!c || !counts) return -EINVAL;
+    std::lock_guard<std::mutex> g(c->mu);
+    cudaSetDevice(c->device);
+    if (int fr = flush_staged_locked(c, bng_map_id(c, "subscriber_ipv6"))) return fr;
+    CU(c, cudaMemcpyAsync(counts, c->v6.plens, LPM6_LENS * 4, cudaMemcpyDeviceToHost, c->L.stream));
+    CU(c, cudaStreamSynchronize(c->L.stream));
+    return 0;
+}
 
 int bng_prof_enable(bng_ctx *c, int on) {
     if (!c) return -EINVAL;

@@ -109,9 +109,52 @@ __device__ __forceinline__ u32 dir_slot_of(const Tbl &dir, u32 addr) {
     const u8 *s = tbl_find<1, false>(dir, &k);
     return s ? (u32)((s - dir.slots) >> 4) : DIR_NONE;
 }
+#ifdef __CUDACC__
+// subscriber_ipv6 (common.cuh): the value of the entry (len, the address's first len bits), if there is one
+__device__ __forceinline__ bool lpm6_probe(const Tbl &t, u32 len, const u32 *a, u32 *val) {
+    u64 kw[LPM6_KW];
+    lpm6_key(kw, len, a);
+    const u8 *s = tbl_find<LPM6_KW, false>(t, kw);
+    if (s) *val = *(const u32 *)(s + t.voff);
+    return s != nullptr;
+}
+// The prefix lengths that have live entries, longest first, in shared memory: built once per block from the table's
+// counts by the whole block (blockDim.x >= 160), so a frame probes only the lengths in use.
+struct V6Lens {
+    u8 len[LPM6_LENS];
+    u32 n, wcnt[5];
+};
+__device__ __forceinline__ void v6_lens_load(V6Lens &s, const u32 *plens) {
+    const u32 t = threadIdx.x, lane = t & 31, w = t >> 5; // thread t stands for length 128 - t
+    const bool live = t < LPM6_LENS && plens[LPM6_LENS - 1 - t] != 0;
+    const u32 m = __ballot_sync(0xffffffffu, live);
+    if (lane == 0 && w < 5) s.wcnt[w] = __popc(m);
+    __syncthreads();
+    if (live) {
+        u32 pos = __popc(m & ((1u << lane) - 1));
+        for (u32 j = 0; j < w; j++) pos += s.wcnt[j];
+        s.len[pos] = (u8)(LPM6_LENS - 1 - t);
+    }
+    if (t == 0) s.n = s.wcnt[0] + s.wcnt[1] + s.wcnt[2] + s.wcnt[3] + s.wcnt[4];
+    __syncthreads();
+}
+// The owner of an IPv6 address: the value of the longest prefix in subscriber_ipv6 that covers it (a subscriber IPv4
+// address in qos_ingress key order).  One probe per prefix length in use until one hits.
+__device__ __forceinline__ bool v6_owner(const Tbl &t, const V6Lens &s, const u32 *a, u32 *owner) {
+    for (u32 k = 0; k < s.n; k++)
+        if (lpm6_probe(t, s.len[k], a, owner)) return true;
+    return false;
+}
+// the 16 address bytes at frame offset off as four little-endian words (off even)
+__device__ __forceinline__ void v6_addr(const u8 *p, u32 off, u32 *a) {
+#pragma unroll
+    for (int j = 0; j < 4; j++) a[j] = rd32(p, off + 4 * j);
+}
+#endif
 // acct: count the frames into the counter records (nullptr: no counting); idle: stamp the idle records of the frames
-// that pass (nullptr: no stamping).  At least one of the two is given.
-cudaError_t run_acct(Launcher &L, const Tbl &dir, const DevBatch &b, int mode, u64 *acct, u64 *idle);
+// that pass (nullptr: no stamping).  At least one of the two is given.  v6: subscriber_ipv6 while it has live entries
+// (IPv6 frames are attributed through it), else nullptr.
+cudaError_t run_acct(Launcher &L, const Tbl &dir, const DevBatch &b, int mode, u64 *acct, u64 *idle, const Tbl *v6);
 // results[i] = 0 / -ENOENT, out[i] zeroed on a miss; acct may be nullptr (every record reads as zero)
 cudaError_t run_acct_read(Launcher &L, const Tbl &dir, const u64 *acct, const u32 *addrs, u64 n, u64 *out, int *results);
 // every directory address with its record, compacted at *count (grows past cap: only cap are written)
@@ -144,6 +187,8 @@ cudaError_t run_idle_load(Launcher &L, const Tbl &dir, u64 *idle, const u32 *add
 cudaError_t run_move_select(Launcher &L, const DevCtx &c, const AddrSet &a, u32 *lists, u32 *cnt);
 // tombstones the listed slots (no log record, no statistic); n[k] entries of table k's list
 cudaError_t run_move_detach(Launcher &L, const DevCtx &c, const u32 *lists, const u32 n[3]);
+// the slots of subscriber_ipv6 whose value is in the address set, listed at `list` (room for every slot), *cnt of them
+cudaError_t run_move_select_v6(Launcher &L, const Tbl &v6, const AddrSet &a, u32 *list, u32 *cnt);
 
 // NAT port-usage census (natuse.cu).  Scratch of its own, zeroed before every census:
 //   set        set_mask + 1 u64 words, 0 = empty: the distinct held triples and ports, overall and per subscriber.  A
@@ -248,7 +293,8 @@ struct LiSrc {
 // UP: before the program (the frame as it entered), reserves the slots and lists the matches; then run_li_verdict
 // after the program.  !UP: after the program, complete records.  attr: classify's attribution words in the pipelines
 // (a SHOT frame without one was dropped by antispoof), else nullptr.
-cudaError_t run_li_capture(Launcher &L, const LiRing &r, const DevBatch &b, const LiSrc &src, bool up);
+// v6: as run_acct's.
+cudaError_t run_li_capture(Launcher &L, const LiRing &r, const DevBatch &b, const LiSrc &src, bool up, const Tbl *v6);
 cudaError_t run_li_verdict(Launcher &L, const LiRing &r, const DevBatch &b, const u32 *attr);
 
 // incremental replication (delta.cu).  A table as the diff sees it: nslots slots whose first kw words are the key (word

@@ -10,6 +10,10 @@
 //   - downstream, k_li_capture<false> AFTER the program: the destination address it leaves with, the frame as the
 //     program left it (after DNAT), the verdict: complete records in one pass (the shape of k_acct<ACCT_DST>).
 // The target set is a few KB at most (<= BNG_LI_MAX_TARGETS addresses at load <= 1/2): its probes stay in L1 / L2.
+// V6 (launched only while subscriber_ipv6 has live entries): an untagged IPv6 frame is captured for the owner of its
+// source (bytes 22-37, upstream) or destination (38-53, downstream), v6_owner; that IPv4 address is probed in the target
+// set and goes into the record.  Downstream only a TC_ACT_OK frame is attributed; upstream k_li_verdict voids a SHOT
+// one, which in a pipeline is antispoof's (NAT and QoS pass every non-IPv4 frame) and elsewhere cannot happen.
 #include "kernels.h"
 #include "progs.cuh"
 
@@ -51,10 +55,12 @@ __device__ __forceinline__ uint4 li_unit(const u8 *p, const u8 *tail, u32 split,
     return w;
 }
 
-template <bool UP>
+template <bool UP, bool V6>
 __global__ void __launch_bounds__(LI_BLOCK) k_li_capture(const __grid_constant__ LiRing r, const __grid_constant__ DevBatch b,
-                                                         const __grid_constant__ LiSrc src) {
+                                                         const __grid_constant__ LiSrc src, const __grid_constant__ Tbl v6) {
     const u32 lane = threadIdx.x & 31, below = (1u << lane) - 1;
+    __shared__ V6Lens lens;
+    if (V6) v6_lens_load(lens, v6.plens);
     const u32 units = (r.rec_bytes - LI_HDR) / 16;
     // warp-uniform trip count: the ballots and the cooperative copy need every lane
     for (u32 base = blockIdx.x * LI_BLOCK + (threadIdx.x & ~31u); base < b.n; base += gridDim.x * LI_BLOCK) {
@@ -73,6 +79,10 @@ __global__ void __launch_bounds__(LI_BLOCK) k_li_capture(const __grid_constant__
             if ((UP || v == TC_OK || v == TC_SHOT) && have >= off + 4 && rd16(p, 12) == ETH_P_IP_LE) {
                 addr = rd32(p, off);
                 t = li_find(r.tgt, addr);
+            } else if (V6 && (UP || v == TC_OK) && have >= (UP ? 38u : 54u) && rd16(p, 12) == ETH_P_IPV6_LE) {
+                u32 a[4];
+                v6_addr(p, UP ? 22 : 38, a);
+                if (v6_owner(v6, lens, a, &addr)) t = li_find(r.tgt, addr);
             }
         }
         const u32 m = __ballot_sync(0xffffffffu, t >= 0);
@@ -144,14 +154,20 @@ static inline int li_grid(const Launcher &L, u64 n, int per_sm) {
     return (int)(want < 1 ? 1 : (want < cap ? want : cap));
 }
 
-cudaError_t run_li_capture(Launcher &L, const LiRing &r, const DevBatch &b, const LiSrc &src, bool up) {
+cudaError_t run_li_capture(Launcher &L, const LiRing &r, const DevBatch &b, const LiSrc &src, bool up, const Tbl *v6) {
     const int grid = li_grid(L, b.n, 8);
-    if (up) {
+    if (up && v6) {
+        prof_begin(L, "k_li_capture<up,v6>");
+        k_li_capture<true, true><<<grid, LI_BLOCK, 0, L.stream>>>(r, b, src, *v6);
+    } else if (up) {
         prof_begin(L, "k_li_capture<up>");
-        k_li_capture<true><<<grid, LI_BLOCK, 0, L.stream>>>(r, b, src);
+        k_li_capture<true, false><<<grid, LI_BLOCK, 0, L.stream>>>(r, b, src, Tbl{});
+    } else if (v6) {
+        prof_begin(L, "k_li_capture<down,v6>");
+        k_li_capture<false, true><<<grid, LI_BLOCK, 0, L.stream>>>(r, b, src, *v6);
     } else {
         prof_begin(L, "k_li_capture<down>");
-        k_li_capture<false><<<grid, LI_BLOCK, 0, L.stream>>>(r, b, src);
+        k_li_capture<false, false><<<grid, LI_BLOCK, 0, L.stream>>>(r, b, src, Tbl{});
     }
     prof_end(L);
     L.launches++;

@@ -11,6 +11,9 @@
 // no log record and touches no counter but the tables' live counts: nothing expired, the state lives on elsewhere.
 // The per-address and per-MAC maps are reached by key through the table-op kernels (tableops.cu), so the subscriber
 // directory stays derived state.
+// subscriber_ipv6 is keyed by prefix and selected by value (the owner's IPv4 address in A): k_move_select_v6 lists its
+// matching slots the same way, launched only while the table has live entries.  Its detach deletes the gathered keys
+// through the table-op path, which keeps the per-length counts.
 #include "kernels.h"
 
 #define MOVE_BLOCK 256
@@ -65,6 +68,20 @@ __global__ void __launch_bounds__(MOVE_BLOCK) k_move_select(const __grid_constan
     if (lane == 0 && s) atomicAdd(cnt + 3, s);
 }
 
+__global__ void __launch_bounds__(MOVE_BLOCK) k_move_select_v6(const __grid_constant__ Tbl t, const AddrSet a, u32 *list, u32 *cnt) {
+    const u64 n = (u64)t.mask + 1;
+    const u32 lane = threadIdx.x & 31;
+    for (u64 base = blockIdx.x * (u64)MOVE_BLOCK + (threadIdx.x & ~31u); base < n; base += (u64)gridDim.x * MOVE_BLOCK) {
+        const u64 i = base + lane;
+        bool take = false;
+        if (i < n) {
+            const u8 *s = t.slots + i * t.slot_bytes;
+            take = __ldg((const unsigned long long *)s) < K_BUSY && aset_has(a, *(const u32 *)(s + t.voff));
+        }
+        move_push(list, cnt, take, (u32)i);
+    }
+}
+
 __global__ void k_move_detach(const __grid_constant__ DevCtx c, const u32 *lists, uint3 n) {
     const u64 ns = (u64)c.sessions.mask + 1, nr = (u64)c.reverse.mask + 1;
     const u64 total = (u64)n.x + n.y + n.z;
@@ -95,6 +112,14 @@ cudaError_t run_move_detach(Launcher &L, const DevCtx &c, const u32 *lists, cons
     if (total == 0) return cudaSuccess;
     prof_begin(L, "k_move_detach");
     k_move_detach<<<move_grid(L, total), MOVE_BLOCK, 0, L.stream>>>(c, lists, make_uint3(n[0], n[1], n[2]));
+    prof_end(L);
+    L.launches++;
+    return cudaGetLastError();
+}
+
+cudaError_t run_move_select_v6(Launcher &L, const Tbl &v6, const AddrSet &a, u32 *list, u32 *cnt) {
+    prof_begin(L, "k_move_select_v6");
+    k_move_select_v6<<<move_grid(L, (u64)v6.mask + 1), MOVE_BLOCK, 0, L.stream>>>(v6, a, list, cnt);
     prof_end(L);
     L.launches++;
     return cudaGetLastError();

@@ -9,6 +9,11 @@ template <int KW>
 __device__ __forceinline__ void load_key(const Tbl &t, const u8 *kb, u64 *kw) {
     if (t.key_size == 4) {
         kw[0] = *(const u32 *)kb;
+    } else if (KW == LPM6_KW) { // 20 bytes, 4-byte aligned in a packed key array; the last word's high half zero
+        const u32 *k = (const u32 *)kb;
+        kw[0] = k[0] | (u64)k[1] << 32;
+        kw[1] = k[2] | (u64)k[3] << 32;
+        kw[2] = k[4];
     } else {
 #pragma unroll
         for (int j = 0; j < KW; j++) kw[j] = *(const u64 *)(kb + 8 * j);
@@ -82,6 +87,24 @@ __global__ void k_table_op(const __grid_constant__ Tbl t, int op, const u8 *keys
         u64 kw[KW];
         load_key<KW>(t, keys + i * t.key_size, kw);
         int r = 0;
+        if (KW == LPM6_KW) { // subscriber_ipv6 (the only table with this key width)
+            const u32 pl = (u32)kw[0];
+            if (pl >= LPM6_LENS) {
+                results[i] = -EINVAL;
+                continue;
+            }
+            const u32 a[4] = {(u32)(kw[0] >> 32), (u32)kw[1], (u32)(kw[1] >> 32), (u32)kw[2]};
+            if (op == TOP_LOOKUP) { // the trie's lookup: the longest prefix of length <= prefixlen covering the address
+                u32 v = 0;
+                r = -ENOENT;
+                for (int l = (int)pl; l >= 0 && r; l--)
+                    if (t.plens[l] && lpm6_probe(t, (u32)l, a, &v)) r = 0;
+                if (!r) *(u32 *)(vals + i * t.value_size) = v;
+                results[i] = r;
+                continue;
+            }
+            lpm6_key(kw, pl, a); // update and delete match (prefixlen, prefix) exactly: bits past prefixlen are masked off
+        }
         if (kw[0] >= K_BUSY) {
             r = (op == TOP_UPDATE) ? -EINVAL : -ENOENT; // reserved key patterns cannot be stored
         } else if (op == TOP_LOOKUP) {
@@ -93,6 +116,7 @@ __global__ void k_table_op(const __grid_constant__ Tbl t, int op, const u8 *keys
         } else if (op == TOP_DELETE) {
             r = tbl_erase<KW>(t, kw) ? 0 : -ENOENT;
             if (!r && dir_role) dir_unset(dir, kw[0], dir_role);
+            if (!r && KW == LPM6_KW) atomicSub(t.plens + (u32)kw[0], 1u);
         } else {
             const u8 *v = vals + i * t.value_size;
             u8 *s = nullptr;
@@ -114,6 +138,7 @@ __global__ void k_table_op(const __grid_constant__ Tbl t, int op, const u8 *keys
                         for (u32 z = 8 * KW; z < t.slot_bytes; z += 8) *(u64 *)(s + z) = 0;
                     val_to_slot(t, s, v);
                     if (created) tbl_publish(s, kw[0]);
+                    if (created && KW == LPM6_KW) atomicAdd(t.plens + (u32)kw[0], 1u);
                 }
             }
             if (!r && dir_role) dir_set(dir, kw[0], dir_role, dir_value(t, s, dir_role), acct, idle);
@@ -166,6 +191,8 @@ cudaError_t run_table_op(Launcher &L, const Tbl &t, int op, const u8 *keys, u8 *
         k_table_op<1><<<grid, block, 0, L.stream>>>(t, op, keys, vals, results, n, flags, dir, dir_role, acct, idle);
     else if (t.key_size == 16)
         k_table_op<2><<<grid, block, 0, L.stream>>>(t, op, keys, vals, results, n, flags, dir, 0, nullptr, nullptr);
+    else if (t.key_size == LPM6_KEY)
+        k_table_op<LPM6_KW><<<grid, block, 0, L.stream>>>(t, op, keys, vals, results, n, flags, dir, 0, nullptr, nullptr);
     else
         k_table_op<4><<<grid, block, 0, L.stream>>>(t, op, keys, vals, results, n, flags, dir, 0, nullptr, nullptr);
     L.launches++;
@@ -197,6 +224,8 @@ cudaError_t run_table_rebuild(Launcher &L, const Tbl &o, const Tbl &nw) {
         k_table_rebuild<1><<<L.num_sms * 8, 256, 0, L.stream>>>(o, nw);
     else if (o.key_size == 16)
         k_table_rebuild<2><<<L.num_sms * 8, 256, 0, L.stream>>>(o, nw);
+    else if (o.key_size == LPM6_KEY)
+        k_table_rebuild<LPM6_KW><<<L.num_sms * 8, 256, 0, L.stream>>>(o, nw);
     else
         k_table_rebuild<4><<<L.num_sms * 8, 256, 0, L.stream>>>(o, nw);
     L.launches++;

@@ -13,7 +13,7 @@ import os
 import numpy as np
 
 from .layouts import as_bytes, bng_acct, bng_idle, bng_li_record, bng_nat_pub_use, bng_nat_sub_use, bng_nat_usage_sum
-from .layouts import bng_lease_pool_use, bng_lease_removed, bng_lease_sum
+from .layouts import bng_ipv6_prefix_key, bng_lease_pool_use, bng_lease_removed, bng_lease_sum
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("BNG_B200_LIB") or os.path.join(HERE, "libbng_b200.so")  # override: A/B builds
@@ -98,6 +98,7 @@ def load_library() -> C.CDLL:
         "bng_shard_of_mac": ([u64, u32], u32),
         "bng_stats_device_ptr": ([vp, C.POINTER(vp), C.POINTER(u32)], i32),
         "bng_launch_count": ([vp], u64),
+        "bng_ipv6_prefix_lengths": ([vp, vp], i32),
         "bng_lru_overflow": ([vp], u64),
         "bng_events_lost": ([vp], u64),
         "bng_prof_enable": ([vp, i32], i32),
@@ -151,7 +152,7 @@ EXPORTED_SYMBOLS = (
     "bng_delta_enable", "bng_delta_export", "bng_delta_apply", "bng_delta_info",
     "bng_idle_enable", "bng_idle_timeout_set", "bng_idle_read", "bng_idle_scan", "bng_nat_usage",
     "bng_dhcp_lease_census", "bng_dhcp_lease_sweep", "bng_lease_table_rebuilds", "bng_dhcp_lease_addr_order",
-    "bng_sub_export", "bng_sub_import",
+    "bng_sub_export", "bng_sub_import", "bng_ipv6_prefix_lengths",
 )
 
 
@@ -290,6 +291,26 @@ class Dataplane:
             order = np.lexsort(keys.T[::-1])
             keys, vals = keys[order], vals[order]
         return keys, vals
+
+    def ipv6_prefixes_set(self, prefixes, lens, addrs=None, remove: bool = False) -> int:
+        """Install subscribers' IPv6 addresses and prefixes (Framed-IPv6-Prefix, Delegated-IPv6-Prefix) in
+        subscriber_ipv6, or with remove=True delete them.  prefixes: u8[n, 16] or 16-byte bytes objects; lens: the
+        prefix lengths; addrs: the owners' IPv4 addresses (u8[n, 4] key bytes or u32 words; not needed to remove).
+        Returns 0 or the first negative errno (a removal that finds a prefix absent reports -ENOENT)."""
+        p = np.asarray([np.frombuffer(x, np.uint8) if isinstance(x, (bytes, bytearray)) else x for x in prefixes], np.uint8)
+        keys = np.zeros(len(p), bng_ipv6_prefix_key)
+        keys["prefixlen"] = np.asarray(lens, np.uint32).reshape(-1)
+        keys["addr"] = p.reshape(-1, 16)
+        if remove:
+            rs = [self.delete("subscriber_ipv6", k) for k in keys]
+            return next((r for r in rs if r), 0)
+        return self.update_batch("subscriber_ipv6", keys, _addr_words(addrs).reshape(-1, 1).view(np.uint8))
+
+    def ipv6_prefix_lengths(self) -> np.ndarray:
+        """Live subscriber_ipv6 entries per prefix length, u32[129]."""
+        out = np.zeros(129, np.uint32)
+        self._chk(self.lib.bng_ipv6_prefix_lengths(self.h, out.ctypes.data), "ipv6_prefix_lengths")
+        return out
 
     def stats(self, name: str) -> np.ndarray:
         """A statistics map (antispoof_stats, qos_stats_map, nat_stats_map, stats_map) as u64[]."""

@@ -289,6 +289,36 @@ class Monitor {
 } // namespace idle
 
 // ===========================================================================
+// Dual-stack subscribers: the IPv6 address or prefix the control plane assigned (DHCPv6 IA_NA / IA_PD, IPv6CP / SLAAC,
+// RADIUS Framed-IPv6-Prefix / Delegated-IPv6-Prefix) -> the subscriber's IPv4 address, in subscriber_ipv6
+// (include/bng_b200.h).  With several shards, shard::Router::Update / Delete with "subscriber_ipv6" route the same
+// calls to the owner of the IPv4 address.
+namespace dualstack {
+
+inline bng_ipv6_prefix_key PrefixKey(const uint8_t addr[16], uint32_t prefixlen) {
+    bng_ipv6_prefix_key k;
+    k.prefixlen = prefixlen;
+    memcpy(k.addr, addr, 16);
+    return k;
+}
+// Installs or replaces the prefix (staged: applied at the next batch boundary, as the per-lease Puts are).
+inline int SetPrefix(bng_ctx *ctx, const uint8_t addr[16], uint32_t prefixlen, uint32_t ip_key, bool staged = true) {
+    const int id = bng_map_id(ctx, "subscriber_ipv6");
+    if (id < 0) return id;
+    const bng_ipv6_prefix_key k = PrefixKey(addr, prefixlen);
+    return staged ? bng_map_update_staged(ctx, id, &k, &ip_key) : bng_map_update(ctx, id, &k, &ip_key, BNG_ANY);
+}
+// Removes it (release, lease expiry, RADIUS Stop): -ENOENT when it was not installed
+inline int ClearPrefix(bng_ctx *ctx, const uint8_t addr[16], uint32_t prefixlen) {
+    const int id = bng_map_id(ctx, "subscriber_ipv6");
+    if (id < 0) return id;
+    const bng_ipv6_prefix_key k = PrefixKey(addr, prefixlen);
+    return bng_map_delete(ctx, id, &k);
+}
+
+} // namespace dualstack
+
+// ===========================================================================
 // Lawful intercept, content of communication (reference pkg/intercept/manager.go:337: Manager.RecordCC(warrant,
 // session, direction, srcIP, dstIP, srcPort, dstPort, protocol, payload)).  StartInterceptSession sets the session's
 // IPv4 address as a target (bng_li_target_set), StopInterceptSession deletes it; PumpCC drains the records and hands
@@ -300,34 +330,53 @@ enum class Direction : uint8_t { Uplink = BNG_LI_UPLINK, Downlink = BNG_LI_DOWNL
 struct CC {
     bng_li_record rec;                // the record's header: target, frame, batch, verdict, timestamp
     Direction direction = Direction::Uplink;
-    IP src, dst;                      // 4 bytes each, wire order; 0.0.0.0 when the capture is too short for it
+    IP src, dst;                      // wire order: 4 bytes (IPv4) or 16 (IPv6); all zero when the capture is too short
     uint16_t src_port = 0, dst_port = 0; // host order
-    uint8_t protocol = 0;
+    uint8_t protocol = 0;             // IPv4 protocol / IPv6 next header
     std::vector<uint8_t> payload;     // the IP packet as captured: bytes 14 .. cap_len of the frame
 };
 
-// The fields RecordCC takes, from one record (header + cap_len captured bytes).  Ports: TCP / UDP source and
-// destination port at 14 + 4 * ihl; ICMP echo request / reply: the echo id, which the NAT translates in place of a port,
-// as the subscriber-side port (src_port uplink, dst_port downlink); 0 for any other protocol or when the capture ends
-// before them.  Returns false when the capture does not hold the IPv4 header's first 20 bytes' addresses.
+// The fields RecordCC takes, from one record (header + cap_len captured bytes).
+//   IPv4 (any record whose ethertype is not 0x86DD): addresses at 26 / 30, protocol at 23; TCP / UDP ports at
+//     14 + 4 * ihl; ICMP echo request / reply: the echo id, which the NAT translates in place of a port, as the
+//     subscriber-side port (src_port uplink, dst_port downlink).
+//   IPv6 (ethertype 0x86DD): 16-byte addresses at 22 / 38, the next header at 20 as the protocol; TCP / UDP ports at
+//     54; ICMPv6 echo request / reply (types 128 / 129): the echo id at 58 as the subscriber-side port.  A next header
+//     that is an extension header is reported as is, with ports 0 (the transport header is not searched for).
+// Ports are 0 for any other protocol or when the capture ends before them.  Returns false when the capture does not
+// hold both addresses.
 inline bool ParseCC(const uint8_t *record, CC *out) {
     memcpy(&out->rec, record, sizeof(bng_li_record));
     const uint8_t *f = record + sizeof(bng_li_record);
     const uint32_t n = out->rec.cap_len;
     out->direction = out->rec.dir == BNG_LI_DOWNLINK ? Direction::Downlink : Direction::Uplink;
+    out->src_port = out->dst_port = 0;
+    out->payload.assign(f + (n > 14 ? 14 : n), f + n);
+    auto be16 = [&](uint32_t off) { return (uint16_t)(f[off] << 8 | f[off + 1]); };
+    uint16_t &sub_port = out->direction == Direction::Uplink ? out->src_port : out->dst_port;
+    if (n >= 14 && f[12] == 0x86 && f[13] == 0xDD) {
+        out->src = n >= 38 ? IP(f + 22, f + 38) : IP(16, 0);
+        out->dst = n >= 54 ? IP(f + 38, f + 54) : IP(16, 0);
+        out->protocol = n >= 21 ? f[20] : 0;
+        if (n < 54) return false;
+        if ((out->protocol == 6 || out->protocol == 17) && n >= 58) {
+            out->src_port = be16(54);
+            out->dst_port = be16(56);
+        } else if (out->protocol == 58 && n >= 60 && (f[54] == 128 || f[54] == 129)) {
+            sub_port = be16(58);
+        }
+        return true;
+    }
     out->src = n >= 30 ? IP(f + 26, f + 30) : IPv4(0, 0, 0, 0);
     out->dst = n >= 34 ? IP(f + 30, f + 34) : IPv4(0, 0, 0, 0);
     out->protocol = n >= 24 ? f[23] : 0;
-    out->src_port = out->dst_port = 0;
-    out->payload.assign(f + (n > 14 ? 14 : n), f + n);
     if (n < 34) return false;
     const uint32_t l4 = 14 + 4u * (f[14] & 0x0f);
-    auto be16 = [&](uint32_t off) { return (uint16_t)(f[off] << 8 | f[off + 1]); };
     if ((out->protocol == 6 || out->protocol == 17) && n >= l4 + 4) {
         out->src_port = be16(l4);
         out->dst_port = be16(l4 + 2);
     } else if (out->protocol == 1 && n >= l4 + 6 && (f[l4] == 0 || f[l4] == 8)) {
-        (out->direction == Direction::Uplink ? out->src_port : out->dst_port) = be16(l4 + 4);
+        sub_port = be16(l4 + 4);
     }
     return true;
 }

@@ -9,6 +9,8 @@
 //   * for the downstream direction (§8f-1) the (public IP, port block) -> shard table.  Blocks are laid out
 //     deterministically by AllocateNAT (pkg/nat/manager.go:433-434: port_start = range_start + k * ports_per_sub),
 //     so the owner of an inbound (dst ip, dst port) is one array lookup;
+//   * for IPv6 (subscriber_ipv6, DESIGN.md §18) the prefix -> IPv4 address table, with a longest-prefix match: a
+//     prefix lives on the shard of its IPv4 address, and a downstream IPv6 frame goes to the owner of its destination;
 //   * replication of the small read-mostly maps (ip_pools, server_config, nat_config_map, alg_ports, hairpin_ips,
 //     antispoof_config, allowed_ranges_v4, nat_pool, nat_private_ranges) to every shard.
 // Router::Update / Lookup / Delete are what a cgo shim binds the Go managers' Map.Put / Lookup / Delete to when
@@ -18,6 +20,8 @@
 #include <string.h>
 
 #include <algorithm>
+#include <array>
+#include <map>
 #include <memory>
 #include <mutex>
 #include <optional>
@@ -31,7 +35,8 @@
 namespace bng {
 namespace shard {
 
-enum class Route { ByMAC, ByPrivateIP, BySessionKey, ByEIMKey, ByReverseKey, Replicated };
+// ByValueIP: the value is the subscriber's IPv4 address (subscriber_ipv6); the entry lives on that address's shard
+enum class Route { ByMAC, ByPrivateIP, BySessionKey, ByEIMKey, ByReverseKey, ByValueIP, Replicated };
 
 inline Route RouteOf(const std::string &map) {
     if (map == "subscriber_bindings" || map == "subscriber_pools") return Route::ByMAC;
@@ -39,6 +44,7 @@ inline Route RouteOf(const std::string &map) {
     if (map == "nat_sessions") return Route::BySessionKey; // struct nat_key: src_ip = the subscriber's address
     if (map == "eim_table") return Route::ByEIMKey;        // struct eim_key: internal_ip
     if (map == "nat_reverse") return Route::ByReverseKey;  // struct nat_key: dst_ip/dst_port = public address, port
+    if (map == "subscriber_ipv6") return Route::ByValueIP; // value: the owner's IPv4 address
     return Route::Replicated;
 }
 
@@ -125,6 +131,50 @@ class Directory {
         }
         return ShardOfIP(priv);
     }
+    // ---- IPv6 prefixes (subscriber_ipv6): prefix -> IPv4 address key, longest-prefix match ----
+    using Addr6 = std::array<uint8_t, 16>;
+    static Addr6 Masked(const uint8_t *addr, uint32_t plen) {
+        Addr6 a;
+        for (uint32_t j = 0; j < 16; j++) {
+            const uint32_t keep = plen >= 8 * (j + 1) ? 8 : (plen > 8 * j ? plen - 8 * j : 0);
+            a[j] = (uint8_t)(addr[j] & (uint8_t)(0xFF00u >> keep));
+        }
+        return a;
+    }
+    // false for prefixlen > 128
+    bool LearnPrefix(const uint8_t *addr, uint32_t plen, uint32_t ip_key) {
+        if (plen > 128) return false;
+        std::lock_guard<std::mutex> g(mu_);
+        v6_[plen][Masked(addr, plen)] = ip_key;
+        return true;
+    }
+    void ForgetPrefix(const uint8_t *addr, uint32_t plen) {
+        if (plen > 128) return;
+        std::lock_guard<std::mutex> g(mu_);
+        v6_[plen].erase(Masked(addr, plen));
+    }
+    // the IPv4 address of exactly this prefix
+    std::optional<uint32_t> PrefixOwner(const uint8_t *addr, uint32_t plen) const {
+        if (plen > 128) return std::nullopt;
+        std::lock_guard<std::mutex> g(mu_);
+        auto it = v6_[plen].find(Masked(addr, plen));
+        if (it == v6_[plen].end()) return std::nullopt;
+        return it->second;
+    }
+    // the IPv4 address of the longest prefix of length <= maxlen covering addr (the dataplane's rule)
+    std::optional<uint32_t> OwnerOfV6(const uint8_t *addr, uint32_t maxlen = 128) const {
+        std::lock_guard<std::mutex> g(mu_);
+        for (int l = (int)std::min<uint32_t>(maxlen, 128); l >= 0; l--) {
+            if (v6_[l].empty()) continue;
+            auto it = v6_[l].find(Masked(addr, (uint32_t)l));
+            if (it != v6_[l].end()) return it->second;
+        }
+        return std::nullopt;
+    }
+    std::optional<uint32_t> ShardOfV6(const uint8_t *addr) const {
+        auto ip = OwnerOfV6(addr);
+        return ip ? ShardOfIP(*ip) : std::nullopt;
+    }
     // ---- frame steering (what the NIC's flow steering does in front of the GPUs) ----
     static uint64_t MacKey(const uint8_t *m) {
         uint64_t k = 0;
@@ -134,8 +184,14 @@ class Directory {
     uint32_t SteerUpstream(const uint8_t *frame, uint32_t len) const { // by source MAC
         return len >= 12 ? ShardOfMAC(MacKey(frame + 6)) : 0;
     }
-    // by destination (public address, port / echo id); frames that are not translatable IPv4 go to `fallback`
+    // IPv4: by destination (public address, port / echo id).  IPv6 (untagged, ethertype 0x86DD): by the owner of the
+    // longest prefix covering the destination (bytes 38-53), the shard that holds its records.  Anything else, and a
+    // destination nobody owns, goes to `fallback`.
     uint32_t SteerDownstream(const uint8_t *f, uint32_t len, uint32_t fallback = 0) const {
+        if (len >= 54 && f[12] == 0x86 && f[13] == 0xDD) {
+            auto s = ShardOfV6(f + 38);
+            return s ? *s : fallback;
+        }
         if (len < 34 || f[12] != 0x08 || f[13] != 0x00) return fallback;
         uint32_t l4 = 14 + (uint32_t)(f[14] & 0x0f) * 4, daddr;
         memcpy(&daddr, f + 30, 4);
@@ -168,6 +224,7 @@ class Directory {
     std::unordered_map<uint64_t, uint32_t> mac_ip_;
     std::unordered_map<uint32_t, uint64_t> ip_mac_;
     std::unordered_map<uint32_t, std::vector<uint32_t>> blocks_; // public ip -> private ip per block index
+    std::array<std::map<Addr6, uint32_t>, 129> v6_;               // per prefix length: masked prefix -> IPv4 key
 };
 
 // N contexts behind one map API.
@@ -179,11 +236,27 @@ class Router {
     Backend &Shard(size_t i) { return *shards_[i]; }
     Directory &Dir() { return *dir_; }
 
-    // -1: replicated, -ENOENT: the owner is not known (the address was never Learn()ed)
-    int Owner(const std::string &map, const void *key) const {
+    // -1: replicated, -ENOENT: the owner is not known (the address was never Learn()ed).  subscriber_ipv6 (ByValueIP):
+    // with the value, the owner of its IPv4 address; without it, the owner of the prefix as the directory learned it.
+    int Owner(const std::string &map, const void *key, const void *value = nullptr) const {
         const uint8_t *k = (const uint8_t *)key;
         uint32_t ip;
         switch (RouteOf(map)) {
+        case Route::ByValueIP: {
+            uint32_t plen;
+            memcpy(&plen, k, 4);
+            if (plen > 128) return -EINVAL;
+            std::optional<uint32_t> a;
+            if (value) {
+                memcpy(&ip, value, 4);
+                a = ip;
+            } else {
+                a = dir_->PrefixOwner(k + 4, plen);
+            }
+            if (!a) return -ENOENT;
+            auto s = dir_->ShardOfIP(*a);
+            return s ? (int)*s : -ENOENT;
+        }
         case Route::ByMAC: {
             uint64_t mac;
             memcpy(&mac, k, 8);
@@ -206,8 +279,18 @@ class Router {
         }
     }
     int Update(const char *map, const void *key, const void *value, uint64_t flags = BNG_ANY, bool staged = false) {
-        int o = Owner(map, key);
-        if (o == -ENOENT) return o;
+        const bool v6 = RouteOf(map) == Route::ByValueIP;
+        int o = Owner(map, key, value);
+        if (o == -ENOENT || o == -EINVAL) return o;
+        if (v6) { // a prefix handed to another subscriber leaves its old shard
+            const int was = Owner(map, key);
+            if (was >= 0 && was != o) {
+                bng_ctx *c = shards_[(size_t)was]->ctx;
+                const int id = bng_map_id(c, map);
+                if (id < 0) return id;
+                if (int r = bng_map_delete(c, id, key); r && r != -ENOENT) return r;
+            }
+        }
         int rc = 0;
         for (size_t i = 0; i < shards_.size(); i++) {
             if (o >= 0 && (size_t)o != i) continue;
@@ -217,10 +300,27 @@ class Router {
             int r = staged && flags == BNG_ANY ? bng_map_update_staged(c, id, key, value) : bng_map_update(c, id, key, value, flags);
             if (r && !rc) rc = r;
         }
+        if (v6 && !rc) {
+            uint32_t plen, a;
+            memcpy(&plen, key, 4);
+            memcpy(&a, value, 4);
+            dir_->LearnPrefix((const uint8_t *)key + 4, plen, a);
+        }
         return rc;
     }
     int Lookup(const char *map, const void *key, void *value_out) {
-        int o = Owner(map, key);
+        int o;
+        if (RouteOf(map) == Route::ByValueIP) { // the longest match: its owner's shard answers
+            uint32_t plen;
+            memcpy(&plen, key, 4);
+            if (plen > 128) return -EINVAL;
+            auto a = dir_->OwnerOfV6((const uint8_t *)key + 4, plen);
+            auto s = a ? dir_->ShardOfIP(*a) : std::nullopt;
+            if (!s) return -ENOENT;
+            o = (int)*s;
+        } else {
+            o = Owner(map, key);
+        }
         if (o == -ENOENT) return o;
         bng_ctx *c = shards_[o < 0 ? 0 : (size_t)o]->ctx; // replicated maps: any copy
         int id = bng_map_id(c, map);
@@ -228,7 +328,12 @@ class Router {
     }
     int Delete(const char *map, const void *key) {
         int o = Owner(map, key);
-        if (o == -ENOENT) return o;
+        if (o == -ENOENT || o == -EINVAL) return o;
+        if (RouteOf(map) == Route::ByValueIP) {
+            uint32_t plen;
+            memcpy(&plen, key, 4);
+            dir_->ForgetPrefix((const uint8_t *)key + 4, plen);
+        }
         int rc = 0;
         for (size_t i = 0; i < shards_.size(); i++) {
             if (o >= 0 && (size_t)o != i) continue;

@@ -121,6 +121,11 @@ bng_acct = np.dtype([(n, "<u8") for n in (
 IDLE_UP, IDLE_DOWN, IDLE_STARTED, IDLE_NEVER = 1, 2, 4, 0xFFFFFFFF
 bng_idle = np.dtype([("up_ns", "<u8"), ("down_ns", "<u8"), ("since_ns", "<u8"), ("timeout_s", "<u4"), ("flags", "<u4")])
 
+# include/bng_b200.h struct bng_ipv6_prefix_key (20 B): the key of subscriber_ipv6 (not a reference map), laid out as a
+# BPF_MAP_TYPE_LPM_TRIE key for IPv6; the value is the subscriber's IPv4 address (4 key bytes of qos_ingress)
+bng_ipv6_prefix_key = np.dtype([("prefixlen", "<u4"), ("addr", "u1", 16)])
+assert bng_ipv6_prefix_key.itemsize == 20
+
 # lawful-intercept record header (include/bng_b200.h: struct bng_li_record, 64 B); the captured bytes follow it
 LI_UPLINK, LI_DOWNLINK = 0, 1
 bng_li_record = np.dtype([
@@ -193,6 +198,7 @@ MAP_DTYPES = {
     "stats_map": ("<u4", dhcp_stats),
     "circuit_id_map": ("<u8", "<u8"),
     "circuit_id_subscribers": (circuit_id_key, pool_assignment),
+    "subscriber_ipv6": (bng_ipv6_prefix_key, ("u1", 4)),
 }
 
 

@@ -216,6 +216,9 @@ int bng_restore(bng_ctx *ctx, const void *buf, uint64_t len);
  *     address it entered the program with (before SNAT): untagged Ethernet II, ethertype 0x0800, bytes 26-29 present.
  *   - Downstream programs (nat44_ingress, qos_egress_prog) charge a frame to the IPv4 DESTINATION address it leaves
  *     with (after DNAT), bytes 30-33: a frame nat44_ingress did not translate keeps its public address.
+ *   - IPv6 (dual-stack subscribers): an untagged Ethernet II frame with ethertype 0x86DD whose 16 address bytes are
+ *     present (source 22-37 upstream, destination 38-53 downstream) is charged to the subscriber_ipv6 owner of that
+ *     address (see below), and only when its verdict is TC_ACT_OK; from there the rules here apply unchanged.
  *   - Verdict TC_ACT_OK counts in the pass pair, TC_ACT_SHOT in the drop pair (NAT port exhaustion, token bucket).
  *     In the two pipelines a frame that antispoof drops is not counted at all: it may have forged its address.
  *   - A frame whose address has no entry when the batch runs is not counted anywhere.
@@ -252,6 +255,8 @@ int64_t bng_acct_dump(bng_ctx *ctx, uint32_t *addrs_out, bng_acct *out, uint64_t
  *     frame entered the program, is a target: untagged Ethernet II, ethertype 0x0800, bytes 26-29 present.
  *   - Downstream programs (nat44_ingress, qos_egress_prog): a frame whose IPv4 DESTINATION, as the frame leaves the
  *     program (after DNAT), is a target: bytes 30-33 present.
+ *   - IPv6: an untagged frame with ethertype 0x86DD whose subscriber_ipv6 owner (see below) is a target, by the same
+ *     attribution as accounting's; `addr` is the owner's IPv4 address.  The bytes are copied as they are.
  *   - The verdict is TC_ACT_OK or TC_ACT_SHOT; both are captured.  In the two pipelines a frame that antispoof drops
  *     is not captured: it may have forged its address.  Other programs never capture.
  *   - A target is any address; it needs no subscriber_nat or qos_ingress entry.  The targets in force are those set
@@ -592,8 +597,40 @@ int64_t bng_dhcp_lease_sweep(bng_ctx *ctx, uint64_t now_ns, uint32_t grace_s, bn
 int bng_dhcp_lease_addr_order(bng_ctx *ctx, uint32_t order); /* -EINVAL for a NULL ctx or another value */
 uint64_t bng_lease_table_rebuilds(bng_ctx *ctx); /* rebuilds of the three lease maps and circuit_id_map by the sweep */
 
+/* ---- dual-stack subscribers: the IPv6 prefix table (not one of the reference's maps) ----
+ * "subscriber_ipv6" (bng_map_id) maps a subscriber's IPv6 address or prefix (Framed-IPv6-Prefix, Delegated-IPv6-Prefix)
+ * to its IPv4 address, the 4 key bytes of qos_ingress.  It is an ordinary map of the registry: bng_map_update, _batch,
+ * _staged, _delete, _dump, _clear, snapshots, restore and deltas carry it.  Reported type BPF_MAP_TYPE_LPM_TRIE (11),
+ * key struct bng_ipv6_prefix_key (20 bytes), value uint32_t, max_entries 2 x max_subscribers (a WAN /64 or /128 and a
+ * delegated prefix per subscriber).
+ *   - prefixlen > 128: -EINVAL (update, staged update, delete, lookup).
+ *   - Update and delete match exactly on (prefixlen, prefix).  Bits of addr past prefixlen are masked off on the way in,
+ *     so two keys that differ only there are one entry, as in the kernel's trie.  Dumps return the masked key, where
+ *     the kernel's trie returns what the caller wrote.
+ *   - bng_map_lookup is the trie's lookup: the value of the longest prefix of length <= key.prefixlen that covers
+ *     key.addr ("whose address is this?"), -ENOENT when none does.
+ * The rule every feature that attributes frames uses (accounting, idle detection, lawful intercept, hand-over): an
+ * untagged Ethernet II frame with ethertype 0x86DD whose 16 address bytes are present in the frame's storage (source
+ * at 22-37 upstream, destination at 38-53 downstream) belongs to the value of the longest prefix in subscriber_ipv6
+ * that covers that address; the IPv4 rule then applies to that address unchanged (its directory entry, its record,
+ * its target).  No covering prefix (a link-local source, say): nobody.  Tagged IPv6 frames: nobody, as tagged IPv4.
+ * No program here drops an IPv6 frame except antispoof_ingress (NAT and QoS pass non-IPv4 frames), so an IPv6 frame
+ * with verdict TC_ACT_SHOT is an antispoof drop, and an IPv6 frame is attributed only when its verdict is TC_ACT_OK.
+ * While the table is empty, every record and every launch is what it is without it: the IPv6 variants of the
+ * attribution kernels run only while the table has live entries.  bng_sub_export carries the entries whose value is
+ * an exported address, in a "subscriber_ipv6" section written only when there is one; BNG_SUB_DETACH removes them.
+ * Memory: 32 bytes per slot of a power of two >= 4 x max_subscribers (128 MiB at the default 1e6), and with change
+ * tracking a shadow of the same size. */
+typedef struct bng_ipv6_prefix_key {
+    uint32_t prefixlen; /* 0..128 */
+    uint8_t addr[16];   /* network order */
+} bng_ipv6_prefix_key;
+
 /* ---- diagnostics ---- */
 uint64_t bng_launch_count(bng_ctx *ctx);  /* kernels launched by this context so far */
+/* Live subscriber_ipv6 entries per prefix length, counts[0..128]: the lengths the IPv6 lookup probes are those with a
+ * non-zero count.  Staged upserts are applied first. */
+int bng_ipv6_prefix_lengths(bng_ctx *ctx, uint32_t *counts /* [129] */);
 uint64_t bng_lru_overflow(bng_ctx *ctx);  /* inserts that found no victim to evict in a full LRU map (should stay 0) */
 uint64_t bng_lru_evictions(bng_ctx *ctx); /* entries evicted from full LRU maps by the data path */
 /* Flow-table rebuilds so far.  nat_sessions / nat_reverse / eim_table are rebuilt (tombstones dropped) together:
