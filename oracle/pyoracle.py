@@ -58,10 +58,11 @@ def available(kind: str) -> bool:
 
 
 class Oracle:
-    """One private instance of an oracle library (own map state)."""
+    """One instance of an oracle library.  The map state lives in the library, so every Oracle built from the same
+    file shares it; `path` names a copy of the library to get a second, independent state."""
 
-    def __init__(self, kind: str = "reference"):
-        path = REF_LIB if kind == "reference" else PORT_LIB
+    def __init__(self, kind: str = "reference", path: str | None = None):
+        path = path or (REF_LIB if kind == "reference" else PORT_LIB)
         if not os.path.exists(path):
             raise FileNotFoundError(f"oracle library missing: {path} (run `make -C oracle`)")
         self.kind = kind
