@@ -11,9 +11,12 @@
 // passed frames raises the record's stamp of the direction to the group's latest clock with one atomicMax.  With one
 // clock for the whole batch the leader reads the stamp first and skips the atomic when it is already there.
 //
-// V6 (launched only while subscriber_ipv6 has live entries): an untagged IPv6 frame with verdict TC_ACT_OK belongs to
-// the owner of its source (bytes 22-37, upstream) or destination (38-53, downstream) address, v6_owner, and from there
-// to that IPv4 address's directory slot.  In ACCT_ATTR mode only frames classify left unattributed read the frame.
+// V6 (launched only while subscriber_ipv6 has live entries): an untagged IPv6 frame belongs to the owner of its source
+// (bytes 22-37, upstream) or destination (38-53, downstream) address, v6_owner, and from there to that IPv4 address's
+// directory slot.  In ACCT_ATTR mode only frames classify left unattributed read the frame, and only with verdict
+// TC_ACT_OK: a pipeline's TC_ACT_SHOT IPv6 frame without an attribution word is antispoof's (a bucket drop has one,
+// k_pipe_classify<V6>).  In the other modes a TC_ACT_SHOT IPv6 frame is a token-bucket drop of a qos program that
+// shapes IPv6 (bng_qos_ipv6_enable); without shaping no program in these modes drops an IPv6 frame.
 #include <errno.h>
 
 #include "kernels.h"
@@ -46,7 +49,7 @@ __global__ void __launch_bounds__(ACCT_BLOCK) k_acct(const __grid_constant__ Tbl
                     const u8 *p = frame_ptr(b, i);
                     if (frame_dlen(b, len) >= off + 4 && rd16(p, 12) == ETH_P_IP_LE) slot = dir_slot_of(dir, rd32(p, off));
                 }
-                if (V6 && slot == DIR_NONE && v == TC_OK) { // untagged IPv6 with the address's sixteen bytes present
+                if (V6 && slot == DIR_NONE && (MODE != ACCT_ATTR || v == TC_OK)) { // untagged IPv6, its sixteen address bytes present
                     const u32 off = MODE == ACCT_DST ? 38 : 22;
                     const u8 *p = frame_ptr(b, i);
                     u32 a[4], owner;

@@ -173,6 +173,9 @@ struct bng_ctx {
     // frames; v6_live is its live-entry count as of the last command that changed it (0: the IPv6 kernels stay off)
     Tbl v6{};
     u32 v6_live = 0;
+    // bng_qos_ipv6_enable: IPv6 frames are shaped by their owner's token bucket (context state: no snapshot, delta or
+    // hand-over blob carries it)
+    bool qos_v6 = false;
 };
 
 namespace {
@@ -1115,6 +1118,7 @@ static int dispatch(bng_ctx *c, int prog, const DevBatch &b, const LiSrc &src = 
     const int li = c->li_targets.empty() ? -1 : k_li_dir[prog]; // no target: not one kernel more
     const bool pipe = prog == P_PIPE_UP || prog == P_PIPE_TC;
     const Tbl *v6 = c->v6_live ? &c->v6 : nullptr; // an empty table launches exactly what it did before it existed
+    const Tbl *qv6 = c->qos_v6 ? v6 : nullptr;     // ... and so does shaping IPv6 with it
     // the upstream classify records attributions: for accounting and idle detection, and in the pipelines to tell
     // antispoof's drops
     c->L.acct_attr = (acct || idle || (li == 0 && pipe)) ? c->L.s.attr : nullptr;
@@ -1131,14 +1135,14 @@ static int dispatch(bng_ctx *c, int prog, const DevBatch &b, const LiSrc &src = 
     }
     switch (prog) {
     case P_ANTISPOOF: e = run_antispoof(c->L, c->dev, b); break;
-    case P_QOS_EG: e = run_qos(c->L, c->dev, b, true); break;
-    case P_QOS_IN: e = run_qos(c->L, c->dev, b, false); break;
+    case P_QOS_EG: e = run_qos(c->L, c->dev, b, true, qv6); break;
+    case P_QOS_IN: e = run_qos(c->L, c->dev, b, false, qv6); break;
     case P_NAT_EG: e = run_nat_egress(c->L, c->dev, b); break;
     case P_NAT_IN: e = run_nat_ingress(c->L, c->dev, b); break;
     case P_NAT_HAIRPIN: e = run_nat_hairpin_xdp(c->L, c->dev, b); break;
     case P_DHCP: e = run_dhcp_fastpath(c->L, c->dev, b); break;
-    case P_PIPE_UP: e = run_pipeline_up(c->L, c->dev, b); break;
-    case P_PIPE_TC: e = run_pipeline_tc(c->L, c->dev, b); break;
+    case P_PIPE_UP: e = run_pipeline_up(c->L, c->dev, b, qv6); break;
+    case P_PIPE_TC: e = run_pipeline_tc(c->L, c->dev, b, qv6); break;
     default: return -EINVAL;
     }
     // after the program, before anything copies the frames out: the downstream modes read the rewritten headers
@@ -3356,6 +3360,13 @@ int bng_stats_device_ptr(bng_ctx *c, void **dptr, uint32_t *n_u64) {
 }
 
 uint64_t bng_launch_count(bng_ctx *c) { return c ? c->L.launches : 0; }
+
+int bng_qos_ipv6_enable(bng_ctx *c, int on) {
+    if (!c) return -EINVAL;
+    std::lock_guard<std::mutex> g(c->mu);
+    c->qos_v6 = on != 0;
+    return 0;
+}
 
 int bng_ipv6_prefix_lengths(bng_ctx *c, uint32_t *counts) {
     if (!c || !counts) return -EINVAL;

@@ -122,22 +122,39 @@ __global__ void __launch_bounds__(BLOCK, AS_MINB) k_antispoof(const __grid_const
 
 // ---------------------------------------------------------------------------
 // qos_egress_prog / qos_ingress_prog: classify
+// V6 (bng_qos_ipv6_enable, while subscriber_ipv6 has live entries): an untagged IPv6 frame whose source (22-37,
+// ingress) or destination (38-53, egress) has a subscriber_ipv6 owner takes the owner's bucket, as an IPv4 frame from
+// or to the owner would: its ordering key is that bucket's slot.
 // ---------------------------------------------------------------------------
+template <bool V6>
 __global__ void __launch_bounds__(BLOCK)
-    k_qos_classify(const __grid_constant__ DevCtx c, const __grid_constant__ DevBatch b, int egress, u32 *skey, u32 *sval, u32 *cnt, u32 *T) {
+    k_qos_classify(const __grid_constant__ DevCtx c, const __grid_constant__ DevBatch b, int egress, u32 *skey, u32 *sval, u32 *cnt, u32 *T,
+                   const __grid_constant__ Tbl v6) {
     __shared__ BlockStats bs;
+    __shared__ V6Lens lens;
     scratch_reset(cnt, T);
     bstats_init(bs);
+    if (V6) v6_lens_load(lens, v6.plens);
     const Tbl &t = egress ? c.qos_eg : c.qos_in;
+    constexpr u32 HB = V6 ? 54 : 34; // header bytes read: through the IPv4 addresses, or through the IPv6 destination
     for (u32 i = blockIdx.x * BLOCK + threadIdx.x; i < b.n; i += gridDim.x * BLOCK) {
         u32 len = b.len[i];
         const u32 dlen = frame_dlen(b, len);
         const u8 *p = frame_ptr(b, i);
         Hdr64 h;
-        hdr_load_wide(h, p, dlen < 34 ? dlen : 34, __all_sync(__activemask(), FRAME_WIDE_OK(b, p)));
+        hdr_load_wide(h, p, dlen < HB ? dlen : HB, __all_sync(__activemask(), FRAME_WIDE_OK(b, p)));
         u32 prio;
         bool prio_set;
-        u32 key = qos_classify_one(c, bs, t, h, len, dlen, egress != 0, &prio, &prio_set);
+        u32 key;
+        if (V6 && dlen >= (egress ? 54u : 38u) && h.b16(12) == ETH_P_IPV6_LE) {
+            u32 a[4], owner;
+#pragma unroll
+            for (int j = 0; j < 4; j++) a[j] = egress ? h.b32(38 + 4 * j) : h.b32(22 + 4 * j); // (constant offsets: h stays in registers)
+            prio_set = false;
+            key = v6_owner(v6, lens, a, &owner) ? qos_bucket_one(bs, t, owner, len, egress != 0, &prio, &prio_set) : NO_KEY;
+        } else {
+            key = qos_classify_one(c, bs, t, h, len, dlen, egress != 0, &prio, &prio_set);
+        }
         if (prio_set && b.priority) b.priority[i] = prio;
         b.verdict[i] = TC_OK;
         skey[i] = key == NO_KEY ? NO_KEY : key_pack(key, len, b.kshift);
@@ -1018,11 +1035,14 @@ cudaError_t run_antispoof(Launcher &L, const DevCtx &c, const DevBatch &b) {
     return cudaGetLastError();
 }
 
-cudaError_t run_qos(Launcher &L, const DevCtx &c, const DevBatch &b0, bool egress) {
+cudaError_t run_qos(Launcher &L, const DevCtx &c, const DevBatch &b0, bool egress, const Tbl *v6) {
     const Tbl &t = egress ? c.qos_eg : c.qos_in;
     DevBatch b = b0;
     b.kshift = kshift_for((u64)t.mask + 1);
-    LAUNCH(k_qos_classify, b.n, 8, c, b, egress ? 1 : 0, L.s.key_a, L.s.val_a, L.s.counters, sort_T(L));
+    if (v6)
+        LAUNCH_AS("k_qos_classify<v6>", k_qos_classify<true>, b.n, 8, c, b, egress ? 1 : 0, L.s.key_a, L.s.val_a, L.s.counters, sort_T(L), *v6);
+    else
+        LAUNCH_AS("k_qos_classify", k_qos_classify<false>, b.n, 8, c, b, egress ? 1 : 0, L.s.key_a, L.s.val_a, L.s.counters, sort_T(L), Tbl{});
     Grouped g;
     cudaError_t e = group_by_key(L, b.n, (u64)t.mask + 1, b.kshift, &g);
     if (e != cudaSuccess) return e;
@@ -1035,18 +1055,31 @@ cudaError_t run_qos(Launcher &L, const DevCtx &c, const DevBatch &b0, bool egres
 
 // The programs keyed on the subscriber directory (nat44_egress, pipeline_up, pipeline_tc): classify, group by
 // directory slot, resolve.  The names are what each launch is timed as; with accounting on, classify is the
-// ACCT instantiation and is timed under its own name.
+// ACCT instantiation and is timed under its own name.  v6 (the pipelines only): IPv6 frames are shaped, classify is
+// the V6 instantiation and is timed under its name with a ", v6>" suffix.
+struct ClassifyNames {
+    const char *plain, *acct, *v6, *acct_v6;
+};
+template <bool AS, bool QOS, bool TC, bool ACCT, bool V6>
+static void launch_classify(Launcher &L, const DevCtx &c, const DevBatch &b, const char *name, const Tbl &v6) {
+    LAUNCH_AS(name, (k_pipe_classify<AS, QOS, TC, ACCT, V6>), b.n, CLASSIFY_BPS(AS), c, b, L.s.key_a, L.s.val_a, L.s.counters, sort_T(L),
+              ACCT ? L.acct_attr : nullptr, v6);
+}
 template <bool AS, bool QOS, bool TC>
-static cudaError_t run_dir_prog(Launcher &L, const DevCtx &c, const DevBatch &b0, const char *classify_name,
-                                const char *classify_acct_name, const char *resolve_name) {
+static cudaError_t run_dir_prog(Launcher &L, const DevCtx &c, const DevBatch &b0, const ClassifyNames &nm, const char *resolve_name,
+                                const Tbl *v6) {
     DevBatch b = b0;
     b.kshift = kshift_for((u64)c.subdir.mask + 1);
-    if (L.acct_attr)
-        LAUNCH_AS(classify_acct_name, (k_pipe_classify<AS, QOS, TC, true>), b.n, CLASSIFY_BPS(AS), c, b, L.s.key_a, L.s.val_a,
-                  L.s.counters, sort_T(L), L.acct_attr);
-    else
-        LAUNCH_AS(classify_name, (k_pipe_classify<AS, QOS, TC>), b.n, CLASSIFY_BPS(AS), c, b, L.s.key_a, L.s.val_a, L.s.counters,
-                  sort_T(L), nullptr);
+    if (QOS && v6) { // (V6 = QOS: nat44_egress has no bucket and is never given the table)
+        if (L.acct_attr)
+            launch_classify<AS, QOS, TC, true, QOS>(L, c, b, nm.acct_v6, *v6);
+        else
+            launch_classify<AS, QOS, TC, false, QOS>(L, c, b, nm.v6, *v6);
+    } else if (L.acct_attr) {
+        launch_classify<AS, QOS, TC, true, false>(L, c, b, nm.acct, Tbl{});
+    } else {
+        launch_classify<AS, QOS, TC, false, false>(L, c, b, nm.plain, Tbl{});
+    }
     Grouped g;
     cudaError_t e = group_by_key(L, b.n, (u64)c.subdir.mask + 1, b.kshift, &g);
     if (e != cudaSuccess) return e;
@@ -1055,8 +1088,8 @@ static cudaError_t run_dir_prog(Launcher &L, const DevCtx &c, const DevBatch &b0
 }
 
 cudaError_t run_nat_egress(Launcher &L, const DevCtx &c, const DevBatch &b) {
-    return run_dir_prog<false, false, false>(L, c, b, "(k_pipe_classify<false, false>)", "(k_pipe_classify<false, false, false, true>)",
-                                             "(k_resolve<true, false, false>)");
+    return run_dir_prog<false, false, false>(L, c, b, {"(k_pipe_classify<false, false>)", "(k_pipe_classify<false, false, false, true>)"},
+                                             "(k_resolve<true, false, false>)", nullptr);
 }
 
 cudaError_t run_nat_ingress(Launcher &L, const DevCtx &c, const DevBatch &b) {
@@ -1069,12 +1102,16 @@ cudaError_t run_nat_hairpin_xdp(Launcher &L, const DevCtx &c, const DevBatch &b)
     return cudaGetLastError();
 }
 
-cudaError_t run_pipeline_up(Launcher &L, const DevCtx &c, const DevBatch &b) {
-    return run_dir_prog<true, true, false>(L, c, b, "(k_pipe_classify<true, true>)", "(k_pipe_classify<true, true, false, true>)",
-                                           "(k_resolve<true, true, false>)");
+cudaError_t run_pipeline_up(Launcher &L, const DevCtx &c, const DevBatch &b, const Tbl *v6) {
+    return run_dir_prog<true, true, false>(L, c, b,
+                                           {"(k_pipe_classify<true, true>)", "(k_pipe_classify<true, true, false, true>)",
+                                            "(k_pipe_classify<true, true, v6>)", "(k_pipe_classify<true, true, false, true, v6>)"},
+                                           "(k_resolve<true, true, false>)", v6);
 }
 
-cudaError_t run_pipeline_tc(Launcher &L, const DevCtx &c, const DevBatch &b) {
-    return run_dir_prog<true, true, true>(L, c, b, "(k_pipe_classify<true, true, true>)", "(k_pipe_classify<true, true, true, true>)",
-                                          "(k_resolve<true, true, false, tc>)");
+cudaError_t run_pipeline_tc(Launcher &L, const DevCtx &c, const DevBatch &b, const Tbl *v6) {
+    return run_dir_prog<true, true, true>(L, c, b,
+                                          {"(k_pipe_classify<true, true, true>)", "(k_pipe_classify<true, true, true, true>)",
+                                           "(k_pipe_classify<true, true, true, v6>)", "(k_pipe_classify<true, true, true, true, v6>)"},
+                                          "(k_resolve<true, true, false, tc>)", v6);
 }

@@ -12,8 +12,10 @@
 // The target set is a few KB at most (<= BNG_LI_MAX_TARGETS addresses at load <= 1/2): its probes stay in L1 / L2.
 // V6 (launched only while subscriber_ipv6 has live entries): an untagged IPv6 frame is captured for the owner of its
 // source (bytes 22-37, upstream) or destination (38-53, downstream), v6_owner; that IPv4 address is probed in the target
-// set and goes into the record.  Downstream only a TC_ACT_OK frame is attributed; upstream k_li_verdict voids a SHOT
-// one, which in a pipeline is antispoof's (NAT and QoS pass every non-IPv4 frame) and elsewhere cannot happen.
+// set and goes into the record.  Downstream a TC_ACT_OK or TC_ACT_SHOT frame is attributed, as an IPv4 one is (SHOT:
+// a token-bucket drop of qos_egress_prog shaping IPv6, bng_qos_ipv6_enable; no other downstream program drops an IPv6
+// frame).  Upstream k_li_verdict voids a SHOT one in a pipeline unless classify attributed it (a bucket drop), so an
+// antispoof drop stays uncaptured.
 #include "kernels.h"
 #include "progs.cuh"
 
@@ -79,7 +81,7 @@ __global__ void __launch_bounds__(LI_BLOCK) k_li_capture(const __grid_constant__
             if ((UP || v == TC_OK || v == TC_SHOT) && have >= off + 4 && rd16(p, 12) == ETH_P_IP_LE) {
                 addr = rd32(p, off);
                 t = li_find(r.tgt, addr);
-            } else if (V6 && (UP || v == TC_OK) && have >= (UP ? 38u : 54u) && rd16(p, 12) == ETH_P_IPV6_LE) {
+            } else if (V6 && (UP || v == TC_OK || v == TC_SHOT) && have >= (UP ? 38u : 54u) && rd16(p, 12) == ETH_P_IPV6_LE) {
                 u32 a[4];
                 v6_addr(p, UP ? 22 : 38, a);
                 if (v6_owner(v6, lens, a, &addr)) t = li_find(r.tgt, addr);

@@ -36,16 +36,25 @@
 // ACCT: traffic accounting is on for this run: attr[i] := the directory slot frame i is charged to (its source
 // address as it entered), or DIR_NONE when the frame is not attributable or antispoof dropped it (acct.cu).  A
 // template parameter, so that the instantiations without it are the code they were.
-template <bool AS, bool QOS, bool TC = false, bool ACCT = false>
+// V6 (bng_qos_ipv6_enable, while subscriber_ipv6 has live entries; QOS only): an untagged IPv6 frame that antispoof
+// passed and whose source (bytes 22-37) has a subscriber_ipv6 owner is shaped by the owner's qos_ingress bucket: it
+// skips the IPv4 directory and session probes, and the directory phase finds the owner (v6_owner) and the owner's
+// directory slot in their place.  The frame gets the owner's ordering key, so the ordered phase charges it in index
+// order with the owner's IPv4 frames; it never carries MISS_FLAG or DEFER_FLAG, so there it meets only the bucket, and
+// nothing of NAT ever sees it.  With ACCT its attribution word is the owner's slot.
+template <bool AS, bool QOS, bool TC = false, bool ACCT = false, bool V6 = false>
 __global__ void __launch_bounds__(BLOCK, CLASSIFY_BPS(AS))
     k_pipe_classify(const __grid_constant__ DevCtx c, const __grid_constant__ DevBatch b, u32 *skey, u32 *sval, u32 *cnt, u32 *T,
-                    u32 *attr) {
+                    u32 *attr, const __grid_constant__ Tbl v6) {
+    static_assert(!V6 || QOS, "IPv6 frames only ever meet a token bucket");
     __shared__ SmallTabs st;
     scratch_reset(cnt, T);
     __shared__ BlockStats bs;
     __shared__ u64 bar;
+    __shared__ V6Lens lens;
     smem_stage_begin(&st, c.small, (u32)sizeof(SmallTabs), &bar);
     bstats_init(bs);
+    if (V6) v6_lens_load(lens, v6.plens);
     smem_stage_wait(&bar);
     const u32 lane = threadIdx.x & 31;
 #define as_cfg (st.as_cfg) /* read from shared memory / the constant bank where used: no live registers */
@@ -66,6 +75,7 @@ __global__ void __launch_bounds__(BLOCK, CLASSIFY_BPS(AS))
 
         // ---- phase 1: keys, and the first probe of every table this frame may need ----
         const bool ip4 = dlen >= 34 && h.b16(12) == ETH_P_IP_LE;
+        const bool ip6 = V6 && dlen >= 38 && h.b16(12) == ETH_P_IPV6_LE; // untagged, the source's 16 bytes present
         const u32 saddr = h.b32(26), daddr = h.b32(30), proto = h.b8(23);
         const bool ihl5 = (h.b8(14) & 0x0f) == 5;
         u64 mk = mac_key(h, 6);
@@ -119,6 +129,7 @@ __global__ void __launch_bounds__(BLOCK, CLASSIFY_BPS(AS))
             __syncwarp();
         }
         const bool alive = act && v != TC_SHOT && ip4;
+        const bool alive6 = V6 && act && v != TC_SHOT && ip6;
 
         // ---- phase 3: the subscriber directory: does this address own a NAT block / a bucket? ----
         u32 nat_slot = DIR_NONE, qos_slot = DIR_NONE, dir_idx = ACCT ? DIR_NONE : 0; // (ACCT: DIR_NONE = no entry)
@@ -133,6 +144,18 @@ __global__ void __launch_bounds__(BLOCK, CLASSIFY_BPS(AS))
                     nat_slot = (u32)w;
                     qos_slot = (u32)(w >> 32);
                     dir_idx = (u32)((de - c.subdir.slots) >> 4);
+                }
+            }
+        }
+        if (V6 && alive6) { // the owner's directory entry stands in for the frame's own
+            u32 a[4], owner;
+#pragma unroll
+            for (int j = 0; j < 4; j++) a[j] = h.b32(22 + 4 * j);
+            if (v6_owner(v6, lens, a, &owner)) {
+                const u32 s = dir_slot_of(c.subdir, owner);
+                if (s != DIR_NONE) {
+                    qos_slot = (u32)(*(const u64 *)(c.subdir.slots + (size_t)s * 16 + 8) >> 32);
+                    dir_idx = s;
                 }
             }
         }
@@ -217,7 +240,7 @@ __global__ void __launch_bounds__(BLOCK, CLASSIFY_BPS(AS))
 
         // ---- phase 5: ordering key = the directory slot ----
         u32 okey = NO_KEY, oval = i;
-        if (alive && v != TC_SHOT) {
+        if ((alive || alive6) && v != TC_SHOT) {
             if (qos_slot != DIR_NONE && (qos_slot & DIR_QOS_UNLIMITED) && !miss) {
                 n_qpass++; // unlimited bucket and nothing left to order (bpf/qos_ratelimit.c:77-78)
                 n_qbytes += len;
@@ -234,7 +257,7 @@ __global__ void __launch_bounds__(BLOCK, CLASSIFY_BPS(AS))
         }
         if (ACCT) {
             // a frame too short for classify's IPv4 parse (bytes 26-29 present, 30-33 not) is still its source's
-            u32 aw = alive ? dir_idx : DIR_NONE;
+            u32 aw = (alive || alive6) ? dir_idx : DIR_NONE;
             if (act && !ip4 && dlen >= 30 && h.b16(12) == ETH_P_IP_LE && (!AS || v != TC_SHOT)) {
                 const u8 *de = tbl_find<1, false>(c.subdir, &sk);
                 if (de) aw = (u32)((de - c.subdir.slots) >> 4);

@@ -246,16 +246,10 @@ __device__ __forceinline__ bool tb_step(TokenBucket &tb, u64 now, u32 pkt_len) {
     return false;
 }
 
-// classify for qos_{egress,ingress}_prog (:126-172, :178-222): returns the
-// ordering key (bucket slot index) when the frame has to go through the
-// ordered token-bucket walk, NO_KEY when its verdict is already final.
-__device__ __forceinline__ u32 qos_classify_one(const DevCtx &c, BlockStats &bs, const Tbl &t, const Hdr64 &h,
-                                                u32 len, u32 dlen, bool egress, u32 *prio_out, bool *prio_set) {
-    *prio_set = false; // dlen: bytes present (bounds checks), len: skb->len (byte counters)
-    if (dlen < 14) return NO_KEY;
-    if (h.b16(12) != ETH_P_IP_LE) return NO_KEY;
-    if (dlen < 34) return NO_KEY;
-    u64 k = egress ? h.b32(30) : h.b32(26);
+// the bucket of a frame whose key is k (an IPv4 address in qos_{egress,ingress} key order): the ordering key (bucket
+// slot index) when the frame has to go through the ordered token-bucket walk, NO_KEY when its verdict is already final
+__device__ __forceinline__ u32 qos_bucket_one(BlockStats &bs, const Tbl &t, u64 k, u32 len, bool egress, u32 *prio_out,
+                                              bool *prio_set) {
     const u8 *slot = tbl_find<1, false>(t, &k);
     if (!slot) return NO_KEY; // no policy: TC_ACT_OK without statistics
     u64 rate = *(const u64 *)(slot + QOS_RATE_COPY); // mirror of rate_bps in the key's sector
@@ -269,6 +263,16 @@ __device__ __forceinline__ u32 qos_classify_one(const DevCtx &c, BlockStats &bs,
         return NO_KEY;
     }
     return (u32)((slot - t.slots) / t.slot_bytes);
+}
+
+// classify for qos_{egress,ingress}_prog (:126-172, :178-222): qos_bucket_one of an IPv4 frame's address
+__device__ __forceinline__ u32 qos_classify_one(const DevCtx &c, BlockStats &bs, const Tbl &t, const Hdr64 &h,
+                                                u32 len, u32 dlen, bool egress, u32 *prio_out, bool *prio_set) {
+    *prio_set = false; // dlen: bytes present (bounds checks), len: skb->len (byte counters)
+    if (dlen < 14) return NO_KEY;
+    if (h.b16(12) != ETH_P_IP_LE) return NO_KEY;
+    if (dlen < 34) return NO_KEY;
+    return qos_bucket_one(bs, t, egress ? h.b32(30) : h.b32(26), len, egress, prio_out, prio_set);
 }
 
 // ---------------------------------------------------------------------------

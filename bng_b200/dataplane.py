@@ -99,6 +99,7 @@ def load_library() -> C.CDLL:
         "bng_stats_device_ptr": ([vp, C.POINTER(vp), C.POINTER(u32)], i32),
         "bng_launch_count": ([vp], u64),
         "bng_ipv6_prefix_lengths": ([vp, vp], i32),
+        "bng_qos_ipv6_enable": ([vp, i32], i32),
         "bng_lru_overflow": ([vp], u64),
         "bng_events_lost": ([vp], u64),
         "bng_prof_enable": ([vp, i32], i32),
@@ -152,7 +153,7 @@ EXPORTED_SYMBOLS = (
     "bng_delta_enable", "bng_delta_export", "bng_delta_apply", "bng_delta_info",
     "bng_idle_enable", "bng_idle_timeout_set", "bng_idle_read", "bng_idle_scan", "bng_nat_usage",
     "bng_dhcp_lease_census", "bng_dhcp_lease_sweep", "bng_lease_table_rebuilds", "bng_dhcp_lease_addr_order",
-    "bng_sub_export", "bng_sub_import", "bng_ipv6_prefix_lengths",
+    "bng_sub_export", "bng_sub_import", "bng_ipv6_prefix_lengths", "bng_qos_ipv6_enable",
 )
 
 
@@ -305,6 +306,12 @@ class Dataplane:
             rs = [self.delete("subscriber_ipv6", k) for k in keys]
             return next((r for r in rs if r), 0)
         return self.update_batch("subscriber_ipv6", keys, _addr_words(addrs).reshape(-1, 1).view(np.uint8))
+
+    def qos_ipv6_enable(self, on: bool = True):
+        """Shape IPv6 frames with their subscriber_ipv6 owner's token bucket (qos_ingress_prog, qos_egress_prog and the
+        two pipelines), from the next run on; off by default.  Context state: snapshots, deltas and hand-over blobs do
+        not carry it."""
+        self._chk(self.lib.bng_qos_ipv6_enable(self.h, 1 if on else 0), "qos_ipv6_enable")
 
     def ipv6_prefix_lengths(self) -> np.ndarray:
         """Live subscriber_ipv6 entries per prefix length, u32[129]."""

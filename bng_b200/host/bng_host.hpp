@@ -927,6 +927,10 @@ struct SubscriberQoS { // manager.go:37-44
 struct ManagerConfig {
     std::string Interface, BPFPath;
     std::shared_ptr<Backend> Backend_;
+    // Shape dual-stack subscribers' IPv6 frames with the same buckets (bng_qos_ipv6_enable), applied by Start().  The
+    // flag is context state that no snapshot or delta carries: a standby's Manager sets it too.  false leaves the
+    // context's flag as it is.
+    bool ShapeIPv6 = false;
 };
 
 class Manager {
@@ -953,6 +957,9 @@ class Manager {
         ingress_ = be_->Map("qos_ingress");
         if (ingress_ < 0) return Error("qos_ingress map not found");
         stats_ = be_->Map("qos_stats_map");
+        if (cfg_.ShapeIPv6) {
+            if (int rc = bng_qos_ipv6_enable(be_->ctx, 1)) return MapErr("failed to enable IPv6 shaping", rc);
+        }
         return Nil();
     }
     Error Stop() {

@@ -412,6 +412,14 @@ class Router {
         }
         return rc;
     }
+    // IPv6 shaping (bng_qos_ipv6_enable) on every shard: one bucket per subscriber whatever the address family.  A
+    // subscriber's IPv6 frames already reach its shard (SteerDownstream, and upstream by MAC), so each shard shapes
+    // them with the bucket it holds.  Returns 0 or the first shard's error.
+    int QoSIPv6Enable(bool on) {
+        for (auto &s : shards_)
+            if (int r = bng_qos_ipv6_enable(s->ctx, on ? 1 : 0)) return r;
+        return 0;
+    }
     // Drains every shard: fn(shard, record, record size) per record, in (batch, frame) order within a shard (batch
     // numbers are per shard).  Returns the number of records or a negative errno.
     template <class F>

@@ -218,7 +218,8 @@ int bng_restore(bng_ctx *ctx, const void *buf, uint64_t len);
  *     with (after DNAT), bytes 30-33: a frame nat44_ingress did not translate keeps its public address.
  *   - IPv6 (dual-stack subscribers): an untagged Ethernet II frame with ethertype 0x86DD whose 16 address bytes are
  *     present (source 22-37 upstream, destination 38-53 downstream) is charged to the subscriber_ipv6 owner of that
- *     address (see below), and only when its verdict is TC_ACT_OK; from there the rules here apply unchanged.
+ *     address (see below), and only when its verdict is TC_ACT_OK; from there the rules here apply unchanged.  With
+ *     IPv6 shaping on (bng_qos_ipv6_enable), a frame its owner's token bucket drops counts in the owner's drop pair.
  *   - Verdict TC_ACT_OK counts in the pass pair, TC_ACT_SHOT in the drop pair (NAT port exhaustion, token bucket).
  *     In the two pipelines a frame that antispoof drops is not counted at all: it may have forged its address.
  *   - A frame whose address has no entry when the batch runs is not counted anywhere.
@@ -256,7 +257,8 @@ int64_t bng_acct_dump(bng_ctx *ctx, uint32_t *addrs_out, bng_acct *out, uint64_t
  *   - Downstream programs (nat44_ingress, qos_egress_prog): a frame whose IPv4 DESTINATION, as the frame leaves the
  *     program (after DNAT), is a target: bytes 30-33 present.
  *   - IPv6: an untagged frame with ethertype 0x86DD whose subscriber_ipv6 owner (see below) is a target, by the same
- *     attribution as accounting's; `addr` is the owner's IPv4 address.  The bytes are copied as they are.
+ *     attribution as accounting's; `addr` is the owner's IPv4 address.  The bytes are copied as they are.  With IPv6
+ *     shaping on (bng_qos_ipv6_enable), a frame its owner's token bucket drops is captured with TC_ACT_SHOT.
  *   - The verdict is TC_ACT_OK or TC_ACT_SHOT; both are captured.  In the two pipelines a frame that antispoof drops
  *     is not captured: it may have forged its address.  Other programs never capture.
  *   - A target is any address; it needs no subscriber_nat or qos_ingress entry.  The targets in force are those set
@@ -614,8 +616,10 @@ uint64_t bng_lease_table_rebuilds(bng_ctx *ctx); /* rebuilds of the three lease 
  * at 22-37 upstream, destination at 38-53 downstream) belongs to the value of the longest prefix in subscriber_ipv6
  * that covers that address; the IPv4 rule then applies to that address unchanged (its directory entry, its record,
  * its target).  No covering prefix (a link-local source, say): nobody.  Tagged IPv6 frames: nobody, as tagged IPv4.
- * No program here drops an IPv6 frame except antispoof_ingress (NAT and QoS pass non-IPv4 frames), so an IPv6 frame
- * with verdict TC_ACT_SHOT is an antispoof drop, and an IPv6 frame is attributed only when its verdict is TC_ACT_OK.
+ * Without IPv6 shaping (below), no program here drops an IPv6 frame except antispoof_ingress (NAT and QoS pass
+ * non-IPv4 frames), so an IPv6 frame with verdict TC_ACT_SHOT is an antispoof drop, and an IPv6 frame is attributed
+ * only when its verdict is TC_ACT_OK.  With shaping on, a frame the owner's token bucket drops is attributed as well
+ * (TC_ACT_SHOT, the drop pair); a frame antispoof drops is still nobody's.
  * While the table is empty, every record and every launch is what it is without it: the IPv6 variants of the
  * attribution kernels run only while the table has live entries.  bng_sub_export carries the entries whose value is
  * an exported address, in a "subscriber_ipv6" section written only when there is one; BNG_SUB_DETACH removes them.
@@ -625,6 +629,23 @@ typedef struct bng_ipv6_prefix_key {
     uint32_t prefixlen; /* 0..128 */
     uint8_t addr[16];   /* network order */
 } bng_ipv6_prefix_key;
+/* IPv6 shaping: one token bucket per subscriber, whatever the address family.  on != 0: from the next bng_prog_run,
+ * qos_ingress_prog, pipeline_up and pipeline_tc shape an IPv6 frame with the qos_ingress bucket of the subscriber_ipv6
+ * owner of its source (bytes 22-37), and qos_egress_prog with the qos_egress bucket of the owner of its destination
+ * (38-53).  Which frames: those the rule above attributes (untagged, ethertype 0x86DD, the 16 address bytes present,
+ * a covering prefix); in the pipelines only those antispoof_ingress passed.
+ *   - The frame is shaped exactly as an IPv4 frame of the same len from the owner (ingress) or to it (egress), at the
+ *     same clock and the same position in the batch, would be: token_bucket_check() runs in index order together with
+ *     the owner's IPv4 frames, an unlimited bucket passes it, qos_stats_map counts it, and a frame qos_egress_prog
+ *     passes gets the bucket's priority.  Its bytes are not changed.
+ *   - Nothing else that happens to an IPv6 frame changes: NAT passes it untouched and uncounted (in pipeline_tc too,
+ *     where NAT runs after the bucket); nat44_*, antispoof_ingress and dhcp_fastpath_prog are not affected.  Frames
+ *     without an owner, tagged frames and frames too short for the address are not shaped.
+ *   - Accounting, idle detection and interception see a bucket drop as they see an IPv4 one (above).
+ *   - While subscriber_ipv6 is empty, "on" launches exactly what "off" launches.
+ * Off by default.  The flag is context state: snapshots, deltas and hand-over blobs do not carry it, so a standby or
+ * the destination of a hand-over sets it itself.  Returns 0, or -EINVAL for a NULL ctx. */
+int bng_qos_ipv6_enable(bng_ctx *ctx, int on);
 
 /* ---- diagnostics ---- */
 uint64_t bng_launch_count(bng_ctx *ctx);  /* kernels launched by this context so far */
