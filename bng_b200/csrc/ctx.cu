@@ -176,6 +176,9 @@ struct bng_ctx {
     // bng_qos_ipv6_enable: IPv6 frames are shaped by their owner's token bucket (context state: no snapshot, delta or
     // hand-over blob carries it)
     bool qos_v6 = false;
+    // bng_nat_icmp_errors_enable: nat44_ingress translates ICMP errors by the flow they quote (context state, as
+    // qos_v6)
+    bool nat_icmp = false;
 };
 
 namespace {
@@ -1138,7 +1141,7 @@ static int dispatch(bng_ctx *c, int prog, const DevBatch &b, const LiSrc &src = 
     case P_QOS_EG: e = run_qos(c->L, c->dev, b, true, qv6); break;
     case P_QOS_IN: e = run_qos(c->L, c->dev, b, false, qv6); break;
     case P_NAT_EG: e = run_nat_egress(c->L, c->dev, b); break;
-    case P_NAT_IN: e = run_nat_ingress(c->L, c->dev, b); break;
+    case P_NAT_IN: e = run_nat_ingress(c->L, c->dev, b, c->nat_icmp); break;
     case P_NAT_HAIRPIN: e = run_nat_hairpin_xdp(c->L, c->dev, b); break;
     case P_DHCP: e = run_dhcp_fastpath(c->L, c->dev, b); break;
     case P_PIPE_UP: e = run_pipeline_up(c->L, c->dev, b, qv6); break;
@@ -1230,7 +1233,7 @@ static int run_host_zero_copy(bng_ctx *c, int prog, bng_batch *bb, u8 *arena_dev
                                   c->s_in));
         } else {
             CU(c, run_gather_frames(c->s_in, c->L.num_sms, chunk_arena, bb->off16 ? c->zc_off[buf] : nullptr, c->zc_len[buf],
-                                    bb->stride, cn, hb, tc, c->zc_hdr[buf], c->zc_len0[buf]));
+                                    bb->stride, cn, hb, tc, prog == P_NAT_IN && c->nat_icmp, c->zc_hdr[buf], c->zc_len0[buf]));
             c->L.launches++;
         }
         CU(c, cudaEventRecord(c->ev_in[buf], c->s_in));
@@ -3365,6 +3368,13 @@ int bng_qos_ipv6_enable(bng_ctx *c, int on) {
     if (!c) return -EINVAL;
     std::lock_guard<std::mutex> g(c->mu);
     c->qos_v6 = on != 0;
+    return 0;
+}
+
+int bng_nat_icmp_errors_enable(bng_ctx *c, int on) {
+    if (!c) return -EINVAL;
+    std::lock_guard<std::mutex> g(c->mu);
+    c->nat_icmp = on != 0;
     return 0;
 }
 

@@ -169,6 +169,9 @@ __global__ void __launch_bounds__(BLOCK)
 // Header in registers, whole-sector probes (nat_reverse slot = key + original tuple in one 32-byte load,
 // nat_sessions sector 0 = key + translation + last_seen), the TCP state CAS only when the state would
 // change, the rewrite stored back as whole sectors.  Frames with IPv4 options take nat_ingress_one().
+// ICMPERR (bng_nat_icmp_errors_enable): an ICMP error frame is keyed by the flow it quotes, not by bytes 4-5 of its
+// ICMP header; it takes nat_icmp_error_one() on its own lane (errors are rare).
+template <bool ICMPERR>
 __global__ void __launch_bounds__(BLOCK) k_nat_ingress(const __grid_constant__ DevCtx c, const __grid_constant__ DevBatch b) {
     __shared__ BlockStats bs;
     bstats_init(bs);
@@ -186,7 +189,14 @@ __global__ void __launch_bounds__(BLOCK) k_nat_ingress(const __grid_constant__ D
         if (act) b.verdict[i] = TC_OK; // nat44_ingress never drops
         const bool ip4 = dlen >= 34 && h.b16(12) == ETH_P_IP_LE;
         if (ip4 && (h.b8(14) & 0x0f) != 5) { // options: fields are not at fixed offsets (rare)
-            nat_ingress_one(c, bs, p, len, dlen, frame_now(b, i), b.nowv != nullptr);
+            nat_ingress_one<ICMPERR>(c, bs, p, len, dlen, frame_now(b, i), b.nowv != nullptr);
+            continue;
+        }
+        if (ICMPERR && ip4 && h.b8(23) == 1 && dlen >= 42 && icmp_error_type(h.b8(34))) {
+            if (nat_icmp_error_one(c, p, h, dlen))
+                n_dnat++;
+            else
+                n_passed++;
             continue;
         }
         const u32 saddr = h.b32(26), daddr = h.b32(30), proto = h.b8(23);
@@ -1092,8 +1102,11 @@ cudaError_t run_nat_egress(Launcher &L, const DevCtx &c, const DevBatch &b) {
                                              "(k_resolve<true, false, false>)", nullptr);
 }
 
-cudaError_t run_nat_ingress(Launcher &L, const DevCtx &c, const DevBatch &b) {
-    LAUNCH(k_nat_ingress, b.n, 6, c, b);
+cudaError_t run_nat_ingress(Launcher &L, const DevCtx &c, const DevBatch &b, bool icmp_errors) {
+    if (icmp_errors)
+        LAUNCH_AS("k_nat_ingress<icmperr>", k_nat_ingress<true>, b.n, 6, c, b);
+    else
+        LAUNCH_AS("k_nat_ingress", k_nat_ingress<false>, b.n, 6, c, b);
     return cudaGetLastError();
 }
 

@@ -49,15 +49,17 @@ cudaError_t run_antispoof(Launcher &L, const DevCtx &c, const DevBatch &b);
 // entries), else nullptr
 cudaError_t run_qos(Launcher &L, const DevCtx &c, const DevBatch &b, bool egress, const Tbl *v6);
 cudaError_t run_nat_egress(Launcher &L, const DevCtx &c, const DevBatch &b);
-cudaError_t run_nat_ingress(Launcher &L, const DevCtx &c, const DevBatch &b);
+// icmp_errors: ICMP errors are translated by the flow they quote (bng_nat_icmp_errors_enable)
+cudaError_t run_nat_ingress(Launcher &L, const DevCtx &c, const DevBatch &b, bool icmp_errors);
 cudaError_t run_nat_hairpin_xdp(Launcher &L, const DevCtx &c, const DevBatch &b);
 cudaError_t run_pipeline_up(Launcher &L, const DevCtx &c, const DevBatch &b, const Tbl *v6);
 cudaError_t run_pipeline_tc(Launcher &L, const DevCtx &c, const DevBatch &b, const Tbl *v6);
 cudaError_t run_dhcp_fastpath(Launcher &L, const DevCtx &c, const DevBatch &b);
 
-// header gather / scatter between a pinned host arena and a compact device copy (hostio.cu)
+// header gather / scatter between a pinned host arena and a compact device copy (hostio.cu); icmp_errors (TC only):
+// also bytes 64-79 of an ICMP error frame, for nat44_ingress with bng_nat_icmp_errors_enable
 cudaError_t run_gather_frames(cudaStream_t st, int blocks, const u8 *arena, const u32 *off16, const u32 *len, u32 stride,
-                              u32 n, u32 slot, bool tc, u8 *dst, u32 *need);
+                              u32 n, u32 slot, bool tc, bool icmp_errors, u8 *dst, u32 *need);
 cudaError_t run_scatter_frames(cudaStream_t st, int blocks, u8 *arena, const u32 *off16, const u32 *need, u32 stride, u32 n,
                                u32 slot, const u8 *src);
 

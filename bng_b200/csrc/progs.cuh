@@ -873,8 +873,15 @@ __device__ __forceinline__ u32 nat_chunk_coop(const DevCtx &c, BlockStats &bs, c
     return take;
 }
 
+// ICMP error messages whose quoted datagram names a flow (RFC 5508): Destination Unreachable, Time Exceeded,
+// Parameter Problem.
+__device__ __forceinline__ bool icmp_error_type(u32 t) { return t == 3 || t == 11 || t == 12; }
+
 // nat44_ingress, :805-948.  Every update is commutative (or made so with a
 // CAS on the state byte), so this is a classify-only program.
+// ICMPERR (bng_nat_icmp_errors_enable): an ICMP error frame is never keyed by its bytes 4-5; here (outer options) it
+// is not translatable and passes as a miss.
+template <bool ICMPERR = false>
 __device__ __forceinline__ int nat_ingress_one(const DevCtx &c, BlockStats &bs, u8 *p, u32 len, u32 dlen, u64 now, bool stamped = false) {
     if (dlen < 14) return TC_OK;
     if (rd16(p, 12) != ETH_P_IP_LE) return TC_OK;
@@ -893,6 +900,10 @@ __device__ __forceinline__ int nat_ingress_one(const DevCtx &c, BlockStats &bs, 
         dport = rd16(p, l4 + 2);
     } else if (proto == 1) {
         if (l4 + 8 > dlen) return TC_OK;
+        if (ICMPERR && icmp_error_type(p[l4])) {
+            bstats_add(bs, ST_NAT_PASSED, 1);
+            return TC_OK;
+        }
         sport = 0;
         dport = rd16(p, l4 + 4);
     } else {
@@ -970,4 +981,70 @@ __device__ __forceinline__ int nat_ingress_one(const DevCtx &c, BlockStats &bs, 
     }
     bstats_add(bs, ST_NAT_DNAT, 1);
     return TC_OK;
+}
+
+// bng_nat_icmp_errors_enable: an ICMP error frame (outer ihl 5, type 3 / 11 / 12, the 8-byte ICMP header present)
+// sent to a public address, translated by the flow it quotes (include/bng_b200.h, DESIGN.md §20).  h holds bytes 0-63;
+// the quoted L4 header continues in chunk 4 (bytes 64-79), loaded here.  Returns whether the frame was translated
+// (packets_dnat); otherwise it is unchanged (packets_passed).  Reads only the reverse entry and the session's
+// immutable orig_ip / orig_port: no table, counter or stamp changes, so the frame's place in the batch is immaterial.
+__device__ __forceinline__ bool nat_icmp_error_one(const DevCtx &c, u8 *p, Hdr64 &h, u32 dlen) {
+    const u32 iproto = h.b8(51), isrc = h.b32(54), idst = h.b32(58);
+    // quoted IPv4 header without options, addressed from where the error is sent to, and the lookup's bytes present:
+    // ports through 65, the ICMP id through 67
+    if (h.b8(42) != 0x45 || (iproto != 6 && iproto != 17 && iproto != 1) || isrc != h.b32(30)) return false;
+    if (dlen < (iproto == 1 ? 68u : 66u)) return false;
+    uint4 x = *(const uint4 *)(p + 64); // x.x = bytes 64-67, x.y = 68-71, x.w = 76-79
+    const u16 pport = iproto == 1 ? (u16)(x.x >> 16) : h.b16(62); // the public port: inner source port or ICMP id
+    // nat_reverse as nat44_egress wrote it for the quoted packet (bpf/nat44.c:733-739)
+    u64 rk[2];
+    rk[0] = (u64)idst | ((u64)isrc << 32);
+    rk[1] = (u64)(iproto == 1 ? 0u : (x.x & 0xffffu)) | ((u64)pport << 16) | ((u64)iproto << 32);
+    const u8 *rs = tbl_find<2, true>(c.reverse, rk);
+    if (!rs) return false;
+    u64 ok[2];
+    ok[0] = *(const u64 *)(rs + 16);
+    ok[1] = *(const u64 *)(rs + 24);
+    const u8 *ses = tbl_find<2, false>(c.sessions, ok);
+    if (!ses) return false; // stale: passed, and the entry is left for an ordinary frame to erase
+    const u32 oip = *(const u32 *)(ses + SES_ORIG_IP);
+    const u16 oport = *(const u16 *)(ses + SES_ORIG_PORT);
+    // outer destination (the ICMP checksum has no pseudo-header)
+    h.s32(30, oip);
+    h.s16(24, csum_upd32(h.b16(24), isrc, oip));
+    // quoted source address and its header checksum, then the quoted port / id; every changed word of the ICMP
+    // message goes into the ICMP checksum, in this order
+    const u16 ihc = h.b16(52), ihc2 = csum_upd32(ihc, isrc, oip);
+    h.s32(54, oip);
+    h.s16(52, ihc2);
+    u16 ic = csum_upd32(h.b16(36), isrc, oip);
+    ic = csum_upd16(ic, ihc, ihc2);
+    ic = csum_upd16(ic, pport, oport);
+    bool c4 = true; // chunk 4 changed
+    if (iproto == 1) {
+        const u16 k0 = (u16)x.x, k1 = csum_upd16(k0, pport, oport);
+        x.x = (u32)k1 | ((u32)oport << 16);
+        ic = csum_upd16(ic, k0, k1);
+    } else {
+        h.s16(62, oport);
+        if (iproto == 17 && dlen >= 70 && (u16)x.y != 0) {
+            const u16 k0 = (u16)x.y;
+            u16 k1 = csum_upd16(csum_upd32(k0, isrc, oip), pport, oport);
+            if (k1 == 0) k1 = 0xffff;
+            x.y = (x.y & 0xffff0000u) | k1;
+            ic = csum_upd16(ic, k0, k1);
+        } else if (iproto == 6 && dlen >= 80) {
+            const u16 k0 = (u16)(x.w >> 16), k1 = csum_upd16(csum_upd32(k0, isrc, oip), pport, oport);
+            x.w = (x.w & 0xffffu) | ((u32)k1 << 16);
+            ic = csum_upd16(ic, k0, k1);
+        } else {
+            c4 = false;
+        }
+    }
+    h.s16(36, ic);
+    hdr_store_chunk(h, p, 1);
+    hdr_store_chunk(h, p, 2);
+    hdr_store_chunk(h, p, 3);
+    if (c4) *(uint4 *)(p + 64) = x;
+    return true;
 }

@@ -1289,6 +1289,10 @@ struct ManagerConfig { // :172-200
     int PortsPerSubscriber = 0, PortRangeStart = 0, PortRangeEnd = 0;
     bool EnableEIM = false, EnableEIF = false, EnableHairpin = false, EnableFTPALG = false, EnableSIPALG = false,
          EnablePortParity = false, EnablePortContiguity = false, EnableLogging = false;
+    // Translate inbound ICMP errors by the flow they quote (bng_nat_icmp_errors_enable), applied by Start().  The flag
+    // is context state that no snapshot or delta carries: a standby's Manager sets it too.  false leaves the context's
+    // flag as it is.
+    bool EnableICMPErrorTranslation = false;
     std::shared_ptr<Backend> Backend_;
 };
 
@@ -1511,6 +1515,9 @@ class Manager {
         if (cfg_.EnableSIPALG) {
             ConfigureALG(5060, 17, ALGTypeSIP, true);
             ConfigureALG(5060, 6, ALGTypeSIP, true);
+        }
+        if (cfg_.EnableICMPErrorTranslation) {
+            if (int rc = bng_nat_icmp_errors_enable(be_->ctx, 1)) return MapErr("failed to enable ICMP error translation", rc);
         }
         return Nil();
     }

@@ -21,6 +21,7 @@
 
 #include <algorithm>
 #include <array>
+#include <atomic>
 #include <map>
 #include <memory>
 #include <mutex>
@@ -186,7 +187,9 @@ class Directory {
     }
     // IPv4: by destination (public address, port / echo id).  IPv6 (untagged, ethertype 0x86DD): by the owner of the
     // longest prefix covering the destination (bytes 38-53), the shard that holds its records.  Anything else, and a
-    // destination nobody owns, goes to `fallback`.
+    // destination nobody owns, goes to `fallback`.  With ICMP error translation on (SetICMPErrors), an ICMP error
+    // (type 3, 11 or 12) goes by the flow it quotes: (quoted source, quoted source port or ICMP id), when the frame is
+    // one nat44_ingress can translate; otherwise to `fallback`, since every shard passes it unchanged.
     uint32_t SteerDownstream(const uint8_t *f, uint32_t len, uint32_t fallback = 0) const {
         if (len >= 54 && f[12] == 0x86 && f[13] == 0xDD) {
             auto s = ShardOfV6(f + 38);
@@ -202,11 +205,28 @@ class Directory {
             poff = l4 + 4;
         else
             return fallback;
+        if (proto == 1 && icmp_errors_.load(std::memory_order_relaxed) && l4 + 8 <= len &&
+            (f[l4] == 3 || f[l4] == 11 || f[l4] == 12)) {
+            // the length first: a quoted byte is read only once the frame holds it (66: the TCP/UDP ports, the least a
+            // translatable error carries)
+            if (l4 != 34 || len < 66) return fallback;
+            const uint32_t ip = f[51];
+            if (f[42] != 0x45 || (ip != 6 && ip != 17 && ip != 1) || memcmp(f + 54, f + 30, 4)) return fallback;
+            const uint32_t qoff = ip == 1 ? 66 : 62; // the quoted ICMP id / source port: the public port
+            if (ip == 1 && len < 68) return fallback;
+            uint32_t qsrc;
+            memcpy(&qsrc, f + 54, 4);
+            auto s = ShardOfPublic(qsrc, (uint16_t)((f[qoff] << 8) | f[qoff + 1]));
+            return s ? *s : fallback;
+        }
         if (poff + 2 > len) return fallback;
         uint16_t port = (uint16_t)((f[poff] << 8) | f[poff + 1]);
         auto s = ShardOfPublic(daddr, port);
         return s ? *s : fallback;
     }
+
+    // SteerDownstream keys ICMP errors by the flow they quote (Router::NatICMPErrorsEnable)
+    void SetICMPErrors(bool on) { icmp_errors_.store(on, std::memory_order_relaxed); }
 
   private:
     uint32_t ShardOfMACLocked(uint64_t mac) const {
@@ -220,6 +240,7 @@ class Directory {
     uint32_t world_;
     std::unordered_map<uint64_t, uint32_t> pins_; // MAC -> shard, set by Router::Move
     uint16_t range_start_, pps_;
+    std::atomic<bool> icmp_errors_{false};
     mutable std::mutex mu_;
     std::unordered_map<uint64_t, uint32_t> mac_ip_;
     std::unordered_map<uint32_t, uint64_t> ip_mac_;
@@ -418,6 +439,15 @@ class Router {
     int QoSIPv6Enable(bool on) {
         for (auto &s : shards_)
             if (int r = bng_qos_ipv6_enable(s->ctx, on ? 1 : 0)) return r;
+        return 0;
+    }
+    // ICMP error translation in nat44_ingress (bng_nat_icmp_errors_enable) on every shard, and SteerDownstream sends an
+    // ICMP error to the shard of the flow it quotes (without it, the error's bytes 4-5 name no block and it goes to
+    // `fallback`, which holds no session).  Returns 0 or the first shard's error.
+    int NatICMPErrorsEnable(bool on) {
+        for (auto &s : shards_)
+            if (int r = bng_nat_icmp_errors_enable(s->ctx, on ? 1 : 0)) return r;
+        dir_->SetICMPErrors(on);
         return 0;
     }
     // Drains every shard: fn(shard, record, record size) per record, in (batch, frame) order within a shard (batch

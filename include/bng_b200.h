@@ -145,6 +145,41 @@ void *bng_stream(bng_ctx *ctx); /* the context's cudaStream_t */
  * recently used entry among the 16 slots next to the new key's home slot instead of failing. */
 int bng_sweep(bng_ctx *ctx, uint64_t now_ns, uint64_t *expired_out);
 
+/* ---- nat44_ingress: inbound ICMP errors to the subscriber whose flow they quote (RFC 5508) ----
+ * nat44_ingress keys every ICMPv4 message by bytes 4-5 of its ICMP header, read as an echo id (bpf/nat44.c:846-851).
+ * In an ICMP error those bytes are unused, a pointer or the next-hop MTU; the flow is named by the datagram the error
+ * quotes.  on != 0: from the next bng_prog_run, nat44_ingress applies the rule below to every ICMP error frame:
+ * untagged Ethernet II, ethertype 0x0800, protocol 1, ICMP type 3, 11 or 12, with the 8-byte ICMP header present (as
+ * the program checks it today: bytes through 14 + ihl*4 + 7).  Such a frame is never keyed by bytes 4-5.  Offsets
+ * below are for an outer header without options: ICMP header 34-41 (checksum 36-37), quoted IPv4 header 42-61
+ * (protocol 51, checksum 52-53, source 54-57, destination 58-61), quoted L4 header from 62 (TCP/UDP ports 62-63 and
+ * 64-65, UDP checksum 68-69, TCP checksum 78-79; ICMP checksum 64-65, id 66-67).
+ *   - Translatable: outer ihl 5; quoted version 4 and ihl 5; quoted protocol 6, 17 or 1; quoted source = outer
+ *     destination; and the bytes the lookup needs present ("present": min(len, the slot), as every bounds check):
+ *     through 65 for TCP/UDP, 67 for ICMP.
+ *   - Lookup: the nat_reverse key nat44_egress wrote for the quoted packet (bpf/nat44.c:733-739): {src_ip = quoted
+ *     destination, dst_ip = quoted source, src_port = quoted destination port (0 for ICMP), dst_port = quoted source
+ *     port (the quoted ICMP id, of any ICMP type), protocol}; its value is the session key, and the session gives
+ *     orig_ip and orig_port.
+ *   - Rewrite (csum_upd32 / csum_upd16 steps): outer destination <- orig_ip (outer IPv4 checksum); quoted source <-
+ *     orig_ip (quoted IPv4 checksum); quoted source port or ICMP id <- orig_port (quoted L4 checksum: UDP only when
+ *     68-69 are present and non-zero, a result of 0 becoming 0xFFFF; TCP only when 78-79 are present; ICMP always,
+ *     for the id alone); and every changed word of the ICMP message into the ICMP checksum (36-37), in that order.
+ *     ICMPv4 has no pseudo-header, so the outer destination is not part of it.
+ *   - Outcome: verdict TC_ACT_OK, as for every nat44_ingress frame.  Translated: packets_dnat.  Not translatable, a
+ *     reverse miss, or a stale reverse entry whose session is gone (the entry is NOT erased): passed unchanged,
+ *     packets_passed.  The session is not refreshed (last_seen, its epoch stamp, packets_in, bytes_in and the TCP
+ *     state stay): anyone on the path can forge an error, and an error must not keep a flow alive.  No other table,
+ *     counter or log record changes, so an error frame's result does not depend on its place in the batch.
+ *   - Everything else is as before: frames that are not ICMP error frames (types 0, 8, 4, 5 among them), and
+ *     nat44_egress, which still keys an upstream ICMP error by bytes 4-5.  Accounting, idle detection and interception
+ *     see a translated error by its new destination, the subscriber's address (captured after DNAT).
+ *   - BNG_MEM_HOST with a pinned arena moves bytes 64-79 of an ICMP error frame for nat44_ingress; a fixed-stride
+ *     arena of 64-byte slots (a header-split ring) does not hold the quoted ports, so its errors pass unchanged.
+ * Off by default: nat44_ingress then runs exactly as before.  The flag is context state: snapshots, deltas and
+ * hand-over blobs do not carry it.  Returns 0, or -EINVAL for a NULL ctx. */
+int bng_nat_icmp_errors_enable(bng_ctx *ctx, int on);
+
 /* ---- NAT flow-state flush (what a subscriber's release / RADIUS Disconnect needs) ----
  * Removes the NAT flow state of a set of subscriber addresses.  Until it expires, a departed subscriber's flow state
  * keeps translating: return traffic to its public ports is DNATed to the private address (nat44_ingress never
