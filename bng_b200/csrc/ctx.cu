@@ -179,6 +179,9 @@ struct bng_ctx {
     // bng_nat_icmp_errors_enable: nat44_ingress translates ICMP errors by the flow they quote (context state, as
     // qos_v6)
     bool nat_icmp = false;
+    // bng_antispoof_ipv6_prefixes_enable: antispoof_ingress allows IPv6 sources in their binding's own subscriber_ipv6
+    // prefixes (context state, as qos_v6)
+    bool as_v6 = false;
 };
 
 namespace {
@@ -1122,6 +1125,7 @@ static int dispatch(bng_ctx *c, int prog, const DevBatch &b, const LiSrc &src = 
     const bool pipe = prog == P_PIPE_UP || prog == P_PIPE_TC;
     const Tbl *v6 = c->v6_live ? &c->v6 : nullptr; // an empty table launches exactly what it did before it existed
     const Tbl *qv6 = c->qos_v6 ? v6 : nullptr;     // ... and so does shaping IPv6 with it
+    const Tbl *as6 = c->as_v6 ? v6 : nullptr;      // ... and antispoof allowing the prefixes' sources
     // the upstream classify records attributions: for accounting and idle detection, and in the pipelines to tell
     // antispoof's drops
     c->L.acct_attr = (acct || idle || (li == 0 && pipe)) ? c->L.s.attr : nullptr;
@@ -1137,15 +1141,15 @@ static int dispatch(bng_ctx *c, int prog, const DevBatch &b, const LiSrc &src = 
         if (e != cudaSuccess) return fail(c, -EIO, "launch k_li_capture: %s", cudaGetErrorString(e));
     }
     switch (prog) {
-    case P_ANTISPOOF: e = run_antispoof(c->L, c->dev, b); break;
+    case P_ANTISPOOF: e = run_antispoof(c->L, c->dev, b, as6); break;
     case P_QOS_EG: e = run_qos(c->L, c->dev, b, true, qv6); break;
     case P_QOS_IN: e = run_qos(c->L, c->dev, b, false, qv6); break;
     case P_NAT_EG: e = run_nat_egress(c->L, c->dev, b); break;
     case P_NAT_IN: e = run_nat_ingress(c->L, c->dev, b, c->nat_icmp); break;
     case P_NAT_HAIRPIN: e = run_nat_hairpin_xdp(c->L, c->dev, b); break;
     case P_DHCP: e = run_dhcp_fastpath(c->L, c->dev, b); break;
-    case P_PIPE_UP: e = run_pipeline_up(c->L, c->dev, b, qv6); break;
-    case P_PIPE_TC: e = run_pipeline_tc(c->L, c->dev, b, qv6); break;
+    case P_PIPE_UP: e = run_pipeline_up(c->L, c->dev, b, qv6, as6); break;
+    case P_PIPE_TC: e = run_pipeline_tc(c->L, c->dev, b, qv6, as6); break;
     default: return -EINVAL;
     }
     // after the program, before anything copies the frames out: the downstream modes read the rewritten headers
@@ -3368,6 +3372,13 @@ int bng_qos_ipv6_enable(bng_ctx *c, int on) {
     if (!c) return -EINVAL;
     std::lock_guard<std::mutex> g(c->mu);
     c->qos_v6 = on != 0;
+    return 0;
+}
+
+int bng_antispoof_ipv6_prefixes_enable(bng_ctx *c, int on) {
+    if (!c) return -EINVAL;
+    std::lock_guard<std::mutex> g(c->mu);
+    c->as_v6 = on != 0;
     return 0;
 }
 

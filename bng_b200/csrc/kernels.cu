@@ -68,14 +68,20 @@ __device__ __forceinline__ void grouped_select(const Grouped &g, const u32 *cnt,
 
 // ---------------------------------------------------------------------------
 // antispoof_ingress
+// V6 (bng_antispoof_ipv6_prefixes_enable, while subscriber_ipv6 has live entries): antispoof_eval<true>, a
+// subscriber's own prefixes count as its IPv6 addresses; only frames on the IPv6 drop path probe the table.
 // ---------------------------------------------------------------------------
 #define AS_MINB 5
-__global__ void __launch_bounds__(BLOCK, AS_MINB) k_antispoof(const __grid_constant__ DevCtx c, const __grid_constant__ DevBatch b) {
+template <bool V6>
+__global__ void __launch_bounds__(BLOCK, AS_MINB) k_antispoof(const __grid_constant__ DevCtx c, const __grid_constant__ DevBatch b,
+                                                              const __grid_constant__ Tbl v6) {
     __shared__ BlockStats bs;
     __shared__ SpoofQ sqs[BLOCK / 32];
+    __shared__ V6Lens lens;
     static_assert(64 <= SPOOFQ_CAP, "a trip's 32 frames must fit in what a flush at 32 leaves free");
     bstats_init(bs);
     spoofq_init(sqs);
+    if (V6) v6_lens_load(lens, v6.plens);
     SpoofQ &sq = sqs[threadIdx.x >> 5];
     u32 cfg = *(const u16 *)c.as_config;
     AsCnt cn = {0, 0};
@@ -112,7 +118,12 @@ __global__ void __launch_bounds__(BLOCK, AS_MINB) k_antispoof(const __grid_const
                 bv = bind_load(tbl_finish<1>(c.bindings, &mk, hi + 1, w1, true));
             }
         }
-        if (act) b.verdict[i] = (u8)antispoof_eval(c, &sq, h, len, i + b.base, frame_now(b, i), bv, cfg, cn);
+        if (V6) {
+            bool own6 = false;
+            if (act) b.verdict[i] = (u8)antispoof_eval<true>(c, &sq, h, len, i + b.base, frame_now(b, i), bv, cfg, cn, &v6, &lens, &own6);
+        } else if (act) {
+            b.verdict[i] = (u8)antispoof_eval(c, &sq, h, len, i + b.base, frame_now(b, i), bv, cfg, cn);
+        }
         ascnt_spill(bs, cn);
     }
     spoof_flush(c, sq);
@@ -1040,8 +1051,11 @@ static void launch_resolve(Launcher &L, const DevCtx &c, const DevBatch &b, cons
     L.launches++;
 }
 
-cudaError_t run_antispoof(Launcher &L, const DevCtx &c, const DevBatch &b) {
-    LAUNCH(k_antispoof, b.n, 8, c, b);
+cudaError_t run_antispoof(Launcher &L, const DevCtx &c, const DevBatch &b, const Tbl *as6) {
+    if (as6)
+        LAUNCH_AS("k_antispoof<v6>", k_antispoof<true>, b.n, 8, c, b, *as6);
+    else
+        LAUNCH_AS("k_antispoof", k_antispoof<false>, b.n, 8, c, b, Tbl{});
     return cudaGetLastError();
 }
 
@@ -1066,21 +1080,33 @@ cudaError_t run_qos(Launcher &L, const DevCtx &c, const DevBatch &b0, bool egres
 // The programs keyed on the subscriber directory (nat44_egress, pipeline_up, pipeline_tc): classify, group by
 // directory slot, resolve.  The names are what each launch is timed as; with accounting on, classify is the
 // ACCT instantiation and is timed under its own name.  v6 (the pipelines only): IPv6 frames are shaped, classify is
-// the V6 instantiation and is timed under its name with a ", v6>" suffix.
+// the V6 instantiation and is timed under its name with a ", v6>" suffix.  as6 (the pipelines only): antispoof allows
+// IPv6 sources in their subscriber's prefixes, classify is the AS6 instantiation, timed with an ", as6>" suffix.
 struct ClassifyNames {
-    const char *plain, *acct, *v6, *acct_v6;
+    const char *plain, *acct, *v6, *acct_v6, *as6, *acct_as6, *v6_as6, *acct_v6_as6;
 };
-template <bool AS, bool QOS, bool TC, bool ACCT, bool V6>
+template <bool AS, bool QOS, bool TC, bool ACCT, bool V6, bool AS6 = false>
 static void launch_classify(Launcher &L, const DevCtx &c, const DevBatch &b, const char *name, const Tbl &v6) {
-    LAUNCH_AS(name, (k_pipe_classify<AS, QOS, TC, ACCT, V6>), b.n, CLASSIFY_BPS(AS), c, b, L.s.key_a, L.s.val_a, L.s.counters, sort_T(L),
-              ACCT ? L.acct_attr : nullptr, v6);
+    LAUNCH_AS(name, (k_pipe_classify<AS, QOS, TC, ACCT, V6, AS6>), b.n, CLASSIFY_BPS(AS), c, b, L.s.key_a, L.s.val_a, L.s.counters,
+              sort_T(L), ACCT ? L.acct_attr : nullptr, v6);
 }
 template <bool AS, bool QOS, bool TC>
 static cudaError_t run_dir_prog(Launcher &L, const DevCtx &c, const DevBatch &b0, const ClassifyNames &nm, const char *resolve_name,
-                                const Tbl *v6) {
+                                const Tbl *v6, const Tbl *as6) {
     DevBatch b = b0;
     b.kshift = kshift_for((u64)c.subdir.mask + 1);
-    if (QOS && v6) { // (V6 = QOS: nat44_egress has no bucket and is never given the table)
+    if (AS && as6) { // (AS6 = AS: nat44_egress has no antispoof stage and is never given the table)
+        if (QOS && v6) {
+            if (L.acct_attr)
+                launch_classify<AS, QOS, TC, true, QOS, AS>(L, c, b, nm.acct_v6_as6, *as6);
+            else
+                launch_classify<AS, QOS, TC, false, QOS, AS>(L, c, b, nm.v6_as6, *as6);
+        } else if (L.acct_attr) {
+            launch_classify<AS, QOS, TC, true, false, AS>(L, c, b, nm.acct_as6, *as6);
+        } else {
+            launch_classify<AS, QOS, TC, false, false, AS>(L, c, b, nm.as6, *as6);
+        }
+    } else if (QOS && v6) { // (V6 = QOS: nat44_egress has no bucket and is never given the table)
         if (L.acct_attr)
             launch_classify<AS, QOS, TC, true, QOS>(L, c, b, nm.acct_v6, *v6);
         else
@@ -1099,7 +1125,7 @@ static cudaError_t run_dir_prog(Launcher &L, const DevCtx &c, const DevBatch &b0
 
 cudaError_t run_nat_egress(Launcher &L, const DevCtx &c, const DevBatch &b) {
     return run_dir_prog<false, false, false>(L, c, b, {"(k_pipe_classify<false, false>)", "(k_pipe_classify<false, false, false, true>)"},
-                                             "(k_resolve<true, false, false>)", nullptr);
+                                             "(k_resolve<true, false, false>)", nullptr, nullptr);
 }
 
 cudaError_t run_nat_ingress(Launcher &L, const DevCtx &c, const DevBatch &b, bool icmp_errors) {
@@ -1115,16 +1141,21 @@ cudaError_t run_nat_hairpin_xdp(Launcher &L, const DevCtx &c, const DevBatch &b)
     return cudaGetLastError();
 }
 
-cudaError_t run_pipeline_up(Launcher &L, const DevCtx &c, const DevBatch &b, const Tbl *v6) {
+cudaError_t run_pipeline_up(Launcher &L, const DevCtx &c, const DevBatch &b, const Tbl *v6, const Tbl *as6) {
     return run_dir_prog<true, true, false>(L, c, b,
                                            {"(k_pipe_classify<true, true>)", "(k_pipe_classify<true, true, false, true>)",
-                                            "(k_pipe_classify<true, true, v6>)", "(k_pipe_classify<true, true, false, true, v6>)"},
-                                           "(k_resolve<true, true, false>)", v6);
+                                            "(k_pipe_classify<true, true, v6>)", "(k_pipe_classify<true, true, false, true, v6>)",
+                                            "(k_pipe_classify<true, true, as6>)", "(k_pipe_classify<true, true, false, true, as6>)",
+                                            "(k_pipe_classify<true, true, v6, as6>)", "(k_pipe_classify<true, true, false, true, v6, as6>)"},
+                                           "(k_resolve<true, true, false>)", v6, as6);
 }
 
-cudaError_t run_pipeline_tc(Launcher &L, const DevCtx &c, const DevBatch &b, const Tbl *v6) {
+cudaError_t run_pipeline_tc(Launcher &L, const DevCtx &c, const DevBatch &b, const Tbl *v6, const Tbl *as6) {
     return run_dir_prog<true, true, true>(L, c, b,
                                           {"(k_pipe_classify<true, true, true>)", "(k_pipe_classify<true, true, true, true>)",
-                                           "(k_pipe_classify<true, true, true, v6>)", "(k_pipe_classify<true, true, true, true, v6>)"},
-                                          "(k_resolve<true, true, false, tc>)", v6);
+                                           "(k_pipe_classify<true, true, true, v6>)", "(k_pipe_classify<true, true, true, true, v6>)",
+                                           "(k_pipe_classify<true, true, true, as6>)", "(k_pipe_classify<true, true, true, true, as6>)",
+                                           "(k_pipe_classify<true, true, true, v6, as6>)",
+                                           "(k_pipe_classify<true, true, true, true, v6, as6>)"},
+                                          "(k_resolve<true, true, false, tc>)", v6, as6);
 }

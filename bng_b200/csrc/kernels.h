@@ -44,7 +44,9 @@ void prof_collect(Launcher &L); // call after the stream has been synchronised
 
 size_t sort_temp_bytes(u32 n);
 
-cudaError_t run_antispoof(Launcher &L, const DevCtx &c, const DevBatch &b);
+// as6 (antispoof_ingress and the pipelines): subscriber_ipv6 when antispoof allows IPv6 sources in their subscriber's
+// prefixes (bng_antispoof_ipv6_prefixes_enable, and the table has live entries), else nullptr
+cudaError_t run_antispoof(Launcher &L, const DevCtx &c, const DevBatch &b, const Tbl *as6);
 // v6: subscriber_ipv6 when IPv6 frames are shaped by their owner's bucket (bng_qos_ipv6_enable, and the table has live
 // entries), else nullptr
 cudaError_t run_qos(Launcher &L, const DevCtx &c, const DevBatch &b, bool egress, const Tbl *v6);
@@ -52,8 +54,8 @@ cudaError_t run_nat_egress(Launcher &L, const DevCtx &c, const DevBatch &b);
 // icmp_errors: ICMP errors are translated by the flow they quote (bng_nat_icmp_errors_enable)
 cudaError_t run_nat_ingress(Launcher &L, const DevCtx &c, const DevBatch &b, bool icmp_errors);
 cudaError_t run_nat_hairpin_xdp(Launcher &L, const DevCtx &c, const DevBatch &b);
-cudaError_t run_pipeline_up(Launcher &L, const DevCtx &c, const DevBatch &b, const Tbl *v6);
-cudaError_t run_pipeline_tc(Launcher &L, const DevCtx &c, const DevBatch &b, const Tbl *v6);
+cudaError_t run_pipeline_up(Launcher &L, const DevCtx &c, const DevBatch &b, const Tbl *v6, const Tbl *as6);
+cudaError_t run_pipeline_tc(Launcher &L, const DevCtx &c, const DevBatch &b, const Tbl *v6, const Tbl *as6);
 cudaError_t run_dhcp_fastpath(Launcher &L, const DevCtx &c, const DevBatch &b);
 
 // header gather / scatter between a pinned host arena and a compact device copy (hostio.cu); icmp_errors (TC only):

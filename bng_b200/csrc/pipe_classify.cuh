@@ -42,11 +42,15 @@
 // directory slot in their place.  The frame gets the owner's ordering key, so the ordered phase charges it in index
 // order with the owner's IPv4 frames; it never carries MISS_FLAG or DEFER_FLAG, so there it meets only the bucket, and
 // nothing of NAT ever sees it.  With ACCT its attribution word is the owner's slot.
-template <bool AS, bool QOS, bool TC = false, bool ACCT = false, bool V6 = false>
+// AS6 (bng_antispoof_ipv6_prefixes_enable, while subscriber_ipv6 has live entries; AS only): antispoof_eval<true>, an
+// IPv6 frame on antispoof's drop path whose source is in its binding's own prefixes is allowed.  The frame's source is
+// already in h.  With V6 too, the owner antispoof found (the binding's ipv4_addr) stands in for phase 3's v6_owner.
+template <bool AS, bool QOS, bool TC = false, bool ACCT = false, bool V6 = false, bool AS6 = false>
 __global__ void __launch_bounds__(BLOCK, CLASSIFY_BPS(AS))
     k_pipe_classify(const __grid_constant__ DevCtx c, const __grid_constant__ DevBatch b, u32 *skey, u32 *sval, u32 *cnt, u32 *T,
                     u32 *attr, const __grid_constant__ Tbl v6) {
     static_assert(!V6 || QOS, "IPv6 frames only ever meet a token bucket");
+    static_assert(!AS6 || AS, "the prefixes widen antispoof's verdicts");
     __shared__ SmallTabs st;
     scratch_reset(cnt, T);
     __shared__ BlockStats bs;
@@ -54,7 +58,7 @@ __global__ void __launch_bounds__(BLOCK, CLASSIFY_BPS(AS))
     __shared__ V6Lens lens;
     smem_stage_begin(&st, c.small, (u32)sizeof(SmallTabs), &bar);
     bstats_init(bs);
-    if (V6) v6_lens_load(lens, v6.plens);
+    if (V6 || AS6) v6_lens_load(lens, v6.plens);
     smem_stage_wait(&bar);
     const u32 lane = threadIdx.x & 31;
 #define as_cfg (st.as_cfg) /* read from shared memory / the constant bank where used: no live registers */
@@ -112,6 +116,7 @@ __global__ void __launch_bounds__(BLOCK, CLASSIFY_BPS(AS))
 
         // ---- phase 2: antispoof_ingress ----
         int v = TC_OK;
+        bool own6 = false; // AS6: antispoof allowed the frame by its binding's prefixes
         if (AS) {
             const u8 *bind = nullptr;
             if (dlen >= 14 && mk < K_BUSY) {
@@ -125,7 +130,10 @@ __global__ void __launch_bounds__(BLOCK, CLASSIFY_BPS(AS))
             }
             __syncwarp();
             bv.has = bind != nullptr;
-            v = antispoof_eval(c, nullptr, h, dlen, i + b.base, act ? frame_now(b, i) : 0, bv, as_cfg, cn); // (the clock is read where it is used: no live register)
+            if (AS6)
+                v = antispoof_eval<true>(c, nullptr, h, dlen, i + b.base, act ? frame_now(b, i) : 0, bv, as_cfg, cn, &v6, &lens, &own6);
+            else
+                v = antispoof_eval(c, nullptr, h, dlen, i + b.base, act ? frame_now(b, i) : 0, bv, as_cfg, cn); // (the clock is read where it is used: no live register)
             __syncwarp();
         }
         const bool alive = act && v != TC_SHOT && ip4;
@@ -151,7 +159,8 @@ __global__ void __launch_bounds__(BLOCK, CLASSIFY_BPS(AS))
             u32 a[4], owner;
 #pragma unroll
             for (int j = 0; j < 4; j++) a[j] = h.b32(22 + 4 * j);
-            if (v6_owner(v6, lens, a, &owner)) {
+            if (AS6 && own6) owner = bv.s.w[2];
+            if ((AS6 && own6) || v6_owner(v6, lens, a, &owner)) {
                 const u32 s = dir_slot_of(c.subdir, owner);
                 if (s != DIR_NONE) {
                     qos_slot = (u32)(*(const u64 *)(c.subdir.slots + (size_t)s * 16 + 8) >> 32);

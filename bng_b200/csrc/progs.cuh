@@ -141,8 +141,14 @@ __device__ __forceinline__ BindVal bind_load(const u8 *slot) {
     if (slot) b.s = ldg256(slot);
     return b;
 }
+// V6 (bng_antispoof_ipv6_prefixes_enable, while subscriber_ipv6 has live entries): on the IPv6 drop path only, a
+// frame from a bound MAC with ipv4_valid whose source's longest covering subscriber_ipv6 prefix has the binding's
+// ipv4_addr as its value is allowed after all (*own6 := true): a subscriber's own prefixes count as its addresses.
+// A template parameter, so that the instantiation without it is the code it was.
+template <bool V6 = false>
 __device__ __forceinline__ int antispoof_eval(const DevCtx &c, SpoofQ *sq, const Hdr64 &h, u32 len, u32 idx, u64 now, const BindVal &bv,
-                                              u32 cfg, AsCnt &cn) {
+                                              u32 cfg, AsCnt &cn, const Tbl *v6 = nullptr, const V6Lens *lens = nullptr,
+                                              bool *own6 = nullptr) {
     u32 &n_allowed = cn.allowed;
     const bool bind = bv.has;
     if (len < 14) return TC_OK; // :195-196, no stats
@@ -191,6 +197,16 @@ __device__ __forceinline__ int antispoof_eval(const DevCtx &c, SpoofQ *sq, const
             allowed = true;
         }
         if (!allowed && mode != 3) {
+            if (V6 && bind && (b_flags & 0xff)) {
+                u32 a[4], owner;
+#pragma unroll
+                for (int k = 0; k < 4; k++) a[k] = h.b32(22 + 4 * k);
+                if (v6_owner(*v6, *lens, a, &owner) && owner == b_ipv4) { // (the 4 bytes the IPv4 branch compares)
+                    *own6 = true;
+                    n_allowed++;
+                    return TC_OK;
+                }
+            }
             if (log_viol) spoof_log(c, sq, cn, idx, now, h, 0, 0, true);
             cn.rare += ASC_V6;
             return TC_SHOT;

@@ -100,6 +100,7 @@ def load_library() -> C.CDLL:
         "bng_launch_count": ([vp], u64),
         "bng_ipv6_prefix_lengths": ([vp, vp], i32),
         "bng_qos_ipv6_enable": ([vp, i32], i32),
+        "bng_antispoof_ipv6_prefixes_enable": ([vp, i32], i32),
         "bng_nat_icmp_errors_enable": ([vp, i32], i32),
         "bng_lru_overflow": ([vp], u64),
         "bng_events_lost": ([vp], u64),
@@ -155,7 +156,7 @@ EXPORTED_SYMBOLS = (
     "bng_idle_enable", "bng_idle_timeout_set", "bng_idle_read", "bng_idle_scan", "bng_nat_usage",
     "bng_dhcp_lease_census", "bng_dhcp_lease_sweep", "bng_lease_table_rebuilds", "bng_dhcp_lease_addr_order",
     "bng_sub_export", "bng_sub_import", "bng_ipv6_prefix_lengths", "bng_qos_ipv6_enable",
-    "bng_nat_icmp_errors_enable",
+    "bng_nat_icmp_errors_enable", "bng_antispoof_ipv6_prefixes_enable",
 )
 
 
@@ -314,6 +315,12 @@ class Dataplane:
         two pipelines), from the next run on; off by default.  Context state: snapshots, deltas and hand-over blobs do
         not carry it."""
         self._chk(self.lib.bng_qos_ipv6_enable(self.h, 1 if on else 0), "qos_ipv6_enable")
+
+    def antispoof_ipv6_prefixes_enable(self, on: bool = True):
+        """Let antispoof_ingress (standalone and in the two pipelines) allow an IPv6 source that lies in its binding's
+        own subscriber_ipv6 prefixes, from the next run on; off by default (include/bng_b200.h).  Context state:
+        snapshots, deltas and hand-over blobs do not carry it."""
+        self._chk(self.lib.bng_antispoof_ipv6_prefixes_enable(self.h, 1 if on else 0), "antispoof_ipv6_prefixes_enable")
 
     def nat_icmp_errors_enable(self, on: bool = True):
         """Translate inbound ICMP errors (Destination Unreachable, Time Exceeded, Parameter Problem) in nat44_ingress

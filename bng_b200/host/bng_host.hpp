@@ -756,6 +756,10 @@ struct ManagerConfig { // :89-94
     Mode DefaultMode = ModeDisabled;
     bool LogViolations = true;
     std::shared_ptr<Backend> Backend_;
+    // Let a binding's own subscriber_ipv6 prefixes (Framed-IPv6-Prefix, Delegated-IPv6-Prefix) count as its IPv6
+    // addresses (bng_antispoof_ipv6_prefixes_enable), applied by Start().  The flag is context state that no snapshot
+    // or delta carries: a standby's Manager sets it too.  false leaves the context's flag as it is.
+    bool ValidateIPv6Prefixes = false;
 };
 
 class Manager {
@@ -788,6 +792,9 @@ class Manager {
             uint32_t key = 0;
             int rc = bng_map_update(be_->ctx, config_, &key, &c, BNG_ANY);
             if (rc) return MapErr("failed to set config", rc);
+        }
+        if (cfg_.ValidateIPv6Prefixes) {
+            if (int rc = bng_antispoof_ipv6_prefixes_enable(be_->ctx, 1)) return MapErr("failed to enable IPv6 prefix validation", rc);
         }
         return Nil();
     }

@@ -441,6 +441,14 @@ class Router {
             if (int r = bng_qos_ipv6_enable(s->ctx, on ? 1 : 0)) return r;
         return 0;
     }
+    // Antispoof by delegated prefix (bng_antispoof_ipv6_prefixes_enable) on every shard.  The rule needs a
+    // subscriber's binding and its prefixes on one shard: the binding is routed ByMAC and subscriber_ipv6 ByValueIP,
+    // the shard of the IPv4 address and so of its MAC.  Returns 0 or the first shard's error.
+    int AntispoofIPv6PrefixesEnable(bool on) {
+        for (auto &s : shards_)
+            if (int r = bng_antispoof_ipv6_prefixes_enable(s->ctx, on ? 1 : 0)) return r;
+        return 0;
+    }
     // ICMP error translation in nat44_ingress (bng_nat_icmp_errors_enable) on every shard, and SteerDownstream sends an
     // ICMP error to the shard of the flow it quotes (without it, the error's bytes 4-5 name no block and it goes to
     // `fallback`, which holds no session).  Returns 0 or the first shard's error.

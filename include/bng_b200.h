@@ -681,6 +681,24 @@ typedef struct bng_ipv6_prefix_key {
  * Off by default.  The flag is context state: snapshots, deltas and hand-over blobs do not carry it, so a standby or
  * the destination of a hand-over sets it itself.  Returns 0, or -EINVAL for a NULL ctx. */
 int bng_qos_ipv6_enable(bng_ctx *ctx, int on);
+/* Antispoof by delegated prefix: a subscriber's own subscriber_ipv6 prefixes count as its IPv6 addresses.  on != 0:
+ * from the next bng_prog_run, antispoof_ingress (standalone, and its stage in pipeline_up and pipeline_tc) allows an
+ * IPv6 frame that the reference would drop when all of these hold:
+ *   - the frame reaches the reference's IPv6 drop: untagged, ethertype 0x86DD at bytes 12-13, at least 54 bytes
+ *     present, mode neither disabled nor log-only, not allowed by the exact match with ipv6_addr or by loose mode;
+ *   - the source MAC has a subscriber_bindings entry with ipv4_valid set;
+ *   - the longest prefix in subscriber_ipv6 that covers the source address (bytes 22-37) has the binding's ipv4_addr
+ *     as its value (the same 4 bytes the IPv4 branch compares with saddr).
+ * Such a frame gets TC_ACT_OK and adds 1 to packets_allowed, and nothing else: no spoof event, no packets_logged,
+ * packets_dropped or ipv6_violations.  From there it is an ordinary passed IPv6 frame: NAT passes it untouched, QoS
+ * passes it (or shapes it with its owner's bucket, bng_qos_ipv6_enable), and accounting, idle detection and
+ * interception attribute it by the rule above.  Every other frame is unchanged: a source whose longest covering prefix
+ * belongs to another subscriber (a longer prefix nested in the binding's own, say), unbound MACs, bindings without
+ * ipv4_valid, tagged and short frames, every non-IPv6 frame.
+ * While subscriber_ipv6 is empty, "on" launches exactly what "off" launches.  Off by default.  The flag is context
+ * state: snapshots, deltas and hand-over blobs do not carry it, so a standby or the destination of a hand-over sets
+ * it itself.  Returns 0, or -EINVAL for a NULL ctx. */
+int bng_antispoof_ipv6_prefixes_enable(bng_ctx *ctx, int on);
 
 /* ---- diagnostics ---- */
 uint64_t bng_launch_count(bng_ctx *ctx);  /* kernels launched by this context so far */
