@@ -182,6 +182,15 @@ struct bng_ctx {
     // bng_antispoof_ipv6_prefixes_enable: antispoof_ingress allows IPv6 sources in their binding's own subscriber_ipv6
     // prefixes (context state, as qos_v6)
     bool as_v6 = false;
+    // The DHCPv6 fast path (not maps of the reference, include/bng_b200.h): dhcpv6_bindings, dhcpv6_server_config, and
+    // the host's copies of what selects k_dhcp_fastpath<v6>: the bindings' live-entry count as of the last command
+    // that changed it, and the server configuration as last written
+    Tbl d6b{};
+    u8 *d6cfg = nullptr;
+    u32 d6_live = 0;
+    u8 d6cfg_host[DHCP6_CFG_BYTES] = {};
+    // bng_dhcpv6_enable: dhcp_fastpath_prog answers bound DHCPv6 clients (context state, as qos_v6)
+    bool dhcp6 = false;
 };
 
 namespace {
@@ -349,6 +358,28 @@ void v6_mask_key(u8 *key) {
     memcpy(key, w, 20);
 }
 
+// ---- dhcpv6_bindings ----
+int d6_refresh_locked(bng_ctx *c) {
+    CU(c, cudaMemcpyAsync(&c->d6_live, c->d6b.count, 4, cudaMemcpyDeviceToHost, c->L.stream));
+    CU(c, cudaStreamSynchronize(c->L.stream));
+    return 0;
+}
+// An entry the fast path could not use the way it reads it (include/bng_b200.h: the update's -EINVAL)
+bool d6_bad_binding(const u8 *key, const u8 *val) {
+    const u32 dl = key[0];
+    if (dl == 0 || dl > 31) return true;
+    for (u32 k = 1 + dl; k < 32; k++)
+        if (key[k]) return true;
+    const u32 flags = val[6], pl = val[7];
+    if ((flags & ~3u) || !flags) return true;
+    if (flags & BNG_DHCPV6_PD) {
+        if (pl == 0 || pl > 128) return true;
+        for (u32 b = pl; b < 128; b++)
+            if ((val[48 + b / 8] >> (7 - b % 8)) & 1) return true;
+    }
+    return false;
+}
+
 // ---- control-plane commands on hash maps ----
 int hash_cmd(bng_ctx *c, MapReg *m, int op, const void *keys, void *vals, u64 n, u32 flags, int *first_err, u64 *n_err = nullptr) {
     const Tbl &t = *m->tbl;
@@ -383,6 +414,7 @@ int hash_cmd(bng_ctx *c, MapReg *m, int op, const void *keys, void *vals, u64 n,
         }
     }
     if (m->tbl == &c->v6 && op != TOP_LOOKUP) return v6_refresh_locked(c);
+    if (m->tbl == &c->d6b && op != TOP_LOOKUP) return d6_refresh_locked(c);
     return 0;
 }
 
@@ -688,6 +720,9 @@ bng_ctx *bng_open(const bng_open_opts *o) {
     // subscriber_ipv6: a WAN /64 or /128 and a delegated prefix per subscriber; 32-byte slots (key words, value at 24)
     OPEN_R(make_table(c, &c->v6, LPM6_KEY, 4, 24, 2 * max_subs));
     OPEN_R(dev_alloc(c, (void **)&c->v6.plens, LPM6_LENS * 4, 0));
+    // dhcpv6_bindings: 96-byte slots (32-byte key, the 64-byte binding at 32)
+    OPEN_R(make_table(c, &c->d6b, 32, 64, 32, max_subs));
+    OPEN_R(dev_alloc(c, (void **)&c->d6cfg, DHCP6_CFG_BYTES, 0));
     // subscriber directory: 16-byte slots, as many as the per-subscriber maps have, room for both maps' keys
     OPEN_R(make_table(c, &d.subdir, 4, 8, 8, max_subs, 0, 16));
     d.subdir.max_entries = std::min<u64>(2ull * max_subs, d.subdir.mask);
@@ -698,7 +733,7 @@ bng_ctx *bng_open(const bng_open_opts *o) {
     OPEN_R(dev_alloc(c, (void **)&d.nat_config, 16, 0));
     OPEN_R(dev_alloc(c, (void **)&d.server_config, 16, 0));
     OPEN_R(dev_alloc(c, (void **)&d.nat_pool, 256 * 16, 0));
-    OPEN_R(dev_alloc(c, (void **)&d.stats, ST_COUNT * 8, 0));
+    OPEN_R(dev_alloc(c, (void **)&d.stats, ST_ALL * 8, 0));
     OPEN_R(make_ring(c, &d.spoof_ev, 56, ev_cap, ST_EV_LOST_SPOOF));
     OPEN_R(make_ring(c, &d.natlog_ev, 40, ev_cap, ST_EV_LOST_NATLOG));
     OPEN_CU(cudaMalloc((void **)&c->L.s.counters, 64));
@@ -736,6 +771,10 @@ bng_ctx *bng_open(const bng_open_opts *o) {
     add_hash(c, "circuit_id_subscribers", T_HASH, 32, 25, max_subs, &d.cid_subs);
     // not a map of the reference: IPv6 prefix -> subscriber IPv4 address (include/bng_b200.h), reported as an LPM trie
     add_hash(c, "subscriber_ipv6", T_LPM, LPM6_KEY, 4, 2 * max_subs, &c->v6);
+    // not maps of the reference: the DHCPv6 fast path's cache (include/bng_b200.h)
+    add_hash(c, "dhcpv6_bindings", T_HASH, 32, 64, max_subs, &c->d6b);
+    add_array(c, "dhcpv6_server_config", DHCP6_CFG_BYTES, 1, &c->d6cfg);
+    add_stats(c, "dhcpv6_stats", T_ARRAY, ST_DHCP6_N * 8, ST_DHCP6);
     c->staged.resize(c->maps.size());
     OPEN_R(small_refresh(c));
     cudaError_t se = cudaStreamSynchronize(c->L.stream);
@@ -801,6 +840,9 @@ int bng_map_update_batch(bng_ctx *c, int map, const void *keys, const void *valu
         // wherever a key repeats (usually nowhere) and the pieces run in order.
         int first = 0, r = 0;
         const u32 ks = m->key_size;
+        if (m->tbl == &c->d6b)
+            for (u64 i = 0; i < n; i++)
+                if (d6_bad_binding((const u8 *)keys + i * ks, (const u8 *)values + i * m->value_size)) return -EINVAL;
         std::vector<u8> masked;
         if (m->tbl == &c->v6) { // two spellings of one prefix are one key
             masked.assign((const u8 *)keys, (const u8 *)keys + n * ks);
@@ -837,12 +879,17 @@ int bng_map_update_batch(bng_ctx *c, int map, const void *keys, const void *valu
             u32 idx = ((const u32 *)keys)[i];
             if (idx >= m->max_entries) return -E2BIG;
             if (flags == BNG_NOEXIST) return -EEXIST;
+            if (m->arr == &c->d6cfg) { // duid_len, dns_count
+                const u8 *v = (const u8 *)values + i * m->value_size;
+                if (v[6] > 32 || v[7] > 2) return -EINVAL;
+            }
             u8 *dst = m->kind == KIND_ARRAY ? *m->arr + (size_t)idx * m->value_size : (u8 *)(c->dev.stats + m->stat_base);
             CU(c, cudaMemcpyAsync(dst, (const u8 *)values + i * m->value_size, m->value_size, cudaMemcpyHostToDevice,
                                   c->L.stream));
         }
         CU(c, cudaStreamSynchronize(c->L.stream));
         if (feeds_small_tabs(m)) c->small_dirty = true;
+        if (m->arr == &c->d6cfg && n) memcpy(c->d6cfg_host, (const u8 *)values + (n - 1) * m->value_size, DHCP6_CFG_BYTES);
         return 0;
     case KIND_LPM:
         for (u64 i = 0; i < n; i++) {
@@ -956,6 +1003,7 @@ int bng_map_clear(bng_ctx *c, int map) {
     CU(c, cudaMemsetAsync(t.count, 0, 4, c->L.stream));
     if (t.plens) CU(c, cudaMemsetAsync(t.plens, 0, LPM6_LENS * 4, c->L.stream));
     if (m->tbl == &c->v6) c->v6_live = 0;
+    if (m->tbl == &c->d6b) c->d6_live = 0;
     if (m->tbl == &c->dev.sub_nat || m->tbl == &c->dev.qos_in)
         CU(c, run_dir_clear_half(c->L, c->dev.subdir, m->tbl == &c->dev.sub_nat ? 1 : 2));
     CU(c, cudaStreamSynchronize(c->L.stream));
@@ -1117,7 +1165,14 @@ static const int k_acct_mode[] = {-1, ACCT_DST, ACCT_SRC, ACCT_ATTR, ACCT_DST, -
 // the interception direction of each program: BNG_LI_UPLINK (0), BNG_LI_DOWNLINK (1), -1: never captures
 static const int k_li_dir[] = {-1, 1, 0, 0, 1, -1, -1, 0, 0};
 
-static int dispatch(bng_ctx *c, int prog, const DevBatch &b, const LiSrc &src = LiSrc{}) {
+// The storage of the caller's frames, for replies longer than their request (k_dhcp_fastpath<v6>): room_stride bytes
+// each, or 0: len rounded up to 16; need: the pinned zero-copy feed's bytes to scatter back, else nullptr.
+struct FrameRoom {
+    u32 room_stride;
+    u32 *need;
+};
+
+static int dispatch(bng_ctx *c, int prog, const DevBatch &b, const LiSrc &src = LiSrc{}, const FrameRoom *room = nullptr) {
     cudaError_t e = cudaSuccess;
     const bool acct = c->acct && ((c->acct_progs >> prog) & 1);
     const bool idle = c->idle && ((c->idle_progs >> prog) & 1);
@@ -1147,7 +1202,18 @@ static int dispatch(bng_ctx *c, int prog, const DevBatch &b, const LiSrc &src = 
     case P_NAT_EG: e = run_nat_egress(c->L, c->dev, b); break;
     case P_NAT_IN: e = run_nat_ingress(c->L, c->dev, b, c->nat_icmp); break;
     case P_NAT_HAIRPIN: e = run_nat_hairpin_xdp(c->L, c->dev, b); break;
-    case P_DHCP: e = run_dhcp_fastpath(c->L, c->dev, b); break;
+    case P_DHCP: {
+        // DHCPv6 needs the switch, a configured server and a binding: otherwise "on" launches what "off" does
+        Dhcp6Args d6{};
+        const bool v6 = c->dhcp6 && c->d6_live && c->d6cfg_host[6];
+        if (v6) {
+            d6.bind = c->d6b, d6.cfg = c->d6cfg, d6.stats = c->dev.stats + ST_DHCP6;
+            d6.room_stride = room ? room->room_stride : (b.off16 ? 0u : b.stride);
+            d6.need = room ? room->need : nullptr;
+        }
+        e = run_dhcp_fastpath(c->L, c->dev, b, v6 ? &d6 : nullptr);
+        break;
+    }
     case P_PIPE_UP: e = run_pipeline_up(c->L, c->dev, b, qv6, as6); break;
     case P_PIPE_TC: e = run_pipeline_tc(c->L, c->dev, b, qv6, as6); break;
     default: return -EINVAL;
@@ -1260,7 +1326,9 @@ static int run_host_zero_copy(bng_ctx *c, int prog, bng_batch *bb, u8 *arena_dev
         b.arena_len = (u64)cn * hb;
         // interception copies the bytes past the compact copy straight from the host arena
         const LiSrc src{chunk_arena, bb->off16 ? c->zc_off[buf] : nullptr, contiguous ? nullptr : c->zc_len0[buf], bb->stride};
-        int r = dispatch(c, prog, b, src);
+        // a DHCPv6 reply may outgrow its request: bounded by the host frame's storage, written back up to its length
+        const FrameRoom room{bb->off16 ? 0u : bb->stride, contiguous ? nullptr : c->zc_len0[buf]};
+        int r = dispatch(c, prog, b, src, &room);
         if (r) return r;
         CU(c, cudaEventRecord(c->ev_comp[buf], sc));
         mark(sc);
@@ -1409,6 +1477,7 @@ int bng_map_update_staged(bng_ctx *c, int map, const void *key, const void *valu
     MapReg *m = get_map(c, map);
     if (!m || !key || !value) return -EINVAL;
     if (m->kind != KIND_HASH) return bng_map_update(c, map, key, value, BNG_ANY); // arrays / tries: nothing to batch
+    if (m->tbl == &c->d6b && d6_bad_binding((const u8 *)key, (const u8 *)value)) return -EINVAL;
     std::lock_guard<std::mutex> g(c->mu);
     bng_ctx::Staged &q = c->staged[map];
     q.keys.insert(q.keys.end(), (const u8 *)key, (const u8 *)key + m->key_size);
@@ -1477,15 +1546,15 @@ int bng_sync_reduce(bng_ctx *c, uint64_t *totals_out) {
     cudaSetDevice(c->device);
     int fr = flush_staged_locked(c, -1);
     if (!c->stats_global) {
-        CU(c, cudaMalloc((void **)&c->stats_global, ST_COUNT * 8));
+        CU(c, cudaMalloc((void **)&c->stats_global, ST_ALL * 8));
         c->allocs.push_back(c->stats_global);
     }
     if (c->comm) {
         NcclApi *a = nccl_api();
-        ncclResult_t r = a->AllReduce(c->dev.stats, c->stats_global, ST_COUNT, ncclUint64, ncclSum, c->comm, c->L.stream);
+        ncclResult_t r = a->AllReduce(c->dev.stats, c->stats_global, ST_ALL, ncclUint64, ncclSum, c->comm, c->L.stream);
         if (r != ncclSuccess) return fail(c, -EIO, "ncclAllReduce: %s", a->GetErrorString ? a->GetErrorString(r) : "error");
     } else {
-        CU(c, cudaMemcpyAsync(c->stats_global, c->dev.stats, ST_COUNT * 8, cudaMemcpyDeviceToDevice, c->L.stream));
+        CU(c, cudaMemcpyAsync(c->stats_global, c->dev.stats, ST_ALL * 8, cudaMemcpyDeviceToDevice, c->L.stream));
     }
     if (totals_out) CU(c, cudaMemcpyAsync(totals_out, c->stats_global, ST_COUNT * 8, cudaMemcpyDeviceToHost, c->L.stream));
     CU(c, cudaStreamSynchronize(c->L.stream));
@@ -3362,11 +3431,18 @@ int bng_sub_import(bng_ctx *c, const void *buf, uint64_t len) {
 int bng_stats_device_ptr(bng_ctx *c, void **dptr, uint32_t *n_u64) {
     if (!c || !dptr) return -EINVAL;
     *dptr = c->dev.stats;
-    if (n_u64) *n_u64 = ST_COUNT;
+    if (n_u64) *n_u64 = ST_COUNT; // dhcpv6_stats follow them in the same buffer (include/bng_b200.h)
     return 0;
 }
 
 uint64_t bng_launch_count(bng_ctx *c) { return c ? c->L.launches : 0; }
+
+int bng_dhcpv6_enable(bng_ctx *c, int on) {
+    if (!c) return -EINVAL;
+    std::lock_guard<std::mutex> g(c->mu);
+    c->dhcp6 = on != 0;
+    return 0;
+}
 
 int bng_qos_ipv6_enable(bng_ctx *c, int on) {
     if (!c) return -EINVAL;

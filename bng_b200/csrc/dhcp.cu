@@ -273,6 +273,241 @@ __device__ __forceinline__ int dhcp_one(const DevCtx &c, BlockStats &bs, u8 *p, 
     return XDP_TX_;
 }
 
+// ---- DHCPv6 (include/bng_b200.h, bng_dhcpv6_enable): a bound client's Solicit / Request / Renew / Rebind answered
+// from dhcpv6_bindings with what pkg/dhcpv6's buildAdvertise / buildReply would send ----
+enum { D6_TOTAL, D6_SOLICIT, D6_REQUEST, D6_RENEW, D6_REBIND, D6_ADVERTISE, D6_REPLY, D6_MISS, D6_EXPIRED, D6_UNSUP, D6_NOROOM, D6_MALFORMED };
+
+__device__ __forceinline__ u32 be16(const u8 *p, u32 o) { return ((u32)p[o] << 8) | p[o + 1]; }
+__device__ __forceinline__ void put16(u8 *p, u32 &o, u32 v) {
+    p[o] = (u8)(v >> 8);
+    p[o + 1] = (u8)v;
+    o += 2;
+}
+__device__ __forceinline__ void put32(u8 *p, u32 &o, u32 v) {
+    put16(p, o, v >> 16);
+    put16(p, o, v);
+}
+__device__ __forceinline__ void put_bytes(u8 *p, u32 &o, const u8 *s, u32 n) {
+    for (u32 k = 0; k < n; k++) p[o + k] = s[k];
+    o += n;
+}
+
+// The L3 offset of a DHCPv6 candidate, 0 for any other frame: tags as dhcp_one parses them, ethertype 0x86DD, the IPv6
+// and UDP headers present, version 6, next header 17, destination port 547, destination ff02::1:2 or server_ip.
+__device__ __forceinline__ u32 dhcpv6_candidate(const u8 *p, u32 dlen, const u8 *cfg) {
+    if (dlen < 14) return 0;
+    u32 proto = rd16(p, 12), l3 = 14;
+    if (proto == 0x0081u || proto == 0xA888u) {
+        if (dlen < 18) return 0;
+        proto = rd16(p, 16);
+        l3 = 18;
+        if (proto == 0x0081u) {
+            if (dlen < 22) return 0;
+            proto = rd16(p, 20);
+            l3 = 22;
+        }
+    }
+    if (proto != 0xDD86u || l3 + 48 > dlen) return 0;
+    if ((p[l3] >> 4) != 6 || p[l3 + 6] != 17 || rd16(p, l3 + 42) != 0x2302u) return 0; // bpf_htons(547)
+    const u32 d0 = rd32(p, l3 + 24), d1 = rd32(p, l3 + 28), d2 = rd32(p, l3 + 32), d3 = rd32(p, l3 + 36);
+    const bool all_servers = d0 == 0x000002FFu && d1 == 0 && d2 == 0 && d3 == 0x02000100u; // ff02::1:2
+    const u32 *sip = (const u32 *)(cfg + 8);
+    const bool ours = d0 == sip[0] && d1 == sip[1] && d2 == sip[2] && d3 == sip[3];
+    return all_servers || ours ? l3 : 0;
+}
+
+// One candidate at L3 offset l3.  The request is parsed completely (the Client ID into the lookup key's registers,
+// the IAs' IAIDs and positions) before the first byte of the reply is written over it.
+__device__ __forceinline__ int dhcpv6_one(const Dhcp6Args &a, u32 *st, u8 *p, u32 &len, const u32 dlen, u64 now, u32 l3) {
+    const u8 *cfg = a.cfg; // server_mac@0 duid_len@6 dns_count@7 server_ip@8 duid@24 dns@56
+    const u32 udp = l3 + 40, m = udp + 8;
+    atomicAdd(&st[D6_TOTAL], 1u);
+    const u32 sduid = cfg[6];
+    if (sduid == 0 || len > 448) {
+        atomicAdd(&st[D6_UNSUP], 1u);
+        return XDP_PASS_;
+    }
+    const u32 ulen = be16(p, udp + 4);
+    if (ulen < 12 || udp + ulen > dlen) {
+        atomicAdd(&st[D6_MALFORMED], 1u);
+        return XDP_PASS_;
+    }
+    const u32 type = p[m];
+    if (type != 1 && type != 3 && type != 5 && type != 6) {
+        atomicAdd(&st[D6_UNSUP], 1u);
+        return XDP_PASS_;
+    }
+    atomicAdd(&st[type == 1 ? D6_SOLICIT : type == 3 ? D6_REQUEST : type == 5 ? D6_RENEW : D6_REBIND], 1u);
+
+    // ---- the option walk ----
+    const u32 end = udp + ulen;
+    u32 cid = 0, cid_len = 0, n_cid = 0, sid = 0, sid_len = 0, n_sid = 0, na = 0, na_len = 0, n_na = 0, pd = 0,
+        pd_len = 0, n_pd = 0, nopt = 0;
+    bool ta = false, rapid = false;
+    for (u32 o = m + 4; o < end;) {
+        if (o + 4 > end || ++nopt > 32) {
+            atomicAdd(&st[D6_MALFORMED], 1u);
+            return XDP_PASS_;
+        }
+        const u32 code = be16(p, o), olen = be16(p, o + 2);
+        if (o + 4 + olen > end) {
+            atomicAdd(&st[D6_MALFORMED], 1u);
+            return XDP_PASS_;
+        }
+        if (code == 1) cid = o + 4, cid_len = olen, n_cid++;
+        else if (code == 2) sid = o + 4, sid_len = olen, n_sid++;
+        else if (code == 3) na = o + 4, na_len = olen, n_na++;
+        else if (code == 4) ta = true;
+        else if (code == 25) pd = o + 4, pd_len = olen, n_pd++;
+        else if (code == 14) rapid = true;
+        o += 4 + olen;
+    }
+    bool unsup = n_cid != 1 || cid_len < 1 || cid_len > 31 || ta || n_na > 1 || n_pd > 1 || (n_na && na_len < 12) ||
+                 (n_pd && pd_len < 12) || (n_na | n_pd) == 0;
+    if (type == 1 || type == 6) unsup = unsup || n_sid != 0;
+    else if (!unsup) {
+        unsup = n_sid != 1 || sid_len != sduid;
+        for (u32 k = 0; k < sid_len && !unsup; k++) unsup = p[sid + k] != cfg[24 + k];
+    }
+    if (unsup) {
+        atomicAdd(&st[D6_UNSUP], 1u);
+        return XDP_PASS_;
+    }
+
+    // ---- the binding ----
+    u64 kw[4] = {cid_len, 0, 0, 0}; // struct bng_dhcpv6_client_key {duid_len; duid[31]}
+#pragma unroll
+    for (int k = 0; k < 31; k++) {
+        const u64 v = (u32)k < cid_len ? p[cid + k] : 0;
+        kw[(k + 1) >> 3] |= v << (((k + 1) & 7) * 8);
+    }
+    const u8 *s = tbl_find_conv<4>(a.bind, kw);
+    const u8 *v = s ? s + a.bind.voff : nullptr; // mac@0 flags@6 pd_len@7 iaid_na@8 iaid_pd@12 preferred@16 valid@20
+                                                 // expires_s@24 addr@32 prefix@48
+    if (!v || *(const u16 *)v != rd16(p, 6) || *(const u16 *)(v + 2) != rd16(p, 8) || *(const u16 *)(v + 4) != rd16(p, 10)) {
+        atomicAdd(&st[D6_MISS], 1u);
+        return XDP_PASS_;
+    }
+    if (now / 1000000000ull > *(const u64 *)(v + 24)) {
+        atomicAdd(&st[D6_EXPIRED], 1u);
+        return XDP_PASS_;
+    }
+    const u32 flags = v[6];
+    const u32 iaid_na = n_na ? (be16(p, na) << 16 | be16(p, na + 2)) : 0, iaid_pd = n_pd ? (be16(p, pd) << 16 | be16(p, pd + 2)) : 0;
+    if ((n_na && (!(flags & 1) || iaid_na != *(const u32 *)(v + 8))) || (n_pd && (!(flags & 2) || iaid_pd != *(const u32 *)(v + 12)))) {
+        atomicAdd(&st[D6_UNSUP], 1u);
+        return XDP_PASS_;
+    }
+    const bool adv = type == 1 && !rapid, rc_reply = type == 1 && rapid;
+    const u32 dns = cfg[7];
+    const u32 total = m + 4 + (4 + cid_len) + (4 + sduid) + (adv ? 5u : 13u) + (n_na ? 44u : 0u) + (n_pd ? 45u : 0u) +
+                      (dns ? 4u + 16u * dns : 0u) + (rc_reply ? 4u : 0u);
+    const u32 room = a.room_stride ? a.room_stride : (len + 15u) & ~15u;
+    if (total > room) {
+        atomicAdd(&st[D6_NOROOM], 1u);
+        return XDP_PASS_;
+    }
+
+    // ---- the reply, over the request ----
+    p[m] = adv ? 2 : 7; // the transaction id stays
+    u32 o = m + 4;
+    put16(p, o, 1);
+    put16(p, o, cid_len);
+#pragma unroll
+    for (int k = 0; k < 31; k++)
+        if ((u32)k < cid_len) p[o + k] = (u8)(kw[(k + 1) >> 3] >> (((k + 1) & 7) * 8));
+    o += cid_len;
+    put16(p, o, 2);
+    put16(p, o, sduid);
+    put_bytes(p, o, cfg + 24, sduid);
+    if (adv) {
+        put16(p, o, 7);
+        put16(p, o, 1);
+        p[o++] = 255;
+    }
+    const u32 pref = *(const u32 *)(v + 16), valid = *(const u32 *)(v + 20);
+    const u32 t1 = pref / 2u, t2 = (pref * 4u) / 5u;
+    if (n_na) {
+        put16(p, o, 3);
+        put16(p, o, 40);
+        put32(p, o, iaid_na);
+        put32(p, o, t1);
+        put32(p, o, t2);
+        put16(p, o, 5);
+        put16(p, o, 24);
+        put_bytes(p, o, v + 32, 16);
+        put32(p, o, pref);
+        put32(p, o, valid);
+    }
+    if (n_pd) {
+        put16(p, o, 25);
+        put16(p, o, 41);
+        put32(p, o, iaid_pd);
+        put32(p, o, t1);
+        put32(p, o, t2);
+        put16(p, o, 26);
+        put16(p, o, 25);
+        put32(p, o, pref);
+        put32(p, o, valid);
+        p[o++] = v[7];
+        put_bytes(p, o, v + 48, 16);
+    }
+    if (dns) {
+        put16(p, o, 23);
+        put16(p, o, 16 * dns);
+        put_bytes(p, o, cfg + 56, 16 * dns);
+    }
+    if (!adv) {
+        put16(p, o, 13);
+        put16(p, o, 9);
+        put16(p, o, 0);
+        put32(p, o, 0x53756363u); // "Success"
+        put16(p, o, 0x6573u);
+        p[o++] = 's';
+    }
+    if (rc_reply) {
+        put16(p, o, 14);
+        put16(p, o, 0);
+    }
+    for (u32 k = o; k & 15; k++) p[k] = 0; // to the reply's next 16-byte boundary (a frame starts on one): no stale byte
+    const u32 ul = o - udp;
+    // Ethernet: back to the client, from the server; the tags stay
+    wr16(p, 0, rd16(p, 6));
+    wr16(p, 2, rd16(p, 8));
+    wr16(p, 4, rd16(p, 10));
+    wr16(p, 6, *(const u16 *)(cfg + 0));
+    wr16(p, 8, *(const u16 *)(cfg + 2));
+    wr16(p, 10, *(const u16 *)(cfg + 4));
+    // IPv6
+    wr32(p, l3, 0x00000060u);
+    wr16(p, l3 + 4, bswap16((u16)ul));
+    p[l3 + 6] = 17;
+    p[l3 + 7] = 64;
+    const u32 *sip = (const u32 *)(cfg + 8);
+#pragma unroll
+    for (int k = 0; k < 4; k++) {
+        wr32(p, l3 + 24 + 4 * k, rd32(p, l3 + 8 + 4 * k));
+        wr32(p, l3 + 8 + 4 * k, sip[k]);
+    }
+    // UDP, with the checksum over the pseudo-header (words read in memory order: the sum is byte-order neutral)
+    wr16(p, udp + 0, 0x2302u); // bpf_htons(547)
+    wr16(p, udp + 2, 0x2202u); // bpf_htons(546)
+    wr16(p, udp + 4, bswap16((u16)ul));
+    wr16(p, udp + 6, 0);
+    u32 sum = bswap16((u16)ul) + 0x1100u; // upper-layer length, next header 17
+#pragma unroll
+    for (int k = 0; k < 16; k++) sum += rd16(p, l3 + 8 + 2 * k);
+    for (u32 k = 0; k + 1 < ul; k += 2) sum += rd16(p, udp + k);
+    if (ul & 1) sum += p[udp + ul - 1];
+    sum = (sum & 0xFFFF) + (sum >> 16);
+    sum = (sum & 0xFFFF) + (sum >> 16);
+    u16 ck = (u16)~sum;
+    wr16(p, udp + 6, ck ? ck : 0xFFFFu);
+    len = o;
+    atomicAdd(&st[adv ? D6_ADVERTISE : D6_REPLY], 1u);
+    return XDP_TX_;
+}
+
 // Tile kernel (one mbarrier per block rather than per-thread barriers without any block-wide synchronisation): a
 // request is up to ~350 bytes that the program reads sparsely and rewrites almost
 // entirely (L2 headers, BOOTP fixed part, 192 zeroed bytes, options), so frames are staged through
@@ -289,10 +524,17 @@ __device__ __forceinline__ int dhcp_one(const DevCtx &c, BlockStats &bs, u8 *p, 
 // contiguous run, so the whole tile moves with ONE bulk copy each way instead of one per frame — the per-frame
 // version issues 2 x 2^22 TMA operations per batch, a few dozen cycles apart on every SM, and that, not HBM,
 // bounds it.  Every other arena (an offset table, or slots that do not fit a staging slot) moves frame by frame.
-__global__ void __launch_bounds__(DH_TILE) k_dhcp_fastpath(const __grid_constant__ DevCtx c, const __grid_constant__ DevBatch b) {
+// V6: DHCPv6 candidates among the frames dhcp_one passed as not IPv4 are answered by dhcpv6_one (bng_dhcpv6_enable)
+template <bool V6>
+__global__ void __launch_bounds__(DH_TILE) k_dhcp_fastpath(const __grid_constant__ DevCtx c, const __grid_constant__ DevBatch b,
+                                                           const __grid_constant__ Dhcp6Args a) {
     extern __shared__ __align__(128) u8 stage[]; // DH_TILE * DH_SLOT
     __shared__ BlockStats bs;
     __shared__ u64 bar, bar1;
+    __shared__ u32 s6[V6 ? ST_DHCP6_N : 1];
+    if constexpr (V6) {
+        if (threadIdx.x < ST_DHCP6_N) s6[threadIdx.x] = 0;
+    }
     bstats_init(bs);
     const u32 bar_a = (u32)__cvta_generic_to_shared(&bar), bar1_a = (u32)__cvta_generic_to_shared(&bar1);
     if (threadIdx.x == 0) {
@@ -352,14 +594,30 @@ __global__ void __launch_bounds__(DH_TILE) k_dhcp_fastpath(const __grid_constant
                 if (rd16(mine, 16) == 0x0081u) l3 = 22;
             }
             direct = l3 + (u32)(mine[l3] & 0x0f) * 4 + 8 + 240 + 64 > DH_SLOT;
+            if constexpr (V6) {
+                if (rd16(mine, l3 - 2) == 0xDD86u) direct = true; // an IPv6 frame is decided by its ethertype
+            }
         }
+        u32 grown = 0; // V6: the bytes of an answered frame, rounded up to 16
         if (act) {
             const u32 l0 = len;
-            int v = dhcp_one(c, bs, direct ? g : mine, len, frame_dlen(b, l0), frame_now(b, i));
+            u8 *fp = direct ? g : mine;
+            const u32 dl = frame_dlen(b, l0);
+            int v = dhcp_one(c, bs, fp, len, dl, frame_now(b, i));
+            if constexpr (V6) {
+                if (v == XDP_PASS_) {
+                    const u32 l3 = dhcpv6_candidate(fp, dl, a.cfg);
+                    if (l3 && (v = dhcpv6_one(a, s6, fp, len, dl, frame_now(b, i), l3)) == XDP_TX_) grown = (len + 15u) & ~15u;
+                }
+            }
             b.verdict[i] = (u8)v;
             if (len != l0) b.len[i] = len;
         }
         if (direct) nbytes = 0;
+        if constexpr (V6) { // a reply can be longer than its request: store it back whole
+            if (!direct && grown > nbytes) nbytes = grown;
+            if (grown && a.need && grown > a.need[i]) a.need[i] = grown;
+        }
         // ---- stage out (every staged frame: a passed frame may have been rewritten, :769) ----
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
         if (tile_mode) {
@@ -380,23 +638,31 @@ __global__ void __launch_bounds__(DH_TILE) k_dhcp_fastpath(const __grid_constant
     }
     if (tile_mode && threadIdx.x == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
     bstats_flush(bs, c.stats);
+    if constexpr (V6) {
+        if (threadIdx.x < ST_DHCP6_N && s6[threadIdx.x]) atomicAdd(&a.stats[threadIdx.x], (u64)s6[threadIdx.x]);
+    }
 }
 
 // (A double-buffered variant — two staging slots per thread, the load of tile i+1 issued before the program runs on
 // tile i — was tried and dropped: it was slower.)
 
-cudaError_t run_dhcp_fastpath(Launcher &L, const DevCtx &c, const DevBatch &b) {
+cudaError_t run_dhcp_fastpath(Launcher &L, const DevCtx &c, const DevBatch &b, const Dhcp6Args *d6) {
     const int smem = DH_TILE * DH_SLOT;
-    if (!L.dhcp_smem_set) { // function attributes are per device: set on the device this context runs on
-        cudaError_t e = cudaFuncSetAttribute(k_dhcp_fastpath, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    int &set = d6 ? L.dhcp6_smem_set : L.dhcp_smem_set;
+    if (!set) { // function attributes are per device: set on the device this context runs on
+        cudaError_t e = cudaFuncSetAttribute(d6 ? k_dhcp_fastpath<true> : k_dhcp_fastpath<false>,
+                                             cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
         if (e != cudaSuccess) return e;
-        L.dhcp_smem_set = 1;
+        set = 1;
     }
     long want = ((long)b.n + DH_TILE - 1) / DH_TILE;
     long cap = (long)L.num_sms * 4; // 4 x 50 KB of staging per SM (of the 228 KB an H100 SM has)
     int grid = (int)(want < cap ? (want < 1 ? 1 : want) : cap);
-    prof_begin(L, "k_dhcp_fastpath");
-    k_dhcp_fastpath<<<grid, DH_TILE, smem, L.stream>>>(c, b);
+    prof_begin(L, d6 ? "k_dhcp_fastpath<v6>" : "k_dhcp_fastpath");
+    if (d6)
+        k_dhcp_fastpath<true><<<grid, DH_TILE, smem, L.stream>>>(c, b, *d6);
+    else
+        k_dhcp_fastpath<false><<<grid, DH_TILE, smem, L.stream>>>(c, b, Dhcp6Args{});
     prof_end(L);
     L.launches++;
     return cudaGetLastError();

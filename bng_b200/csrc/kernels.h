@@ -28,6 +28,7 @@ struct Launcher {
     // per-context (= per-device) launch configuration, filled on first use: nothing here may be process-wide,
     // one process can hold contexts on several GPUs
     int dhcp_smem_set;  // cudaFuncAttributeMaxDynamicSharedMemorySize applied on this context's device
+    int dhcp6_smem_set; // ... and to k_dhcp_fastpath<v6>
     int resolve_bps[16]; // resident blocks per SM of the k_resolve instantiations, by <NAT, QOS, EGRESS, TC> bits
     int prof;
     ProfPending pend[32];
@@ -56,7 +57,23 @@ cudaError_t run_nat_ingress(Launcher &L, const DevCtx &c, const DevBatch &b, boo
 cudaError_t run_nat_hairpin_xdp(Launcher &L, const DevCtx &c, const DevBatch &b);
 cudaError_t run_pipeline_up(Launcher &L, const DevCtx &c, const DevBatch &b, const Tbl *v6, const Tbl *as6);
 cudaError_t run_pipeline_tc(Launcher &L, const DevCtx &c, const DevBatch &b, const Tbl *v6, const Tbl *as6);
-cudaError_t run_dhcp_fastpath(Launcher &L, const DevCtx &c, const DevBatch &b);
+// The DHCPv6 fast path (include/bng_b200.h, bng_dhcpv6_enable): its tables and where its counters go.  The counters
+// follow the ST_COUNT of the packed statistics vector, which then holds ST_ALL; the kernels' per-block accumulators
+// (BlockStats) keep ST_COUNT.
+#define ST_DHCP6 ST_COUNT
+#define ST_DHCP6_N 12
+#define ST_ALL (ST_COUNT + ST_DHCP6_N)
+#define DHCP6_CFG_BYTES 96
+struct Dhcp6Args {
+    Tbl bind;         // dhcpv6_bindings: 32-byte key (4 words), 64-byte value at 32
+    const u8 *cfg;    // dhcpv6_server_config[0]
+    u64 *stats;       // ST_DHCP6_N counters
+    u32 room_stride;  // a frame's storage: room_stride bytes, or 0: its len rounded up to 16 (an offset table)
+    u32 *need;        // pinned zero-copy feed: bytes the scatter writes back, raised to cover a grown reply; else nullptr
+};
+// d6: the DHCPv6 tables when the fast path answers DHCPv6 (bng_dhcpv6_enable, a configured server and live bindings),
+// else nullptr
+cudaError_t run_dhcp_fastpath(Launcher &L, const DevCtx &c, const DevBatch &b, const Dhcp6Args *d6);
 
 // header gather / scatter between a pinned host arena and a compact device copy (hostio.cu); icmp_errors (TC only):
 // also bytes 64-79 of an ICMP error frame, for nat44_ingress with bng_nat_icmp_errors_enable

@@ -568,12 +568,15 @@ class Loader {
         serverConfigMap_ = be_->Map("server_config");
         circuitIDMap_ = be_->Map("circuit_id_map");
         circuitIDSubscribers_ = be_->Map("circuit_id_subscribers");
+        dhcpv6Bindings_ = be_->Map("dhcpv6_bindings");
+        dhcpv6ServerConfig_ = be_->Map("dhcpv6_server_config");
         loaded_ = true;
         return ResetStats();
     }
     Error Close() { // idempotent, loader_test.go:989-1003
         loaded_ = false;
         subscriberPools_ = vlanSubscriberPools_ = ipPools_ = statsMap_ = serverConfigMap_ = circuitIDMap_ = circuitIDSubscribers_ = -1;
+        dhcpv6Bindings_ = dhcpv6ServerConfig_ = -1;
         be_.reset();
         return Nil();
     }
@@ -588,6 +591,42 @@ class Loader {
         return MapErr("delete", bng_map_delete(be_->ctx, subscriberPools_, &mac));
     }
     Result<PoolAssignment> GetSubscriber(uint64_t mac) { return lookup<PoolAssignment>(subscriberPools_, "subscriber_pools map not loaded", &mac); }
+
+    // The DHCPv6 fast-path cache (include/bng_b200.h, "dhcpv6_bindings"): what pkg/dhcpv6's server would put when its
+    // buildReply binds a client, so that the client's next Solicit / Request / Renew / Rebind is answered on the GPU.
+    // The key is the Client Identifier option's data (1-31 bytes).  AddDHCPv6Binding is staged (visible from the next
+    // batch) and returns -EINVAL for a binding the fast path could not use.
+    static bng_dhcpv6_client_key DHCPv6Key(const uint8_t *duid, size_t len) {
+        bng_dhcpv6_client_key k{};
+        k.duid_len = (uint8_t)(len > 31 ? 0 : len); // a longer DUID is refused by the update
+        if (len <= 31) memcpy(k.duid, duid, len);
+        return k;
+    }
+    Error SetDHCPv6ServerConfig(const bng_dhcpv6_server_config &c) {
+        if (dhcpv6ServerConfig_ < 0) return Error("dhcpv6_server_config map not loaded");
+        uint32_t key = 0;
+        return MapErr("update", bng_map_update(be_->ctx, dhcpv6ServerConfig_, &key, &c, BNG_ANY));
+    }
+    Error AddDHCPv6Binding(const uint8_t *duid, size_t len, const bng_dhcpv6_binding &b) {
+        if (dhcpv6Bindings_ < 0) return Error("dhcpv6_bindings map not loaded");
+        if (len == 0 || len > 31) return MapErr("update", -EINVAL);
+        bng_dhcpv6_client_key k = DHCPv6Key(duid, len);
+        return MapErr("update", bng_map_update_staged(be_->ctx, dhcpv6Bindings_, &k, &b));
+    }
+    Error RemoveDHCPv6Binding(const uint8_t *duid, size_t len) {
+        if (dhcpv6Bindings_ < 0) return Error("dhcpv6_bindings map not loaded");
+        bng_dhcpv6_client_key k = DHCPv6Key(duid, len);
+        return MapErr("delete", bng_map_delete(be_->ctx, dhcpv6Bindings_, &k));
+    }
+    Result<bng_dhcpv6_binding> GetDHCPv6Binding(const uint8_t *duid, size_t len) {
+        bng_dhcpv6_client_key k = DHCPv6Key(duid, len);
+        return lookup<bng_dhcpv6_binding>(dhcpv6Bindings_, "dhcpv6_bindings map not loaded", &k);
+    }
+    // bng_dhcpv6_enable: context state that no snapshot or delta carries, so a standby's Loader calls it too
+    Error EnableDHCPv6FastPath(bool on) {
+        if (!be_ || !be_->ctx) return Error("dataplane not loaded");
+        return MapErr("bng_dhcpv6_enable", bng_dhcpv6_enable(be_->ctx, on ? 1 : 0));
+    }
 
     Error AddVLANSubscriber(uint16_t sTag, uint16_t cTag, const PoolAssignment &a) {
         if (vlanSubscriberPools_ < 0) return Error("vlan_subscriber_pools map not loaded");
@@ -720,7 +759,7 @@ class Loader {
     std::shared_ptr<Backend> be_;
     bool loaded_ = false;
     int subscriberPools_ = -1, vlanSubscriberPools_ = -1, ipPools_ = -1, statsMap_ = -1, serverConfigMap_ = -1,
-        circuitIDMap_ = -1, circuitIDSubscribers_ = -1;
+        circuitIDMap_ = -1, circuitIDSubscribers_ = -1, dhcpv6Bindings_ = -1, dhcpv6ServerConfig_ = -1;
 };
 
 } // namespace ebpf

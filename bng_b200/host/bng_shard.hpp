@@ -36,8 +36,10 @@
 namespace bng {
 namespace shard {
 
-// ByValueIP: the value is the subscriber's IPv4 address (subscriber_ipv6); the entry lives on that address's shard
-enum class Route { ByMAC, ByPrivateIP, BySessionKey, ByEIMKey, ByReverseKey, ByValueIP, Replicated };
+// ByValueIP: the value is the subscriber's IPv4 address (subscriber_ipv6); the entry lives on that address's shard.
+// ByValueMAC: the value starts with the client's MAC (dhcpv6_bindings); the entry lives on that MAC's shard, where the
+// client's upstream frames are steered.
+enum class Route { ByMAC, ByPrivateIP, BySessionKey, ByEIMKey, ByReverseKey, ByValueIP, ByValueMAC, Replicated };
 
 inline Route RouteOf(const std::string &map) {
     if (map == "subscriber_bindings" || map == "subscriber_pools") return Route::ByMAC;
@@ -46,6 +48,7 @@ inline Route RouteOf(const std::string &map) {
     if (map == "eim_table") return Route::ByEIMKey;        // struct eim_key: internal_ip
     if (map == "nat_reverse") return Route::ByReverseKey;  // struct nat_key: dst_ip/dst_port = public address, port
     if (map == "subscriber_ipv6") return Route::ByValueIP; // value: the owner's IPv4 address
+    if (map == "dhcpv6_bindings") return Route::ByValueMAC; // value: struct bng_dhcpv6_binding, mac first
     return Route::Replicated;
 }
 
@@ -283,6 +286,12 @@ class Router {
             memcpy(&mac, k, 8);
             return (int)dir_->ShardOfMAC(mac);
         }
+        case Route::ByValueMAC: { // with the value, the shard of its MAC; without it, the shard that holds the key
+            if (value) return (int)dir_->ShardOfMAC(Directory::MacKey((const uint8_t *)value));
+            std::lock_guard<std::mutex> g(home_mu_);
+            auto it = home_.find(std::string((const char *)key, 32));
+            return it == home_.end() ? -ENOENT : (int)it->second;
+        }
         case Route::ByPrivateIP:
         case Route::BySessionKey:
         case Route::ByEIMKey: {
@@ -312,6 +321,17 @@ class Router {
                 if (int r = bng_map_delete(c, id, key); r && r != -ENOENT) return r;
             }
         }
+        if (RouteOf(map) == Route::ByValueMAC) { // a client re-bound under another MAC leaves its old shard
+            const int was = Owner(map, key);
+            if (was >= 0 && was != o) {
+                bng_ctx *c = shards_[(size_t)was]->ctx;
+                const int id = bng_map_id(c, map);
+                if (id < 0) return id;
+                if (int r = bng_map_delete(c, id, key); r && r != -ENOENT) return r;
+                std::lock_guard<std::mutex> g(home_mu_);
+                home_.erase(std::string((const char *)key, 32));
+            }
+        }
         int rc = 0;
         for (size_t i = 0; i < shards_.size(); i++) {
             if (o >= 0 && (size_t)o != i) continue;
@@ -320,6 +340,10 @@ class Router {
             if (id < 0) return id;
             int r = staged && flags == BNG_ANY ? bng_map_update_staged(c, id, key, value) : bng_map_update(c, id, key, value, flags);
             if (r && !rc) rc = r;
+        }
+        if (RouteOf(map) == Route::ByValueMAC && !rc) {
+            std::lock_guard<std::mutex> g(home_mu_);
+            home_[std::string((const char *)key, 32)] = (size_t)o;
         }
         if (v6 && !rc) {
             uint32_t plen, a;
@@ -363,6 +387,10 @@ class Router {
             if (id < 0) return id;
             int r = bng_map_delete(c, id, key);
             if (r && !rc) rc = r;
+        }
+        if (RouteOf(map) == Route::ByValueMAC && (!rc || rc == -ENOENT)) {
+            std::lock_guard<std::mutex> g(home_mu_);
+            home_.erase(std::string((const char *)key, 32));
         }
         return rc;
     }
@@ -444,6 +472,14 @@ class Router {
     // Antispoof by delegated prefix (bng_antispoof_ipv6_prefixes_enable) on every shard.  The rule needs a
     // subscriber's binding and its prefixes on one shard: the binding is routed ByMAC and subscriber_ipv6 ByValueIP,
     // the shard of the IPv4 address and so of its MAC.  Returns 0 or the first shard's error.
+    // The DHCPv6 fast path (bng_dhcpv6_enable) on every shard.  dhcpv6_bindings is routed ByValueMAC and
+    // dhcpv6_server_config replicated, and upstream frames are steered by source MAC (SteerUpstream), so a client's
+    // messages reach the shard that holds its binding.  Returns 0 or the first shard's error.
+    int DHCPv6Enable(bool on) {
+        for (auto &s : shards_)
+            if (int r = bng_dhcpv6_enable(s->ctx, on ? 1 : 0)) return r;
+        return 0;
+    }
     int AntispoofIPv6PrefixesEnable(bool on) {
         for (auto &s : shards_)
             if (int r = bng_antispoof_ipv6_prefixes_enable(s->ctx, on ? 1 : 0)) return r;
@@ -723,6 +759,10 @@ class Router {
   private:
     std::vector<std::shared_ptr<Backend>> shards_;
     std::shared_ptr<Directory> dir_;
+    // dhcpv6_bindings (ByValueMAC): the shard that holds each key, so that delete and lookup find it and a re-bind
+    // under another MAC can leave the old shard
+    mutable std::mutex home_mu_;
+    std::unordered_map<std::string, size_t> home_;
 };
 
 } // namespace shard

@@ -126,6 +126,22 @@ bng_idle = np.dtype([("up_ns", "<u8"), ("down_ns", "<u8"), ("since_ns", "<u8"), 
 bng_ipv6_prefix_key = np.dtype([("prefixlen", "<u4"), ("addr", "u1", 16)])
 assert bng_ipv6_prefix_key.itemsize == 20
 
+# include/bng_b200.h: the DHCPv6 fast path's cache (not reference maps).  dhcpv6_bindings: key (32 B) -> binding (64 B);
+# dhcpv6_server_config: one 96-byte entry; dhcpv6_stats: BNG_DHCPV6_NUM_STATS u64 counters
+DHCPV6_NA, DHCPV6_PD = 1, 2
+bng_dhcpv6_client_key = np.dtype([("duid_len", "u1"), ("duid", "u1", 31)])
+bng_dhcpv6_binding = np.dtype([
+    ("mac", "u1", 6), ("flags", "u1"), ("pd_len", "u1"), ("iaid_na", "<u4"), ("iaid_pd", "<u4"),
+    ("preferred_lft", "<u4"), ("valid_lft", "<u4"), ("expires_s", "<u8"), ("addr", "u1", 16), ("prefix", "u1", 16)])
+bng_dhcpv6_server_config = np.dtype([
+    ("server_mac", "u1", 6), ("duid_len", "u1"), ("dns_count", "u1"), ("server_ip", "u1", 16), ("duid", "u1", 32),
+    ("dns", "u1", (2, 16)), ("_pad", "u1", 8)])
+DHCPV6_STATS = ("total", "solicit", "request", "renew", "rebind", "advertise", "reply", "miss", "expired", "unsupported",
+                "no_room", "malformed")
+dhcpv6_stats = np.dtype([(n, "<u8") for n in DHCPV6_STATS])
+assert bng_dhcpv6_client_key.itemsize == 32 and bng_dhcpv6_binding.itemsize == 64
+assert bng_dhcpv6_server_config.itemsize == 96 and dhcpv6_stats.itemsize == 96
+
 # lawful-intercept record header (include/bng_b200.h: struct bng_li_record, 64 B); the captured bytes follow it
 LI_UPLINK, LI_DOWNLINK = 0, 1
 bng_li_record = np.dtype([
@@ -199,6 +215,9 @@ MAP_DTYPES = {
     "circuit_id_map": ("<u8", "<u8"),
     "circuit_id_subscribers": (circuit_id_key, pool_assignment),
     "subscriber_ipv6": (bng_ipv6_prefix_key, ("u1", 4)),
+    "dhcpv6_bindings": (bng_dhcpv6_client_key, bng_dhcpv6_binding),
+    "dhcpv6_server_config": ("<u4", bng_dhcpv6_server_config),
+    "dhcpv6_stats": ("<u4", dhcpv6_stats),
 }
 
 

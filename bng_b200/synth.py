@@ -280,3 +280,67 @@ def flow_frames(fl: dict, pick: np.ndarray, lens: np.ndarray, gw_mac: int = 0x02
         ck = np.where(zero, 0, base)
     return ipv4_headers(sub_mac_key(sub), np.uint64(gw_mac), sub_ip(sub), fl["dst_ip"][pick], fl["proto"][pick],
                         fl["sport"][pick], fl["dport"][pick], lens, l4_check=ck)
+
+
+# ---------------------------------------------------------------------------
+# DHCPv6 (include/bng_b200.h: the DHCPv6 fast path)
+# ---------------------------------------------------------------------------
+DHCPV6_ALL_SERVERS = bytes.fromhex("ff020000000000000000000000010002")
+
+
+def dhcpv6_option(code: int, data: bytes = b"") -> bytes:
+    return code.to_bytes(2, "big") + len(data).to_bytes(2, "big") + bytes(data)
+
+
+def dhcpv6_ia(code: int, iaid: int, t1: int = 0, t2: int = 0, sub: bytes = b"") -> bytes:
+    """An IA_NA (3) or IA_PD (25) option as a client sends it: IAID, T1, T2, then any sub-options."""
+    return dhcpv6_option(code, iaid.to_bytes(4, "big") + t1.to_bytes(4, "big") + t2.to_bytes(4, "big") + sub)
+
+
+def udp6_checksum(src: bytes, dst: bytes, udp: bytes) -> int:
+    """The UDP checksum over the IPv6 pseudo-header (RFC 8200 §8.1) of a UDP datagram whose checksum field is 0."""
+    data = src + dst + len(udp).to_bytes(4, "big") + b"\x00\x00\x00\x11" + udp
+    if len(data) & 1:
+        data += b"\x00"
+    s = int(np.frombuffer(data, ">u2").astype(np.uint64).sum())
+    while s >> 16:
+        s = (s & 0xFFFF) + (s >> 16)
+    c = ~s & 0xFFFF
+    return c or 0xFFFF
+
+
+def dhcpv6_frame(src_mac: bytes, msg_type: int, xid: int, options: bytes, dst_mac: bytes = b"\x33\x33\x00\x01\x00\x02",
+                 src_ip: bytes | None = None, dst_ip: bytes = DHCPV6_ALL_SERVERS, tags=(), sport: int = 546,
+                 dport: int = 547, next_header: int = 17, hop_limit: int = 1) -> bytes:
+    """An Ethernet frame carrying one DHCPv6 client message: type, 24-bit transaction id, the options as given.
+    tags: (tpid, vid) pairs outermost first.  The source defaults to the link-local EUI-64 address of src_mac."""
+    if src_ip is None:
+        eui = bytes([src_mac[0] ^ 2]) + src_mac[1:3] + b"\xff\xfe" + src_mac[3:6]
+        src_ip = b"\xfe\x80" + bytes(6) + eui
+    msg = bytes([msg_type]) + (int(xid) & 0xFFFFFF).to_bytes(3, "big") + options
+    udp = sport.to_bytes(2, "big") + dport.to_bytes(2, "big") + (8 + len(msg)).to_bytes(2, "big") + b"\x00\x00" + msg
+    ck = udp6_checksum(src_ip, dst_ip, udp)
+    udp = udp[:6] + ck.to_bytes(2, "big") + udp[8:]
+    ip = (b"\x60\x00\x00\x00" + len(udp).to_bytes(2, "big") + bytes([next_header, hop_limit]) + src_ip + dst_ip)
+    l2 = bytes(dst_mac) + bytes(src_mac)
+    for tpid, vid in tags:
+        l2 += tpid.to_bytes(2, "big") + (vid & 0xFFF).to_bytes(2, "big")
+    return l2 + b"\x86\xdd" + ip + udp
+
+
+def dhcpv6_client_key(duid: bytes) -> np.ndarray:
+    k = np.zeros(1, L.bng_dhcpv6_client_key)
+    k["duid_len"] = len(duid)
+    k["duid"][0, :len(duid)] = np.frombuffer(bytes(duid), np.uint8)
+    return k
+
+
+def dhcpv6_duid(i: int, length: int = 14) -> bytes:
+    """A DUID-LLT-shaped client identifier of `length` bytes for client i (distinct per i for length >= 5)."""
+    base = b"\x00\x01\x00\x01" + int(0x2A000000 + i).to_bytes(4, "big") + (0x020000000000 + i).to_bytes(6, "big")
+    base += bytes(32)
+    b = bytearray(base[:length])
+    if length < 10:  # keep short DUIDs distinct
+        v = (i * 2654435761) & ((1 << (8 * length)) - 1)
+        b = bytearray(v.to_bytes(length, "big"))
+    return bytes(b)

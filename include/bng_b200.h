@@ -700,6 +700,90 @@ int bng_qos_ipv6_enable(bng_ctx *ctx, int on);
  * it itself.  Returns 0, or -EINVAL for a NULL ctx. */
 int bng_antispoof_ipv6_prefixes_enable(bng_ctx *ctx, int on);
 
+/* ---- DHCPv6 fast path (not one of the reference's maps or programs) ----
+ * The DHCPv6 server (pkg/dhcpv6) caches each bound client's answer here, and dhcp_fastpath_prog answers a bound
+ * client's Solicit, Request, Renew and Rebind on the GPU with what the server would send.  Three registry maps, carried
+ * by every generic path (update, batch, staged, delete, dump, clear, snapshot, restore, deltas); none is carried by
+ * bng_sub_export, so a moved client's messages pass to the slow path on the destination until it binds again.
+ *   - "dhcpv6_bindings": BPF_MAP_TYPE_HASH, key struct bng_dhcpv6_client_key (32 B), value struct bng_dhcpv6_binding
+ *     (64 B), max_entries = max_subscribers.  An update (plain, batch or staged) returns -EINVAL, and a batch applies
+ *     none of its entries, when duid_len is 0 or > 31, a key byte past duid_len is non-zero, flags has bits other than
+ *     NA | PD or neither, PD is set with pd_len 0 or > 128, or prefix has bits set past pd_len.
+ *   - "dhcpv6_server_config": BPF_MAP_TYPE_ARRAY, one struct bng_dhcpv6_server_config (96 B).  duid_len 0 means
+ *     unconfigured; duid_len > 32 or dns_count > 2 returns -EINVAL.
+ *   - "dhcpv6_stats": BPF_MAP_TYPE_ARRAY, one entry of BNG_DHCPV6_NUM_STATS u64 counters (the BNG_DHCPV6_ST_* order).
+ *     They follow the BNG_NUM_STATS counters of the packed statistics vector in the same device buffer
+ *     (bng_stats_device_ptr still reports BNG_NUM_STATS), and bng_sync_reduce all-reduces them with the others;
+ *     totals_out keeps its BNG_NUM_STATS entries.
+ * bng_dhcpv6_enable(ctx, on): on != 0 applies the rule below from the next bng_prog_run of dhcp_fastpath_prog; DHCPv4
+ * frames and every other program are unchanged.  Off by default; -EINVAL for a NULL ctx.  The flag is context state:
+ * snapshots, deltas and hand-over blobs do not carry it.  While dhcpv6_bindings is empty or the server is
+ * unconfigured, "on" launches exactly what "off" launches and counts nothing.
+ * The rule.  Bytes are "present" as far as frame_dlen goes: min(len, stride) in a fixed-stride arena, len with an
+ * offset table.  A frame that dhcp_one has found not to be IPv4 (stats_map counts it as it always did, vlan_packets
+ * included) is a DHCPv6 candidate when it is untagged or carries one or two tags parsed as for DHCPv4 (0x8100 / 0x88A8,
+ * then an inner 0x8100), its ethertype is 0x86DD, the 40-byte IPv6 header is present with version 6 and next header 17,
+ * the UDP header is present with destination port 547, and the IPv6 destination is ff02::1:2 or server_ip.  For a
+ * candidate, total += 1; the first of these that applies passes it (XDP_PASS, frame untouched, one counter):
+ *   1. server unconfigured or len > 448: unsupported; UDP length < 12 or past the bytes present: malformed;
+ *   2. message type not Solicit (1), Request (3), Renew (5) or Rebind (6): unsupported; otherwise the type's own
+ *      counter also counts, whatever follows;
+ *   3. the option walk from message byte 4 to the UDP end finds an option running past the end, or more than 32
+ *      options: malformed;
+ *   4. unsupported: not exactly one Client ID of 1-31 bytes; an IA_TA; more than one IA_NA or IA_PD; an IA_NA or IA_PD
+ *      shorter than 12 bytes; neither IA_NA nor IA_PD; a Server ID on a Solicit or Rebind; a Request or Renew without
+ *      exactly one Server ID byte-equal to (duid, duid_len);
+ *   5. no dhcpv6_bindings entry for the Client ID, or its mac is not the Ethernet source: miss;
+ *   6. now_s > expires_s (now_s = the frame's clock / 1e9, as DHCPv4's lease_expiry): expired;
+ *   7. an IA_NA while the binding lacks NA or has another iaid_na, or the same for IA_PD: unsupported;
+ *   8. the reply does not fit the frame's storage (stride in a fixed-stride arena, len rounded up to 16 with an offset
+ *      table): no_room.
+ * Otherwise the frame is answered in place: XDP_TX, len = the reply's length, advertise or reply += 1.  Ethernet dst =
+ * the request's source, src = server_mac, tags as they were; IPv6 0x60000000, payload length, next header 17, hop
+ * limit 64, src = server_ip, dst = the request's source; UDP 547 -> 546, its length and its checksum (0 sent as
+ * 0xFFFF); the message: type, the transaction id, then Client ID (copied), Server ID, Preference 255 (Advertise
+ * only), IA_NA {IAID, T1, T2, IAADDR {addr, preferred, valid}} if requested, IA_PD {IAID, T1, T2, IAPREFIX {preferred,
+ * valid, pd_len, prefix}} if requested, DNS servers (23) when dns_count > 0, Status Code {0, "Success"} (Reply only),
+ * Rapid Commit (a Solicit answered with a Reply).  The bytes from the reply's end to the next multiple of 16 (counted
+ * from the frame's start) are zeroed; every other byte of the frame's storage is unchanged.  A Solicit with Rapid Commit gets a Reply, any other Solicit an
+ * Advertise, the other three types a Reply.  T1 = preferred / 2, T2 = preferred * 4 / 5 in 32-bit unsigned arithmetic.
+ * The request's UDP checksum is not verified.  The program writes no table, and no frame's outcome depends on another,
+ * so the rule holds frame by frame, wherever the frame sits in the batch. */
+#define BNG_DHCPV6_NA 1
+#define BNG_DHCPV6_PD 2
+#define BNG_DHCPV6_NUM_STATS 12
+enum {
+    BNG_DHCPV6_ST_TOTAL, BNG_DHCPV6_ST_SOLICIT, BNG_DHCPV6_ST_REQUEST, BNG_DHCPV6_ST_RENEW, BNG_DHCPV6_ST_REBIND,
+    BNG_DHCPV6_ST_ADVERTISE, BNG_DHCPV6_ST_REPLY, BNG_DHCPV6_ST_MISS, BNG_DHCPV6_ST_EXPIRED, BNG_DHCPV6_ST_UNSUPPORTED,
+    BNG_DHCPV6_ST_NO_ROOM, BNG_DHCPV6_ST_MALFORMED
+};
+typedef struct bng_dhcpv6_client_key {
+    uint8_t duid_len; /* 1..31 */
+    uint8_t duid[31]; /* the Client Identifier option's data, zero past duid_len */
+} bng_dhcpv6_client_key;
+typedef struct bng_dhcpv6_binding {
+    uint8_t mac[6];         /* the client's Ethernet address: the request's source must equal it */
+    uint8_t flags;          /* BNG_DHCPV6_NA | BNG_DHCPV6_PD */
+    uint8_t pd_len;         /* 1..128 with PD */
+    uint32_t iaid_na;       /* host order */
+    uint32_t iaid_pd;
+    uint32_t preferred_lft; /* seconds */
+    uint32_t valid_lft;
+    uint64_t expires_s;     /* compared with the frame's clock / 1e9 */
+    uint8_t addr[16];       /* IA_NA address, network order */
+    uint8_t prefix[16];     /* IA_PD prefix, zero past pd_len */
+} bng_dhcpv6_binding;
+typedef struct bng_dhcpv6_server_config {
+    uint8_t server_mac[6];
+    uint8_t duid_len;       /* 0 = unconfigured, at most 32 */
+    uint8_t dns_count;      /* 0..2 */
+    uint8_t server_ip[16];  /* the reply's source, normally link-local */
+    uint8_t duid[32];       /* the Server Identifier option's data */
+    uint8_t dns[2][16];
+    uint8_t _pad[8];
+} bng_dhcpv6_server_config;
+int bng_dhcpv6_enable(bng_ctx *ctx, int on);
+
 /* ---- diagnostics ---- */
 uint64_t bng_launch_count(bng_ctx *ctx);  /* kernels launched by this context so far */
 /* Live subscriber_ipv6 entries per prefix length, counts[0..128]: the lengths the IPv6 lookup probes are those with a
