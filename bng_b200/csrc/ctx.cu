@@ -191,6 +191,15 @@ struct bng_ctx {
     u8 d6cfg_host[DHCP6_CFG_BYTES] = {};
     // bng_dhcpv6_enable: dhcp_fastpath_prog answers bound DHCPv6 clients (context state, as qos_v6)
     bool dhcp6 = false;
+    // Router and Neighbor Solicitations (not maps of the reference, include/bng_b200.h): nd_bindings, nd_config, the
+    // host's copy of the configuration as last written (it selects k_dhcp_fastpath<nd>) and the bindings' live-entry
+    // count as of the last command that changed it (bng_sub_export looks them up only while there are some)
+    Tbl ndb{};
+    u8 *ndcfg = nullptr;
+    u32 nd_live = 0;
+    u8 ndcfg_host[ND_CFG_BYTES] = {};
+    // bng_nd_enable: dhcp_fastpath_prog answers Router and Neighbor Solicitations (context state, as qos_v6)
+    bool nd = false;
 };
 
 namespace {
@@ -380,6 +389,55 @@ bool d6_bad_binding(const u8 *key, const u8 *val) {
     return false;
 }
 
+// ---- nd_bindings, nd_config ----
+int nd_refresh_locked(bng_ctx *c) {
+    CU(c, cudaMemcpyAsync(&c->nd_live, c->ndb.count, 4, cudaMemcpyDeviceToHost, c->L.stream));
+    CU(c, cudaStreamSynchronize(c->L.stream));
+    return 0;
+}
+// A binding the fast path could not use the way it reads it (include/bng_b200.h: the update's -EINVAL).  val: struct
+// bng_nd_binding: prefix@0 prefix_len@16 pio_flags@17 pad@18 valid@20 preferred@24 pad@28 expires_s@32 pad@40
+bool nd_bad_binding(const u8 *val) {
+    const u32 pl = val[16], fl = val[17];
+    if (pl > 128 || (fl & ~(u32)(BNG_ND_PIO_L | BNG_ND_PIO_A))) return true;
+    if (pl == 0 && fl) return true;
+    for (u32 b = pl; b < 128; b++)
+        if ((val[b / 8] >> (7 - b % 8)) & 1) return true;
+    for (u32 k : {18u, 19u, 28u, 29u, 30u, 31u, 40u, 41u, 42u, 43u, 44u, 45u, 46u, 47u})
+        if (val[k]) return true;
+    return false;
+}
+// The RA template's options from `o` to `end`: each has a length byte >= 1 and the walk ends exactly at `end`
+bool nd_options_ok(const u8 *ra, u32 o, u32 end) {
+    while (o < end) {
+        if (o + 2 > end || ra[o + 1] == 0) return false;
+        o += 8u * ra[o + 1];
+    }
+    return o == end;
+}
+// A configuration the fast path could not copy as its rule says (include/bng_b200.h: the update's -EINVAL).  v: struct
+// bng_nd_config: router_mac@0 pad@6 ra_head_len@8 ra_tail_len@10 pad@12 router_ll@16 ra@32
+bool nd_bad_config(const u8 *v) {
+    u16 head, tail;
+    memcpy(&head, v + 8, 2);
+    memcpy(&tail, v + 10, 2);
+    if (head == 0) { // unconfigured: all zero past the MAC
+        for (u32 k = 6; k < ND_CFG_BYTES; k++)
+            if (v[k]) return true;
+        return false;
+    }
+    if (v[6] || v[7] || v[12] || v[13] || v[14] || v[15]) return true;
+    if (head < 16 || (head & 7) || (tail & 7) || head + tail > 288) return true;
+    const u8 *ra = v + 32;
+    if (ra[0] != 134 || ra[1] != 0 || ra[2] || ra[3]) return true;
+    if (!nd_options_ok(ra, 16, head) || !nd_options_ok(ra, head, head + tail)) return true;
+    if (v[16] != 0xFE || (v[17] & 0xC0) != 0x80) return true; // fe80::/10
+    if ((v[0] & 1) || !(v[0] | v[1] | v[2] | v[3] | v[4] | v[5])) return true;
+    for (u32 k = head + tail; k < 288; k++)
+        if (ra[k]) return true;
+    return false;
+}
+
 // ---- control-plane commands on hash maps ----
 int hash_cmd(bng_ctx *c, MapReg *m, int op, const void *keys, void *vals, u64 n, u32 flags, int *first_err, u64 *n_err = nullptr) {
     const Tbl &t = *m->tbl;
@@ -415,6 +473,7 @@ int hash_cmd(bng_ctx *c, MapReg *m, int op, const void *keys, void *vals, u64 n,
     }
     if (m->tbl == &c->v6 && op != TOP_LOOKUP) return v6_refresh_locked(c);
     if (m->tbl == &c->d6b && op != TOP_LOOKUP) return d6_refresh_locked(c);
+    if (m->tbl == &c->ndb && op != TOP_LOOKUP) return nd_refresh_locked(c);
     return 0;
 }
 
@@ -723,6 +782,9 @@ bng_ctx *bng_open(const bng_open_opts *o) {
     // dhcpv6_bindings: 96-byte slots (32-byte key, the 64-byte binding at 32)
     OPEN_R(make_table(c, &c->d6b, 32, 64, 32, max_subs));
     OPEN_R(dev_alloc(c, (void **)&c->d6cfg, DHCP6_CFG_BYTES, 0));
+    // nd_bindings: 64-byte slots (the MAC word, the 48-byte binding at 8)
+    OPEN_R(make_table(c, &c->ndb, 8, 48, 8, max_subs));
+    OPEN_R(dev_alloc(c, (void **)&c->ndcfg, ND_CFG_BYTES, 0));
     // subscriber directory: 16-byte slots, as many as the per-subscriber maps have, room for both maps' keys
     OPEN_R(make_table(c, &d.subdir, 4, 8, 8, max_subs, 0, 16));
     d.subdir.max_entries = std::min<u64>(2ull * max_subs, d.subdir.mask);
@@ -775,6 +837,10 @@ bng_ctx *bng_open(const bng_open_opts *o) {
     add_hash(c, "dhcpv6_bindings", T_HASH, 32, 64, max_subs, &c->d6b);
     add_array(c, "dhcpv6_server_config", DHCP6_CFG_BYTES, 1, &c->d6cfg);
     add_stats(c, "dhcpv6_stats", T_ARRAY, ST_DHCP6_N * 8, ST_DHCP6);
+    // not maps of the reference: Router and Neighbor Solicitations answered on the GPU (include/bng_b200.h)
+    add_hash(c, "nd_bindings", T_HASH, 8, 48, max_subs, &c->ndb);
+    add_array(c, "nd_config", ND_CFG_BYTES, 1, &c->ndcfg);
+    add_stats(c, "nd_stats", T_ARRAY, ST_ND_N * 8, ST_ND);
     c->staged.resize(c->maps.size());
     OPEN_R(small_refresh(c));
     cudaError_t se = cudaStreamSynchronize(c->L.stream);
@@ -843,6 +909,9 @@ int bng_map_update_batch(bng_ctx *c, int map, const void *keys, const void *valu
         if (m->tbl == &c->d6b)
             for (u64 i = 0; i < n; i++)
                 if (d6_bad_binding((const u8 *)keys + i * ks, (const u8 *)values + i * m->value_size)) return -EINVAL;
+        if (m->tbl == &c->ndb)
+            for (u64 i = 0; i < n; i++)
+                if (nd_bad_binding((const u8 *)values + i * m->value_size)) return -EINVAL;
         std::vector<u8> masked;
         if (m->tbl == &c->v6) { // two spellings of one prefix are one key
             masked.assign((const u8 *)keys, (const u8 *)keys + n * ks);
@@ -883,6 +952,7 @@ int bng_map_update_batch(bng_ctx *c, int map, const void *keys, const void *valu
                 const u8 *v = (const u8 *)values + i * m->value_size;
                 if (v[6] > 32 || v[7] > 2) return -EINVAL;
             }
+            if (m->arr == &c->ndcfg && nd_bad_config((const u8 *)values + i * m->value_size)) return -EINVAL;
             u8 *dst = m->kind == KIND_ARRAY ? *m->arr + (size_t)idx * m->value_size : (u8 *)(c->dev.stats + m->stat_base);
             CU(c, cudaMemcpyAsync(dst, (const u8 *)values + i * m->value_size, m->value_size, cudaMemcpyHostToDevice,
                                   c->L.stream));
@@ -890,6 +960,7 @@ int bng_map_update_batch(bng_ctx *c, int map, const void *keys, const void *valu
         CU(c, cudaStreamSynchronize(c->L.stream));
         if (feeds_small_tabs(m)) c->small_dirty = true;
         if (m->arr == &c->d6cfg && n) memcpy(c->d6cfg_host, (const u8 *)values + (n - 1) * m->value_size, DHCP6_CFG_BYTES);
+        if (m->arr == &c->ndcfg && n) memcpy(c->ndcfg_host, (const u8 *)values + (n - 1) * m->value_size, ND_CFG_BYTES);
         return 0;
     case KIND_LPM:
         for (u64 i = 0; i < n; i++) {
@@ -1004,6 +1075,7 @@ int bng_map_clear(bng_ctx *c, int map) {
     if (t.plens) CU(c, cudaMemsetAsync(t.plens, 0, LPM6_LENS * 4, c->L.stream));
     if (m->tbl == &c->v6) c->v6_live = 0;
     if (m->tbl == &c->d6b) c->d6_live = 0;
+    if (m->tbl == &c->ndb) c->nd_live = 0;
     if (m->tbl == &c->dev.sub_nat || m->tbl == &c->dev.qos_in)
         CU(c, run_dir_clear_half(c->L, c->dev.subdir, m->tbl == &c->dev.sub_nat ? 1 : 2));
     CU(c, cudaStreamSynchronize(c->L.stream));
@@ -1165,7 +1237,7 @@ static const int k_acct_mode[] = {-1, ACCT_DST, ACCT_SRC, ACCT_ATTR, ACCT_DST, -
 // the interception direction of each program: BNG_LI_UPLINK (0), BNG_LI_DOWNLINK (1), -1: never captures
 static const int k_li_dir[] = {-1, 1, 0, 0, 1, -1, -1, 0, 0};
 
-// The storage of the caller's frames, for replies longer than their request (k_dhcp_fastpath<v6>): room_stride bytes
+// The storage of the caller's frames, for replies longer than their request (k_dhcp_fastpath<v6>, <nd>): room_stride bytes
 // each, or 0: len rounded up to 16; need: the pinned zero-copy feed's bytes to scatter back, else nullptr.
 struct FrameRoom {
     u32 room_stride;
@@ -1211,7 +1283,15 @@ static int dispatch(bng_ctx *c, int prog, const DevBatch &b, const LiSrc &src = 
             d6.room_stride = room ? room->room_stride : (b.off16 ? 0u : b.stride);
             d6.need = room ? room->need : nullptr;
         }
-        e = run_dhcp_fastpath(c->L, c->dev, b, v6 ? &d6 : nullptr);
+        // ND needs the switch and a configured nd_config (NS answers need no binding)
+        NdArgs nd{};
+        const bool ndo = c->nd && (c->ndcfg_host[8] | c->ndcfg_host[9]);
+        if (ndo) {
+            nd.bind = c->ndb, nd.cfg = c->ndcfg, nd.stats = c->dev.stats + ST_ND;
+            nd.room_stride = room ? room->room_stride : (b.off16 ? 0u : b.stride);
+            nd.need = room ? room->need : nullptr;
+        }
+        e = run_dhcp_fastpath(c->L, c->dev, b, v6 ? &d6 : nullptr, ndo ? &nd : nullptr);
         break;
     }
     case P_PIPE_UP: e = run_pipeline_up(c->L, c->dev, b, qv6, as6); break;
@@ -1326,7 +1406,7 @@ static int run_host_zero_copy(bng_ctx *c, int prog, bng_batch *bb, u8 *arena_dev
         b.arena_len = (u64)cn * hb;
         // interception copies the bytes past the compact copy straight from the host arena
         const LiSrc src{chunk_arena, bb->off16 ? c->zc_off[buf] : nullptr, contiguous ? nullptr : c->zc_len0[buf], bb->stride};
-        // a DHCPv6 reply may outgrow its request: bounded by the host frame's storage, written back up to its length
+        // a DHCPv6 or ND reply may outgrow its request: bounded by the host frame's storage, written back up to its length
         const FrameRoom room{bb->off16 ? 0u : bb->stride, contiguous ? nullptr : c->zc_len0[buf]};
         int r = dispatch(c, prog, b, src, &room);
         if (r) return r;
@@ -1478,6 +1558,7 @@ int bng_map_update_staged(bng_ctx *c, int map, const void *key, const void *valu
     if (!m || !key || !value) return -EINVAL;
     if (m->kind != KIND_HASH) return bng_map_update(c, map, key, value, BNG_ANY); // arrays / tries: nothing to batch
     if (m->tbl == &c->d6b && d6_bad_binding((const u8 *)key, (const u8 *)value)) return -EINVAL;
+    if (m->tbl == &c->ndb && nd_bad_binding((const u8 *)value)) return -EINVAL;
     std::lock_guard<std::mutex> g(c->mu);
     bng_ctx::Staged &q = c->staged[map];
     q.keys.insert(q.keys.end(), (const u8 *)key, (const u8 *)key + m->key_size);
@@ -3172,6 +3253,11 @@ int bng_sub_export(bng_ctx *c, const uint32_t *addrs, uint64_t n_addrs, const ui
     for (int k = 0; k < 2; k++) mm_v[k] = at, mm_r[k] = al256(at + nm * mm[k]->value_size), at = al256(mm_r[k] + nm * 4);
     if (c->acct) acct_v = at, acct_r = al256(at + na * sizeof(bng_acct)), at = al256(acct_r + na * 4);
     if (c->idle) idle_v = at, idle_r = al256(at + na * sizeof(bng_idle)), at = al256(idle_r + na * 4);
+    // nd_bindings by MAC, only while it has entries: an export from a context that never used it launches nothing more
+    MapReg *ndm = get_map(c, bng_map_id(c, "nd_bindings"));
+    const bool nd = nm && c->nd_live;
+    size_t nd_v = 0, nd_r = 0;
+    if (nd) nd_v = at, nd_r = al256(at + nm * ndm->value_size), at = al256(nd_r + nm * 4);
     const size_t flow0 = at;
     if (int r = mv_grow(c, flow0, 0)) return r;
     // the inputs are built in the pinned staging buffer and copied on the context's stream, ahead of the kernels that
@@ -3194,6 +3280,7 @@ int bng_sub_export(bng_ctx *c, const uint32_t *addrs, uint64_t n_addrs, const ui
         CU(c, run_table_op(c->L, *am[k]->tbl, TOP_LOOKUP, dv + aoff, dv + am_v[k], (int *)(dv + am_r[k]), na, 0, d.subdir, 0, nullptr, nullptr));
     for (int k = 0; k < 2; k++)
         CU(c, run_table_op(c->L, *mm[k]->tbl, TOP_LOOKUP, dv + moff, dv + mm_v[k], (int *)(dv + mm_r[k]), nm, 0, d.subdir, 0, nullptr, nullptr));
+    if (nd) CU(c, run_table_op(c->L, c->ndb, TOP_LOOKUP, dv + moff, dv + nd_v, (int *)(dv + nd_r), nm, 0, d.subdir, 0, nullptr, nullptr));
     if (c->acct) CU(c, run_acct_read(c->L, d.subdir, c->acct, (const u32 *)(dv + aoff), na, (u64 *)(dv + acct_v), (int *)(dv + acct_r)));
     if (c->idle) CU(c, run_idle_read(c->L, d.subdir, c->idle, (const u32 *)(dv + aoff), na, (u64 *)(dv + idle_v), (int *)(dv + idle_r)));
     u32 *cnt = (u32 *)(dv + coff);
@@ -3239,7 +3326,7 @@ int bng_sub_export(bng_ctx *c, const uint32_t *addrs, uint64_t n_addrs, const ui
     std::vector<u8> out(kMoveMagic, kMoveMagic + 8);
     out.resize(16);
     u64 nsec = 0;
-    auto by_key = [&](MapReg *m, const u8 *keys, u64 n, size_t voff, size_t roff) {
+    auto by_key = [&](MapReg *m, const u8 *keys, u64 n, size_t voff, size_t roff, bool skip_empty = false) {
         const int *res = (const int *)host(roff);
         const u8 *vals = host(voff);
         std::vector<u8> kv, vv;
@@ -3249,13 +3336,17 @@ int bng_sub_export(bng_ctx *c, const uint32_t *addrs, uint64_t n_addrs, const ui
                 vv.insert(vv.end(), vals + i * m->value_size, vals + (i + 1) * m->value_size);
             }
         const u64 k = kv.size() / m->key_size;
+        if (skip_empty && !k) return false;
         put_section(out, m->name, KIND_HASH, m->key_size, m->value_size, 0, k);
         out.insert(out.end(), kv.begin(), kv.end());
         out.insert(out.end(), vv.begin(), vv.end());
         nsec++;
+        return true;
     };
     for (int k = 0; k < 3; k++) by_key(am[k], (const u8 *)A.data(), na, am_v[k], am_r[k]);
     for (int k = 0; k < 2; k++) by_key(mm[k], (const u8 *)M.data(), nm, mm_v[k], mm_r[k]);
+    // only when there is one, so that blobs without ND bindings stay as they were
+    const bool nd_sec = nd && by_key(ndm, (const u8 *)M.data(), nm, nd_v, nd_r, true);
     for (int k = 0; k < 3; k++) {
         const MapReg *m = fm[k];
         put_section(out, m->name, KIND_HASH, m->key_size, m->value_size, 0, n4[k]);
@@ -3311,6 +3402,7 @@ int bng_sub_export(bng_ctx *c, const uint32_t *addrs, uint64_t n_addrs, const ui
                            k < 3 ? na : nm, 0, d.subdir, role, c->acct, c->idle));
     }
     if (n6) CU(c, run_table_op(c->L, c->v6, TOP_DELETE, dv + v6k, nullptr, (int *)(dv + v6r), n6, 0, d.subdir, 0, nullptr, nullptr));
+    if (nd_sec) CU(c, run_table_op(c->L, c->ndb, TOP_DELETE, dv + moff, nullptr, (int *)(dv + nd_r), nm, 0, d.subdir, 0, nullptr, nullptr));
     if (!li_a.empty()) {
         for (u32 a : li_a) c->li_targets.erase(a);
         c->li_dirty = true;
@@ -3319,6 +3411,9 @@ int bng_sub_export(bng_ctx *c, const uint32_t *addrs, uint64_t n_addrs, const ui
     prof_collect(c->L);
     if (n6) {
         if (int r = v6_refresh_locked(c)) return r;
+    }
+    if (nd_sec) {
+        if (int r = nd_refresh_locked(c)) return r;
     }
     // the flush's rebuild rule; a rebuild that finds no memory leaves the tables as they were, and the detach stands
     if (rebuild_if_tombstoned_locked(c, n4[3] + n4[0])) cudaGetLastError();
@@ -3431,7 +3526,7 @@ int bng_sub_import(bng_ctx *c, const void *buf, uint64_t len) {
 int bng_stats_device_ptr(bng_ctx *c, void **dptr, uint32_t *n_u64) {
     if (!c || !dptr) return -EINVAL;
     *dptr = c->dev.stats;
-    if (n_u64) *n_u64 = ST_COUNT; // dhcpv6_stats follow them in the same buffer (include/bng_b200.h)
+    if (n_u64) *n_u64 = ST_COUNT; // dhcpv6_stats and nd_stats follow them in the same buffer (include/bng_b200.h)
     return 0;
 }
 
@@ -3441,6 +3536,13 @@ int bng_dhcpv6_enable(bng_ctx *c, int on) {
     if (!c) return -EINVAL;
     std::lock_guard<std::mutex> g(c->mu);
     c->dhcp6 = on != 0;
+    return 0;
+}
+
+int bng_nd_enable(bng_ctx *c, int on) {
+    if (!c) return -EINVAL;
+    std::lock_guard<std::mutex> g(c->mu);
+    c->nd = on != 0;
     return 0;
 }
 

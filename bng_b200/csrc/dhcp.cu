@@ -508,6 +508,176 @@ __device__ __forceinline__ int dhcpv6_one(const Dhcp6Args &a, u32 *st, u8 *p, u3
     return XDP_TX_;
 }
 
+// ---- Router and Neighbor Solicitations (include/bng_b200.h, bng_nd_enable): an RS answered with the nd_config
+// template and the subscriber's own Prefix Information option, an NS for router_ll with a Neighbor Advertisement ----
+enum { ND_TOTAL, ND_RS, ND_NS, ND_RA, ND_NA, ND_MISS, ND_EXPIRED, ND_NOT_TARGET, ND_MALFORMED, ND_UNSUP, ND_NOROOM };
+
+// The L3 offset of an ND candidate, 0 for any other frame: tags as dhcp_one parses them, ethertype 0x86DD, the IPv6
+// header and the first ICMPv6 byte present, version 6, next header 58, and an RS to ff02::2 or router_ll or an NS to
+// router_ll or its solicited-node address.
+__device__ __forceinline__ u32 nd_candidate(const u8 *p, u32 dlen, const u8 *cfg) {
+    if (dlen < 14) return 0;
+    u32 proto = rd16(p, 12), l3 = 14;
+    if (proto == 0x0081u || proto == 0xA888u) {
+        if (dlen < 18) return 0;
+        proto = rd16(p, 16);
+        l3 = 18;
+        if (proto == 0x0081u) {
+            if (dlen < 22) return 0;
+            proto = rd16(p, 20);
+            l3 = 22;
+        }
+    }
+    if (proto != 0xDD86u || l3 + 41 > dlen) return 0;
+    if ((p[l3] >> 4) != 6 || p[l3 + 6] != 58) return 0;
+    const u32 t = p[l3 + 40];
+    if (t != 133 && t != 135) return 0;
+    const u32 d0 = rd32(p, l3 + 24), d1 = rd32(p, l3 + 28), d2 = rd32(p, l3 + 32), d3 = rd32(p, l3 + 36);
+    const u32 *ll = (const u32 *)(cfg + 16); // router_ll, words in memory order
+    if (d0 == ll[0] && d1 == ll[1] && d2 == ll[2] && d3 == ll[3]) return l3;
+    if (d0 != 0x000002FFu || d1 != 0) return 0;
+    if (t == 133) return d2 == 0 && d3 == 0x02000000u ? l3 : 0;              // ff02::2
+    return d2 == 0x01000000u && d3 == ((ll[3] & 0xFFFFFF00u) | 0xFFu) ? l3 : 0; // ff02::1:ff00:0/104 | router_ll's low 24 bits
+}
+
+// One candidate at L3 offset l3.  Everything the reply needs from the request (its MAC and IPv6 source) is read before
+// the first byte of the reply is written; the reply's ICMPv6 part is written in 2-byte stores.
+__device__ __forceinline__ int nd_one(const NdArgs &a, u32 *st, u8 *p, u32 &len, const u32 dlen, u64 now, u32 l3) {
+    const u8 *cfg = a.cfg; // router_mac@0 ra_head_len@8 ra_tail_len@10 router_ll@16 ra@32
+    const u32 icmp = l3 + 40;
+    const bool rs = p[icmp] == 133;
+    atomicAdd(&st[ND_TOTAL], 1u);
+    const u32 head = *(const u16 *)(cfg + 8), tail = *(const u16 *)(cfg + 10);
+    if (head == 0 || len > 448) {
+        atomicAdd(&st[ND_UNSUP], 1u);
+        return XDP_PASS_;
+    }
+    const u32 plen = be16(p, l3 + 4);
+    if (plen < (rs ? 8u : 24u) || icmp + plen > dlen) {
+        atomicAdd(&st[ND_MALFORMED], 1u);
+        return XDP_PASS_;
+    }
+    atomicAdd(&st[rs ? ND_RS : ND_NS], 1u);
+
+    // ---- validity (RFC 4861 §6.1.1, §7.1.1) ----
+    const u32 s0 = rd32(p, l3 + 8), s1 = rd32(p, l3 + 12), s2 = rd32(p, l3 + 16), s3 = rd32(p, l3 + 20);
+    const bool unspec = (s0 | s1 | s2 | s3) == 0;
+    bool bad = p[l3 + 7] != 255 || p[icmp + 1] != 0;
+    // the checksum over the pseudo-header (words read in memory order: the sum is byte-order neutral)
+    u32 sum = bswap16((u16)plen) + 0x3A00u; // upper-layer length, next header 58
+#pragma unroll
+    for (int k = 0; k < 16; k++) sum += rd16(p, l3 + 8 + 2 * k);
+    for (u32 k = 0; k + 1 < plen; k += 2) sum += rd16(p, icmp + k);
+    if (plen & 1) sum += p[icmp + plen - 1];
+    sum = (sum & 0xFFFF) + (sum >> 16);
+    sum = (sum & 0xFFFF) + (sum >> 16);
+    bad = bad || sum != 0xFFFFu;
+    const u32 end = icmp + plen;
+    u32 nopt = 0;
+    bool slla = false;
+    for (u32 o = icmp + (rs ? 8u : 24u); o < end && !bad;) {
+        if (o + 2 > end || p[o + 1] == 0 || o + 8u * p[o + 1] > end || ++nopt > 32) {
+            bad = true;
+            break;
+        }
+        slla = slla || p[o] == 1;
+        o += 8u * p[o + 1];
+    }
+    bad = bad || (unspec && slla);
+    if (!rs) bad = bad || p[icmp + 8] == 0xFF || (unspec && p[l3 + 24] != 0xFF); // multicast target; :: to router_ll
+    if (bad) {
+        atomicAdd(&st[ND_MALFORMED], 1u);
+        return XDP_PASS_;
+    }
+    const u32 *ll = (const u32 *)(cfg + 16);
+    if (!rs && (rd32(p, icmp + 8) != ll[0] || rd32(p, icmp + 12) != ll[1] || rd32(p, icmp + 16) != ll[2] ||
+                rd32(p, icmp + 20) != ll[3])) {
+        atomicAdd(&st[ND_NOT_TARGET], 1u);
+        return XDP_PASS_;
+    }
+
+    // ---- the binding (RS) ----
+    const u8 *v = nullptr; // prefix@0 prefix_len@16 pio_flags@17 valid@20 preferred@24 expires_s@32
+    if (rs) {
+        u64 mk = 0;
+#pragma unroll
+        for (int k = 0; k < 6; k++) mk = (mk << 8) | p[6 + k];
+        const u8 *s = tbl_find_conv<1>(a.bind, &mk);
+        if (!s) {
+            atomicAdd(&st[ND_MISS], 1u);
+            return XDP_PASS_;
+        }
+        v = s + a.bind.voff;
+        if (now / 1000000000ull > *(const u64 *)(v + 32)) {
+            atomicAdd(&st[ND_EXPIRED], 1u);
+            return XDP_PASS_;
+        }
+    }
+    const u32 pl = rs ? v[16] : 0;
+    const u32 ilen = rs ? head + (pl ? 32u : 0u) + tail : 32u;
+    const u32 room = a.room_stride ? a.room_stride : (len + 15u) & ~15u;
+    if (icmp + ilen > room) {
+        atomicAdd(&st[ND_NOROOM], 1u);
+        return XDP_PASS_;
+    }
+
+    // ---- the reply, over the request ----
+    u32 o = icmp;
+    if (rs) {
+        const u8 *ra = cfg + 32;
+        for (u32 k = 0; k < head; k += 4) wr32(p, o + k, *(const u32 *)(ra + k));
+        o += head;
+        if (pl) {
+            wr16(p, o, 0x0403u);
+            wr16(p, o + 2, (u16)(pl | (u32)v[17] << 8));
+            wr32(p, o + 4, __byte_perm(*(const u32 *)(v + 20), 0, 0x0123));
+            wr32(p, o + 8, __byte_perm(*(const u32 *)(v + 24), 0, 0x0123));
+            wr32(p, o + 12, 0);
+#pragma unroll
+            for (int k = 0; k < 4; k++) wr32(p, o + 16 + 4 * k, *(const u32 *)(v + 4 * k));
+            o += 32;
+        }
+        for (u32 k = 0; k < tail; k += 4) wr32(p, o + k, *(const u32 *)(ra + head + k));
+        o += tail;
+    } else {
+        wr32(p, o, 0x00000088u); // type 136, code 0, checksum 0 for now
+        wr32(p, o + 4, unspec ? 0xA0u : 0xE0u);
+#pragma unroll
+        for (int k = 0; k < 4; k++) wr32(p, o + 8 + 4 * k, ll[k]);
+        wr16(p, o + 24, 0x0102u); // Target Link-Layer Address, 1 x 8 bytes
+#pragma unroll
+        for (int k = 0; k < 3; k++) wr16(p, o + 26 + 2 * k, *(const u16 *)(cfg + 2 * k));
+        o += 32;
+    }
+    for (u32 k = o; k & 15; k += 2) wr16(p, k, 0); // to the reply's next 16-byte boundary (a frame starts on one)
+    // Ethernet: back to the requester, from the router; the tags stay
+    wr16(p, 0, rd16(p, 6));
+    wr16(p, 2, rd16(p, 8));
+    wr16(p, 4, rd16(p, 10));
+#pragma unroll
+    for (int k = 0; k < 3; k++) wr16(p, 6 + 2 * k, *(const u16 *)(cfg + 2 * k));
+    // IPv6
+    wr32(p, l3, 0x00000060u);
+    wr16(p, l3 + 4, bswap16((u16)ilen));
+    wr16(p, l3 + 6, 0xFF3Au); // next header 58, hop limit 255
+#pragma unroll
+    for (int k = 0; k < 4; k++) wr32(p, l3 + 8 + 4 * k, ll[k]);
+    wr32(p, l3 + 24, unspec ? 0x000002FFu : s0); // ff02::1 for ::
+    wr32(p, l3 + 28, unspec ? 0u : s1);
+    wr32(p, l3 + 32, unspec ? 0u : s2);
+    wr32(p, l3 + 36, unspec ? 0x01000000u : s3);
+    u32 ck = bswap16((u16)ilen) + 0x3A00u;
+#pragma unroll
+    for (int k = 0; k < 16; k++) ck += rd16(p, l3 + 8 + 2 * k);
+    for (u32 k = 0; k < ilen; k += 2) ck += rd16(p, icmp + k);
+    ck = (ck & 0xFFFF) + (ck >> 16);
+    ck = (ck & 0xFFFF) + (ck >> 16);
+    wr16(p, icmp + 2, (u16)~ck);
+    len = o;
+    atomicAdd(&st[rs ? ND_RA : ND_NA], 1u);
+    return XDP_TX_;
+}
+
 // Tile kernel (one mbarrier per block rather than per-thread barriers without any block-wide synchronisation): a
 // request is up to ~350 bytes that the program reads sparsely and rewrites almost
 // entirely (L2 headers, BOOTP fixed part, 192 zeroed bytes, options), so frames are staged through
@@ -525,15 +695,20 @@ __device__ __forceinline__ int dhcpv6_one(const Dhcp6Args &a, u32 *st, u8 *p, u3
 // version issues 2 x 2^22 TMA operations per batch, a few dozen cycles apart on every SM, and that, not HBM,
 // bounds it.  Every other arena (an offset table, or slots that do not fit a staging slot) moves frame by frame.
 // V6: DHCPv6 candidates among the frames dhcp_one passed as not IPv4 are answered by dhcpv6_one (bng_dhcpv6_enable)
-template <bool V6>
+// ND: so are Router and Neighbor Solicitations among the frames still passed, by nd_one (bng_nd_enable)
+template <bool V6, bool ND>
 __global__ void __launch_bounds__(DH_TILE) k_dhcp_fastpath(const __grid_constant__ DevCtx c, const __grid_constant__ DevBatch b,
-                                                           const __grid_constant__ Dhcp6Args a) {
+                                                           const __grid_constant__ Dhcp6Args a, const __grid_constant__ NdArgs na) {
     extern __shared__ __align__(128) u8 stage[]; // DH_TILE * DH_SLOT
     __shared__ BlockStats bs;
     __shared__ u64 bar, bar1;
     __shared__ u32 s6[V6 ? ST_DHCP6_N : 1];
     if constexpr (V6) {
         if (threadIdx.x < ST_DHCP6_N) s6[threadIdx.x] = 0;
+    }
+    __shared__ u32 snd[ND ? ST_ND_N : 1];
+    if constexpr (ND) {
+        if (threadIdx.x < ST_ND_N) snd[threadIdx.x] = 0;
     }
     bstats_init(bs);
     const u32 bar_a = (u32)__cvta_generic_to_shared(&bar), bar1_a = (u32)__cvta_generic_to_shared(&bar1);
@@ -594,11 +769,11 @@ __global__ void __launch_bounds__(DH_TILE) k_dhcp_fastpath(const __grid_constant
                 if (rd16(mine, 16) == 0x0081u) l3 = 22;
             }
             direct = l3 + (u32)(mine[l3] & 0x0f) * 4 + 8 + 240 + 64 > DH_SLOT;
-            if constexpr (V6) {
+            if constexpr (V6 || ND) {
                 if (rd16(mine, l3 - 2) == 0xDD86u) direct = true; // an IPv6 frame is decided by its ethertype
             }
         }
-        u32 grown = 0; // V6: the bytes of an answered frame, rounded up to 16
+        u32 grown = 0; // V6, ND: the bytes of an answered frame, rounded up to 16
         if (act) {
             const u32 l0 = len;
             u8 *fp = direct ? g : mine;
@@ -610,13 +785,20 @@ __global__ void __launch_bounds__(DH_TILE) k_dhcp_fastpath(const __grid_constant
                     if (l3 && (v = dhcpv6_one(a, s6, fp, len, dl, frame_now(b, i), l3)) == XDP_TX_) grown = (len + 15u) & ~15u;
                 }
             }
+            if constexpr (ND) { // disjoint from DHCPv6's candidates: next header 58, not 17
+                if (v == XDP_PASS_) {
+                    const u32 l3 = nd_candidate(fp, dl, na.cfg);
+                    if (l3 && (v = nd_one(na, snd, fp, len, dl, frame_now(b, i), l3)) == XDP_TX_) grown = (len + 15u) & ~15u;
+                }
+            }
             b.verdict[i] = (u8)v;
             if (len != l0) b.len[i] = len;
         }
         if (direct) nbytes = 0;
-        if constexpr (V6) { // a reply can be longer than its request: store it back whole
+        if constexpr (V6 || ND) { // a reply can be longer than its request: store it back whole
+            u32 *need = V6 ? a.need : na.need;
             if (!direct && grown > nbytes) nbytes = grown;
-            if (grown && a.need && grown > a.need[i]) a.need[i] = grown;
+            if (grown && need && grown > need[i]) need[i] = grown;
         }
         // ---- stage out (every staged frame: a passed frame may have been rewritten, :769) ----
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
@@ -641,28 +823,29 @@ __global__ void __launch_bounds__(DH_TILE) k_dhcp_fastpath(const __grid_constant
     if constexpr (V6) {
         if (threadIdx.x < ST_DHCP6_N && s6[threadIdx.x]) atomicAdd(&a.stats[threadIdx.x], (u64)s6[threadIdx.x]);
     }
+    if constexpr (ND) {
+        if (threadIdx.x < ST_ND_N && snd[threadIdx.x]) atomicAdd(&na.stats[threadIdx.x], (u64)snd[threadIdx.x]);
+    }
 }
 
 // (A double-buffered variant — two staging slots per thread, the load of tile i+1 issued before the program runs on
 // tile i — was tried and dropped: it was slower.)
 
-cudaError_t run_dhcp_fastpath(Launcher &L, const DevCtx &c, const DevBatch &b, const Dhcp6Args *d6) {
+cudaError_t run_dhcp_fastpath(Launcher &L, const DevCtx &c, const DevBatch &b, const Dhcp6Args *d6, const NdArgs *nd) {
     const int smem = DH_TILE * DH_SLOT;
-    int &set = d6 ? L.dhcp6_smem_set : L.dhcp_smem_set;
+    int &set = nd ? L.nd_smem_set[d6 ? 1 : 0] : (d6 ? L.dhcp6_smem_set : L.dhcp_smem_set);
+    auto *k = nd ? (d6 ? k_dhcp_fastpath<true, true> : k_dhcp_fastpath<false, true>)
+                 : (d6 ? k_dhcp_fastpath<true, false> : k_dhcp_fastpath<false, false>);
     if (!set) { // function attributes are per device: set on the device this context runs on
-        cudaError_t e = cudaFuncSetAttribute(d6 ? k_dhcp_fastpath<true> : k_dhcp_fastpath<false>,
-                                             cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+        cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
         if (e != cudaSuccess) return e;
         set = 1;
     }
     long want = ((long)b.n + DH_TILE - 1) / DH_TILE;
     long cap = (long)L.num_sms * 4; // 4 x 50 KB of staging per SM (of the 228 KB an H100 SM has)
     int grid = (int)(want < cap ? (want < 1 ? 1 : want) : cap);
-    prof_begin(L, d6 ? "k_dhcp_fastpath<v6>" : "k_dhcp_fastpath");
-    if (d6)
-        k_dhcp_fastpath<true><<<grid, DH_TILE, smem, L.stream>>>(c, b, *d6);
-    else
-        k_dhcp_fastpath<false><<<grid, DH_TILE, smem, L.stream>>>(c, b, Dhcp6Args{});
+    prof_begin(L, nd ? (d6 ? "k_dhcp_fastpath<v6,nd>" : "k_dhcp_fastpath<nd>") : (d6 ? "k_dhcp_fastpath<v6>" : "k_dhcp_fastpath"));
+    k<<<grid, DH_TILE, smem, L.stream>>>(c, b, d6 ? *d6 : Dhcp6Args{}, nd ? *nd : NdArgs{});
     prof_end(L);
     L.launches++;
     return cudaGetLastError();

@@ -29,6 +29,7 @@ struct Launcher {
     // one process can hold contexts on several GPUs
     int dhcp_smem_set;  // cudaFuncAttributeMaxDynamicSharedMemorySize applied on this context's device
     int dhcp6_smem_set; // ... and to k_dhcp_fastpath<v6>
+    int nd_smem_set[2]; // ... and to k_dhcp_fastpath<nd>, <v6,nd>
     int resolve_bps[16]; // resident blocks per SM of the k_resolve instantiations, by <NAT, QOS, EGRESS, TC> bits
     int prof;
     ProfPending pend[32];
@@ -62,7 +63,6 @@ cudaError_t run_pipeline_tc(Launcher &L, const DevCtx &c, const DevBatch &b, con
 // (BlockStats) keep ST_COUNT.
 #define ST_DHCP6 ST_COUNT
 #define ST_DHCP6_N 12
-#define ST_ALL (ST_COUNT + ST_DHCP6_N)
 #define DHCP6_CFG_BYTES 96
 struct Dhcp6Args {
     Tbl bind;         // dhcpv6_bindings: 32-byte key (4 words), 64-byte value at 32
@@ -71,9 +71,22 @@ struct Dhcp6Args {
     u32 room_stride;  // a frame's storage: room_stride bytes, or 0: its len rounded up to 16 (an offset table)
     u32 *need;        // pinned zero-copy feed: bytes the scatter writes back, raised to cover a grown reply; else nullptr
 };
+// Router and Neighbor Solicitations (include/bng_b200.h, bng_nd_enable): their counters follow dhcpv6_stats
+#define ST_ND (ST_DHCP6 + ST_DHCP6_N)
+#define ST_ND_N 11
+#define ST_ALL (ST_COUNT + ST_DHCP6_N + ST_ND_N)
+#define ND_CFG_BYTES 320
+struct NdArgs {
+    Tbl bind;         // nd_bindings: the 8-byte MAC word, 48-byte value at 8
+    const u8 *cfg;    // nd_config[0]
+    u64 *stats;       // ST_ND_N counters
+    u32 room_stride;  // as Dhcp6Args
+    u32 *need;
+};
 // d6: the DHCPv6 tables when the fast path answers DHCPv6 (bng_dhcpv6_enable, a configured server and live bindings),
-// else nullptr
-cudaError_t run_dhcp_fastpath(Launcher &L, const DevCtx &c, const DevBatch &b, const Dhcp6Args *d6);
+// else nullptr; nd: the ND tables when it answers Router and Neighbor Solicitations (bng_nd_enable and a configured
+// nd_config), else nullptr
+cudaError_t run_dhcp_fastpath(Launcher &L, const DevCtx &c, const DevBatch &b, const Dhcp6Args *d6, const NdArgs *nd);
 
 // header gather / scatter between a pinned host arena and a compact device copy (hostio.cu); icmp_errors (TC only):
 // also bytes 64-79 of an ICMP error frame, for nat44_ingress with bng_nat_icmp_errors_enable

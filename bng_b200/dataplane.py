@@ -103,6 +103,7 @@ def load_library() -> C.CDLL:
         "bng_antispoof_ipv6_prefixes_enable": ([vp, i32], i32),
         "bng_nat_icmp_errors_enable": ([vp, i32], i32),
         "bng_dhcpv6_enable": ([vp, i32], i32),
+        "bng_nd_enable": ([vp, i32], i32),
         "bng_lru_overflow": ([vp], u64),
         "bng_events_lost": ([vp], u64),
         "bng_prof_enable": ([vp, i32], i32),
@@ -157,7 +158,7 @@ EXPORTED_SYMBOLS = (
     "bng_idle_enable", "bng_idle_timeout_set", "bng_idle_read", "bng_idle_scan", "bng_nat_usage",
     "bng_dhcp_lease_census", "bng_dhcp_lease_sweep", "bng_lease_table_rebuilds", "bng_dhcp_lease_addr_order",
     "bng_sub_export", "bng_sub_import", "bng_ipv6_prefix_lengths", "bng_qos_ipv6_enable",
-    "bng_nat_icmp_errors_enable", "bng_antispoof_ipv6_prefixes_enable", "bng_dhcpv6_enable",
+    "bng_nat_icmp_errors_enable", "bng_antispoof_ipv6_prefixes_enable", "bng_dhcpv6_enable", "bng_nd_enable",
 )
 
 
@@ -328,6 +329,12 @@ class Dataplane:
         from the next run on; off by default (include/bng_b200.h).  Context state: snapshots, deltas and hand-over
         blobs do not carry it."""
         self._chk(self.lib.bng_dhcpv6_enable(self.h, 1 if on else 0), "dhcpv6_enable")
+
+    def nd_enable(self, on: bool = True):
+        """Let dhcp_fastpath_prog answer IPv6 Router Solicitations with a per-subscriber Router Advertisement (nd_config,
+        nd_bindings) and Neighbor Solicitations for the router's link-local address, from the next run on; off by
+        default (include/bng_b200.h).  Context state: snapshots, deltas and hand-over blobs do not carry it."""
+        self._chk(self.lib.bng_nd_enable(self.h, 1 if on else 0), "nd_enable")
 
     def nat_icmp_errors_enable(self, on: bool = True):
         """Translate inbound ICMP errors (Destination Unreachable, Time Exceeded, Parameter Problem) in nat44_ingress

@@ -319,6 +319,122 @@ inline int ClearPrefix(bng_ctx *ctx, const uint8_t addr[16], uint32_t prefixlen)
 } // namespace dualstack
 
 // ===========================================================================
+// Router Advertisements (reference pkg/slaac/radvd.go: NewServer's defaults, buildRA, buildPrefixOption,
+// buildRDNSSOption, buildDNSSLOption), restated to fill nd_config (include/bng_b200.h, bng_nd_enable): the RA the
+// daemon would send, split where the GPU inserts each subscriber's own Prefix Information option.
+namespace slaac {
+
+struct Prefix {
+    uint8_t addr[16]; // as net.ParseCIDR gives it: masked to len
+    uint8_t len;
+};
+// slaac.Config as NewServer reads it, plus what the daemon takes from the interface: its MAC (buildRA's Source
+// Link-Layer Address) and its link-local address (the RA's source).
+struct RouterConfig {
+    uint8_t router_mac[6] = {};
+    uint8_t router_ll[16] = {};
+    std::vector<Prefix> prefixes;                  // the shared prefixes: L, A = !managed, valid 30 days, preferred 7
+    uint32_t mtu = 0;                              // 0: no MTU option
+    bool managed = false, other = false;           // M, O
+    std::vector<std::vector<uint8_t>> dns_servers; // 16 bytes each; IPv4-mapped ones are dropped, as NewServer does
+    std::vector<std::string> dns_domains;
+    uint16_t default_lifetime = 0;                 // router lifetime in seconds, 0 = 1800
+};
+
+namespace detail {
+inline void put32(std::vector<uint8_t> &b, size_t o, uint32_t v) {
+    b[o] = (uint8_t)(v >> 24), b[o + 1] = (uint8_t)(v >> 16), b[o + 2] = (uint8_t)(v >> 8), b[o + 3] = (uint8_t)v;
+}
+// encodeDNSLabel / splitDomain: labels split on '.', empty ones skipped, then a terminating zero
+inline std::vector<uint8_t> EncodeDNSLabel(const std::string &domain) {
+    std::vector<uint8_t> out;
+    std::string cur;
+    auto flush = [&] {
+        if (cur.empty()) return;
+        out.push_back((uint8_t)cur.size());
+        out.insert(out.end(), cur.begin(), cur.end());
+        cur.clear();
+    };
+    for (char ch : domain) {
+        if (ch == '.') flush();
+        else cur += ch;
+    }
+    flush();
+    out.push_back(0);
+    return out;
+}
+} // namespace detail
+
+// buildRA's bytes as nd_config: head = RA header, SLLA, MTU, the shared prefixes; tail = RDNSS, DNSSL.  An error when
+// they do not fit the 288 bytes nd_config holds.
+inline Result<bng_nd_config> BuildRA(const RouterConfig &rc) {
+    Result<bng_nd_config> r;
+    const uint16_t lifetime = rc.default_lifetime ? rc.default_lifetime : 1800;
+    std::vector<uint8_t> head(16, 0), tail;
+    head[0] = 134;
+    head[4] = 64; // curHopLimit
+    head[5] = (uint8_t)((rc.managed ? 0x80 : 0) | (rc.other ? 0x40 : 0));
+    head[6] = (uint8_t)(lifetime >> 8), head[7] = (uint8_t)lifetime; // reachable time and retrans timer stay 0
+    head.insert(head.end(), {1, 1});                                  // Source Link-Layer Address
+    head.insert(head.end(), rc.router_mac, rc.router_mac + 6);
+    if (rc.mtu) {
+        const size_t o = head.size();
+        head.resize(o + 8, 0);
+        head[o] = 5, head[o + 1] = 1;
+        detail::put32(head, o + 4, rc.mtu);
+    }
+    for (const Prefix &p : rc.prefixes) {
+        const size_t o = head.size();
+        head.resize(o + 32, 0);
+        head[o] = 3, head[o + 1] = 4, head[o + 2] = p.len;
+        head[o + 3] = (uint8_t)(0x80 | (rc.managed ? 0 : 0x40));
+        detail::put32(head, o + 4, 2592000);
+        detail::put32(head, o + 8, 604800);
+        for (int k = 0; k < 16; k++) {
+            const int bits = std::min(8, std::max(0, (int)p.len - 8 * k));
+            head[o + 16 + k] = (uint8_t)(p.addr[k] & (uint8_t)(0xFF00 >> bits));
+        }
+    }
+    std::vector<std::vector<uint8_t>> dns;
+    static const uint8_t v4mapped[12] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0xff, 0xff};
+    for (const auto &d : rc.dns_servers)
+        if (d.size() == 16 && memcmp(d.data(), v4mapped, 12)) dns.push_back(d);
+    if (!dns.empty()) {
+        tail.resize(8 + 16 * dns.size(), 0);
+        tail[0] = 25, tail[1] = (uint8_t)(1 + 2 * dns.size());
+        detail::put32(tail, 4, (uint32_t)lifetime * 3);
+        for (size_t i = 0; i < dns.size(); i++) memcpy(&tail[8 + 16 * i], dns[i].data(), 16);
+    }
+    if (!rc.dns_domains.empty()) {
+        std::vector<uint8_t> names;
+        for (const auto &d : rc.dns_domains) {
+            auto e = detail::EncodeDNSLabel(d);
+            names.insert(names.end(), e.begin(), e.end());
+        }
+        names.resize(names.size() + (8 - (8 + names.size()) % 8) % 8, 0);
+        const size_t o = tail.size();
+        tail.resize(o + 8, 0);
+        tail[o] = 31, tail[o + 1] = (uint8_t)((8 + names.size()) / 8);
+        detail::put32(tail, o + 4, (uint32_t)lifetime * 3);
+        tail.insert(tail.end(), names.begin(), names.end());
+    }
+    if (head.size() + tail.size() > sizeof(((bng_nd_config *)nullptr)->ra)) {
+        r.err = Error("router advertisement of " + std::to_string(head.size() + tail.size()) + " bytes does not fit nd_config");
+        return r;
+    }
+    bng_nd_config c{};
+    memcpy(c.router_mac, rc.router_mac, 6);
+    memcpy(c.router_ll, rc.router_ll, 16);
+    c.ra_head_len = (uint16_t)head.size(), c.ra_tail_len = (uint16_t)tail.size();
+    memcpy(c.ra, head.data(), head.size());
+    if (!tail.empty()) memcpy(c.ra + head.size(), tail.data(), tail.size());
+    r.value = c;
+    return r;
+}
+
+} // namespace slaac
+
+// ===========================================================================
 // Lawful intercept, content of communication (reference pkg/intercept/manager.go:337: Manager.RecordCC(warrant,
 // session, direction, srcIP, dstIP, srcPort, dstPort, protocol, payload)).  StartInterceptSession sets the session's
 // IPv4 address as a target (bng_li_target_set), StopInterceptSession deletes it; PumpCC drains the records and hands
@@ -570,13 +686,15 @@ class Loader {
         circuitIDSubscribers_ = be_->Map("circuit_id_subscribers");
         dhcpv6Bindings_ = be_->Map("dhcpv6_bindings");
         dhcpv6ServerConfig_ = be_->Map("dhcpv6_server_config");
+        ndConfig_ = be_->Map("nd_config");
+        ndBindings_ = be_->Map("nd_bindings");
         loaded_ = true;
         return ResetStats();
     }
     Error Close() { // idempotent, loader_test.go:989-1003
         loaded_ = false;
         subscriberPools_ = vlanSubscriberPools_ = ipPools_ = statsMap_ = serverConfigMap_ = circuitIDMap_ = circuitIDSubscribers_ = -1;
-        dhcpv6Bindings_ = dhcpv6ServerConfig_ = -1;
+        dhcpv6Bindings_ = dhcpv6ServerConfig_ = ndConfig_ = ndBindings_ = -1;
         be_.reset();
         return Nil();
     }
@@ -626,6 +744,30 @@ class Loader {
     Error EnableDHCPv6FastPath(bool on) {
         if (!be_ || !be_->ctx) return Error("dataplane not loaded");
         return MapErr("bng_dhcpv6_enable", bng_dhcpv6_enable(be_->ctx, on ? 1 : 0));
+    }
+
+    // Router and Neighbor Solicitations answered on the GPU (include/bng_b200.h, "nd_config" / "nd_bindings"): the RA
+    // template (slaac::BuildRA) and, per subscriber MAC, the subscriber's own prefix and lifetimes for its RA.
+    // AddNDBinding is staged (visible from the next batch) and returns -EINVAL for a binding the fast path could not
+    // use.  A subscriber without a binding is answered by the slow path; NS for router_ll needs none.
+    Error SetNDConfig(const bng_nd_config &c) {
+        if (ndConfig_ < 0) return Error("nd_config map not loaded");
+        uint32_t key = 0;
+        return MapErr("update", bng_map_update(be_->ctx, ndConfig_, &key, &c, BNG_ANY));
+    }
+    Error AddNDBinding(uint64_t mac, const bng_nd_binding &b) {
+        if (ndBindings_ < 0) return Error("nd_bindings map not loaded");
+        return MapErr("update", bng_map_update_staged(be_->ctx, ndBindings_, &mac, &b));
+    }
+    Error RemoveNDBinding(uint64_t mac) {
+        if (ndBindings_ < 0) return Error("nd_bindings map not loaded");
+        return MapErr("delete", bng_map_delete(be_->ctx, ndBindings_, &mac));
+    }
+    Result<bng_nd_binding> GetNDBinding(uint64_t mac) { return lookup<bng_nd_binding>(ndBindings_, "nd_bindings map not loaded", &mac); }
+    // bng_nd_enable: context state that no snapshot or delta carries, so a standby's Loader calls it too
+    Error EnableNDFastPath(bool on) {
+        if (!be_ || !be_->ctx) return Error("dataplane not loaded");
+        return MapErr("bng_nd_enable", bng_nd_enable(be_->ctx, on ? 1 : 0));
     }
 
     Error AddVLANSubscriber(uint16_t sTag, uint16_t cTag, const PoolAssignment &a) {
@@ -759,7 +901,8 @@ class Loader {
     std::shared_ptr<Backend> be_;
     bool loaded_ = false;
     int subscriberPools_ = -1, vlanSubscriberPools_ = -1, ipPools_ = -1, statsMap_ = -1, serverConfigMap_ = -1,
-        circuitIDMap_ = -1, circuitIDSubscribers_ = -1, dhcpv6Bindings_ = -1, dhcpv6ServerConfig_ = -1;
+        circuitIDMap_ = -1, circuitIDSubscribers_ = -1, dhcpv6Bindings_ = -1, dhcpv6ServerConfig_ = -1, ndConfig_ = -1,
+        ndBindings_ = -1;
 };
 
 } // namespace ebpf

@@ -42,7 +42,7 @@ namespace shard {
 enum class Route { ByMAC, ByPrivateIP, BySessionKey, ByEIMKey, ByReverseKey, ByValueIP, ByValueMAC, Replicated };
 
 inline Route RouteOf(const std::string &map) {
-    if (map == "subscriber_bindings" || map == "subscriber_pools") return Route::ByMAC;
+    if (map == "subscriber_bindings" || map == "subscriber_pools" || map == "nd_bindings") return Route::ByMAC;
     if (map == "subscriber_nat" || map == "qos_ingress" || map == "qos_egress") return Route::ByPrivateIP;
     if (map == "nat_sessions") return Route::BySessionKey; // struct nat_key: src_ip = the subscriber's address
     if (map == "eim_table") return Route::ByEIMKey;        // struct eim_key: internal_ip
@@ -483,6 +483,14 @@ class Router {
     int AntispoofIPv6PrefixesEnable(bool on) {
         for (auto &s : shards_)
             if (int r = bng_antispoof_ipv6_prefixes_enable(s->ctx, on ? 1 : 0)) return r;
+        return 0;
+    }
+    // Router and Neighbor Solicitations answered on the GPU (bng_nd_enable) on every shard.  nd_bindings is routed ByMAC
+    // and nd_config replicated, and upstream frames are steered by source MAC, so a subscriber's RS reaches the shard
+    // that holds its binding.  Returns 0 or the first shard's error.
+    int NDEnable(bool on) {
+        for (auto &s : shards_)
+            if (int r = bng_nd_enable(s->ctx, on ? 1 : 0)) return r;
         return 0;
     }
     // ICMP error translation in nat44_ingress (bng_nat_icmp_errors_enable) on every shard, and SteerDownstream sends an

@@ -142,6 +142,20 @@ dhcpv6_stats = np.dtype([(n, "<u8") for n in DHCPV6_STATS])
 assert bng_dhcpv6_client_key.itemsize == 32 and bng_dhcpv6_binding.itemsize == 64
 assert bng_dhcpv6_server_config.itemsize == 96 and dhcpv6_stats.itemsize == 96
 
+# include/bng_b200.h: Router and Neighbor Solicitations answered on the GPU (not reference maps).  nd_config: one
+# 320-byte entry (the RA template); nd_bindings: the subscriber_bindings MAC word -> binding (48 B); nd_stats:
+# BNG_ND_NUM_STATS u64 counters
+ND_PIO_L, ND_PIO_A = 0x80, 0x40
+bng_nd_config = np.dtype([
+    ("router_mac", "u1", 6), ("_pad0", "u1", 2), ("ra_head_len", "<u2"), ("ra_tail_len", "<u2"), ("_pad1", "u1", 4),
+    ("router_ll", "u1", 16), ("ra", "u1", 288)])
+bng_nd_binding = np.dtype([
+    ("prefix", "u1", 16), ("prefix_len", "u1"), ("pio_flags", "u1"), ("_pad0", "u1", 2), ("valid_lft", "<u4"),
+    ("preferred_lft", "<u4"), ("_pad1", "u1", 4), ("expires_s", "<u8"), ("_pad2", "u1", 8)])
+ND_STATS = ("total", "rs", "ns", "ra", "na", "miss", "expired", "not_target", "malformed", "unsupported", "no_room")
+nd_stats = np.dtype([(n, "<u8") for n in ND_STATS])
+assert bng_nd_config.itemsize == 320 and bng_nd_binding.itemsize == 48 and nd_stats.itemsize == 88
+
 # lawful-intercept record header (include/bng_b200.h: struct bng_li_record, 64 B); the captured bytes follow it
 LI_UPLINK, LI_DOWNLINK = 0, 1
 bng_li_record = np.dtype([
@@ -218,6 +232,9 @@ MAP_DTYPES = {
     "dhcpv6_bindings": (bng_dhcpv6_client_key, bng_dhcpv6_binding),
     "dhcpv6_server_config": ("<u4", bng_dhcpv6_server_config),
     "dhcpv6_stats": ("<u4", dhcpv6_stats),
+    "nd_bindings": ("<u8", bng_nd_binding),
+    "nd_config": ("<u4", bng_nd_config),
+    "nd_stats": ("<u4", nd_stats),
 }
 
 

@@ -344,3 +344,75 @@ def dhcpv6_duid(i: int, length: int = 14) -> bytes:
         v = (i * 2654435761) & ((1 << (8 * length)) - 1)
         b = bytearray(v.to_bytes(length, "big"))
     return bytes(b)
+
+
+# ---------------------------------------------------------------------------
+# ICMPv6 Router and Neighbor Solicitations (include/bng_b200.h: bng_nd_enable)
+# ---------------------------------------------------------------------------
+ALL_NODES = bytes.fromhex("ff020000000000000000000000000001")
+ALL_ROUTERS = bytes.fromhex("ff020000000000000000000000000002")
+
+
+def link_local(mac: bytes) -> bytes:
+    """The EUI-64 link-local address of a MAC (RFC 4291 appendix A)."""
+    return b"\xfe\x80" + bytes(6) + bytes([mac[0] ^ 2]) + mac[1:3] + b"\xff\xfe" + mac[3:6]
+
+
+def solicited_node(addr: bytes) -> bytes:
+    """ff02::1:ffXX:XXXX with the address's low 24 bits (RFC 4291 §2.7.1)."""
+    return bytes.fromhex("ff0200000000000000000001ff") + bytes(addr[13:16])
+
+
+def icmp6_checksum(src: bytes, dst: bytes, msg: bytes) -> int:
+    """The ICMPv6 checksum (RFC 4443 §2.3) of a message whose checksum field is 0."""
+    data = src + dst + len(msg).to_bytes(4, "big") + b"\x00\x00\x00\x3a" + msg
+    if len(data) & 1:
+        data += b"\x00"
+    s = int(np.frombuffer(data, ">u2").astype(np.uint64).sum())
+    while s >> 16:
+        s = (s & 0xFFFF) + (s >> 16)
+    return ~s & 0xFFFF
+
+
+def icmp6_frame(src_mac: bytes, msg: bytes, src_ip: bytes, dst_ip: bytes, dst_mac: bytes | None = None, tags=(),
+                hop_limit: int = 255, next_header: int = 58, checksum: bool = True) -> bytes:
+    """An Ethernet frame carrying one ICMPv6 message (bytes 2-3, the checksum, filled in unless checksum=False).
+    dst_mac defaults to the destination's multicast MAC (33:33 + its low 32 bits); tags: (tpid, vid) outermost first."""
+    if checksum:
+        msg = msg[:2] + b"\x00\x00" + msg[4:]
+        msg = msg[:2] + icmp6_checksum(src_ip, dst_ip, msg).to_bytes(2, "big") + msg[4:]
+    if dst_mac is None:
+        dst_mac = b"\x33\x33" + dst_ip[12:16]
+    ip = b"\x60\x00\x00\x00" + len(msg).to_bytes(2, "big") + bytes([next_header, hop_limit]) + src_ip + dst_ip
+    l2 = bytes(dst_mac) + bytes(src_mac)
+    for tpid, vid in tags:
+        l2 += tpid.to_bytes(2, "big") + (vid & 0xFFF).to_bytes(2, "big")
+    return l2 + b"\x86\xdd" + ip + msg
+
+
+def nd_option(kind: int, data: bytes) -> bytes:
+    """An ND option (RFC 4861 §4.6): type, length in units of 8 bytes, data padded to the length."""
+    n = (2 + len(data) + 7) // 8
+    return bytes([kind, n]) + data + bytes(n * 8 - 2 - len(data))
+
+
+def rs_frame(src_mac: bytes, src_ip: bytes | None = None, dst_ip: bytes = ALL_ROUTERS, slla: bool = True,
+             options: bytes = b"", code: int = 0, **kw) -> bytes:
+    """A Router Solicitation (RFC 4861 §4.1) from src_mac, from its link-local address unless src_ip is given, with a
+    Source Link-Layer Address option when slla."""
+    if src_ip is None:
+        src_ip = link_local(src_mac)
+    msg = bytes([133, code, 0, 0]) + bytes(4) + (nd_option(1, src_mac) if slla else b"") + options
+    return icmp6_frame(src_mac, msg, src_ip, dst_ip, **kw)
+
+
+def ns_frame(src_mac: bytes, target: bytes, src_ip: bytes | None = None, dst_ip: bytes | None = None, slla: bool = True,
+             options: bytes = b"", code: int = 0, **kw) -> bytes:
+    """A Neighbor Solicitation (RFC 4861 §4.3) for target, to its solicited-node address unless dst_ip is given; src_ip
+    defaults to src_mac's link-local address (pass bytes(16) for duplicate address detection)."""
+    if src_ip is None:
+        src_ip = link_local(src_mac)
+    if dst_ip is None:
+        dst_ip = solicited_node(target)
+    msg = bytes([135, code, 0, 0]) + bytes(4) + bytes(target) + (nd_option(1, src_mac) if slla else b"") + options
+    return icmp6_frame(src_mac, msg, src_ip, dst_ip, **kw)

@@ -784,6 +784,94 @@ typedef struct bng_dhcpv6_server_config {
 } bng_dhcpv6_server_config;
 int bng_dhcpv6_enable(bng_ctx *ctx, int on);
 
+/* ---- Router and Neighbor Solicitations (not one of the reference's maps or programs) ----
+ * dhcp_fastpath_prog answers a subscriber's IPv6 Router Solicitation with a Router Advertisement of its own (the
+ * shared options pkg/slaac's buildRA would send, plus the subscriber's own Prefix Information option), and a Neighbor
+ * Solicitation for the router's link-local address with a Neighbor Advertisement, on the GPU.  Three registry maps,
+ * carried by every generic path (update, batch, staged, delete, dump, clear, snapshot, restore, deltas):
+ *   - "nd_config": BPF_MAP_TYPE_ARRAY, one struct bng_nd_config (320 B).  ra[0, ra_head_len) is the RA message from its
+ *     type byte through the options that precede the per-subscriber prefix (RA header, Source Link-Layer Address, MTU,
+ *     the shared Prefix Information options); ra[ra_head_len, ra_head_len + ra_tail_len) the options that follow it
+ *     (RDNSS, DNSSL): buildRA's order, split where the subscriber's prefix goes.  ra_head_len 0 means unconfigured, and
+ *     then every byte past router_mac must be 0.  Otherwise an update returns -EINVAL unless ra_head_len >= 16 and a
+ *     multiple of 8, ra_tail_len a multiple of 8, head + tail <= 288, ra[0] = 134, ra[1] = 0, ra[2] = ra[3] = 0, each
+ *     part's option walk (length byte >= 1, in units of 8 bytes) ends exactly at the part's end, router_ll is in
+ *     fe80::/10, router_mac is a non-zero unicast address, and ra's bytes past head + tail are 0.  The GPU copies the
+ *     template; it does not interpret it.
+ *   - "nd_bindings": BPF_MAP_TYPE_HASH, key the 8-byte MAC word of subscriber_bindings, value struct bng_nd_binding
+ *     (48 B), max_entries = max_subscribers.  prefix_len 0: no per-subscriber prefix (a DHCPv6-managed subscriber still
+ *     gets its default route).  An update (plain, batch or staged) returns -EINVAL, and a batch applies none of its
+ *     entries, when prefix_len > 128, prefix has bits set past prefix_len, prefix_len is 0 with a non-zero prefix or
+ *     pio_flags, pio_flags has bits other than L (0x80) and A (0x40), or a pad byte is non-zero.
+ *   - "nd_stats": BPF_MAP_TYPE_ARRAY, one entry of BNG_ND_NUM_STATS u64 counters (the BNG_ND_ST_* order), stored after
+ *     dhcpv6_stats in the same device buffer; bng_sync_reduce all-reduces them.  bng_stats_device_ptr's count and
+ *     totals_out are unchanged.
+ * bng_sub_export carries the nd_bindings entries keyed by a MAC it is given, in an "nd_bindings" section written only
+ * when there is one; BNG_SUB_DETACH removes them and bng_sub_import inserts them.
+ * bng_nd_enable(ctx, on): on != 0 applies the rule below from the next bng_prog_run of dhcp_fastpath_prog; every other
+ * frame and program is unchanged.  Off by default; -EINVAL for a NULL ctx.  The flag is context state: snapshots,
+ * deltas and hand-over blobs do not carry it.  While nd_config is unconfigured, "on" launches exactly what "off"
+ * launches and counts nothing.
+ * The rule.  Bytes are "present" as far as frame_dlen goes, as for DHCPv6.  A frame that dhcp_one has found not to be
+ * IPv4 and that the DHCPv6 rule did not take (it needs next header 17) is a candidate when it is untagged or carries
+ * one or two tags parsed as for DHCPv4 and DHCPv6, its ethertype is 0x86DD, the 40-byte IPv6 header is present with
+ * version 6 and next header 58 (no extension headers), the first ICMPv6 byte is present, and it is a Router
+ * Solicitation (133) to ff02::2 or router_ll, or a Neighbor Solicitation (135) to router_ll or to router_ll's
+ * solicited-node address ff02::1:ffXX:XXXX.  Every other frame is untouched and counted nowhere new; stats_map counts
+ * every frame as it always did.  For a candidate, total += 1; the first of these that applies passes it (XDP_PASS,
+ * frame untouched, one counter):
+ *   1. unconfigured or len > 448: unsupported; payload length < 8 (RS) or < 24 (NS), or 40 + payload length past the
+ *      bytes present: malformed;
+ *   2. (from here on rs or ns also counts, whatever follows)
+ *   3. malformed (RFC 4861 §6.1.1, §7.1.1): hop limit != 255; ICMP code != 0; the ICMPv6 checksum over the
+ *      pseudo-header and payload length bytes does not sum to 0xFFFF; an option (after the 8-byte RS or 24-byte NS
+ *      body) of length 0 or running past the payload's end; more than 32 options; an unspecified (::) source with a
+ *      Source Link-Layer Address option; for NS, a multicast target, or an unspecified source sent to router_ll
+ *      rather than to its solicited-node address;
+ *   4. NS whose target is not router_ll: not_target (a subscriber's own duplicate address detection lands here);
+ *   5. RS with no nd_bindings entry for the Ethernet source: miss; RS with now_s > expires_s (now_s = the frame's
+ *      clock / 1e9): expired;
+ *   6. the reply does not fit the frame's storage (the stride, or len rounded up to 16 with an offset table): no_room.
+ * Otherwise the frame is answered in place: XDP_TX, len = the reply's length, ra or na += 1.  Ethernet dst = the
+ * request's source, src = router_mac, tags as they were; IPv6 0x60000000, payload length, next header 58, hop limit
+ * 255, src = router_ll, dst = the request's source, or ff02::1 when that is ::.  An RA is the template's head, then,
+ * when prefix_len > 0, the binding's Prefix Information option {3, 4, prefix_len, pio_flags, valid_lft,
+ * preferred_lft, 0, prefix}, then the template's tail, with the ICMPv6 checksum.  An NA is 32 bytes of ICMPv6: type
+ * 136, code 0, the checksum, flags R|S|O (0xE0), or R|O (0xA0) when the source is ::, three zero bytes, target =
+ * router_ll, and the Target Link-Layer Address option {2, 1, router_mac}.  The bytes from the reply's end to the next
+ * multiple of 16 (counted from the frame's start) are zeroed; every other byte of the frame's storage is unchanged.
+ * NS answers need no binding: they name only the router's own address.  The program writes no table, and no frame's
+ * outcome depends on another, so the rule holds frame by frame, wherever the frame sits in the batch.  The largest
+ * reply is 22 + 40 + 288 + 32 = 382 bytes. */
+#define BNG_ND_PIO_L 0x80
+#define BNG_ND_PIO_A 0x40
+#define BNG_ND_NUM_STATS 11
+enum {
+    BNG_ND_ST_TOTAL, BNG_ND_ST_RS, BNG_ND_ST_NS, BNG_ND_ST_RA, BNG_ND_ST_NA, BNG_ND_ST_MISS, BNG_ND_ST_EXPIRED,
+    BNG_ND_ST_NOT_TARGET, BNG_ND_ST_MALFORMED, BNG_ND_ST_UNSUPPORTED, BNG_ND_ST_NO_ROOM
+};
+typedef struct bng_nd_config {
+    uint8_t router_mac[6];   /* the replies' Ethernet source and Target Link-Layer Address */
+    uint8_t _pad0[2];
+    uint16_t ra_head_len;    /* 0 = unconfigured */
+    uint16_t ra_tail_len;
+    uint8_t _pad1[4];
+    uint8_t router_ll[16];   /* the router's link-local address: the replies' source, the NS target answered */
+    uint8_t ra[288];         /* head, then tail; the checksum bytes 0 */
+} bng_nd_config;
+typedef struct bng_nd_binding {
+    uint8_t prefix[16];      /* network order, zero past prefix_len */
+    uint8_t prefix_len;      /* 0 = no per-subscriber prefix */
+    uint8_t pio_flags;       /* BNG_ND_PIO_L | BNG_ND_PIO_A */
+    uint8_t _pad0[2];
+    uint32_t valid_lft;      /* seconds, host order */
+    uint32_t preferred_lft;
+    uint8_t _pad1[4];
+    uint64_t expires_s;      /* compared with the frame's clock / 1e9 */
+    uint8_t _pad2[8];
+} bng_nd_binding;
+int bng_nd_enable(bng_ctx *ctx, int on);
+
 /* ---- diagnostics ---- */
 uint64_t bng_launch_count(bng_ctx *ctx);  /* kernels launched by this context so far */
 /* Live subscriber_ipv6 entries per prefix length, counts[0..128]: the lengths the IPv6 lookup probes are those with a
