@@ -22,6 +22,7 @@
 #include <vector>
 
 #include "../../include/bng_b200.h"
+#include "blob.hpp"
 #include "kernels.h"
 
 namespace {
@@ -2533,77 +2534,137 @@ uint64_t bng_li_lost(bng_ctx *c) {
 }
 
 // ---------------------------------------------------------------------------
-// snapshot / restore (SURVEY.md §8f-4: device-table state for HA hand-over, reference pkg/ha)
-// A snapshot is a self-describing blob: header, then per map { name, kind, key size, value size, entry count,
-// keys, values } for every hash / array / LPM / statistics map (event rings are not state).  Restore clears
-// each map it finds in the blob and loads the entries through the ordinary update path, so derived state
-// (subscriber directory, the shared-memory image of the small maps) is rebuilt on the way and a snapshot
-// taken with one set of table capacities restores into another.
+// state blobs: snapshot / restore, incremental replication, subscriber hand-over.  All three share the section
+// framing of blob.hpp; each entry point keeps its own policy for the sections it reads.
 // ---------------------------------------------------------------------------
 namespace {
-const char kSnapMagic[8] = {'B', 'N', 'G', 'S', 'N', 'A', 'P', '2'};
-struct SnapMapHdr {
-    char name[40];
-    u32 kind, key_size, value_size, pad;
-    u64 count;
-};
-// Trailing section of the accounting records: (address, struct bng_acct) pairs.  No map has this name, so a library
-// without accounting steps over it; a context that never allocated records writes no such section.
-const char kSnapAcct[] = "subscriber_acct";
-const u32 kSnapAcctKind = 5;
-// Trailing section of the interception targets: (address, target id) pairs, by address.  Written by a context that
-// has used interception; the records are not state and stay out.
-const char kSnapLi[] = "li_targets";
-const u32 kSnapLiKind = 6;
-// Trailing section of the idle timeouts: (address, uint32 timeout_s) pairs, by address.  Written once idle records
-// exist; the clocks are not state (another node's clock, or this one's minutes ago, says nothing about activity now).
-const char kSnapIdle[] = "subscriber_idle";
-const u32 kSnapIdleKind = 7;
+using blob::kAcct, blob::kLi, blob::kIdle;
 
-// one (address, u32) section
-void put_pairs(std::vector<u8> &out, const char *name, u32 kind, const std::vector<u32> &a, const std::vector<u32> &v) {
-    SnapMapHdr h{};
-    snprintf(h.name, sizeof(h.name), "%s", name);
-    h.kind = kind, h.key_size = 4, h.value_size = 4, h.count = a.size();
-    out.insert(out.end(), (u8 *)&h, (u8 *)&h + sizeof(h));
-    out.insert(out.end(), (const u8 *)a.data(), (const u8 *)(a.data() + a.size()));
-    out.insert(out.end(), (const u8 *)v.data(), (const u8 *)(v.data() + v.size()));
+// a grow-only device buffer of at least `bytes`; keep: bytes at the start that survive the growth
+int dev_grow(bng_ctx *c, const char *what, u8 **p, u64 *cap, u64 bytes, u64 keep = 0) {
+    if (bytes <= *cap) return 0;
+    const u64 nb = std::max<u64>(bytes + bytes / 2, 1 << 20);
+    u8 *q = nullptr;
+    if (cudaMalloc((void **)&q, nb) != cudaSuccess) {
+        cudaGetLastError();
+        return fail(c, -ENOMEM, "%s: %llu bytes of device memory", what, (unsigned long long)nb);
+    }
+    if (keep) CU(c, cudaMemcpyAsync(q, *p, keep, cudaMemcpyDeviceToDevice, c->L.stream));
+    CU(c, cudaStreamSynchronize(c->L.stream));
+    if (*p) cudaFree(*p);
+    *p = q;
+    *cap = nb;
+    return 0;
+}
+
+// a non-event map, whole, as one section
+int map_section_locked(bng_ctx *c, MapReg *m, blob::Writer &w) {
+    u64 cnt = m->max_entries;
+    if (m->kind == KIND_HASH) {
+        u32 n32 = 0;
+        CU(c, cudaMemcpy(&n32, m->tbl->count, 4, cudaMemcpyDeviceToHost));
+        cnt = n32;
+    } else if (m->kind == KIND_LPM) {
+        cnt = m->lpm_host.size() / 3;
+    } else if (m->kind == KIND_STATS) {
+        cnt = 1;
+    }
+    std::vector<u8> keys((size_t)std::max<u64>(cnt, 1) * m->key_size), vals((size_t)std::max<u64>(cnt, 1) * m->value_size);
+    const int64_t got = cnt ? map_dump_locked(c, m, keys.data(), vals.data(), cnt) : 0;
+    if (got < 0) return (int)got;
+    w.section(m->name, (u32)m->kind, m->key_size, m->value_size, (u64)got, keys.data(), vals.data());
+    return 0;
+}
+
+// the interception targets, by address
+std::vector<std::pair<u32, u32>> li_sorted(const bng_ctx *c) {
+    std::vector<std::pair<u32, u32>> t(c->li_targets.begin(), c->li_targets.end());
+    std::sort(t.begin(), t.end());
+    return t;
+}
+
+void li_section(blob::Writer &w, const std::vector<std::pair<u32, u32>> &t) {
+    std::vector<u32> a, id;
+    for (const auto &e : t) a.push_back(e.first), id.push_back(e.second);
+    w.pairs(kLi, blob::kLiKind, a, id);
+}
+
+// a map emptied ahead of loading a blob's section into it
+int map_clear_for_load(bng_ctx *c, int id) {
+    MapReg *m = get_map(c, id);
+    if (m->kind == KIND_HASH) return bng_map_clear(c, id);
+    if (m->kind != KIND_LPM) return 0;
+    std::lock_guard<std::mutex> g(c->mu);
+    cudaSetDevice(c->device);
+    m->lpm_host.clear();
+    return lpm_upload(c, m);
+}
+
+// every accounting record and idle record at zero, no interception target: what a full load starts from
+int records_reset_locked(bng_ctx *c) {
+    if (c->acct) CU(c, cudaMemsetAsync(c->acct, 0, ((size_t)c->dev.subdir.mask + 1) * sizeof(bng_acct), c->L.stream));
+    if (c->idle) CU(c, cudaMemsetAsync(c->idle, 0, ((size_t)c->dev.subdir.mask + 1) * sizeof(bng_idle), c->L.stream));
+    CU(c, cudaStreamSynchronize(c->L.stream));
+    if (!c->li_targets.empty()) c->li_targets.clear(), c->li_dirty = true;
+    return 0;
+}
+
+size_t al256(size_t v) { return (v + 255) & ~(size_t)255; }
+
+// n (address, record) pairs into the addresses' directory slots, chunked through the staging buffers: accounting
+// records (rs = sizeof(bng_acct)) or whole idle records (rs = sizeof(bng_idle))
+int load_records_locked(bng_ctx *c, const u8 *addrs, const u8 *recs, u64 n, size_t rs) {
+    const bool acct = rs == sizeof(bng_acct);
+    if (int r = acct ? acct_alloc_locked(c) : idle_alloc_locked(c)) return r;
+    const u64 chunk_max = 1u << 16;
+    for (u64 done = 0; done < n; done += chunk_max) {
+        const u64 k = std::min(chunk_max, n - done);
+        const size_t roff = al256(k * 4);
+        if (int r = ensure_io(c, roff + k * rs)) return r;
+        memcpy(c->io_host, addrs + done * 4, k * 4);
+        memcpy(c->io_host + roff, recs + done * rs, k * rs);
+        CU(c, cudaMemcpyAsync(c->io_dev, c->io_host, roff + k * rs, cudaMemcpyHostToDevice, c->L.stream));
+        if (acct)
+            CU(c, run_acct_load(c->L, c->dev.subdir, c->acct, (const u32 *)c->io_dev, (const u64 *)(c->io_dev + roff), k));
+        else
+            CU(c, run_idle_load(c->L, c->dev.subdir, c->idle, (const u32 *)c->io_dev, (const u64 *)(c->io_dev + roff), k));
+        CU(c, cudaStreamSynchronize(c->L.stream));
+    }
+    return 0;
+}
+
+// n (address, target id) pairs into the interception targets; replace: they are the only targets afterwards
+int li_targets_load_locked(bng_ctx *c, const u8 *addrs, const u8 *ids, u64 n, bool replace) {
+    if (int r = li_alloc_locked(c)) return r;
+    if (replace) c->li_targets.clear();
+    for (u64 k = 0; k < n; k++) {
+        u32 a, id;
+        memcpy(&a, addrs + k * 4, 4);
+        memcpy(&id, ids + k * 4, 4);
+        c->li_targets[a] = id;
+    }
+    c->li_dirty = true;
+    return 0;
 }
 } // namespace
 
+// ---------------------------------------------------------------------------
+// snapshot / restore (SURVEY.md §8f-4: device-table state for HA hand-over, reference pkg/ha)
+// A snapshot is a self-describing blob: header, then one section per hash / array / LPM / statistics map (event rings
+// are not state), then the records.  Restore clears each map it finds in the blob and loads the entries through the
+// ordinary update path, so derived state (subscriber directory, the shared-memory image of the small maps) is rebuilt
+// on the way and a snapshot taken with one set of table capacities restores into another.
+// ---------------------------------------------------------------------------
 int64_t bng_snapshot(bng_ctx *c, void *buf, uint64_t cap) {
     if (!c) return -EINVAL;
     std::lock_guard<std::mutex> g(c->mu);
     cudaSetDevice(c->device);
     if (int fr = flush_staged_locked(c, -1)) return fr;
     CU(c, cudaStreamSynchronize(c->L.stream));
-    std::vector<u8> out(kSnapMagic, kSnapMagic + 8);
-    u64 nmaps = 0;
-    size_t nmaps_at = out.size();
-    out.resize(out.size() + 8);
-    for (size_t mi = 0; mi < c->maps.size(); mi++) {
-        MapReg *m = &c->maps[mi];
-        if (m->kind == KIND_EVENT) continue;
-        u64 cnt = m->max_entries;
-        if (m->kind == KIND_HASH) {
-            u32 n32 = 0;
-            CU(c, cudaMemcpy(&n32, m->tbl->count, 4, cudaMemcpyDeviceToHost));
-            cnt = n32;
-        } else if (m->kind == KIND_LPM) {
-            cnt = m->lpm_host.size() / 3;
-        } else if (m->kind == KIND_STATS) {
-            cnt = 1;
-        }
-        std::vector<u8> keys((size_t)std::max<u64>(cnt, 1) * m->key_size), vals((size_t)std::max<u64>(cnt, 1) * m->value_size);
-        int64_t got = cnt ? map_dump_locked(c, m, keys.data(), vals.data(), cnt) : 0;
-        if (got < 0) return got;
-        SnapMapHdr h{};
-        snprintf(h.name, sizeof(h.name), "%s", m->name);
-        h.kind = (u32)m->kind, h.key_size = m->key_size, h.value_size = m->value_size, h.count = (u64)got;
-        out.insert(out.end(), (u8 *)&h, (u8 *)&h + sizeof(h));
-        out.insert(out.end(), keys.begin(), keys.begin() + (size_t)got * m->key_size);
-        out.insert(out.end(), vals.begin(), vals.begin() + (size_t)got * m->value_size);
-        nmaps++;
+    blob::Writer w(16);
+    for (auto &m : c->maps) {
+        if (m.kind == KIND_EVENT) continue;
+        if (int r = map_section_locked(c, &m, w)) return r;
     }
     if (c->acct) {
         u32 n32 = 0;
@@ -2613,145 +2674,75 @@ int64_t bng_snapshot(bng_ctx *c, void *buf, uint64_t cap) {
         std::vector<bng_acct> recs(cnt);
         int64_t got = acct_dump_locked(c, addrs.data(), recs.data(), cnt);
         if (got < 0) return got;
-        SnapMapHdr h{};
-        snprintf(h.name, sizeof(h.name), "%s", kSnapAcct);
-        h.kind = kSnapAcctKind, h.key_size = 4, h.value_size = sizeof(bng_acct), h.count = (u64)got;
-        out.insert(out.end(), (u8 *)&h, (u8 *)&h + sizeof(h));
-        out.insert(out.end(), (u8 *)addrs.data(), (u8 *)(addrs.data() + got));
-        out.insert(out.end(), (u8 *)recs.data(), (u8 *)(recs.data() + got));
-        nmaps++;
+        w.section(kAcct, blob::kAcctKind, 4, sizeof(bng_acct), (u64)got, addrs.data(), recs.data());
     }
-    if (c->li_ctl) {
-        std::vector<std::pair<u32, u32>> t(c->li_targets.begin(), c->li_targets.end());
-        std::sort(t.begin(), t.end());
-        SnapMapHdr h{};
-        snprintf(h.name, sizeof(h.name), "%s", kSnapLi);
-        h.kind = kSnapLiKind, h.key_size = 4, h.value_size = 4, h.count = t.size();
-        out.insert(out.end(), (u8 *)&h, (u8 *)&h + sizeof(h));
-        for (auto &e : t) out.insert(out.end(), (u8 *)&e.first, (u8 *)&e.first + 4);
-        for (auto &e : t) out.insert(out.end(), (u8 *)&e.second, (u8 *)&e.second + 4);
-        nmaps++;
-    }
+    if (c->li_ctl) li_section(w, li_sorted(c));
     if (c->idle) {
         std::vector<u32> a, t;
         if (int r = idle_timeouts_dump_locked(c, &a, &t)) return r;
-        put_pairs(out, kSnapIdle, kSnapIdleKind, a, t);
-        nmaps++;
+        w.pairs(kIdle, blob::kIdleKind, a, t);
     }
-    memcpy(&out[nmaps_at], &nmaps, 8);
-    if (buf && cap >= out.size()) memcpy(buf, out.data(), out.size());
-    return (int64_t)out.size(); // the size needed; nothing was copied when cap is smaller
+    memcpy(w.out.data(), blob::kSnapMagic, 8);
+    memcpy(w.out.data() + 8, &w.sections, 8);
+    if (buf && cap >= w.out.size()) memcpy(buf, w.out.data(), w.out.size());
+    return (int64_t)w.out.size(); // the size needed; nothing was copied when cap is smaller
 }
 
 int bng_restore(bng_ctx *c, const void *buf, uint64_t len) {
-    if (!c || !buf || len < 16 || memcmp(buf, kSnapMagic, 8)) return -EINVAL;
-    const u8 *p = (const u8 *)buf, *end = p + len;
-    u64 nmaps;
-    memcpy(&nmaps, p + 8, 8);
-    p += 16;
-    { // the blob's records replace these; a blob without them leaves every record at zero
+    if (!c || !buf || len < 16 || memcmp(buf, blob::kSnapMagic, 8)) return -EINVAL;
+    u64 n;
+    memcpy(&n, (const u8 *)buf + 8, 8);
+    std::vector<blob::Section> secs;
+    std::string err;
+    if (!blob::read_sections((const u8 *)buf + 16, (const u8 *)buf + len, n, false, false, secs, err))
+        return fail(c, -EINVAL, "snapshot: %s", err.c_str());
+    // the whole blob is checked before anything changes: maps this library does not have are skipped, the records
+    // are taken once the maps (and so the directory) are in place
+    std::vector<std::pair<int, const blob::Section *>> maps;
+    const blob::Section *acct = nullptr, *li = nullptr, *idle = nullptr;
+    for (const blob::Section &s : secs) {
+        const blob::SectionHdr &h = s.h;
+        bool ok = h.key_size == 4;
+        if (!strcmp(h.name, kAcct)) {
+            ok = ok && h.value_size == sizeof(bng_acct), acct = &s;
+        } else if (!strcmp(h.name, kLi)) {
+            ok = ok && h.value_size == 4 && h.count <= BNG_LI_MAX_TARGETS, li = &s;
+        } else if (!strcmp(h.name, kIdle)) {
+            ok = ok && h.value_size == 4, idle = &s;
+        } else {
+            const int id = bng_map_id(c, h.name);
+            if (id < 0) continue;
+            const MapReg *m = get_map(c, id);
+            ok = m->key_size == h.key_size && m->value_size == h.value_size;
+            maps.emplace_back(id, &s);
+        }
+        if (!ok) return fail(c, -EINVAL, "snapshot: %s has another layout", h.name);
+    }
+    { // the blob's records replace these; a blob without them leaves every record at zero and every clock restarts
         std::lock_guard<std::mutex> g(c->mu);
         cudaSetDevice(c->device);
-        if (c->acct) {
-            CU(c, cudaMemsetAsync(c->acct, 0, ((size_t)c->dev.subdir.mask + 1) * sizeof(bng_acct), c->L.stream));
-            CU(c, cudaStreamSynchronize(c->L.stream));
-        }
-        if (!c->li_targets.empty()) { // the same for the interception targets
-            c->li_targets.clear();
-            c->li_dirty = true;
-        }
-        if (c->idle) { // and for the idle timeouts; every clock restarts
-            CU(c, cudaMemsetAsync(c->idle, 0, ((size_t)c->dev.subdir.mask + 1) * sizeof(bng_idle), c->L.stream));
-            CU(c, cudaStreamSynchronize(c->L.stream));
+        if (int r = records_reset_locked(c)) return r;
+    }
+    for (const auto &[id, s] : maps) {
+        if (int r = map_clear_for_load(c, id)) return r;
+        if (s->h.count) {
+            if (int r = bng_map_update_batch(c, id, s->keys, s->vals, s->h.count, BNG_ANY))
+                return fail(c, r, "snapshot: loading %s failed", s->h.name);
         }
     }
-    const u8 *acct_p = nullptr, *li_p = nullptr, *idle_p = nullptr;
-    u64 acct_n = 0, li_n = 0, idle_n = 0;
-    for (u64 k = 0; k < nmaps; k++) {
-        if (p + sizeof(SnapMapHdr) > end) return -EINVAL;
-        SnapMapHdr h;
-        memcpy(&h, p, sizeof(h));
-        p += sizeof(h);
-        h.name[sizeof(h.name) - 1] = 0;
-        const u64 kb = h.count * h.key_size, vb = h.count * h.value_size;
-        if (p + kb + vb > end) return -EINVAL;
-        if (!strcmp(h.name, kSnapAcct)) { // applied below, once the maps (and so the directory) are in place
-            if (h.key_size != 4 || h.value_size != sizeof(bng_acct)) return fail(c, -EINVAL, "snapshot: %s has another layout", h.name);
-            acct_p = p;
-            acct_n = h.count;
-            p += kb + vb;
-            continue;
-        }
-        if (!strcmp(h.name, kSnapLi)) {
-            if (h.key_size != 4 || h.value_size != 4 || h.count > BNG_LI_MAX_TARGETS)
-                return fail(c, -EINVAL, "snapshot: %s has another layout", h.name);
-            li_p = p;
-            li_n = h.count;
-            p += kb + vb;
-            continue;
-        }
-        if (!strcmp(h.name, kSnapIdle)) { // applied below, once the directory is in place
-            if (h.key_size != 4 || h.value_size != 4) return fail(c, -EINVAL, "snapshot: %s has another layout", h.name);
-            idle_p = p;
-            idle_n = h.count;
-            p += kb + vb;
-            continue;
-        }
-        int id = bng_map_id(c, h.name);
-        if (id >= 0) {
-            MapReg *m = get_map(c, id);
-            if (m->key_size != h.key_size || m->value_size != h.value_size) return fail(c, -EINVAL, "snapshot: %s has another layout", h.name);
-            if (m->kind == KIND_HASH) {
-                int r = bng_map_clear(c, id);
-                if (r) return r;
-            } else if (m->kind == KIND_LPM) {
-                std::lock_guard<std::mutex> g(c->mu);
-                cudaSetDevice(c->device);
-                m->lpm_host.clear();
-                int r = lpm_upload(c, m);
-                if (r) return r;
-            }
-            if (h.count) {
-                int r = bng_map_update_batch(c, id, p, p + kb, h.count, BNG_ANY);
-                if (r) return fail(c, r, "snapshot: loading %s failed", h.name);
-            }
-        }
-        p += kb + vb;
+    std::lock_guard<std::mutex> g(c->mu);
+    cudaSetDevice(c->device);
+    if (acct && acct->h.count) {
+        if (int r = load_records_locked(c, acct->keys, acct->vals, acct->h.count, sizeof(bng_acct))) return r;
     }
-    if (acct_n) {
-        std::lock_guard<std::mutex> g(c->mu);
-        cudaSetDevice(c->device);
-        if (int r = acct_alloc_locked(c)) return r;
-        const u64 chunk_max = 1u << 16;
-        for (u64 done = 0; done < acct_n; done += chunk_max) {
-            const u64 k = std::min(chunk_max, acct_n - done);
-            const size_t roff = (k * 4 + 255) & ~(size_t)255;
-            if (int r = ensure_io(c, roff + k * sizeof(bng_acct))) return r;
-            memcpy(c->io_host, acct_p + done * 4, k * 4);
-            memcpy(c->io_host + roff, acct_p + acct_n * 4 + done * sizeof(bng_acct), k * sizeof(bng_acct));
-            CU(c, cudaMemcpyAsync(c->io_dev, c->io_host, roff + k * sizeof(bng_acct), cudaMemcpyHostToDevice, c->L.stream));
-            CU(c, run_acct_load(c->L, c->dev.subdir, c->acct, (const u32 *)c->io_dev, (const u64 *)(c->io_dev + roff), k));
-            CU(c, cudaStreamSynchronize(c->L.stream));
-        }
+    if (li && li->h.count) {
+        if (int r = li_targets_load_locked(c, li->keys, li->vals, li->h.count, true)) return r;
     }
-    if (li_n) {
-        std::lock_guard<std::mutex> g(c->mu);
-        cudaSetDevice(c->device);
-        if (int r = li_alloc_locked(c)) return r;
-        for (u64 k = 0; k < li_n; k++) {
-            u32 a, id;
-            memcpy(&a, li_p + k * 4, 4);
-            memcpy(&id, li_p + li_n * 4 + k * 4, 4);
-            c->li_targets[a] = id;
-        }
-        c->li_dirty = true;
-    }
-    if (idle_p) {
-        std::lock_guard<std::mutex> g(c->mu);
-        cudaSetDevice(c->device);
-        std::vector<u32> a(idle_n), t(idle_n);
-        if (idle_n) memcpy(a.data(), idle_p, idle_n * 4), memcpy(t.data(), idle_p + idle_n * 4, idle_n * 4);
-        if (int r = idle_timeouts_locked(c, a.data(), t.data(), idle_n, nullptr)) return r;
+    if (idle) {
+        const u64 k = idle->h.count;
+        std::vector<u32> a(k), t(k);
+        if (k) memcpy(a.data(), idle->keys, k * 4), memcpy(t.data(), idle->vals, k * 4);
+        if (int r = idle_timeouts_locked(c, a.data(), t.data(), k, nullptr)) return r;
         if (int r = idle_restart_locked(c)) return r;
     }
     return 0;
@@ -2761,14 +2752,6 @@ int bng_restore(bng_ctx *c, const void *buf, uint64_t len) {
 // incremental replication (delta.cu; the blob is described in include/bng_b200.h)
 // ---------------------------------------------------------------------------
 namespace {
-const char kDeltaMagic[8] = {'B', 'N', 'G', 'D', 'E', 'L', 'T', '1'};
-struct DeltaHdr {
-    char magic[8];
-    u64 stream, seq_from, seq_to;
-    u32 flags, sections;
-};
-static_assert(sizeof(DeltaHdr) == 40 && sizeof(SnapMapHdr) == 64, "the delta framing of include/bng_b200.h");
-
 // shadow ids beside the hash maps' (map ids): the accounting records, the idle records
 const int kShadowAcct = -1, kShadowIdle = -2;
 
@@ -2830,7 +2813,7 @@ int delta_shadow_locked(bng_ctx *c, int map, const Tbl &t, u32 sw) {
     const size_t bytes = s.nslots * sw * 8;
     if (cudaMalloc((void **)&s.words, bytes) != cudaSuccess) {
         cudaGetLastError();
-        return fail(c, -ENOMEM, "delta_enable: %zu bytes of device memory for the shadow of %s", bytes, map == kShadowAcct ? kSnapAcct : (map == kShadowIdle ? kSnapIdle : c->maps[map].name));
+        return fail(c, -ENOMEM, "delta_enable: %zu bytes of device memory for the shadow of %s", bytes, map == kShadowAcct ? kAcct : (map == kShadowIdle ? kIdle : c->maps[map].name));
     }
     c->dshadow.push_back(s);
     CU(c, cudaMemsetAsync(s.words, 0xFF, bytes, c->L.stream)); // every slot empty: nothing sent yet
@@ -2851,30 +2834,6 @@ void delta_free_locked(bng_ctx *c) {
     cudaStreamSynchronize(c->L.stream);
     for (auto &s : c->dshadow) cudaFree(s.words);
     c->dshadow.clear();
-}
-
-// a grow-only device buffer of at least `bytes`; keep: bytes at the start that survive the growth
-int delta_grow(bng_ctx *c, u8 **p, u64 *cap, u64 bytes, u64 keep = 0) {
-    if (bytes <= *cap) return 0;
-    const u64 nb = std::max<u64>(bytes + bytes / 2, 1 << 20);
-    u8 *q = nullptr;
-    if (cudaMalloc((void **)&q, nb) != cudaSuccess) {
-        cudaGetLastError();
-        return fail(c, -ENOMEM, "delta_export: %llu bytes of device memory", (unsigned long long)nb);
-    }
-    if (keep) CU(c, cudaMemcpyAsync(q, *p, keep, cudaMemcpyDeviceToDevice, c->L.stream));
-    CU(c, cudaStreamSynchronize(c->L.stream));
-    if (*p) cudaFree(*p);
-    *p = q;
-    *cap = nb;
-    return 0;
-}
-
-void put_section(std::vector<u8> &out, const char *name, u32 kind, u32 ks, u32 vs, u32 n_del, u64 n_up) {
-    SnapMapHdr h{};
-    snprintf(h.name, sizeof(h.name), "%s", name);
-    h.kind = kind, h.key_size = ks, h.value_size = vs, h.pad = n_del, h.count = n_up;
-    out.insert(out.end(), (u8 *)&h, (u8 *)&h + sizeof(h));
 }
 } // namespace
 
@@ -2941,8 +2900,7 @@ int bng_delta_export(bng_ctx *c, uint64_t refresh_ns, uint32_t flags, void *buf,
         if ((r = delta_shadow_locked(c, kShadowIdle, c->dev.subdir, 2)) != 0) return r;
     }
     const bool full = (flags & BNG_DELTA_FULL) || c->delta_full, exact = flags & BNG_DELTA_EXACT;
-    std::vector<u8> out(sizeof(DeltaHdr));
-    u32 sections = 0;
+    blob::Writer w(sizeof(blob::DeltaHdr));
     struct Pending {
         DeltaTbl t;
         u64 at;
@@ -2960,54 +2918,40 @@ int bng_delta_export(bng_ctx *c, uint64_t refresh_ns, uint32_t flags, void *buf,
         CU(c, cudaMemcpyAsync(n, cnt, 8, cudaMemcpyDeviceToHost, c->L.stream));
         CU(c, cudaStreamSynchronize(c->L.stream));
         const u64 kb_del = (u64)n[0] * t.key_size, kb_up = (u64)n[1] * t.key_size, vb = (u64)n[1] * t.value_size;
-        if ((r = delta_grow(c, &c->demit, &c->demit_cap, kb_del + kb_up + vb)) != 0) return r;
-        if ((r = delta_grow(c, (u8 **)&c->dsent, &c->dsent_cap, (sent_used + n[0] + n[1]) * 4, sent_used * 4)) != 0) return r;
+        if ((r = dev_grow(c, "delta_export", &c->demit, &c->demit_cap, kb_del + kb_up + vb)) != 0) return r;
+        if ((r = dev_grow(c, "delta_export", (u8 **)&c->dsent, &c->dsent_cap, (sent_used + n[0] + n[1]) * 4, sent_used * 4)) != 0) return r;
         CU(c, run_delta_emit(c->L, t, del, n[0], up, n[1], c->demit, c->demit + kb_del, c->demit + kb_del + kb_up));
         if (n[0]) CU(c, cudaMemcpyAsync(c->dsent + sent_used, del, (u64)n[0] * 4, cudaMemcpyDeviceToDevice, c->L.stream));
         if (n[1]) CU(c, cudaMemcpyAsync(c->dsent + sent_used + n[0], up, (u64)n[1] * 4, cudaMemcpyDeviceToDevice, c->L.stream));
         commits.push_back({t, sent_used, n[0], n[1]});
         sent_used += n[0] + n[1];
         if (s.map == kShadowAcct)
-            put_section(out, kSnapAcct, kSnapAcctKind, 4, sizeof(bng_acct), n[0], n[1]);
+            w.header(kAcct, blob::kAcctKind, 4, sizeof(bng_acct), n[1], n[0]);
         else if (s.map == kShadowIdle)
-            put_section(out, kSnapIdle, kSnapIdleKind, 4, 4, n[0], n[1]);
+            w.header(kIdle, blob::kIdleKind, 4, 4, n[1], n[0]);
         else
-            put_section(out, c->maps[s.map].name, KIND_HASH, t.key_size, t.value_size, n[0], n[1]);
-        sections++;
-        const size_t at = out.size();
-        out.resize(at + kb_del + kb_up + vb);
-        if (out.size() > at) CU(c, cudaMemcpyAsync(out.data() + at, c->demit, kb_del + kb_up + vb, cudaMemcpyDeviceToHost, c->L.stream));
+            w.header(c->maps[s.map].name, KIND_HASH, t.key_size, t.value_size, n[1], n[0]);
+        const size_t at = w.out.size();
+        w.out.resize(at + kb_del + kb_up + vb);
+        if (w.out.size() > at) CU(c, cudaMemcpyAsync(w.out.data() + at, c->demit, kb_del + kb_up + vb, cudaMemcpyDeviceToHost, c->L.stream));
         CU(c, cudaStreamSynchronize(c->L.stream));
     }
     for (auto &m : c->maps) { // the small maps, whole
         if (m.kind == KIND_HASH || m.kind == KIND_EVENT) continue;
-        const u64 cnt_e = m.kind == KIND_LPM ? m.lpm_host.size() / 3 : (m.kind == KIND_STATS ? 1 : m.max_entries);
-        std::vector<u8> keys((size_t)std::max<u64>(cnt_e, 1) * m.key_size), vals((size_t)std::max<u64>(cnt_e, 1) * m.value_size);
-        const int64_t got = cnt_e ? map_dump_locked(c, &m, keys.data(), vals.data(), cnt_e) : 0;
-        if (got < 0) return (int)got;
-        put_section(out, m.name, (u32)m.kind, m.key_size, m.value_size, 0, (u64)got);
-        out.insert(out.end(), keys.begin(), keys.begin() + (size_t)got * m.key_size);
-        out.insert(out.end(), vals.begin(), vals.begin() + (size_t)got * m.value_size);
-        sections++;
+        if ((r = map_section_locked(c, &m, w)) != 0) return r;
     }
-    std::vector<std::pair<u32, u32>> li(c->li_targets.begin(), c->li_targets.end());
-    std::sort(li.begin(), li.end());
+    const std::vector<std::pair<u32, u32>> li = li_sorted(c);
     const bool li_send = c->li_ctl && (full || !c->delta_li_sent || li != c->delta_li);
-    if (li_send) {
-        put_section(out, kSnapLi, kSnapLiKind, 4, 4, 0, li.size());
-        for (auto &e : li) out.insert(out.end(), (u8 *)&e.first, (u8 *)&e.first + 4);
-        for (auto &e : li) out.insert(out.end(), (u8 *)&e.second, (u8 *)&e.second + 4);
-        sections++;
-    }
-    DeltaHdr h{};
-    memcpy(h.magic, kDeltaMagic, 8);
+    if (li_send) li_section(w, li);
+    blob::DeltaHdr h{};
+    memcpy(h.magic, blob::kDeltaMagic, 8);
     h.stream = c->delta_stream, h.seq_from = c->delta_seq, h.seq_to = c->delta_seq + 1;
-    h.flags = (full ? BNG_DELTA_FULL : 0) | (exact ? BNG_DELTA_EXACT : 0), h.sections = sections;
-    memcpy(out.data(), &h, sizeof(h));
-    *len_out = out.size();
+    h.flags = (full ? BNG_DELTA_FULL : 0) | (exact ? BNG_DELTA_EXACT : 0), h.sections = (u32)w.sections;
+    memcpy(w.out.data(), &h, sizeof(h));
+    *len_out = w.out.size();
     prof_collect(c->L);
-    if (cap < out.size()) return -ENOSPC; // the shadows are as they were: the next call covers the same changes
-    memcpy(buf, out.data(), out.size());
+    if (cap < w.out.size()) return -ENOSPC; // the shadows are as they were: the next call covers the same changes
+    memcpy(buf, w.out.data(), w.out.size());
     // the baseline moves to what this delta carries
     if (full)
         for (const auto &s : c->dshadow) CU(c, cudaMemsetAsync(s.words, 0xFF, s.nslots * s.sw * 8, c->L.stream));
@@ -3021,49 +2965,37 @@ int bng_delta_export(bng_ctx *c, uint64_t refresh_ns, uint32_t flags, void *buf,
 }
 
 int bng_delta_apply(bng_ctx *c, const void *buf, uint64_t len) {
-    if (!c || !buf || len < sizeof(DeltaHdr)) return -EINVAL;
-    DeltaHdr h;
+    if (!c || !buf || len < sizeof(blob::DeltaHdr)) return -EINVAL;
+    blob::DeltaHdr h;
     memcpy(&h, buf, sizeof(h));
-    if (memcmp(h.magic, kDeltaMagic, 8)) return fail(c, -EINVAL, "delta_apply: not a delta");
+    if (memcmp(h.magic, blob::kDeltaMagic, 8)) return fail(c, -EINVAL, "delta_apply: not a delta");
     const bool full = h.flags & BNG_DELTA_FULL;
-    // the whole blob is checked before anything changes
-    struct Sec {
-        SnapMapHdr h;
-        const u8 *p;
+    std::vector<blob::Section> all;
+    std::string err;
+    if (!blob::read_sections((const u8 *)buf + sizeof(h), (const u8 *)buf + len, h.sections, true, false, all, err))
+        return fail(c, -EINVAL, "delta_apply: %s", err.c_str());
+    // the whole blob is checked before anything changes; maps this library does not have are skipped
+    enum { ACCT = -2, LI = -3, IDLE = -4 };
+    std::vector<std::pair<int, const blob::Section *>> secs;
+    for (const blob::Section &s : all) {
+        const blob::SectionHdr &sh = s.h;
+        if (sh.count > (1ull << 40) || sh.key_size > 64 || sh.value_size > 4096)
+            return fail(c, -EINVAL, "delta_apply: %s has a bad header", sh.name);
         int id;
-    };
-    std::vector<Sec> secs;
-    const u8 *p = (const u8 *)buf + sizeof(h), *end = (const u8 *)buf + len;
-    for (u32 k = 0; k < h.sections; k++) {
-        Sec s{};
-        if ((u64)(end - p) < sizeof(SnapMapHdr)) return fail(c, -EINVAL, "delta_apply: truncated");
-        memcpy(&s.h, p, sizeof(s.h));
-        p += sizeof(s.h);
-        s.h.name[sizeof(s.h.name) - 1] = 0;
-        if (s.h.count > (1ull << 40) || s.h.key_size > 64 || s.h.value_size > 4096)
-            return fail(c, -EINVAL, "delta_apply: %s has a bad header", s.h.name);
-        const u64 need = (u64)s.h.pad * s.h.key_size + s.h.count * (s.h.key_size + s.h.value_size);
-        if ((u64)(end - p) < need) return fail(c, -EINVAL, "delta_apply: %s is truncated", s.h.name);
-        s.p = p;
-        p += need;
-        if (!strcmp(s.h.name, kSnapAcct)) {
-            if (s.h.key_size != 4 || s.h.value_size != sizeof(bng_acct)) return fail(c, -EINVAL, "delta_apply: %s has another layout", s.h.name);
-            s.id = -2;
-        } else if (!strcmp(s.h.name, kSnapLi)) {
-            if (s.h.key_size != 4 || s.h.value_size != 4 || s.h.count > BNG_LI_MAX_TARGETS)
-                return fail(c, -EINVAL, "delta_apply: %s has another layout", s.h.name);
-            s.id = -3;
-        } else if (!strcmp(s.h.name, kSnapIdle)) {
-            if (s.h.key_size != 4 || s.h.value_size != 4) return fail(c, -EINVAL, "delta_apply: %s has another layout", s.h.name);
-            s.id = -4;
+        bool ok = sh.key_size == 4;
+        if (!strcmp(sh.name, kAcct)) {
+            id = ACCT, ok = ok && sh.value_size == sizeof(bng_acct);
+        } else if (!strcmp(sh.name, kLi)) {
+            id = LI, ok = ok && sh.value_size == 4 && sh.count <= BNG_LI_MAX_TARGETS;
+        } else if (!strcmp(sh.name, kIdle)) {
+            id = IDLE, ok = ok && sh.value_size == 4;
         } else {
-            s.id = bng_map_id(c, s.h.name);
-            if (s.id < 0) continue; // a map this library does not have
-            const MapReg *m = get_map(c, s.id);
-            if (m->key_size != s.h.key_size || m->value_size != s.h.value_size || (u32)m->kind != s.h.kind || (m->kind != KIND_HASH && s.h.pad))
-                return fail(c, -EINVAL, "delta_apply: %s has another layout", s.h.name);
+            if ((id = bng_map_id(c, sh.name)) < 0) continue;
+            const MapReg *m = get_map(c, id);
+            ok = m->key_size == sh.key_size && m->value_size == sh.value_size && (u32)m->kind == sh.kind && (m->kind == KIND_HASH || !s.n_del);
         }
-        secs.push_back(s);
+        if (!ok) return fail(c, -EINVAL, "delta_apply: %s has another layout", sh.name);
+        secs.emplace_back(id, &s);
     }
     {
         std::lock_guard<std::mutex> g(c->mu);
@@ -3073,69 +3005,40 @@ int bng_delta_apply(bng_ctx *c, const void *buf, uint64_t len) {
                         (unsigned long long)h.seq_from, (unsigned long long)c->dapply_stream, (unsigned long long)c->dapply_seq);
         c->dapply_stream = 0; // until this apply has completed, only a FULL delta is accepted
         if (full) {
-            if (c->acct) CU(c, cudaMemsetAsync(c->acct, 0, ((size_t)c->dev.subdir.mask + 1) * sizeof(bng_acct), c->L.stream));
-            if (c->idle) CU(c, cudaMemsetAsync(c->idle, 0, ((size_t)c->dev.subdir.mask + 1) * sizeof(bng_idle), c->L.stream));
-            CU(c, cudaStreamSynchronize(c->L.stream));
-            if (!c->li_targets.empty()) c->li_targets.clear(), c->li_dirty = true;
+            if (int r = records_reset_locked(c)) return r;
         }
     }
-    for (const Sec &s : secs) {
-        if (s.id < 0) continue;
-        MapReg *m = get_map(c, s.id);
-        const u8 *dk = s.p, *uk = dk + (u64)s.h.pad * s.h.key_size, *uv = uk + s.h.count * s.h.key_size;
-        if (m->kind == KIND_HASH) {
-            if (full) {
-                if (int r = bng_map_clear(c, s.id)) return r;
-            }
-            if (s.h.pad) {
-                std::lock_guard<std::mutex> g(c->mu);
-                cudaSetDevice(c->device);
-                if (int r = flush_staged_locked(c, s.id)) return r;
-                int first = 0; // a key the standby no longer has is no error
-                if (int r = hash_cmd(c, m, TOP_DELETE, dk, nullptr, s.h.pad, 0, &first)) return r;
-                if (feeds_small_tabs(m)) c->small_dirty = true;
-            }
-        } else if (m->kind == KIND_LPM) {
+    for (const auto &[id, s] : secs) {
+        if (id < 0) continue;
+        MapReg *m = get_map(c, id);
+        if (full || m->kind != KIND_HASH) {
+            if (int r = map_clear_for_load(c, id)) return r;
+        }
+        if (s->n_del) {
             std::lock_guard<std::mutex> g(c->mu);
             cudaSetDevice(c->device);
-            m->lpm_host.clear();
-            if (int r = lpm_upload(c, m)) return r;
+            if (int r = flush_staged_locked(c, id)) return r;
+            int first = 0; // a key the standby no longer has is no error
+            if (int r = hash_cmd(c, m, TOP_DELETE, s->dels, nullptr, s->n_del, 0, &first)) return r;
+            if (feeds_small_tabs(m)) c->small_dirty = true;
         }
-        if (s.h.count) {
-            if (int r = bng_map_update_batch(c, s.id, uk, uv, s.h.count, BNG_ANY)) return fail(c, r, "delta_apply: loading %s failed", s.h.name);
+        if (s->h.count) {
+            if (int r = bng_map_update_batch(c, id, s->keys, s->vals, s->h.count, BNG_ANY)) return fail(c, r, "delta_apply: loading %s failed", s->h.name);
         }
     }
+    // after the maps: the records go to the addresses' directory slots
     std::lock_guard<std::mutex> g(c->mu);
     cudaSetDevice(c->device);
-    for (const Sec &s : secs) {
-        const u8 *uk = s.p + (u64)s.h.pad * s.h.key_size, *uv = uk + s.h.count * s.h.key_size;
-        if (s.id == -2 && s.h.count) { // after the maps: the records go to the addresses' directory slots
-            if (int r = acct_alloc_locked(c)) return r;
-            const u64 chunk_max = 1u << 16;
-            for (u64 done = 0; done < s.h.count; done += chunk_max) {
-                const u64 k = std::min(chunk_max, s.h.count - done);
-                const size_t roff = (k * 4 + 255) & ~(size_t)255;
-                if (int r = ensure_io(c, roff + k * sizeof(bng_acct))) return r;
-                memcpy(c->io_host, uk + done * 4, k * 4);
-                memcpy(c->io_host + roff, uv + done * sizeof(bng_acct), k * sizeof(bng_acct));
-                CU(c, cudaMemcpyAsync(c->io_dev, c->io_host, roff + k * sizeof(bng_acct), cudaMemcpyHostToDevice, c->L.stream));
-                CU(c, run_acct_load(c->L, c->dev.subdir, c->acct, (const u32 *)c->io_dev, (const u64 *)(c->io_dev + roff), k));
-                CU(c, cudaStreamSynchronize(c->L.stream));
-            }
-        } else if (s.id == -3) {
-            if (int r = li_alloc_locked(c)) return r;
-            c->li_targets.clear();
-            for (u64 k = 0; k < s.h.count; k++) {
-                u32 a, id;
-                memcpy(&a, uk + k * 4, 4);
-                memcpy(&id, uv + k * 4, 4);
-                c->li_targets[a] = id;
-            }
-            c->li_dirty = true;
-        } else if (s.id == -4) {
-            std::vector<u32> a(s.h.count), t(s.h.count);
-            if (s.h.count) memcpy(a.data(), uk, s.h.count * 4), memcpy(t.data(), uv, s.h.count * 4);
-            if (int r = idle_timeouts_locked(c, a.data(), t.data(), s.h.count, nullptr)) return r;
+    for (const auto &[id, s] : secs) {
+        const u64 n = s->h.count;
+        if (id == ACCT && n) {
+            if (int r = load_records_locked(c, s->keys, s->vals, n, sizeof(bng_acct))) return r;
+        } else if (id == LI) {
+            if (int r = li_targets_load_locked(c, s->keys, s->vals, n, true)) return r;
+        } else if (id == IDLE) {
+            std::vector<u32> a(n), t(n);
+            if (n) memcpy(a.data(), s->keys, n * 4), memcpy(t.data(), s->vals, n * 4);
+            if (int r = idle_timeouts_locked(c, a.data(), t.data(), n, nullptr)) return r;
         }
     }
     // every clock restarts: at a takeover no clock here started before the last delta applied
@@ -3159,54 +3062,10 @@ int bng_delta_info(bng_ctx *c, uint64_t *stream_id, uint64_t *seq) {
 // subscriber hand-over between contexts (move.cu; the blob is described in include/bng_b200.h)
 // ---------------------------------------------------------------------------
 namespace {
-const char kMoveMagic[8] = {'B', 'N', 'G', 'M', 'O', 'V', 'E', '1'};
-// Whole idle records, (address, struct bng_idle): a name of its own, so that bng_restore and bng_delta_apply, which
-// take only timeouts under kSnapIdle, step over it.
-const char kMoveIdle[] = "subscriber_idle_rec";
-const u32 kMoveIdleKind = 8;
 // what a subscriber owns: maps keyed by its address, by its MAC, and the flow tables (selected by k_move_select)
 const char *const kMoveAddrMaps[] = {"subscriber_nat", "qos_ingress", "qos_egress"};
 const char *const kMoveMacMaps[] = {"subscriber_bindings", "subscriber_pools"};
 const char *const kMoveFlowMaps[] = {"nat_sessions", "nat_reverse", "eim_table"};
-
-size_t al256(size_t v) { return (v + 255) & ~(size_t)255; }
-
-// the staging buffer of bng_sub_export, grown to `bytes` with its first `keep` bytes kept
-int mv_grow(bng_ctx *c, u64 bytes, u64 keep) {
-    if (bytes <= c->mv_cap) return 0;
-    const u64 nb = std::max<u64>(bytes + bytes / 4, 1 << 20);
-    u8 *q = nullptr;
-    if (cudaMalloc((void **)&q, nb) != cudaSuccess) {
-        cudaGetLastError();
-        return fail(c, -ENOMEM, "sub_export: %llu bytes of device memory", (unsigned long long)nb);
-    }
-    if (keep) CU(c, cudaMemcpyAsync(q, c->mv_buf, keep, cudaMemcpyDeviceToDevice, c->L.stream));
-    CU(c, cudaStreamSynchronize(c->L.stream));
-    if (c->mv_buf) cudaFree(c->mv_buf);
-    c->mv_buf = q;
-    c->mv_cap = nb;
-    return 0;
-}
-
-// n (address, record) pairs into the addresses' directory slots, chunked through the staging buffers: accounting
-// records (rs = sizeof(bng_acct)) or whole idle records (rs = sizeof(bng_idle))
-int mv_load_records_locked(bng_ctx *c, const u8 *addrs, const u8 *recs, u64 n, size_t rs) {
-    const u64 chunk_max = 1u << 16;
-    for (u64 done = 0; done < n; done += chunk_max) {
-        const u64 k = std::min(chunk_max, n - done);
-        const size_t roff = al256(k * 4);
-        if (int r = ensure_io(c, roff + k * rs)) return r;
-        memcpy(c->io_host, addrs + done * 4, k * 4);
-        memcpy(c->io_host + roff, recs + done * rs, k * rs);
-        CU(c, cudaMemcpyAsync(c->io_dev, c->io_host, roff + k * rs, cudaMemcpyHostToDevice, c->L.stream));
-        if (rs == sizeof(bng_acct))
-            CU(c, run_acct_load(c->L, c->dev.subdir, c->acct, (const u32 *)c->io_dev, (const u64 *)(c->io_dev + roff), k));
-        else
-            CU(c, run_idle_load(c->L, c->dev.subdir, c->idle, (const u32 *)c->io_dev, (const u64 *)(c->io_dev + roff), k));
-        CU(c, cudaStreamSynchronize(c->L.stream));
-    }
-    return 0;
-}
 } // namespace
 
 int bng_sub_export(bng_ctx *c, const uint32_t *addrs, uint64_t n_addrs, const uint64_t *macs, uint64_t n_macs, uint32_t flags,
@@ -3259,7 +3118,7 @@ int bng_sub_export(bng_ctx *c, const uint32_t *addrs, uint64_t n_addrs, const ui
     size_t nd_v = 0, nd_r = 0;
     if (nd) nd_v = at, nd_r = al256(at + nm * ndm->value_size), at = al256(nd_r + nm * 4);
     const size_t flow0 = at;
-    if (int r = mv_grow(c, flow0, 0)) return r;
+    if (int r = dev_grow(c, "sub_export", &c->mv_buf, &c->mv_cap, flow0)) return r;
     // the inputs are built in the pinned staging buffer and copied on the context's stream, ahead of the kernels that
     // read them (as bng_nat_flush does)
     if (int r = ensure_io(c, out0)) return r;
@@ -3301,7 +3160,7 @@ int bng_sub_export(bng_ctx *c, const uint32_t *addrs, uint64_t n_addrs, const ui
     const u32 n6 = n4[4];
     const size_t v6k = at, v6v = al256(v6k + (size_t)n6 * LPM6_KEY), v6r = al256(v6v + (size_t)n6 * 4); // v6r: the detach's results
     if (n6) at = al256(v6r + (size_t)n6 * 4);
-    if (int r = mv_grow(c, at, flow0)) return r;
+    if (int r = dev_grow(c, "sub_export", &c->mv_buf, &c->mv_cap, at, flow0)) return r;
     dv = c->mv_buf;
     for (int k = 0; k < 3 && c->mv_lists; k++) {
         const u32 *lists[3] = {c->mv_lists, c->mv_lists + ns, c->mv_lists + ns + nr};
@@ -3323,9 +3182,7 @@ int bng_sub_export(bng_ctx *c, const uint32_t *addrs, uint64_t n_addrs, const ui
     prof_collect(c->L);
     auto host = [&](size_t off) { return got.data() + (off - out0); };
     // the blob: snapshot framing, one section per map, then the records and the interception targets
-    std::vector<u8> out(kMoveMagic, kMoveMagic + 8);
-    out.resize(16);
-    u64 nsec = 0;
+    blob::Writer w(16);
     auto by_key = [&](MapReg *m, const u8 *keys, u64 n, size_t voff, size_t roff, bool skip_empty = false) {
         const int *res = (const int *)host(roff);
         const u8 *vals = host(voff);
@@ -3337,10 +3194,7 @@ int bng_sub_export(bng_ctx *c, const uint32_t *addrs, uint64_t n_addrs, const ui
             }
         const u64 k = kv.size() / m->key_size;
         if (skip_empty && !k) return false;
-        put_section(out, m->name, KIND_HASH, m->key_size, m->value_size, 0, k);
-        out.insert(out.end(), kv.begin(), kv.end());
-        out.insert(out.end(), vv.begin(), vv.end());
-        nsec++;
+        w.section(m->name, KIND_HASH, m->key_size, m->value_size, k, kv.data(), vv.data());
         return true;
     };
     for (int k = 0; k < 3; k++) by_key(am[k], (const u8 *)A.data(), na, am_v[k], am_r[k]);
@@ -3349,31 +3203,21 @@ int bng_sub_export(bng_ctx *c, const uint32_t *addrs, uint64_t n_addrs, const ui
     const bool nd_sec = nd && by_key(ndm, (const u8 *)M.data(), nm, nd_v, nd_r, true);
     for (int k = 0; k < 3; k++) {
         const MapReg *m = fm[k];
-        put_section(out, m->name, KIND_HASH, m->key_size, m->value_size, 0, n4[k]);
-        out.insert(out.end(), host(fk[k]), host(fk[k]) + (size_t)n4[k] * m->key_size);
-        out.insert(out.end(), host(fv[k]), host(fv[k]) + (size_t)n4[k] * m->value_size);
-        nsec++;
+        w.section(m->name, KIND_HASH, m->key_size, m->value_size, n4[k], host(fk[k]), host(fv[k]));
     }
     const MapReg *m6 = get_map(c, bng_map_id(c, "subscriber_ipv6"));
-    if (n6) { // only when there is one, so that blobs without IPv6 prefixes stay as they were
-        put_section(out, m6->name, KIND_HASH, m6->key_size, m6->value_size, 0, n6);
-        out.insert(out.end(), host(v6k), host(v6k) + (size_t)n6 * LPM6_KEY);
-        out.insert(out.end(), host(v6v), host(v6v) + (size_t)n6 * 4);
-        nsec++;
-    }
+    // only when there is one, so that blobs without IPv6 prefixes stay as they were
+    if (n6) w.section(m6->name, KIND_HASH, m6->key_size, m6->value_size, n6, host(v6k), host(v6v));
     auto records = [&](const char *name, u32 kind, size_t rs, size_t voff, size_t roff) {
         const int *res = (const int *)host(roff);
         std::vector<u32> a;
         std::vector<u8> v;
         for (u64 i = 0; i < na; i++)
             if (res[i] == 0) a.push_back(A[i]), v.insert(v.end(), host(voff) + i * rs, host(voff) + (i + 1) * rs);
-        put_section(out, name, kind, 4, (u32)rs, 0, a.size());
-        out.insert(out.end(), (const u8 *)a.data(), (const u8 *)(a.data() + a.size()));
-        out.insert(out.end(), v.begin(), v.end());
-        nsec++;
+        w.section(name, kind, 4, (u32)rs, a.size(), a.data(), v.data());
     };
-    if (c->acct) records(kSnapAcct, kSnapAcctKind, sizeof(bng_acct), acct_v, acct_r);
-    if (c->idle) records(kMoveIdle, kMoveIdleKind, sizeof(bng_idle), idle_v, idle_r);
+    if (c->acct) records(kAcct, blob::kAcctKind, sizeof(bng_acct), acct_v, acct_r);
+    if (c->idle) records(blob::kIdleRec, blob::kIdleRecKind, sizeof(bng_idle), idle_v, idle_r);
     std::vector<u32> li_a;
     if (c->li_ctl) {
         std::vector<u32> ids;
@@ -3381,13 +3225,13 @@ int bng_sub_export(bng_ctx *c, const uint32_t *addrs, uint64_t n_addrs, const ui
             auto it = c->li_targets.find(a);
             if (it != c->li_targets.end()) li_a.push_back(a), ids.push_back(it->second);
         }
-        put_pairs(out, kSnapLi, kSnapLiKind, li_a, ids);
-        nsec++;
+        w.pairs(kLi, blob::kLiKind, li_a, ids);
     }
-    memcpy(&out[8], &nsec, 8);
-    *len_out = out.size();
-    if (cap < out.size()) return -ENOSPC; // nothing written, nothing removed
-    memcpy(buf, out.data(), out.size());
+    memcpy(w.out.data(), blob::kMoveMagic, 8);
+    memcpy(w.out.data() + 8, &w.sections, 8);
+    *len_out = w.out.size();
+    if (cap < w.out.size()) return -ENOSPC; // nothing written, nothing removed
+    memcpy(buf, w.out.data(), w.out.size());
     if (!(flags & BNG_SUB_DETACH)) return 0;
     // Detach exactly what was exported: the listed flow slots, then the keyed entries through the table-op path (the
     // subscriber directory follows subscriber_nat and qos_ingress, and with it the records' lifetime).  Every input is
@@ -3422,58 +3266,46 @@ int bng_sub_export(bng_ctx *c, const uint32_t *addrs, uint64_t n_addrs, const ui
 
 int bng_sub_import(bng_ctx *c, const void *buf, uint64_t len) {
     if (!c) return -EINVAL;
-    if (!buf || len < 16 || memcmp(buf, kMoveMagic, 8)) return fail(c, -EINVAL, "sub_import: not a hand-over blob");
-    // the whole blob is checked before anything changes
-    struct Sec {
-        SnapMapHdr h;
-        const u8 *p;
-        int id; // map id, or -1 accounting records, -2 idle records, -3 interception targets
-    };
-    std::vector<Sec> secs;
-    u64 nsec;
-    memcpy(&nsec, (const u8 *)buf + 8, 8);
-    const u8 *p = (const u8 *)buf + 16, *end = (const u8 *)buf + len;
-    for (u64 k = 0; k < nsec; k++) {
-        Sec s{};
-        if ((u64)(end - p) < sizeof(SnapMapHdr)) return fail(c, -EINVAL, "sub_import: truncated");
-        memcpy(&s.h, p, sizeof(s.h));
-        p += sizeof(s.h);
-        s.h.name[sizeof(s.h.name) - 1] = 0;
-        const u64 per = (u64)s.h.key_size + s.h.value_size;
-        if (per == 0 || s.h.count > (u64)(end - p) / per) return fail(c, -EINVAL, "sub_import: %s is truncated", s.h.name);
-        s.p = p;
-        p += s.h.count * per;
-        if (!strcmp(s.h.name, kSnapAcct)) {
-            if (s.h.kind != kSnapAcctKind || s.h.key_size != 4 || s.h.value_size != sizeof(bng_acct)) s.id = -100;
-            else s.id = -1;
-        } else if (!strcmp(s.h.name, kMoveIdle)) {
-            if (s.h.kind != kMoveIdleKind || s.h.key_size != 4 || s.h.value_size != sizeof(bng_idle)) s.id = -100;
-            else s.id = -2;
-        } else if (!strcmp(s.h.name, kSnapLi)) {
-            if (s.h.kind != kSnapLiKind || s.h.key_size != 4 || s.h.value_size != 4 || s.h.count > BNG_LI_MAX_TARGETS) s.id = -100;
-            else s.id = -3;
+    if (!buf || len < 16 || memcmp(buf, blob::kMoveMagic, 8)) return fail(c, -EINVAL, "sub_import: not a hand-over blob");
+    u64 n;
+    memcpy(&n, (const u8 *)buf + 8, 8);
+    std::vector<blob::Section> all;
+    std::string err;
+    if (!blob::read_sections((const u8 *)buf + 16, (const u8 *)buf + len, n, false, true, all, err))
+        return fail(c, -EINVAL, "sub_import: %s", err.c_str());
+    // the whole blob is checked before anything changes: every section must be one this library writes
+    enum { ACCT = -1, IDLE = -2, LI = -3 };
+    std::vector<std::pair<int, const blob::Section *>> secs;
+    for (const blob::Section &s : all) {
+        const blob::SectionHdr &sh = s.h;
+        int id;
+        bool ok = sh.key_size == 4;
+        if (!strcmp(sh.name, kAcct)) {
+            id = ACCT, ok = ok && sh.kind == blob::kAcctKind && sh.value_size == sizeof(bng_acct);
+        } else if (!strcmp(sh.name, blob::kIdleRec)) {
+            id = IDLE, ok = ok && sh.kind == blob::kIdleRecKind && sh.value_size == sizeof(bng_idle);
+        } else if (!strcmp(sh.name, kLi)) {
+            id = LI, ok = ok && sh.kind == blob::kLiKind && sh.value_size == 4 && sh.count <= BNG_LI_MAX_TARGETS;
         } else {
-            s.id = bng_map_id(c, s.h.name);
-            const MapReg *m = s.id >= 0 ? get_map(c, s.id) : nullptr;
-            if (!m || m->kind != KIND_HASH || s.h.kind != KIND_HASH || m->key_size != s.h.key_size || m->value_size != s.h.value_size)
-                s.id = -100;
+            id = bng_map_id(c, sh.name);
+            const MapReg *m = id >= 0 ? get_map(c, id) : nullptr;
+            ok = m && m->kind == KIND_HASH && sh.kind == KIND_HASH && m->key_size == sh.key_size && m->value_size == sh.value_size;
         }
-        if (s.id == -100) return fail(c, -EINVAL, "sub_import: %s is not a section of this library's layout", s.h.name);
-        secs.push_back(s);
+        if (!ok) return fail(c, -EINVAL, "sub_import: %s is not a section of this library's layout", sh.name);
+        secs.emplace_back(id, &s);
     }
-    if (p != end) return fail(c, -EINVAL, "sub_import: %llu bytes after the last section", (unsigned long long)(end - p));
     {   // room: nothing may be refused or evicted part way
         std::lock_guard<std::mutex> g(c->mu);
         cudaSetDevice(c->device);
         if (int fr = flush_staged_locked(c, -1)) return fr;
         std::unordered_map<int, u64> want;
         std::unordered_set<u32> li_new;
-        for (const Sec &s : secs) {
-            if (s.id >= 0) want[s.id] += s.h.count;
-            if (s.id == -3)
-                for (u64 k = 0; k < s.h.count; k++) {
+        for (const auto &[id, s] : secs) {
+            if (id >= 0) want[id] += s->h.count;
+            if (id == LI)
+                for (u64 k = 0; k < s->h.count; k++) {
                     u32 a;
-                    memcpy(&a, s.p + k * 4, 4);
+                    memcpy(&a, s->keys + k * 4, 4);
                     if (!c->li_targets.count(a)) li_new.insert(a);
                 }
         }
@@ -3489,32 +3321,20 @@ int bng_sub_import(bng_ctx *c, const void *buf, uint64_t len) {
         if (c->li_targets.size() + li_new.size() > BNG_LI_MAX_TARGETS)
             return fail(c, -E2BIG, "sub_import: more than %d interception targets", BNG_LI_MAX_TARGETS);
     }
-    for (const Sec &s : secs) {
-        if (s.id < 0 || !s.h.count) continue;
-        const u8 *keys = s.p, *vals = s.p + s.h.count * s.h.key_size;
-        if (int r = bng_map_update_batch(c, s.id, keys, vals, s.h.count, BNG_ANY)) return fail(c, r, "sub_import: loading %s failed", s.h.name);
+    for (const auto &[id, s] : secs) {
+        if (id < 0 || !s->h.count) continue;
+        if (int r = bng_map_update_batch(c, id, s->keys, s->vals, s->h.count, BNG_ANY)) return fail(c, r, "sub_import: loading %s failed", s->h.name);
     }
     // after the maps: the records go to the addresses' (new) directory slots
     std::lock_guard<std::mutex> g(c->mu);
     cudaSetDevice(c->device);
-    for (const Sec &s : secs) {
-        const u8 *keys = s.p, *vals = s.p + s.h.count * s.h.key_size;
-        if (!s.h.count) continue;
-        if (s.id == -1) {
-            if (int r = acct_alloc_locked(c)) return r;
-            if (int r = mv_load_records_locked(c, keys, vals, s.h.count, sizeof(bng_acct))) return r;
-        } else if (s.id == -2) {
-            if (int r = idle_alloc_locked(c)) return r;
-            if (int r = mv_load_records_locked(c, keys, vals, s.h.count, sizeof(bng_idle))) return r;
-        } else if (s.id == -3) {
-            if (int r = li_alloc_locked(c)) return r;
-            for (u64 k = 0; k < s.h.count; k++) {
-                u32 a, id;
-                memcpy(&a, keys + k * 4, 4);
-                memcpy(&id, vals + k * 4, 4);
-                c->li_targets[a] = id;
-            }
-            c->li_dirty = true;
+    for (const auto &[id, s] : secs) {
+        const u64 n = s->h.count;
+        if (!n) continue;
+        if (id == ACCT || id == IDLE) {
+            if (int r = load_records_locked(c, s->keys, s->vals, n, id == ACCT ? sizeof(bng_acct) : sizeof(bng_idle))) return r;
+        } else if (id == LI) {
+            if (int r = li_targets_load_locked(c, s->keys, s->vals, n, false)) return r;
         }
     }
     return 0;

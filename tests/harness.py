@@ -12,6 +12,7 @@ from __future__ import annotations
 
 import hashlib
 import os
+from typing import NamedTuple
 
 import numpy as np
 
@@ -404,3 +405,44 @@ def save_golden(path: str, res: dict):
 def load_golden(path: str) -> dict:
     with np.load(path) as z:
         return {k: z[k] for k in z.files}
+
+
+# ---------------------------------------------------------------------------
+# state blobs: the section framing of include/bng_b200.h, shared by bng_snapshot (header 16 bytes), bng_sub_export
+# (16) and bng_delta_export (40, sections with deleted keys)
+# ---------------------------------------------------------------------------
+class Section(NamedTuple):
+    start: int  # offset of the section header in the blob
+    name: str
+    kind: int
+    dels: np.ndarray  # deleted keys u8[n_del, key_size]; empty unless with_del
+    keys: np.ndarray  # u8[count, key_size]
+    vals: np.ndarray  # u8[count, value_size]
+
+
+def blob_sections(blob: bytes, hdr_len: int = 16, with_del: bool = False) -> list:
+    """The sections of a state blob, in order.  A 16-byte header counts them in the u64 at offset 8, a delta header in
+    its sections field; with_del reads the pad word as the count of deleted keys ahead of each section's keys."""
+    b = np.frombuffer(blob, np.uint8)
+    n = int(b[:hdr_len].view(L.delta_header)[0]["sections"]) if with_del else int(b[8:16].view("<u8")[0])
+    p, out = hdr_len, []
+    for _ in range(n):
+        s = b[p:p + L.delta_section.itemsize].view(L.delta_section)[0]
+        ks, vs, nd, c = int(s["key_size"]), int(s["value_size"]), int(s["n_del"]) if with_del else 0, int(s["n_up"])
+        q = p + L.delta_section.itemsize
+        dk = b[q:q + nd * ks].reshape(nd, ks)
+        k = b[q + nd * ks:q + (nd + c) * ks].reshape(c, ks)
+        v = b[q + (nd + c) * ks:q + (nd + c) * ks + c * vs].reshape(c, vs)
+        out.append(Section(p, s["name"].decode(), int(s["kind"]), dk, k, v))
+        p = q + (nd + c) * ks + c * vs
+    assert p == len(b), f"{len(b) - p} bytes after the last section"
+    return out
+
+
+def strip_section(blob: bytes, name: str) -> bytes:
+    """A snapshot or hand-over blob without its section `name`, which it must have."""
+    secs = blob_sections(blob)
+    ends = [s.start for s in secs[1:]] + [len(blob)]
+    kept = [blob[s.start:e] for s, e in zip(secs, ends) if s.name != name]
+    assert len(kept) == len(secs) - 1, f"the blob has no {name} section"
+    return blob[:8] + len(kept).to_bytes(8, "little") + b"".join(kept)

@@ -381,24 +381,6 @@ def test_header_split_ring_past_2_pow_32_bytes(pinned):
 # ---------------------------------------------------------------------------
 # 5. snapshot / restore
 # ---------------------------------------------------------------------------
-def _strip_section(blob, name=b"subscriber_acct"):
-    import struct
-    out = bytearray(blob[:16])
-    nmaps = struct.unpack_from("<Q", blob, 8)[0]
-    p, kept = 16, 0
-    for _ in range(nmaps):
-        hname, = struct.unpack_from("40s", blob, p)
-        _, ks, vs, _, cnt = struct.unpack_from("<IIIIQ", blob, p + 40)
-        end = p + 64 + cnt * (ks + vs)
-        if hname.rstrip(b"\0") != name:
-            out += blob[p:end]
-            kept += 1
-        p = end
-    assert kept == nmaps - 1, "the snapshot has no accounting section"
-    struct.pack_into("<Q", out, 8, kept)
-    return bytes(out)
-
-
 def test_snapshot_carries_records(ora_kind):
     from bng_b200 import Dataplane
     be, _ = run_accounted(scenarios.ALL_SCRIPTS["pipeline"], False, ora_kind)
@@ -409,7 +391,7 @@ def test_snapshot_carries_records(ora_kind):
         with Dataplane(max_subscribers=1 << 11, max_nat_sessions=1 << 15, max_eim_mappings=1 << 15, max_batch=1 << 12) as other:
             other.restore(blob)  # another size; accounting never enabled there
             assert _as_dict(*other.acct_dump()) == want
-        stripped = _strip_section(blob)
+        stripped = harness.strip_section(blob, "subscriber_acct")
         with Dataplane(max_subscribers=1 << 12, max_batch=1 << 12) as other:
             other.acct_enable("pipeline_up")
             other.restore(stripped)

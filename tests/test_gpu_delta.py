@@ -3,6 +3,7 @@ active's tables, accounting records and interception targets, and after a failov
 have computed."""
 import ctypes as C
 import errno
+import hashlib
 import os
 
 import numpy as np
@@ -34,22 +35,11 @@ def dumps(dp, maps=ALL_MAPS):
     return out
 
 
-def snap_sections(blob):
-    """{name: (keys, values)} of a bng_snapshot blob."""
-    b = np.frombuffer(blob, np.uint8)
-    n, p, out = int(b[8:16].view("<u8")[0]), 16, {}
-    for _ in range(n):
-        s = b[p:p + 64].view(L.delta_section)[0]
-        p += 64
-        ks, vs, c = int(s["key_size"]), int(s["value_size"]), int(s["n_up"])
-        out[s["name"].decode()] = (b[p:p + c * ks].reshape(c, ks), b[p + c * ks:p + c * (ks + vs)].reshape(c, vs))
-        p += c * (ks + vs)
-    return out
-
-
 def li_targets(dp):
-    k, v = snap_sections(dp.snapshot()).get("li_targets", (np.zeros((0, 4), np.uint8), np.zeros((0, 4), np.uint8)))
-    return sorted(zip(k.view("<u4").reshape(-1).tolist(), v.view("<u4").reshape(-1).tolist()))
+    s = next((s for s in harness.blob_sections(dp.snapshot()) if s.name == "li_targets"), None)
+    if s is None:
+        return []
+    return sorted(zip(s.keys.view("<u4").reshape(-1).tolist(), s.vals.view("<u4").reshape(-1).tolist()))
 
 
 def acct(dp):
@@ -542,3 +532,85 @@ def test_sharded_replication(world):
     finally:
         for x in act + peers:
             x.close()
+
+
+# ---------------------------------------------------------------------------
+# the three state blobs of one richly configured context, section by section
+# ---------------------------------------------------------------------------
+BLOB_SECTIONS = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "blob_sections.json")
+
+
+def _rich():
+    """A context with a section of every kind: pipeline_up state, accounting and idle records, interception targets,
+    IPv6 prefixes and ND bindings."""
+    from bng_b200 import synth as S
+    from test_gpu_move import _small
+    dp, _, ips = _small(n_subs=40)
+    v6 = np.zeros((20, 16), np.uint8)
+    v6[:, :4] = [0x20, 0x01, 0x0D, 0xB8]
+    v6[:, 5] = np.arange(20)
+    assert dp.ipv6_prefixes_set(v6, [56] * 20, ips[:20]) == 0
+    nd = np.zeros(20, L.bng_nd_binding)
+    nd["prefix"], nd["prefix_len"], nd["pio_flags"] = v6, 64, 0xC0
+    nd["valid_lft"], nd["preferred_lft"], nd["expires_s"] = 7200, 3600, 2_000_000
+    assert dp.update_batch("nd_bindings", S.sub_mac_key(np.arange(20)), nd) == 0
+    return dp, ips, S.sub_mac_key(np.arange(len(ips)))
+
+
+def _section_list(secs):
+    """(name, kind, key_size, value_size, n_del, count, digest of the sorted rows) per section, in blob order."""
+    out = []
+    for s in secs:
+        rows = sorted(bytes(r) for r in np.concatenate([s.keys, harness.mask_padding(s.name, s.vals)], axis=1))
+        h = hashlib.sha256(b"".join(sorted(bytes(r) for r in s.dels)) + b"|" + b"".join(rows)).hexdigest()[:16]
+        out.append([s.name, s.kind, s.keys.shape[1], s.vals.shape[1], len(s.dels), len(s.keys), h])
+    return out
+
+
+def blob_section_lists():
+    """The section lists of a snapshot, a FULL delta and a hand-over export of every other subscriber."""
+    dp, ips, macs = _rich()
+    try:
+        snap = harness.blob_sections(dp.snapshot())
+        dp.delta_enable()
+        delta = harness.blob_sections(dp.delta_export(full=True), L.delta_header.itemsize, with_del=True)
+        move = harness.blob_sections(dp.sub_export(ips[1::2], macs[::2]))
+        return {"snapshot": _section_list(snap), "delta": _section_list(delta), "sub_export": _section_list(move)}
+    finally:
+        dp.close()
+
+
+def test_blob_sections_are_pinned():
+    """Section order, headers and contents of all three blobs, as the library wrote them before their framing was
+    shared (tests/golden/blob_sections.json)."""
+    import json
+    with open(BLOB_SECTIONS) as f:
+        want = json.load(f)
+    got = blob_section_lists()
+    for producer in want:
+        assert [s[:6] for s in got[producer]] == [s[:6] for s in want[producer]], producer
+        assert got[producer] == want[producer], f"{producer}: rows differ"
+
+
+def test_restore_refuses_a_wrapping_section_whole():
+    """A snapshot whose second section claims 2^61 four-byte keys and values, so that count * (key_size + value_size)
+    wraps to 0, is refused before anything changes: not even the valid first section is loaded into its emptied map."""
+    dp, ips, _ = _rich()
+    try:
+        blob = dp.snapshot()
+        secs = harness.blob_sections(blob)
+        bad_hdr = np.zeros(1, L.delta_section)
+        bad_hdr["name"], bad_hdr["kind"], bad_hdr["key_size"], bad_hdr["value_size"] = b"subscriber_idle", 7, 4, 4
+        bad_hdr["n_up"] = 1 << 61
+        bad = blob[:8] + (2).to_bytes(8, "little") + blob[16:secs[1].start] + bad_hdr.tobytes() + bytes(64)
+        assert secs[0].name == "subscriber_bindings" and len(secs[0].keys)
+        dp.clear("subscriber_bindings")
+        before = dumps(dp), acct(dp), li_targets(dp), dp.idle_read(ips)
+        assert dp.lib.bng_restore(dp.h, bad, len(bad)) == -errno.EINVAL
+        after = dumps(dp), acct(dp), li_targets(dp), dp.idle_read(ips)
+        for m in ALL_MAPS:
+            assert np.array_equal(before[0][m][0], after[0][m][0]) and np.array_equal(before[0][m][1], after[0][m][1]), m
+        assert all(np.array_equal(x, y) for x, y in zip(before[1] + before[3], after[1] + after[3]))
+        assert before[2] == after[2] and len(before[2]) == 2
+    finally:
+        dp.close()

@@ -16,7 +16,7 @@ from bng_b200 import synth as S
 from bng_b200 import workloads as W
 from bng_b200.layouts import as_bytes
 from test_gpu_acct import (ACCOUNTED, FEED_IDS, FEEDS, PIPES, SCRIPTS, UP, _addr_keys, _frame_fields, _pipeline_batch,
-                           _pipeline_corpus, _qos_frames, _strip_section, _unlimited)
+                           _pipeline_corpus, _qos_frames, _unlimited)
 from test_oracle_fuzz import fuzz_script
 
 pytestmark = pytest.mark.gpu
@@ -569,7 +569,7 @@ def test_snapshot_carries_timeouts_and_restarts_clocks():
             other.restore(blob)  # another size; idle detection never enabled there
             _assert_restarted(other, keys, tos)
             assert other.idle_scan(61 * SEC)[2] == 0  # restarted: the first scan starts them
-        stripped = _strip_section(blob, b"subscriber_idle")
+        stripped = harness.strip_section(blob, "subscriber_idle")
         with Dataplane(max_subscribers=1 << 12, max_batch=1 << 12) as other:
             other.idle_enable("qos_ingress_prog")
             other.restore(stripped)

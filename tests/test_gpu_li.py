@@ -440,24 +440,6 @@ def _targets_of(dp, addrs, n=64):
     return {int(x["addr"]): int(x["target_id"]) for x in h}
 
 
-def _strip_section(blob, name):
-    import struct
-    out = bytearray(blob[:16])
-    nmaps = struct.unpack_from("<Q", blob, 8)[0]
-    p, kept = 16, 0
-    for _ in range(nmaps):
-        hname, = struct.unpack_from("40s", blob, p)
-        _, ks, vs, _, cnt = struct.unpack_from("<IIIIQ", blob, p + 40)
-        end = p + 64 + cnt * (ks + vs)
-        if hname.rstrip(b"\0") != name:
-            out += blob[p:end]
-            kept += 1
-        p = end
-    assert kept == nmaps - 1, f"the snapshot has no {name} section"
-    struct.pack_into("<Q", out, 8, kept)
-    return bytes(out)
-
-
 def test_snapshot_carries_targets():
     from bng_b200 import Dataplane
     addrs = S.ip_bytes(S.sub_ip(np.arange(40))).view("<u4").reshape(-1)
@@ -470,7 +452,7 @@ def test_snapshot_carries_targets():
             assert other.li_record_size == 0
             other.restore(blob)
             assert _targets_of(other, addrs) == t
-        stripped = _strip_section(blob, b"li_targets")
+        stripped = harness.strip_section(blob, "li_targets")
         with Dataplane(max_batch=1 << 10, max_subscribers=1 << 11) as other:
             other.li_target_set(int(addrs[35]), 5)
             other.restore(stripped)  # restoring over live targets: the blob's (none) replace them

@@ -23,7 +23,6 @@ TABLES = FLOW + ("subscriber_nat", "qos_ingress", "qos_egress", "subscriber_bind
 KEYED_BY_SUBSCRIBER = {"subscriber_bindings": "mac", "subscriber_pools": "mac", "qos_ingress": "ip", "qos_egress": "ip",
                        "subscriber_nat": "ip"}
 EINVAL, ENOSPC, E2BIG = 22, 28, 7
-SEC = np.dtype([("name", "S40"), ("kind", "<u4"), ("ks", "<u4"), ("vs", "<u4"), ("pad", "<u4"), ("count", "<u8")])
 
 
 def _words(b):
@@ -46,19 +45,8 @@ def _rows(name, k, v):
 def parse_blob(blob):
     """{section name: (keys u8[n, ks], values u8[n, vs])} and the offsets where sections start."""
     assert blob[:8] == b"BNGMOVE1"
-    n, p, out, starts = int.from_bytes(blob[8:16], "little"), 16, {}, []
-    for _ in range(n):
-        starts.append(p)
-        h = np.frombuffer(blob[p:p + 64], SEC)[0]
-        p += 64
-        c, ks, vs = int(h["count"]), int(h["ks"]), int(h["vs"])
-        k = np.frombuffer(blob[p:p + c * ks], np.uint8).reshape(c, ks)
-        p += c * ks
-        v = np.frombuffer(blob[p:p + c * vs], np.uint8).reshape(c, vs)
-        p += c * vs
-        out[h["name"].decode()] = (k, v)
-    assert p == len(blob)
-    return out, starts
+    secs = harness.blob_sections(blob)
+    return {s.name: (s.keys, s.vals) for s in secs}, [s.start for s in secs]
 
 
 def _state(dp):
