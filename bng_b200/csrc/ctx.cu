@@ -180,6 +180,9 @@ struct bng_ctx {
     // bng_nat_icmp_errors_enable: nat44_ingress translates ICMP errors by the flow they quote (context state, as
     // qos_v6)
     bool nat_icmp = false;
+    // bng_nat_icmp_errors_egress_enable: nat44_egress and the pipelines translate subscribers' ICMP errors by the flow
+    // they quote (context state, as qos_v6)
+    bool nat_icmp_eg = false;
     // bng_antispoof_ipv6_prefixes_enable: antispoof_ingress allows IPv6 sources in their binding's own subscriber_ipv6
     // prefixes (context state, as qos_v6)
     bool as_v6 = false;
@@ -1272,7 +1275,7 @@ static int dispatch(bng_ctx *c, int prog, const DevBatch &b, const LiSrc &src = 
     case P_ANTISPOOF: e = run_antispoof(c->L, c->dev, b, as6); break;
     case P_QOS_EG: e = run_qos(c->L, c->dev, b, true, qv6); break;
     case P_QOS_IN: e = run_qos(c->L, c->dev, b, false, qv6); break;
-    case P_NAT_EG: e = run_nat_egress(c->L, c->dev, b); break;
+    case P_NAT_EG: e = run_nat_egress(c->L, c->dev, b, c->nat_icmp_eg); break;
     case P_NAT_IN: e = run_nat_ingress(c->L, c->dev, b, c->nat_icmp); break;
     case P_NAT_HAIRPIN: e = run_nat_hairpin_xdp(c->L, c->dev, b); break;
     case P_DHCP: {
@@ -1295,8 +1298,8 @@ static int dispatch(bng_ctx *c, int prog, const DevBatch &b, const LiSrc &src = 
         e = run_dhcp_fastpath(c->L, c->dev, b, v6 ? &d6 : nullptr, ndo ? &nd : nullptr);
         break;
     }
-    case P_PIPE_UP: e = run_pipeline_up(c->L, c->dev, b, qv6, as6); break;
-    case P_PIPE_TC: e = run_pipeline_tc(c->L, c->dev, b, qv6, as6); break;
+    case P_PIPE_UP: e = run_pipeline_up(c->L, c->dev, b, qv6, as6, c->nat_icmp_eg); break;
+    case P_PIPE_TC: e = run_pipeline_tc(c->L, c->dev, b, qv6, as6, c->nat_icmp_eg); break;
     default: return -EINVAL;
     }
     // after the program, before anything copies the frames out: the downstream modes read the rewritten headers
@@ -1384,7 +1387,10 @@ static int run_host_zero_copy(bng_ctx *c, int prog, bng_batch *bb, u8 *arena_dev
                                   c->s_in));
         } else {
             CU(c, run_gather_frames(c->s_in, c->L.num_sms, chunk_arena, bb->off16 ? c->zc_off[buf] : nullptr, c->zc_len[buf],
-                                    bb->stride, cn, hb, tc, prog == P_NAT_IN && c->nat_icmp, c->zc_hdr[buf], c->zc_len0[buf]));
+                                    bb->stride, cn, hb, tc,
+                                    (prog == P_NAT_IN && c->nat_icmp) ||
+                                        ((prog == P_NAT_EG || prog == P_PIPE_UP || prog == P_PIPE_TC) && c->nat_icmp_eg),
+                                    c->zc_hdr[buf], c->zc_len0[buf]));
             c->L.launches++;
         }
         CU(c, cudaEventRecord(c->ev_in[buf], c->s_in));
@@ -3384,6 +3390,13 @@ int bng_nat_icmp_errors_enable(bng_ctx *c, int on) {
     if (!c) return -EINVAL;
     std::lock_guard<std::mutex> g(c->mu);
     c->nat_icmp = on != 0;
+    return 0;
+}
+
+int bng_nat_icmp_errors_egress_enable(bng_ctx *c, int on) {
+    if (!c) return -EINVAL;
+    std::lock_guard<std::mutex> g(c->mu);
+    c->nat_icmp_eg = on != 0;
     return 0;
 }
 

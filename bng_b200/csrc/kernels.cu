@@ -662,13 +662,31 @@ __global__ void __launch_bounds__(BLOCK) k_heads(const __grid_constant__ Grouped
 // never calls it, and its registers (the frame header, three table probes, the translation) must not cost the
 // staging loop and the token-bucket walk theirs.  Returns true for a frame nat44_egress dropped (port exhaustion).
 // The sequential nat44_egress of one frame, out of line (rare; keeps its registers and code out of the walk).
+// ICMPERR: an ICMP error frame (outer ihl 5) first meets the rule of bng_nat_icmp_errors_egress_enable, which
+// translates it by the flow it quotes; where that does not apply, nat44_egress as always.  `fresh` (a frame the token
+// bucket deferred): the parse's hairpin statistic is still to be counted.
+template <bool ICMPERR>
 static __device__ __noinline__ int nat_egress_seq(const DevCtx &c, BlockStats &bs, const DevBatch &b, u8 *sub, u32 idx, u32 len, NatPend *pend,
                                                  bool fresh) {
+    if (ICMPERR) {
+        u8 *p = frame_ptr(b, idx);
+        const u32 dlen = frame_dlen(b, len);
+        if (icmp_error_frame(p, dlen) && nat_icmp_error_egress_one(c, p, dlen)) {
+            if (fresh && (*(const u32 *)c.nat_config & NATF_HAIRPIN)) {
+                u64 hk = rd32(p, 30);
+                if (tbl_find<1, false>(c.hairpin, &hk)) bstats_add(bs, ST_NAT_HAIRPIN, 1);
+            }
+            bstats_add(bs, ST_NAT_SNAT, 1);
+            return TC_OK;
+        }
+    }
     NatOut o = nat_egress_one<true>(c, bs, frame_ptr(b, idx), sub, len, frame_dlen(b, len), idx + b.base, frame_now(b, idx), pend, fresh,
                                     b.nowv != nullptr);
     return o.verdict;
 }
 
+// ICMPERR: an ICMP error frame ends nat_chunk_coop's prefix and goes through nat_egress_seq<true>() in its turn.
+template <bool ICMPERR>
 __device__ __forceinline__ bool resolve_nat_chunk(const DevCtx &c, const DevBatch &b, BlockStats &bs, u8 *sub, u32 idx, u32 len,
                                                       bool is_miss, bool fresh, u32 mm, u32 lane) {
     NatPend pend;
@@ -696,14 +714,14 @@ __device__ __forceinline__ bool resolve_nat_chunk(const DevCtx &c, const DevBatc
     u32 todo = mm;
     while (todo) {
         // the longest prefix of the remaining new flows that does not interact: all at once
-        const u32 took = nat_chunk_coop(c, bs, b, sub, is_miss && ((todo >> lane) & 1), idx, len, pend, lane, fresh);
+        const u32 took = nat_chunk_coop<ICMPERR>(c, bs, b, sub, is_miss && ((todo >> lane) & 1), idx, len, pend, lane, fresh);
         todo &= ~took;
         if (lane == 0 && took) bstats_add(bs, ST_NAT_COOP, __popc(took));
         if (!todo) break;
         const u32 l = __ffs(todo) - 1; // ... then the frame that does, through the sequential code
         todo &= todo - 1;
         if (lane == l) {
-            if (nat_egress_seq(c, bs, b, sub, idx, len, &pend, fresh) == TC_SHOT) {
+            if (nat_egress_seq<ICMPERR>(c, bs, b, sub, idx, len, &pend, fresh) == TC_SHOT) {
                 b.verdict[idx] = TC_SHOT;
                 dropped = true;
             }
@@ -718,7 +736,9 @@ __device__ __forceinline__ bool resolve_nat_chunk(const DevCtx &c, const DevBatc
 
 // TC (pipeline_tc): the token bucket runs BEFORE the NAT stage: QoS walk first, then nat44_egress — hits and
 // new flows alike — for the frames it passed (DEFER_FLAG), with the parse-stage counters still to be counted.
-template <bool NAT, bool QOS, bool EGRESS, bool TC = false>
+// ICMPERR (bng_nat_icmp_errors_egress_enable): an ICMP error frame in the NAT stage is looked up by the flow it quotes
+// first (resolve_nat_chunk).
+template <bool NAT, bool QOS, bool EGRESS, bool TC = false, bool ICMPERR = false>
 __global__ void __launch_bounds__(RS_TEAM, 16) k_resolve(const __grid_constant__ DevCtx c, const __grid_constant__ DevBatch b,
                                                       const __grid_constant__ Grouped g, const u32 *seg, u32 *cnt) {
     constexpr int STAGE = RS_TEAM * RS_PER_THREAD;
@@ -817,7 +837,7 @@ __global__ void __launch_bounds__(RS_TEAM, 16) k_resolve(const __grid_constant__
                     }
                     const u32 mm = __ballot_sync(0xffffffffu, is_miss);
                     if (!mm) continue; // (the steady state: nothing to create, the call below never happens)
-                    if (resolve_nat_chunk(c, b, bs, sub, sv & IDX_MASK, valid ? s_len[j] : 0, is_miss, fresh, mm, lane)) s_sv[j] = sv | DROP_FLAG;
+                    if (resolve_nat_chunk<ICMPERR>(c, b, bs, sub, sv & IDX_MASK, valid ? s_len[j] : 0, is_miss, fresh, mm, lane)) s_sv[j] = sv | DROP_FLAG;
                 }
               }
             };
@@ -1036,17 +1056,18 @@ static inline u32 kshift_for(u64 key_space) { return bits_for(key_space) <= KEY_
 
 // k_resolve walks one group per block and a batch of n frames can hold n groups: the grid is sized for n blocks,
 // capped at what the GPU holds at once (the blocks loop over the groups).
-template <bool NAT, bool QOS, bool EGRESS, bool TC = false>
+template <bool NAT, bool QOS, bool EGRESS, bool TC = false, bool ICMPERR = false>
 static void launch_resolve(Launcher &L, const DevCtx &c, const DevBatch &b, const Grouped &g, const char *name) {
-    int &per_sm = L.resolve_bps[NAT * 8 + QOS * 4 + EGRESS * 2 + TC]; // resident blocks per SM of this instantiation
+    int &per_sm = L.resolve_bps[ICMPERR * 16 + NAT * 8 + QOS * 4 + EGRESS * 2 + TC]; // resident blocks per SM of this instantiation
     if (!per_sm) {
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_resolve<NAT, QOS, EGRESS, TC>, RS_TEAM, 0) != cudaSuccess || per_sm < 1)
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_resolve<NAT, QOS, EGRESS, TC, ICMPERR>, RS_TEAM, 0) != cudaSuccess ||
+            per_sm < 1)
             per_sm = 8;
     }
     long cap = (long)L.num_sms * per_sm, want = b.n ? b.n : 1;
     int grid = (int)(want < cap ? want : cap);
     prof_begin(L, name);
-    launch_dep(k_resolve<NAT, QOS, EGRESS, TC>, grid, RS_TEAM, L.stream, c, b, g, L.s.qslot, L.s.counters);
+    launch_dep(k_resolve<NAT, QOS, EGRESS, TC, ICMPERR>, grid, RS_TEAM, L.stream, c, b, g, L.s.qslot, L.s.counters);
     prof_end(L);
     L.launches++;
 }
@@ -1085,12 +1106,14 @@ cudaError_t run_qos(Launcher &L, const DevCtx &c, const DevBatch &b0, bool egres
 struct ClassifyNames {
     const char *plain, *acct, *v6, *acct_v6, *as6, *acct_as6, *v6_as6, *acct_v6_as6;
 };
-template <bool AS, bool QOS, bool TC, bool ACCT, bool V6, bool AS6 = false>
+template <bool AS, bool QOS, bool TC, bool ACCT, bool V6, bool AS6 = false, bool ICMPERR = false>
 static void launch_classify(Launcher &L, const DevCtx &c, const DevBatch &b, const char *name, const Tbl &v6) {
-    LAUNCH_AS(name, (k_pipe_classify<AS, QOS, TC, ACCT, V6, AS6>), b.n, CLASSIFY_BPS(AS), c, b, L.s.key_a, L.s.val_a, L.s.counters,
+    LAUNCH_AS(name, (k_pipe_classify<AS, QOS, TC, ACCT, V6, AS6, ICMPERR>), b.n, CLASSIFY_BPS(AS), c, b, L.s.key_a, L.s.val_a, L.s.counters,
               sort_T(L), ACCT ? L.acct_attr : nullptr, v6);
 }
-template <bool AS, bool QOS, bool TC>
+// ICMPERR (bng_nat_icmp_errors_egress_enable): the ICMPERR instantiations of classify and resolve, timed under their
+// names with an ", icmperr>" suffix.
+template <bool AS, bool QOS, bool TC, bool ICMPERR = false>
 static cudaError_t run_dir_prog(Launcher &L, const DevCtx &c, const DevBatch &b0, const ClassifyNames &nm, const char *resolve_name,
                                 const Tbl *v6, const Tbl *as6) {
     DevBatch b = b0;
@@ -1098,32 +1121,36 @@ static cudaError_t run_dir_prog(Launcher &L, const DevCtx &c, const DevBatch &b0
     if (AS && as6) { // (AS6 = AS: nat44_egress has no antispoof stage and is never given the table)
         if (QOS && v6) {
             if (L.acct_attr)
-                launch_classify<AS, QOS, TC, true, QOS, AS>(L, c, b, nm.acct_v6_as6, *as6);
+                launch_classify<AS, QOS, TC, true, QOS, AS, ICMPERR>(L, c, b, nm.acct_v6_as6, *as6);
             else
-                launch_classify<AS, QOS, TC, false, QOS, AS>(L, c, b, nm.v6_as6, *as6);
+                launch_classify<AS, QOS, TC, false, QOS, AS, ICMPERR>(L, c, b, nm.v6_as6, *as6);
         } else if (L.acct_attr) {
-            launch_classify<AS, QOS, TC, true, false, AS>(L, c, b, nm.acct_as6, *as6);
+            launch_classify<AS, QOS, TC, true, false, AS, ICMPERR>(L, c, b, nm.acct_as6, *as6);
         } else {
-            launch_classify<AS, QOS, TC, false, false, AS>(L, c, b, nm.as6, *as6);
+            launch_classify<AS, QOS, TC, false, false, AS, ICMPERR>(L, c, b, nm.as6, *as6);
         }
     } else if (QOS && v6) { // (V6 = QOS: nat44_egress has no bucket and is never given the table)
         if (L.acct_attr)
-            launch_classify<AS, QOS, TC, true, QOS>(L, c, b, nm.acct_v6, *v6);
+            launch_classify<AS, QOS, TC, true, QOS, false, ICMPERR>(L, c, b, nm.acct_v6, *v6);
         else
-            launch_classify<AS, QOS, TC, false, QOS>(L, c, b, nm.v6, *v6);
+            launch_classify<AS, QOS, TC, false, QOS, false, ICMPERR>(L, c, b, nm.v6, *v6);
     } else if (L.acct_attr) {
-        launch_classify<AS, QOS, TC, true, false>(L, c, b, nm.acct, Tbl{});
+        launch_classify<AS, QOS, TC, true, false, false, ICMPERR>(L, c, b, nm.acct, Tbl{});
     } else {
-        launch_classify<AS, QOS, TC, false, false>(L, c, b, nm.plain, Tbl{});
+        launch_classify<AS, QOS, TC, false, false, false, ICMPERR>(L, c, b, nm.plain, Tbl{});
     }
     Grouped g;
     cudaError_t e = group_by_key(L, b.n, (u64)c.subdir.mask + 1, b.kshift, &g);
     if (e != cudaSuccess) return e;
-    launch_resolve<true, QOS, false, TC>(L, c, b, g, resolve_name);
+    launch_resolve<true, QOS, false, TC, ICMPERR>(L, c, b, g, resolve_name);
     return cudaGetLastError();
 }
 
-cudaError_t run_nat_egress(Launcher &L, const DevCtx &c, const DevBatch &b) {
+cudaError_t run_nat_egress(Launcher &L, const DevCtx &c, const DevBatch &b, bool icmp_errors_eg) {
+    if (icmp_errors_eg)
+        return run_dir_prog<false, false, false, true>(
+            L, c, b, {"(k_pipe_classify<false, false, icmperr>)", "(k_pipe_classify<false, false, false, true, icmperr>)"},
+            "(k_resolve<true, false, false, icmperr>)", nullptr, nullptr);
     return run_dir_prog<false, false, false>(L, c, b, {"(k_pipe_classify<false, false>)", "(k_pipe_classify<false, false, false, true>)"},
                                              "(k_resolve<true, false, false>)", nullptr, nullptr);
 }
@@ -1141,7 +1168,15 @@ cudaError_t run_nat_hairpin_xdp(Launcher &L, const DevCtx &c, const DevBatch &b)
     return cudaGetLastError();
 }
 
-cudaError_t run_pipeline_up(Launcher &L, const DevCtx &c, const DevBatch &b, const Tbl *v6, const Tbl *as6) {
+cudaError_t run_pipeline_up(Launcher &L, const DevCtx &c, const DevBatch &b, const Tbl *v6, const Tbl *as6, bool icmp_errors_eg) {
+    if (icmp_errors_eg)
+        return run_dir_prog<true, true, false, true>(
+            L, c, b,
+            {"(k_pipe_classify<true, true, icmperr>)", "(k_pipe_classify<true, true, false, true, icmperr>)",
+             "(k_pipe_classify<true, true, v6, icmperr>)", "(k_pipe_classify<true, true, false, true, v6, icmperr>)",
+             "(k_pipe_classify<true, true, as6, icmperr>)", "(k_pipe_classify<true, true, false, true, as6, icmperr>)",
+             "(k_pipe_classify<true, true, v6, as6, icmperr>)", "(k_pipe_classify<true, true, false, true, v6, as6, icmperr>)"},
+            "(k_resolve<true, true, false, icmperr>)", v6, as6);
     return run_dir_prog<true, true, false>(L, c, b,
                                            {"(k_pipe_classify<true, true>)", "(k_pipe_classify<true, true, false, true>)",
                                             "(k_pipe_classify<true, true, v6>)", "(k_pipe_classify<true, true, false, true, v6>)",
@@ -1150,7 +1185,15 @@ cudaError_t run_pipeline_up(Launcher &L, const DevCtx &c, const DevBatch &b, con
                                            "(k_resolve<true, true, false>)", v6, as6);
 }
 
-cudaError_t run_pipeline_tc(Launcher &L, const DevCtx &c, const DevBatch &b, const Tbl *v6, const Tbl *as6) {
+cudaError_t run_pipeline_tc(Launcher &L, const DevCtx &c, const DevBatch &b, const Tbl *v6, const Tbl *as6, bool icmp_errors_eg) {
+    if (icmp_errors_eg)
+        return run_dir_prog<true, true, true, true>(
+            L, c, b,
+            {"(k_pipe_classify<true, true, true, icmperr>)", "(k_pipe_classify<true, true, true, true, icmperr>)",
+             "(k_pipe_classify<true, true, true, v6, icmperr>)", "(k_pipe_classify<true, true, true, true, v6, icmperr>)",
+             "(k_pipe_classify<true, true, true, as6, icmperr>)", "(k_pipe_classify<true, true, true, true, as6, icmperr>)",
+             "(k_pipe_classify<true, true, true, v6, as6, icmperr>)", "(k_pipe_classify<true, true, true, true, v6, as6, icmperr>)"},
+            "(k_resolve<true, true, false, tc, icmperr>)", v6, as6);
     return run_dir_prog<true, true, true>(L, c, b,
                                           {"(k_pipe_classify<true, true, true>)", "(k_pipe_classify<true, true, true, true>)",
                                            "(k_pipe_classify<true, true, true, v6>)", "(k_pipe_classify<true, true, true, true, v6>)",

@@ -30,7 +30,7 @@ struct Launcher {
     int dhcp_smem_set;  // cudaFuncAttributeMaxDynamicSharedMemorySize applied on this context's device
     int dhcp6_smem_set; // ... and to k_dhcp_fastpath<v6>
     int nd_smem_set[2]; // ... and to k_dhcp_fastpath<nd>, <v6,nd>
-    int resolve_bps[16]; // resident blocks per SM of the k_resolve instantiations, by <NAT, QOS, EGRESS, TC> bits
+    int resolve_bps[32]; // resident blocks per SM of the k_resolve instantiations, by <NAT, QOS, EGRESS, TC, ICMPERR> bits
     int prof;
     ProfPending pend[32];
     int npend;
@@ -52,12 +52,14 @@ cudaError_t run_antispoof(Launcher &L, const DevCtx &c, const DevBatch &b, const
 // v6: subscriber_ipv6 when IPv6 frames are shaped by their owner's bucket (bng_qos_ipv6_enable, and the table has live
 // entries), else nullptr
 cudaError_t run_qos(Launcher &L, const DevCtx &c, const DevBatch &b, bool egress, const Tbl *v6);
-cudaError_t run_nat_egress(Launcher &L, const DevCtx &c, const DevBatch &b);
+// icmp_errors_eg (nat44_egress and the pipelines): subscribers' ICMP errors are translated by the flow they quote
+// (bng_nat_icmp_errors_egress_enable)
+cudaError_t run_nat_egress(Launcher &L, const DevCtx &c, const DevBatch &b, bool icmp_errors_eg);
 // icmp_errors: ICMP errors are translated by the flow they quote (bng_nat_icmp_errors_enable)
 cudaError_t run_nat_ingress(Launcher &L, const DevCtx &c, const DevBatch &b, bool icmp_errors);
 cudaError_t run_nat_hairpin_xdp(Launcher &L, const DevCtx &c, const DevBatch &b);
-cudaError_t run_pipeline_up(Launcher &L, const DevCtx &c, const DevBatch &b, const Tbl *v6, const Tbl *as6);
-cudaError_t run_pipeline_tc(Launcher &L, const DevCtx &c, const DevBatch &b, const Tbl *v6, const Tbl *as6);
+cudaError_t run_pipeline_up(Launcher &L, const DevCtx &c, const DevBatch &b, const Tbl *v6, const Tbl *as6, bool icmp_errors_eg);
+cudaError_t run_pipeline_tc(Launcher &L, const DevCtx &c, const DevBatch &b, const Tbl *v6, const Tbl *as6, bool icmp_errors_eg);
 // The DHCPv6 fast path (include/bng_b200.h, bng_dhcpv6_enable): its tables and where its counters go.  The counters
 // follow the ST_COUNT of the packed statistics vector, which then holds ST_ALL; the kernels' per-block accumulators
 // (BlockStats) keep ST_COUNT.
@@ -89,7 +91,8 @@ struct NdArgs {
 cudaError_t run_dhcp_fastpath(Launcher &L, const DevCtx &c, const DevBatch &b, const Dhcp6Args *d6, const NdArgs *nd);
 
 // header gather / scatter between a pinned host arena and a compact device copy (hostio.cu); icmp_errors (TC only):
-// also bytes 64-79 of an ICMP error frame, for nat44_ingress with bng_nat_icmp_errors_enable
+// also bytes 64-79 of an ICMP error frame, for nat44_ingress with bng_nat_icmp_errors_enable and for nat44_egress and
+// the pipelines with bng_nat_icmp_errors_egress_enable
 cudaError_t run_gather_frames(cudaStream_t st, int blocks, const u8 *arena, const u32 *off16, const u32 *len, u32 stride,
                               u32 n, u32 slot, bool tc, bool icmp_errors, u8 *dst, u32 *need);
 cudaError_t run_scatter_frames(cudaStream_t st, int blocks, u8 *arena, const u32 *off16, const u32 *need, u32 stride, u32 n,

@@ -45,7 +45,10 @@
 // AS6 (bng_antispoof_ipv6_prefixes_enable, while subscriber_ipv6 has live entries; AS only): antispoof_eval<true>, an
 // IPv6 frame on antispoof's drop path whose source is in its binding's own prefixes is allowed.  The frame's source is
 // already in h.  With V6 too, the owner antispoof found (the binding's ipv4_addr) stands in for phase 3's v6_owner.
-template <bool AS, bool QOS, bool TC = false, bool ACCT = false, bool V6 = false, bool AS6 = false>
+// ICMPERR (bng_nat_icmp_errors_egress_enable): an ICMP error frame (protocol 1, type 3 / 11 / 12) on the SNAT path
+// does not take the session probe: it becomes a miss (MISS_FLAG, an ordering key), so that the ordered phase looks up
+// the flow it quotes in index order with the subscriber's other new flows (DESIGN.md §24).  No load past h.
+template <bool AS, bool QOS, bool TC = false, bool ACCT = false, bool V6 = false, bool AS6 = false, bool ICMPERR = false>
 __global__ void __launch_bounds__(BLOCK, CLASSIFY_BPS(AS))
     k_pipe_classify(const __grid_constant__ DevCtx c, const __grid_constant__ DevBatch b, u32 *skey, u32 *sval, u32 *cnt, u32 *T,
                     u32 *attr, const __grid_constant__ Tbl v6) {
@@ -188,7 +191,8 @@ __global__ void __launch_bounds__(BLOCK, CLASSIFY_BPS(AS))
         __syncwarp();
         if (go && (nflags & NATF_HAIRPIN) && hp_contains(st, daddr)) bstats_add(bs, ST_NAT_HAIRPIN, 1);
         __syncwarp();
-        u8 *ses = go ? tbl_finish<2>(c.sessions, key, hi, kw0, kw1 == key[1]) : nullptr;
+        const bool err = ICMPERR && go && proto == 1 && icmp_error_type(h.b8(34)); // (go: ihl 5, bytes 0-41 present)
+        u8 *ses = go && !err ? tbl_finish<2>(c.sessions, key, hi, kw0, kw1 == key[1]) : nullptr;
         __syncwarp();
 
         // ---- phase 4: session hit: counters and the SNAT rewrite (:674-680, :752-798) ----

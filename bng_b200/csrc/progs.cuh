@@ -590,6 +590,15 @@ __device__ __forceinline__ NatOut nat_egress_one(const DevCtx &c, BlockStats &bs
     return o;
 }
 
+// ICMP error messages whose quoted datagram names a flow (RFC 5508): Destination Unreachable, Time Exceeded,
+// Parameter Problem.
+__device__ __forceinline__ bool icmp_error_type(u32 t) { return t == 3 || t == 11 || t == 12; }
+// An IPv4 frame (the caller checked the ethertype) that is an ICMP error with no outer options and its ICMP header
+// present: the frames bng_nat_icmp_errors_egress_enable's rule looks at.
+__device__ __forceinline__ bool icmp_error_frame(const u8 *p, u32 dlen) {
+    return dlen >= 42 && (p[14] & 0x0f) == 5 && p[23] == 1 && icmp_error_type(p[34]);
+}
+
 // ---------------------------------------------------------------------------
 // The ordered phase, warp-cooperatively: up to 32 new-flow frames of ONE subscriber (consecutive in index
 // order) are created together.  The sequential walk above spends ~15 dependent table accesses per flow
@@ -609,6 +618,9 @@ __device__ __forceinline__ NatOut nat_egress_one(const DevCtx &c, BlockStats &bs
 // max_entries: those chunks go frame by frame.
 // Exhaustion never happens on the cooperative path: every proposed port is inside the block.
 // ---------------------------------------------------------------------------
+// ICMPERR (bng_nat_icmp_errors_egress_enable): an ICMP error frame also ends the prefix; the sequential code looks up
+// the flow it quotes.
+template <bool ICMPERR = false>
 __device__ __forceinline__ u32 nat_chunk_coop(const DevCtx &c, BlockStats &bs, const DevBatch &b, u8 *sub, bool mine, u32 idx,
                                               u32 len, NatPend &pend, u32 lane, const bool count_parse = false) {
     const u32 cfg_flags = *(const u32 *)c.nat_config;
@@ -652,6 +664,7 @@ __device__ __forceinline__ u32 nat_chunk_coop(const DevCtx &c, BlockStats &bs, c
     // (nothing is counted here: a frame that is not in the committed prefix comes back and is parsed again)
     if (mine && !fast) f = nat_parse(c, bs, p, dlen, idx + b.base, now, sub, cfg_flags, false);
     const bool go = mine && f.ok;
+    const bool err = ICMPERR && go && f.proto == 1 && f.l4 == 34 && icmp_error_type(fast ? h.b8(34) : p[34]);
     // ---- probes: where the flow's entries are, or would go ----
     u64 key[2] = {0, 0}, ek = 0;
     u8 *ses = nullptr, *m = nullptr;
@@ -667,7 +680,7 @@ __device__ __forceinline__ u32 nat_chunk_coop(const DevCtx &c, BlockStats &bs, c
     const bool alloc = create && !m;         // ... and a port (EIM: a new mapping)
     const u32 below = (1u << lane) - 1;
     const u32 cmask = __ballot_sync(0xffffffffu, create), amask = __ballot_sync(0xffffffffu, alloc);
-    bool clash = false, all_clash = false; // clash: this frame ends the prefix; all_clash: nothing can be committed
+    bool clash = err, all_clash = false; // clash: this frame ends the prefix; all_clash: nothing can be committed
     if (cmask) {
         // same 5-tuple as an earlier creating lane?
         const u32 g0 = __match_any_sync(0xffffffffu, create ? key[0] : (u64)lane | (1ull << 63));
@@ -889,10 +902,6 @@ __device__ __forceinline__ u32 nat_chunk_coop(const DevCtx &c, BlockStats &bs, c
     return take;
 }
 
-// ICMP error messages whose quoted datagram names a flow (RFC 5508): Destination Unreachable, Time Exceeded,
-// Parameter Problem.
-__device__ __forceinline__ bool icmp_error_type(u32 t) { return t == 3 || t == 11 || t == 12; }
-
 // nat44_ingress, :805-948.  Every update is commutative (or made so with a
 // CAS on the state byte), so this is a classify-only program.
 // ICMPERR (bng_nat_icmp_errors_enable): an ICMP error frame is never keyed by its bytes 4-5; here (outer options) it
@@ -999,6 +1008,49 @@ __device__ __forceinline__ int nat_ingress_one(const DevCtx &c, BlockStats &bs, 
     return TC_OK;
 }
 
+// The quoted datagram's half of an ICMP error's translation, both directions (RFC 5508): h holds bytes 0-63, x bytes
+// 64-79.  The quoted address at AOFF (54: source, 58: destination) ia -> na, with the quoted IPv4 checksum (52-53);
+// then the quoted TCP/UDP port at POFF (62 or 64), or the quoted ICMP id (66-67), op -> np, with the quoted L4
+// checksum (UDP 68-69 when present and non-zero, 0 becoming 0xFFFF; TCP 78-79 when present; ICMP 64-65 for the id
+// alone); every changed word of the ICMP message goes into the ICMP checksum (36-37), in this order.  The outer
+// header is the caller's.  Returns whether x changed.
+template <u32 AOFF, u32 POFF>
+__device__ __forceinline__ bool icmp_quote_rewrite(Hdr64 &h, uint4 &x, u32 iproto, u32 dlen, u32 ia, u32 na, u16 op, u16 np) {
+    static_assert((AOFF == 54 || AOFF == 58) && (POFF == 62 || POFF == 64), "quoted source or destination");
+    const u16 ihc = h.b16(52), ihc2 = csum_upd32(ihc, ia, na);
+    h.s32(AOFF, na);
+    h.s16(52, ihc2);
+    u16 ic = csum_upd32(h.b16(36), ia, na);
+    ic = csum_upd16(ic, ihc, ihc2);
+    ic = csum_upd16(ic, op, np);
+    bool c4 = true;
+    if (iproto == 1) {
+        const u16 k0 = (u16)x.x, k1 = csum_upd16(k0, op, np);
+        x.x = (u32)k1 | ((u32)np << 16);
+        ic = csum_upd16(ic, k0, k1);
+    } else {
+        if (POFF == 62)
+            h.s16(62, np);
+        else
+            x.x = (x.x & 0xffff0000u) | np;
+        if (iproto == 17 && dlen >= 70 && (u16)x.y != 0) {
+            const u16 k0 = (u16)x.y;
+            u16 k1 = csum_upd16(csum_upd32(k0, ia, na), op, np);
+            if (k1 == 0) k1 = 0xffff;
+            x.y = (x.y & 0xffff0000u) | k1;
+            ic = csum_upd16(ic, k0, k1);
+        } else if (iproto == 6 && dlen >= 80) {
+            const u16 k0 = (u16)(x.w >> 16), k1 = csum_upd16(csum_upd32(k0, ia, na), op, np);
+            x.w = (x.w & 0xffffu) | ((u32)k1 << 16);
+            ic = csum_upd16(ic, k0, k1);
+        } else {
+            c4 = POFF == 64;
+        }
+    }
+    h.s16(36, ic);
+    return c4;
+}
+
 // bng_nat_icmp_errors_enable: an ICMP error frame (outer ihl 5, type 3 / 11 / 12, the 8-byte ICMP header present)
 // sent to a public address, translated by the flow it quotes (include/bng_b200.h, DESIGN.md §20).  h holds bytes 0-63;
 // the quoted L4 header continues in chunk 4 (bytes 64-79), loaded here.  Returns whether the frame was translated
@@ -1028,39 +1080,50 @@ __device__ __forceinline__ bool nat_icmp_error_one(const DevCtx &c, u8 *p, Hdr64
     // outer destination (the ICMP checksum has no pseudo-header)
     h.s32(30, oip);
     h.s16(24, csum_upd32(h.b16(24), isrc, oip));
-    // quoted source address and its header checksum, then the quoted port / id; every changed word of the ICMP
-    // message goes into the ICMP checksum, in this order
-    const u16 ihc = h.b16(52), ihc2 = csum_upd32(ihc, isrc, oip);
-    h.s32(54, oip);
-    h.s16(52, ihc2);
-    u16 ic = csum_upd32(h.b16(36), isrc, oip);
-    ic = csum_upd16(ic, ihc, ihc2);
-    ic = csum_upd16(ic, pport, oport);
-    bool c4 = true; // chunk 4 changed
-    if (iproto == 1) {
-        const u16 k0 = (u16)x.x, k1 = csum_upd16(k0, pport, oport);
-        x.x = (u32)k1 | ((u32)oport << 16);
-        ic = csum_upd16(ic, k0, k1);
-    } else {
-        h.s16(62, oport);
-        if (iproto == 17 && dlen >= 70 && (u16)x.y != 0) {
-            const u16 k0 = (u16)x.y;
-            u16 k1 = csum_upd16(csum_upd32(k0, isrc, oip), pport, oport);
-            if (k1 == 0) k1 = 0xffff;
-            x.y = (x.y & 0xffff0000u) | k1;
-            ic = csum_upd16(ic, k0, k1);
-        } else if (iproto == 6 && dlen >= 80) {
-            const u16 k0 = (u16)(x.w >> 16), k1 = csum_upd16(csum_upd32(k0, isrc, oip), pport, oport);
-            x.w = (x.w & 0xffffu) | ((u32)k1 << 16);
-            ic = csum_upd16(ic, k0, k1);
-        } else {
-            c4 = false;
-        }
-    }
-    h.s16(36, ic);
+    const bool c4 = icmp_quote_rewrite<54, 62>(h, x, iproto, dlen, isrc, oip, pport, oport);
     hdr_store_chunk(h, p, 1);
     hdr_store_chunk(h, p, 2);
     hdr_store_chunk(h, p, 3);
     if (c4) *(uint4 *)(p + 64) = x;
+    return true;
+}
+
+// bng_nat_icmp_errors_egress_enable: an ICMP error frame a subscriber sends about a frame it received, translated by
+// the flow it quotes (include/bng_b200.h, DESIGN.md §24).  The caller has established that p is an ICMP error frame
+// (untagged IPv4, outer ihl 5, protocol 1, type 3 / 11 / 12, bytes through 41 present) from a private source with a
+// subscriber_nat entry.  Bytes 16-79 are loaded here.  The nat_sessions key is the one nat44_egress created for the
+// flow the quoted packet belongs to: one probe, no nat_reverse step.  Returns whether the frame was translated; the
+// session is only read (no refresh, no counter), and nothing is created.  Otherwise the frame is untouched.
+__device__ __forceinline__ bool nat_icmp_error_egress_one(const DevCtx &c, u8 *p, u32 dlen) {
+    if (dlen < 66) return false; // the quoted ports end at 65: nothing shorter is translatable
+    Hdr64 h;
+    h.w[0] = h.w[1] = h.w[2] = h.w[3] = 0; // (chunk 0 is neither read nor stored)
+#pragma unroll
+    for (int k = 1; k < 4; k++) {
+        const uint4 v = *(const uint4 *)(p + 16 * k);
+        h.w[4 * k] = v.x, h.w[4 * k + 1] = v.y, h.w[4 * k + 2] = v.z, h.w[4 * k + 3] = v.w;
+    }
+    uint4 x = *(const uint4 *)(p + 64); // x.x = bytes 64-67, x.y = 68-71, x.w = 76-79
+    const u32 iproto = h.b8(51), isrc = h.b32(54), idst = h.b32(58), osrc = h.b32(26);
+    // quoted IPv4 header without options, quoting a packet sent to the error's source, the lookup's bytes present
+    if (h.b8(42) != 0x45 || (iproto != 6 && iproto != 17 && iproto != 1) || idst != osrc) return false;
+    if (iproto == 1 && dlen < 68) return false;
+    // the private port: quoted destination port or ICMP id
+    const u16 pport = iproto == 1 ? (u16)(x.x >> 16) : (u16)x.x;
+    u64 key[2]; // nat44_egress's key for the flow (bpf/nat44.c:655-665)
+    key[0] = (u64)idst | ((u64)isrc << 32);
+    key[1] = (u64)pport | ((u64)(iproto == 1 ? (u16)0 : h.b16(62)) << 16) | ((u64)iproto << 32);
+    const u8 *ses = tbl_find<2, true, true>(c.sessions, key);
+    if (!ses) return false;
+    const u32 nat_ip = *(const u32 *)(ses + SES_NAT_IP);
+    const u16 nat_port = (u16)*(const volatile u32 *)(ses + SES_NAT_PORT);
+    // outer source (the ICMP checksum has no pseudo-header)
+    h.s32(26, nat_ip);
+    h.s16(24, csum_upd32(h.b16(24), osrc, nat_ip));
+    icmp_quote_rewrite<58, 64>(h, x, iproto, dlen, idst, nat_ip, pport, nat_port);
+    hdr_store_chunk(h, p, 1);
+    hdr_store_chunk(h, p, 2);
+    hdr_store_chunk(h, p, 3);
+    *(uint4 *)(p + 64) = x; // the quoted port or ICMP id is always in it
     return true;
 }

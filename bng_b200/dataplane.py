@@ -102,6 +102,7 @@ def load_library() -> C.CDLL:
         "bng_qos_ipv6_enable": ([vp, i32], i32),
         "bng_antispoof_ipv6_prefixes_enable": ([vp, i32], i32),
         "bng_nat_icmp_errors_enable": ([vp, i32], i32),
+        "bng_nat_icmp_errors_egress_enable": ([vp, i32], i32),
         "bng_dhcpv6_enable": ([vp, i32], i32),
         "bng_nd_enable": ([vp, i32], i32),
         "bng_lru_overflow": ([vp], u64),
@@ -159,6 +160,7 @@ EXPORTED_SYMBOLS = (
     "bng_dhcp_lease_census", "bng_dhcp_lease_sweep", "bng_lease_table_rebuilds", "bng_dhcp_lease_addr_order",
     "bng_sub_export", "bng_sub_import", "bng_ipv6_prefix_lengths", "bng_qos_ipv6_enable",
     "bng_nat_icmp_errors_enable", "bng_antispoof_ipv6_prefixes_enable", "bng_dhcpv6_enable", "bng_nd_enable",
+    "bng_nat_icmp_errors_egress_enable",
 )
 
 
@@ -341,6 +343,12 @@ class Dataplane:
         by the flow they quote, from the next run on; off by default (include/bng_b200.h).  Context state: snapshots,
         deltas and hand-over blobs do not carry it."""
         self._chk(self.lib.bng_nat_icmp_errors_enable(self.h, 1 if on else 0), "nat_icmp_errors_enable")
+
+    def nat_icmp_errors_egress_enable(self, on: bool = True):
+        """Translate subscribers' ICMP errors (Destination Unreachable, Time Exceeded, Parameter Problem) in
+        nat44_egress, pipeline_up and pipeline_tc by the flow they quote, from the next run on; off by default
+        (include/bng_b200.h).  Context state: snapshots, deltas and hand-over blobs do not carry it."""
+        self._chk(self.lib.bng_nat_icmp_errors_egress_enable(self.h, 1 if on else 0), "nat_icmp_errors_egress_enable")
 
     def ipv6_prefix_lengths(self) -> np.ndarray:
         """Live subscriber_ipv6 entries per prefix length, u32[129]."""

@@ -1482,6 +1482,9 @@ struct ManagerConfig { // :172-200
     // is context state that no snapshot or delta carries: a standby's Manager sets it too.  false leaves the context's
     // flag as it is.
     bool EnableICMPErrorTranslation = false;
+    // Translate subscribers' (upstream) ICMP errors by the flow they quote (bng_nat_icmp_errors_egress_enable), applied
+    // by Start(); context state as EnableICMPErrorTranslation.  false leaves the context's flag as it is.
+    bool EnableUpstreamICMPErrorTranslation = false;
     std::shared_ptr<Backend> Backend_;
 };
 
@@ -1707,6 +1710,10 @@ class Manager {
         }
         if (cfg_.EnableICMPErrorTranslation) {
             if (int rc = bng_nat_icmp_errors_enable(be_->ctx, 1)) return MapErr("failed to enable ICMP error translation", rc);
+        }
+        if (cfg_.EnableUpstreamICMPErrorTranslation) {
+            if (int rc = bng_nat_icmp_errors_egress_enable(be_->ctx, 1))
+                return MapErr("failed to enable upstream ICMP error translation", rc);
         }
         return Nil();
     }

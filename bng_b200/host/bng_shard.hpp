@@ -502,6 +502,14 @@ class Router {
         dir_->SetICMPErrors(on);
         return 0;
     }
+    // Upstream ICMP error translation (bng_nat_icmp_errors_egress_enable) on every shard.  No steering change:
+    // SteerUpstream goes by source MAC, so a subscriber's error reaches its own shard, which holds the quoted session.
+    // Returns 0 or the first shard's error.
+    int NatICMPErrorsEgressEnable(bool on) {
+        for (auto &s : shards_)
+            if (int r = bng_nat_icmp_errors_egress_enable(s->ctx, on ? 1 : 0)) return r;
+        return 0;
+    }
     // Drains every shard: fn(shard, record, record size) per record, in (batch, frame) order within a shard (batch
     // numbers are per shard).  Returns the number of records or a negative errno.
     template <class F>

@@ -172,13 +172,50 @@ int bng_sweep(bng_ctx *ctx, uint64_t now_ns, uint64_t *expired_out);
  *     state stay): anyone on the path can forge an error, and an error must not keep a flow alive.  No other table,
  *     counter or log record changes, so an error frame's result does not depend on its place in the batch.
  *   - Everything else is as before: frames that are not ICMP error frames (types 0, 8, 4, 5 among them), and
- *     nat44_egress, which still keys an upstream ICMP error by bytes 4-5.  Accounting, idle detection and interception
+ *     nat44_egress, whose upstream ICMP errors bng_nat_icmp_errors_egress_enable covers.  Accounting, idle detection and interception
  *     see a translated error by its new destination, the subscriber's address (captured after DNAT).
  *   - BNG_MEM_HOST with a pinned arena moves bytes 64-79 of an ICMP error frame for nat44_ingress; a fixed-stride
  *     arena of 64-byte slots (a header-split ring) does not hold the quoted ports, so its errors pass unchanged.
  * Off by default: nat44_ingress then runs exactly as before.  The flag is context state: snapshots, deltas and
  * hand-over blobs do not carry it.  Returns 0, or -EINVAL for a NULL ctx. */
 int bng_nat_icmp_errors_enable(bng_ctx *ctx, int on);
+
+/* ---- nat44_egress: subscribers' ICMP errors by the flow they quote (RFC 5508, the upstream direction) ----
+ * nat44_egress keys every ICMPv4 message by bytes 4-5 of its ICMP header, read as an echo id (bpf/nat44.c:643-649).
+ * A subscriber's Destination Unreachable, Time Exceeded or Parameter Problem about a frame it received then creates
+ * a bogus ICMP session (a port, a nat_reverse entry, a SESSION_CREATE record), its bytes 4-5 (a pointer, the MTU) are
+ * overwritten with the NAT port, and its quote still names the private address and port.  on != 0: from the next
+ * bng_prog_run, wherever nat44_egress runs (standalone, pipeline_up, pipeline_tc), the rule below applies at the
+ * session lookup, after the private-source check, the subscriber_nat lookup (otherwise packets_passed) and the
+ * hairpin statistic, which stay as they are.  It applies to an ICMP error frame: untagged Ethernet II, ethertype
+ * 0x0800, protocol 1, ICMP type 3, 11 or 12, the 8-byte ICMP header present.  Offsets as for
+ * bng_nat_icmp_errors_enable: quoted IPv4 header 42-61, quoted L4 header from 62.
+ *   - Translatable: outer ihl 5; quoted version 4 and ihl 5; quoted protocol 6, 17 or 1; quoted destination (58-61)
+ *     = outer source (26-29), so that the quoted flow is the sending subscriber's; and the bytes the lookup needs
+ *     present ("present": min(len, the slot)): through 65 for TCP/UDP, 67 for ICMP.
+ *   - Lookup: one nat_sessions probe with the key nat44_egress created for the flow the quoted packet belongs to:
+ *     {src_ip = quoted destination, dst_ip = quoted source, src_port = quoted destination port (64-65) or the quoted
+ *     ICMP id (66-67), dst_port = quoted source port (62-63), 0 for ICMP, protocol = quoted protocol}.
+ *   - Rewrite, when the session is live (csum_upd32 / csum_upd16 steps): outer source <- nat_ip (outer IPv4
+ *     checksum); quoted destination <- nat_ip (quoted IPv4 checksum); quoted destination port or ICMP id <- nat_port
+ *     (quoted L4 checksum: UDP only when 68-69 are present and non-zero, a result of 0 becoming 0xFFFF; TCP only when
+ *     78-79 are present; ICMP always, for the id alone); and every changed word of the ICMP message into the ICMP
+ *     checksum (36-37), in that order.  ICMPv4 has no pseudo-header, so the outer source is not part of it.
+ *   - Outcome of a translated error: verdict TC_ACT_OK, packets_snat.  The session is not refreshed (last_seen, its
+ *     epoch stamp, packets_out, bytes_out and the TCP state stay), and nothing is created: no session, nat_reverse or
+ *     EIM entry, no port, no log record.
+ *   - Everything else is exactly as before, keyed by bytes 4-5 (an echo-keyed session hit or created): errors that
+ *     are not translatable, errors whose quoted flow has no live session, frames with outer options, types 0, 8, 4
+ *     and 5, and every frame that is not ICMP.  Only the frames the rule translates change.
+ *   - The rule reads the tables as the frames before it in the batch (index order) left them: a flow created, or a
+ *     session evicted, by an earlier frame of the same subscriber is seen, as in sequential execution.
+ *   - Accounting, idle detection and interception see an error by the source address it entered with (captured as
+ *     the subscriber sent it).
+ *   - BNG_MEM_HOST with a pinned arena moves bytes 64-79 of an ICMP error frame for these programs; a fixed-stride
+ *     arena of 64-byte slots (a header-split ring) does not hold the quoted ports, so its errors take today's path.
+ * Off by default: the programs then run exactly as before.  The flag is context state: snapshots, deltas and
+ * hand-over blobs do not carry it.  Returns 0, or -EINVAL for a NULL ctx. */
+int bng_nat_icmp_errors_egress_enable(bng_ctx *ctx, int on);
 
 /* ---- NAT flow-state flush (what a subscriber's release / RADIUS Disconnect needs) ----
  * Removes the NAT flow state of a set of subscriber addresses.  Until it expires, a departed subscriber's flow state
