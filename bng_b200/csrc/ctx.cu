@@ -23,6 +23,7 @@
 
 #include "../../include/bng_b200.h"
 #include "blob.hpp"
+#include "devbuf.hpp"
 #include "kernels.h"
 
 namespace {
@@ -61,25 +62,24 @@ struct bng_ctx {
     std::vector<MapReg> maps;
     std::vector<void *> allocs;
     std::string err;
+    // the batch arrays that L.s points into (ensure_scratch)
+    DevBuf<u32> key_a, key_b, val_a, val_b, qslot, attr;
+    DevBuf<u8> cub_tmp;
     // staging for control-plane commands
-    u8 *io_dev = nullptr;
-    u8 *io_host = nullptr; // pinned
-    size_t io_bytes = 0;
+    DevBuf<u8> io_dev;
+    PinnedBuf<u8> io_host;
     // staging for BNG_MEM_HOST batches
-    u8 *hb_pkts = nullptr;
-    u32 *hb_off = nullptr, *hb_len = nullptr, *hb_prio = nullptr;
-    u64 *hb_now = nullptr;
-    u64 *zc_now[ZC_BUFS] = {};
-    u8 *hb_verdict = nullptr;
-    size_t hb_arena = 0;
-    u32 hb_n = 0;
+    DevBuf<u8> hb_pkts;
+    DevBuf<u32> hb_off, hb_len, hb_prio;
+    DevBuf<u64> hb_now;
+    DevBuf<u8> hb_verdict;
     u64 lost_base[2] = {0, 0};
     // zero-copy pipeline for BNG_MEM_HOST batches in pinned memory: two chunk buffers, three streams
     cudaStream_t s_in = nullptr, s_out = nullptr;
     cudaEvent_t ev_in[ZC_BUFS] = {}, ev_comp[ZC_BUFS] = {}, ev_out[ZC_BUFS] = {};
-    u8 *zc_hdr[ZC_BUFS] = {}, *zc_verdict[ZC_BUFS] = {};
-    u32 *zc_off[ZC_BUFS] = {}, *zc_len[ZC_BUFS] = {}, *zc_len0[ZC_BUFS] = {}, *zc_prio[ZC_BUFS] = {};
-    u32 zc_hb = 0;
+    DevBuf<u8> zc_hdr[ZC_BUFS], zc_verdict[ZC_BUFS];
+    DevBuf<u32> zc_off[ZC_BUFS], zc_len[ZC_BUFS], zc_len0[ZC_BUFS], zc_prio[ZC_BUFS];
+    DevBuf<u64> zc_now[ZC_BUFS];
     u32 zc_chunk = 1u << 18; // frames per chunk of the zero-copy pipeline
     // staged upserts (bng_map_update_staged): per map, keys/values in arrival order, applied at the next batch boundary
     struct Staged {
@@ -92,44 +92,38 @@ struct bng_ctx {
     u64 evict_at_rebuild = 0; // ST_LRU_EVICT when the flow tables were last rebuilt
     // BNG_MEM_DEVICE batches do not synchronise: each one queues a copy of ST_LRU_EVICT into evict_word and records
     // evict_ev; a later call looks at the copy once the event has completed (poll_compact_locked)
-    u64 *evict_word = nullptr; // pinned
+    PinnedBuf<u64> evict_word;
     cudaEvent_t evict_ev = nullptr;
     bool evict_pending = false;
     bool small_dirty = false; // a map feeding the SmallTabs image changed since the image was built
-    // grow-only scratch of map dumps (no cudaMalloc / cudaFree per call)
-    u8 *dump_k = nullptr, *dump_v = nullptr;
-    u32 *dump_c = nullptr;
-    size_t dump_kb = 0, dump_vb = 0;
+    // grow-only scratch of map dumps (no allocation per call)
+    DevBuf<u8> dump_k, dump_v;
+    DevBuf<u32> dump_c;
     // multi-GPU reconciliation (bng_comm_init / bng_sync_reduce)
     ncclComm_t comm = nullptr;
     u32 comm_rank = 0, comm_world = 1;
-    u64 *stats_global = nullptr; // device: all-reduced counter vector
+    DevBuf<u64> stats_global; // all-reduced counter vector
     // per-subscriber traffic accounting (bng_acct_*): records index-aligned with the subscriber directory, allocated
     // by the first bng_acct_enable (or a restore that carries records); acct_progs: bit p = program p is accounted
-    u64 *acct = nullptr;
+    DevBuf<u64> acct;
     u32 acct_progs = 0;
-    u8 *acct_dump_buf = nullptr; // grow-only scratch of bng_acct_dump: records, then addresses
-    u64 acct_dump_cap = 0;
+    DevBuf<u8> acct_dump_buf; // grow-only scratch of bng_acct_dump: records, then addresses
     // per-subscriber idle detection (bng_idle_*, idle.cu): records index-aligned with the subscriber directory, allocated
     // by the first bng_idle_enable / bng_idle_timeout_set (or a restore / delta that carries timeouts); idle_progs: bit
     // p = program p stamps
-    u64 *idle = nullptr;
+    DevBuf<u64> idle;
     u32 idle_progs = 0;
-    u8 *idle_scan_buf = nullptr; // grow-only scratch of bng_idle_scan: records, then addresses, then the count
-    u64 idle_scan_cap = 0;
+    DevBuf<u8> idle_scan_buf; // grow-only scratch of bng_idle_scan: records, then addresses, then the count
     // NAT port-usage census (bng_nat_usage, natuse.cu): scratch allocated by the first call (nu_sum != null)
-    u64 *nu_set = nullptr, *nu_pub = nullptr, *nu_sum = nullptr;
-    u32 *nu_sub = nullptr;
+    DevBuf<u64> nu_set, nu_pub, nu_sum;
+    DevBuf<u32> nu_sub;
     u32 nu_set_mask = 0, nu_pub_mask = 0;
-    u8 *nu_out = nullptr; // grow-only: the qualifying records and their addresses
-    u64 nu_out_bytes = 0;
+    DevBuf<u8> nu_out; // grow-only: the qualifying records and their addresses
     // DHCP lease census and sweep (leases.cu): scratch allocated by the first call that needs it
-    u64 *ls_set = nullptr, *ls_pools = nullptr, *ls_sum = nullptr; // the census's (ls_sum != null), kernels.h: LeaseUse
+    DevBuf<u64> ls_set, ls_pools, ls_sum; // the census's (ls_sum != null), kernels.h: LeaseUse
     u32 ls_set_mask = 0, ls_unk_mask = 0;
-    u8 *ls_out = nullptr; // grow-only: the records of either call, then the census's pool ids
-    u64 ls_out_bytes = 0;
-    u64 *ls_macs = nullptr; // grow-only: the sweep's words (LS_W_WORDS), then its MAC set
-    u64 ls_mac_slots = 0;
+    DevBuf<u8> ls_out;   // grow-only: the records of either call, then the census's pool ids
+    DevBuf<u64> ls_macs; // grow-only: the sweep's words (LS_W_WORDS), then its MAC set
     u32 ls_wire = 0; // bng_dhcp_lease_addr_order
     u64 lease_rebuilds = 0; // rebuilds of the lease maps and circuit_id_map (not part of `rebuilds`)
     u64 seq = 0; // the batch sequence in 64 bits (dev.batch_seq holds its low 32): bng_li_record.batch
@@ -140,16 +134,16 @@ struct bng_ctx {
     u32 li_mask = 0;
     bool li_dirty = false;   // the host's targets changed since the device copy was made
     std::unordered_map<u32, u32> li_targets; // authoritative: address -> target id
-    u8 *li_ring = nullptr;
+    DevBuf<u8> li_ring;
     u32 li_cap = 0, li_rec = 0, li_snap = 0;
-    uint2 *li_match = nullptr; // [L.s.cap]
+    DevBuf<uint2> li_match; // [L.s.cap]
     std::vector<u8> li_pending; // records copied out of the ring, ordered, not yet drained
     u64 li_lost_host = 0;       // records discarded by a reconfiguration
     // incremental replication (bng_delta_*, delta.cu).  Exporter: one shadow per hash map (map id), and one of the
     // accounting records (map -1) once they exist; empty while tracking is off.
     struct DeltaShadow {
         int map;
-        u64 *words;
+        DevBuf<u64> words;
         u64 nslots;
         u32 sw;
     };
@@ -158,18 +152,14 @@ struct bng_ctx {
     u64 delta_stream = 0, delta_seq = 0;    // exporter: stream id, sequence of the last export
     std::vector<std::pair<u32, u32>> delta_li; // interception targets as last sent, by address
     bool delta_li_sent = false;
-    u32 *dlist = nullptr;                   // diff lists of one table: deletions at [0, n), upserts at [n, 2n)
-    u64 dlist_slots = 0;
-    u32 *dsent = nullptr;                   // the lists of every table of an export, kept for the commit
-    u64 dsent_cap = 0;
-    u8 *demit = nullptr;                    // records of one table
-    u64 demit_cap = 0;
+    DevBuf<u32> dlist;                      // diff lists of one table: deletions at [0, n), upserts at [n, 2n)
+    DevBuf<u32> dsent;                      // the lists of every table of an export, kept for the commit
+    DevBuf<u8> demit;                       // records of one table
     u64 dapply_stream = 0, dapply_seq = 0;  // applier: the last delta applied
     // subscriber hand-over (bng_sub_export, move.cu): the flow tables' slot lists, allocated by the first export, and
     // a grow-only staging buffer (address set and keys in, gathered entries and lookups out)
-    u32 *mv_lists = nullptr;
-    u8 *mv_buf = nullptr;
-    u64 mv_cap = 0;
+    DevBuf<u32> mv_lists;
+    DevBuf<u8> mv_buf;
     // subscriber_ipv6 (not a map of the reference): IPv6 prefix -> subscriber IPv4 address, the attribution of IPv6
     // frames; v6_live is its live-entry count as of the last command that changed it (0: the IPv6 kernels stay off)
     Tbl v6{};
@@ -265,38 +255,34 @@ int make_table(bng_ctx *c, Tbl *t, u32 key_size, u32 value_size, u32 voff, u32 m
     return dev_alloc(c, (void **)&t->count, 16, 0);
 }
 
-int ensure_scratch(bng_ctx *c, u32 n) {
+// A growth of devbuf.hpp that failed, as the caller's error: -ENOMEM when the allocation was refused, else (a replacing
+// growth's copy or stream synchronisation) -EIO with the runtime's text.
+int grow_failed(bng_ctx *c, const char *what, size_t bytes, const char *of = nullptr, cudaError_t e = cudaErrorMemoryAllocation) {
+    if (e != cudaErrorMemoryAllocation) return fail(c, -EIO, "%s: %s", what, cudaGetErrorString(e));
+    return fail(c, -ENOMEM, "%s: %zu bytes of device memory%s%s", what, bytes, of ? " for the " : "", of ? of : "");
+}
+
+// The batch arrays of L.s for cap frames, all of them or none (L.s then holds null pointers and cap 0).  attr: with the
+// attribution words (accounting, idle detection and interception use them), li: with interception's match list.
+int scratch_locked(bng_ctx *c, u32 cap, bool attr, bool li) {
     Scratch &s = c->L.s;
-    if (n <= s.cap) return 0;
-    u32 cap = std::max<u32>(n, 1024);
-    void **ptrs[] = {(void **)&s.key_a, (void **)&s.key_b, (void **)&s.val_a, (void **)&s.val_b, (void **)&s.qslot, (void **)&s.attr};
-    for (void **pp : ptrs) {
-        if (pp == (void **)&s.attr && !c->acct && !c->idle && !c->li_ctl) continue; // the attribution words exist once accounting, idle detection or interception does
-        if (*pp) cudaFree(*pp);
-        CU(c, cudaMalloc(pp, (size_t)cap * 4));
-    }
-    if (c->li_ctl) {
-        if (c->li_match) cudaFree(c->li_match);
-        CU(c, cudaMalloc((void **)&c->li_match, (size_t)cap * sizeof(uint2)));
-    }
-    if (s.cub_tmp) cudaFree(s.cub_tmp);
-    s.cub_tmp_bytes = sort_temp_bytes(cap);
-    CU(c, cudaMalloc(&s.cub_tmp, s.cub_tmp_bytes ? s.cub_tmp_bytes : 16));
-    s.cap = cap;
-    return 0;
+    const size_t w = (size_t)cap * 4, m = li ? (size_t)cap * sizeof(uint2) : 0, sort = std::max<size_t>(sort_temp_bytes(cap), 16);
+    const bool ok = devbuf::grow_all({{&c->key_a, w}, {&c->key_b, w}, {&c->val_a, w}, {&c->val_b, w}, {&c->qslot, w},
+                                      {&c->attr, attr ? w : 0}, {&c->li_match, m}, {&c->cub_tmp, sort}});
+    s.key_a = c->key_a, s.key_b = c->key_b, s.val_a = c->val_a, s.val_b = c->val_b, s.qslot = c->qslot, s.attr = c->attr;
+    s.cub_tmp = c->cub_tmp, s.cub_tmp_bytes = ok ? sort_temp_bytes(cap) : 0;
+    s.cap = ok ? cap : 0;
+    return ok ? 0 : grow_failed(c, "batch scratch", (attr ? 6 : 5) * w + m + sort);
+}
+
+int ensure_scratch(bng_ctx *c, u32 n) {
+    if (n <= c->L.s.cap) return 0;
+    return scratch_locked(c, std::max<u32>(n, 1024), c->acct || c->idle || c->li_ctl, c->li_ctl);
 }
 
 int ensure_io(bng_ctx *c, size_t bytes) {
-    if (bytes <= c->io_bytes) return 0;
-    size_t nb = std::max<size_t>(bytes, 1 << 20);
-    if (c->io_dev) cudaFree(c->io_dev);
-    if (c->io_host) cudaFreeHost(c->io_host);
-    c->io_dev = nullptr;
-    c->io_host = nullptr;
-    c->io_bytes = 0;
-    CU(c, cudaMalloc((void **)&c->io_dev, nb));
-    CU(c, cudaMallocHost((void **)&c->io_host, nb));
-    c->io_bytes = nb;
+    const size_t nb = std::max<size_t>(bytes, 1 << 20);
+    if (!devbuf::grow_all({{&c->io_dev, nb}, {&c->io_host, nb}})) return grow_failed(c, "staging", 2 * nb);
     return 0;
 }
 
@@ -681,21 +667,8 @@ int bng_close(bng_ctx *c) {
             c->comm = nullptr;
         }
         for (void *p : c->allocs) cudaFree(p);
-        Scratch &s = c->L.s;
-        void *sp[] = {s.key_a, s.key_b, s.val_a, s.val_b, s.qslot, s.attr, s.cub_tmp, s.counters, c->acct_dump_buf, c->idle_scan_buf, c->li_ring, c->li_match,
-                      c->io_dev, c->hb_pkts, c->hb_off, c->hb_len, c->hb_prio, c->hb_verdict, c->hb_now, c->dump_k, c->dump_v, c->dump_c,
-                      c->dlist, c->dsent, c->demit, c->nu_set, c->nu_pub, c->nu_sum, c->nu_sub, c->nu_out,
-                      c->ls_set, c->ls_pools, c->ls_sum, c->ls_out, c->ls_macs, c->mv_lists, c->mv_buf};
-        for (void *p : sp)
-            if (p) cudaFree(p);
-        for (auto &s : c->dshadow) cudaFree(s.words);
-        if (c->io_host) cudaFreeHost(c->io_host);
-        if (c->evict_word) cudaFreeHost(c->evict_word);
         if (c->evict_ev) cudaEventDestroy(c->evict_ev);
         for (int i = 0; i < ZC_BUFS; i++) {
-            void *zp[] = {c->zc_hdr[i], c->zc_verdict[i], c->zc_off[i], c->zc_len[i], c->zc_len0[i], c->zc_prio[i], c->zc_now[i]};
-            for (void *p : zp)
-                if (p) cudaFree(p);
             if (c->ev_in[i]) cudaEventDestroy(c->ev_in[i]);
             if (c->ev_comp[i]) cudaEventDestroy(c->ev_comp[i]);
             if (c->ev_out[i]) cudaEventDestroy(c->ev_out[i]);
@@ -704,7 +677,7 @@ int bng_close(bng_ctx *c) {
         if (c->s_out) cudaStreamDestroy(c->s_out);
         if (c->L.stream) cudaStreamDestroy(c->L.stream);
     }
-    delete c;
+    delete c; // and with it the buffers it owns (devbuf.hpp)
     return 0;
 }
 
@@ -802,7 +775,7 @@ bng_ctx *bng_open(const bng_open_opts *o) {
     OPEN_R(dev_alloc(c, (void **)&d.stats, ST_ALL * 8, 0));
     OPEN_R(make_ring(c, &d.spoof_ev, 56, ev_cap, ST_EV_LOST_SPOOF));
     OPEN_R(make_ring(c, &d.natlog_ev, 40, ev_cap, ST_EV_LOST_NATLOG));
-    OPEN_CU(cudaMalloc((void **)&c->L.s.counters, 64));
+    OPEN_R(dev_alloc(c, (void **)&c->L.s.counters, 64, 0));
     OPEN_R(ensure_scratch(c, opts.max_batch ? opts.max_batch : (1u << 22)));
     OPEN_R(ensure_io(c, 1 << 20));
     OPEN_R(dev_alloc(c, (void **)&d.small, sizeof(SmallTabs), 0xFF));
@@ -1183,17 +1156,9 @@ static int64_t map_dump_locked(bng_ctx *c, MapReg *m, void *keys_out, void *valu
     if (m->kind != KIND_HASH) return -EINVAL;
     if (cap == 0) return 0;
     const Tbl &t = *m->tbl;
-    if (cap * t.key_size > c->dump_kb || cap * t.value_size > c->dump_vb || !c->dump_c) {
-        if (c->dump_k) cudaFree(c->dump_k);
-        if (c->dump_v) cudaFree(c->dump_v);
-        c->dump_k = c->dump_v = nullptr;
-        c->dump_kb = c->dump_vb = 0;
-        size_t kb = std::max<size_t>(cap * t.key_size, 1 << 16), vb = std::max<size_t>(cap * t.value_size, 1 << 16);
-        if (cudaMalloc((void **)&c->dump_k, kb) != cudaSuccess || cudaMalloc((void **)&c->dump_v, vb) != cudaSuccess)
-            return fail(c, -ENOMEM, "dump: out of device memory");
-        if (!c->dump_c && cudaMalloc((void **)&c->dump_c, 16) != cudaSuccess) return fail(c, -ENOMEM, "dump: out of device memory");
-        c->dump_kb = kb, c->dump_vb = vb;
-    }
+    const size_t kb = std::max<size_t>(cap * t.key_size, 1 << 16), vb = std::max<size_t>(cap * t.value_size, 1 << 16);
+    if (kb > c->dump_k.size() || vb > c->dump_v.size()) c->dump_k.reset(), c->dump_v.reset(); // both are sized for this dump
+    if (!devbuf::grow_all({{&c->dump_k, kb}, {&c->dump_v, vb}, {&c->dump_c, 16}})) return grow_failed(c, "dump", kb + vb + 16);
     u8 *dk = c->dump_k, *dv = c->dump_v;
     u32 *dc = c->dump_c;
     int rc = 0;
@@ -1303,7 +1268,7 @@ static int dispatch(bng_ctx *c, int prog, const DevBatch &b, const LiSrc &src = 
     default: return -EINVAL;
     }
     // after the program, before anything copies the frames out: the downstream modes read the rewritten headers
-    if (e == cudaSuccess && (acct || idle)) e = run_acct(c->L, c->dev.subdir, b, k_acct_mode[prog], acct ? c->acct : nullptr, idle ? c->idle : nullptr, v6);
+    if (e == cudaSuccess && (acct || idle)) e = run_acct(c->L, c->dev.subdir, b, k_acct_mode[prog], acct ? c->acct.get() : nullptr, idle ? c->idle.get() : nullptr, v6);
     if (e == cudaSuccess && li == 0) e = run_li_verdict(c->L, r, b, pipe ? c->L.s.attr : nullptr);
     if (e == cudaSuccess && li == 1) e = run_li_capture(c->L, r, b, src, false, v6);
     if (e != cudaSuccess) return fail(c, -EIO, "launch %s: %s", k_prog_names[prog], cudaGetErrorString(e));
@@ -1332,30 +1297,19 @@ static int run_host_zero_copy(bng_ctx *c, int prog, bng_batch *bb, u8 *arena_dev
     // The TC programs write below byte 16 only in frames with ihl = 0, but the first 16 bytes are written back all
     // the same: ONE 64-byte PCIe write per frame rather than a 16- and a 32-byte one (what the link counts is TLPs,
     // not bytes).
-    if (!c->s_in) {
-        CU(c, cudaStreamCreateWithFlags(&c->s_in, cudaStreamNonBlocking));
-        CU(c, cudaStreamCreateWithFlags(&c->s_out, cudaStreamNonBlocking));
-        for (int i = 0; i < ZC_BUFS; i++) {
-            CU(c, cudaEventCreateWithFlags(&c->ev_in[i], cudaEventDisableTiming));
-            CU(c, cudaEventCreateWithFlags(&c->ev_comp[i], cudaEventDisableTiming));
-            CU(c, cudaEventCreateWithFlags(&c->ev_out[i], cudaEventDisableTiming));
-            CU(c, cudaMalloc((void **)&c->zc_off[i], ZC_CHUNK * 4));
-            CU(c, cudaMalloc((void **)&c->zc_len[i], ZC_CHUNK * 4));
-            CU(c, cudaMalloc((void **)&c->zc_len0[i], ZC_CHUNK * 4));
-            CU(c, cudaMalloc((void **)&c->zc_prio[i], ZC_CHUNK * 4));
-            CU(c, cudaMalloc((void **)&c->zc_verdict[i], ZC_CHUNK));
-            CU(c, cudaMalloc((void **)&c->zc_now[i], (size_t)ZC_CHUNK * 8));
-        }
+    for (cudaStream_t *st : {&c->s_in, &c->s_out})
+        if (!*st) CU(c, cudaStreamCreateWithFlags(st, cudaStreamNonBlocking));
+    for (int i = 0; i < ZC_BUFS; i++)
+        for (cudaEvent_t *ev : {&c->ev_in[i], &c->ev_comp[i], &c->ev_out[i]})
+            if (!*ev) CU(c, cudaEventCreateWithFlags(ev, cudaEventDisableTiming));
+    devbuf::Want zc[ZC_BUFS * 7];
+    const size_t cw = (size_t)ZC_CHUNK * 4, hdr = (size_t)ZC_CHUNK * hb + 64;
+    for (int i = 0; i < ZC_BUFS; i++) {
+        devbuf::Want *w = zc + 7 * i;
+        w[0] = {&c->zc_off[i], cw}, w[1] = {&c->zc_len[i], cw}, w[2] = {&c->zc_len0[i], cw}, w[3] = {&c->zc_prio[i], cw};
+        w[4] = {&c->zc_verdict[i], ZC_CHUNK}, w[5] = {&c->zc_now[i], (size_t)ZC_CHUNK * 8}, w[6] = {&c->zc_hdr[i], hdr};
     }
-    if (c->zc_hb < hb) {
-        for (int i = 0; i < ZC_BUFS; i++) {
-            if (c->zc_hdr[i]) cudaFree(c->zc_hdr[i]);
-            c->zc_hdr[i] = nullptr;
-        }
-        c->zc_hb = 0;
-        for (int i = 0; i < ZC_BUFS; i++) CU(c, cudaMalloc((void **)&c->zc_hdr[i], (size_t)ZC_CHUNK * hb + 64));
-        c->zc_hb = hb;
-    }
+    if (!devbuf::grow_all(zc)) return grow_failed(c, "zero-copy staging", ZC_BUFS * (6 * cw + hdr));
     cudaStream_t sc = c->L.stream;
     const u32 nchunks = (bb->n + ZC_CHUNK - 1) / ZC_CHUNK;
     // BNG_ZC_TRACE=1: a timeline of the three stages of every chunk on stderr (timing events on the three streams)
@@ -1386,7 +1340,7 @@ static int run_host_zero_copy(bng_ctx *c, int prog, bng_batch *bb, u8 *arena_dev
             CU(c, cudaMemcpyAsync(c->zc_hdr[buf], (u8 *)bb->pkts + (size_t)base * hb, (size_t)cn * hb, cudaMemcpyHostToDevice,
                                   c->s_in));
         } else {
-            CU(c, run_gather_frames(c->s_in, c->L.num_sms, chunk_arena, bb->off16 ? c->zc_off[buf] : nullptr, c->zc_len[buf],
+            CU(c, run_gather_frames(c->s_in, c->L.num_sms, chunk_arena, bb->off16 ? c->zc_off[buf].get() : nullptr, c->zc_len[buf],
                                     bb->stride, cn, hb, tc,
                                     (prog == P_NAT_IN && c->nat_icmp) ||
                                         ((prog == P_NAT_EG || prog == P_PIPE_UP || prog == P_PIPE_TC) && c->nat_icmp_eg),
@@ -1403,18 +1357,18 @@ static int run_host_zero_copy(bng_ctx *c, int prog, bng_batch *bb, u8 *arena_dev
         b.off16 = nullptr;
         b.len = c->zc_len[buf];
         b.verdict = c->zc_verdict[buf];
-        b.priority = bb->priority ? c->zc_prio[buf] : nullptr;
+        b.priority = bb->priority ? c->zc_prio[buf].get() : nullptr;
         b.n = cn;
         b.stride = hb;
         b.now = bb->now_ns;
-        b.nowv = bb->now_ns_v ? c->zc_now[buf] : nullptr;
+        b.nowv = bb->now_ns_v ? c->zc_now[buf].get() : nullptr;
         b.base = base;
         b.cap = hb; // bounds checks never look past a compact slot (a no-op for whole frames: hostio.cu)
         b.arena_len = (u64)cn * hb;
         // interception copies the bytes past the compact copy straight from the host arena
-        const LiSrc src{chunk_arena, bb->off16 ? c->zc_off[buf] : nullptr, contiguous ? nullptr : c->zc_len0[buf], bb->stride};
+        const LiSrc src{chunk_arena, bb->off16 ? c->zc_off[buf].get() : nullptr, contiguous ? nullptr : c->zc_len0[buf].get(), bb->stride};
         // a DHCPv6 or ND reply may outgrow its request: bounded by the host frame's storage, written back up to its length
-        const FrameRoom room{bb->off16 ? 0u : bb->stride, contiguous ? nullptr : c->zc_len0[buf]};
+        const FrameRoom room{bb->off16 ? 0u : bb->stride, contiguous ? nullptr : c->zc_len0[buf].get()};
         int r = dispatch(c, prog, b, src, &room);
         if (r) return r;
         CU(c, cudaEventRecord(c->ev_comp[buf], sc));
@@ -1426,7 +1380,7 @@ static int run_host_zero_copy(bng_ctx *c, int prog, bng_batch *bb, u8 *arena_dev
             CU(c, cudaMemcpyAsync((u8 *)bb->pkts + (size_t)base * hb, c->zc_hdr[buf], (size_t)cn * hb, cudaMemcpyDeviceToHost,
                                   c->s_out));
         } else {
-            CU(c, run_scatter_frames(c->s_out, c->L.num_sms, chunk_arena, bb->off16 ? c->zc_off[buf] : nullptr, c->zc_len0[buf],
+            CU(c, run_scatter_frames(c->s_out, c->L.num_sms, chunk_arena, bb->off16 ? c->zc_off[buf].get() : nullptr, c->zc_len0[buf],
                                      bb->stride, cn, hb, c->zc_hdr[buf]));
             c->L.launches++;
         }
@@ -1506,38 +1460,21 @@ int bng_prog_run(bng_ctx *c, int prog, bng_batch *bb) {
     size_t arena = bb->off16 ? (size_t)bb->arena_bytes * 16 : (size_t)bb->n * bb->stride;
     if (arena == 0) return -EINVAL;
     cudaStream_t st = c->L.stream;
-    if (arena > c->hb_arena) {
-        if (c->hb_pkts) cudaFree(c->hb_pkts);
-        c->hb_pkts = nullptr;
-        c->hb_arena = 0;
-        CU(c, cudaMalloc((void **)&c->hb_pkts, arena));
-        c->hb_arena = arena;
-    }
-    if (bb->n > c->hb_n) {
-        void **pp[] = {(void **)&c->hb_off, (void **)&c->hb_len, (void **)&c->hb_prio, (void **)&c->hb_verdict, (void **)&c->hb_now};
-        for (void **p : pp) {
-            if (*p) cudaFree(*p);
-            *p = nullptr;
-        }
-        c->hb_n = 0;
-        CU(c, cudaMalloc((void **)&c->hb_off, (size_t)bb->n * 4));
-        CU(c, cudaMalloc((void **)&c->hb_len, (size_t)bb->n * 4));
-        CU(c, cudaMalloc((void **)&c->hb_prio, (size_t)bb->n * 4));
-        CU(c, cudaMalloc((void **)&c->hb_verdict, (size_t)bb->n));
-        CU(c, cudaMalloc((void **)&c->hb_now, (size_t)bb->n * 8));
-        c->hb_n = bb->n;
-    }
+    const size_t fw = (size_t)bb->n * 4;
+    if (!devbuf::grow_all({{&c->hb_pkts, arena}, {&c->hb_off, fw}, {&c->hb_len, fw}, {&c->hb_prio, fw}, {&c->hb_verdict, bb->n},
+                           {&c->hb_now, (size_t)bb->n * 8}}))
+        return grow_failed(c, "host staging", arena + (size_t)bb->n * 21);
     CU(c, cudaMemcpyAsync(c->hb_pkts, bb->pkts, arena, cudaMemcpyHostToDevice, st));
     if (bb->off16) CU(c, cudaMemcpyAsync(c->hb_off, bb->off16, (size_t)bb->n * 4, cudaMemcpyHostToDevice, st));
     CU(c, cudaMemcpyAsync(c->hb_len, bb->len, (size_t)bb->n * 4, cudaMemcpyHostToDevice, st));
     if (bb->priority) CU(c, cudaMemcpyAsync(c->hb_prio, bb->priority, (size_t)bb->n * 4, cudaMemcpyHostToDevice, st));
     if (bb->now_ns_v) CU(c, cudaMemcpyAsync(c->hb_now, bb->now_ns_v, (size_t)bb->n * 8, cudaMemcpyHostToDevice, st));
-    b.nowv = bb->now_ns_v ? c->hb_now : nullptr;
+    b.nowv = bb->now_ns_v ? c->hb_now.get() : nullptr;
     b.pkts = c->hb_pkts;
-    b.off16 = bb->off16 ? c->hb_off : nullptr;
+    b.off16 = bb->off16 ? c->hb_off.get() : nullptr;
     b.len = c->hb_len;
     b.verdict = c->hb_verdict;
-    b.priority = bb->priority ? c->hb_prio : nullptr;
+    b.priority = bb->priority ? c->hb_prio.get() : nullptr;
     r = dispatch(c, prog, b);
     if (r) return r;
     CU(c, cudaMemcpyAsync(bb->pkts, c->hb_pkts, arena, cudaMemcpyDeviceToHost, st));
@@ -1633,10 +1570,7 @@ int bng_sync_reduce(bng_ctx *c, uint64_t *totals_out) {
     std::lock_guard<std::mutex> g(c->mu);
     cudaSetDevice(c->device);
     int fr = flush_staged_locked(c, -1);
-    if (!c->stats_global) {
-        CU(c, cudaMalloc((void **)&c->stats_global, ST_ALL * 8));
-        c->allocs.push_back(c->stats_global);
-    }
+    if (!c->stats_global.grow(ST_ALL * 8)) return grow_failed(c, "sync_reduce", ST_ALL * 8);
     if (c->comm) {
         NcclApi *a = nccl_api();
         ncclResult_t r = a->AllReduce(c->dev.stats, c->stats_global, ST_ALL, ncclUint64, ncclSum, c->comm, c->L.stream);
@@ -1660,27 +1594,19 @@ static int table_rebuild_locked(bng_ctx *c, Tbl *t, bool flow = true) {
     nw.lru = LRU_NONE;
     nw.max_entries = nw.mask; // the copy must never refuse or evict
     size_t bytes = ((size_t)t->mask + 1) * t->slot_bytes;
-    CU(c, cudaMalloc((void **)&nw.slots, bytes));
-    u32 *cnt = nullptr;
-    cudaError_t e = cudaMalloc((void **)&cnt, 16);
-    if (e != cudaSuccess) {
-        cudaFree(nw.slots);
-        return fail(c, -ENOMEM, "rebuild: out of device memory");
-    }
-    nw.count = cnt;
-    e = cudaMemsetAsync(nw.slots, 0xFF, bytes, c->L.stream);
+    DevBuf<u8> slots;
+    DevBuf<u32> cnt;
+    if (!devbuf::grow_all({{&slots, bytes}, {&cnt, 16}})) return grow_failed(c, "rebuild", bytes + 16);
+    nw.slots = slots, nw.count = cnt;
+    cudaError_t e = cudaMemsetAsync(nw.slots, 0xFF, bytes, c->L.stream);
     if (e == cudaSuccess) e = cudaMemsetAsync(cnt, 0, 16, c->L.stream);
     if (e == cudaSuccess) e = run_table_rebuild(c->L, *t, nw);
     if (e == cudaSuccess) e = cudaStreamSynchronize(c->L.stream);
-    cudaFree(cnt);
-    if (e != cudaSuccess) {
-        cudaFree(nw.slots);
-        return fail(c, -EIO, "rebuild: %s", cudaGetErrorString(e));
-    }
+    if (e != cudaSuccess) return fail(c, -EIO, "rebuild: %s", cudaGetErrorString(e));
     for (auto &p : c->allocs)
         if (p == t->slots) p = nw.slots;
-    cudaFree(t->slots);
-    t->slots = nw.slots;
+    DevBuf<u8> old(t->slots, bytes); // the table's slots before the rebuild, freed on return
+    t->slots = slots.release();
     (flow ? c->rebuilds : c->lease_rebuilds)++;
     return 0;
 }
@@ -1711,7 +1637,7 @@ static int maybe_compact_locked(bng_ctx *c) {
 // the next bng_prog_run / bng_sweep applies the rule to it if the copy has landed by then (else a later call does).
 // The steady state costs one 8-byte copy per batch and no host wait; only a rebuild itself synchronises.
 static int queue_evict_read_locked(bng_ctx *c) {
-    if (!c->evict_word) CU(c, cudaHostAlloc((void **)&c->evict_word, 8, cudaHostAllocDefault));
+    if (!c->evict_word.grow(8)) return grow_failed(c, "evict_word", 8);
     if (!c->evict_ev) CU(c, cudaEventCreateWithFlags(&c->evict_ev, cudaEventDisableTiming));
     CU(c, cudaMemcpyAsync(c->evict_word, c->dev.stats + ST_LRU_EVICT, 8, cudaMemcpyDeviceToHost, c->L.stream));
     CU(c, cudaEventRecord(c->evict_ev, c->L.stream));
@@ -1785,7 +1711,7 @@ int bng_nat_flush(bng_ctx *c, const uint32_t *addrs, uint64_t n, uint64_t now_ns
     int r = flow_pass_begin_locked(c);
     if (r) return r;
     if ((r = ensure_io(c, slots * 8)) != 0) return r;
-    u64 *set = (u64 *)c->io_host;
+    u64 *set = (u64 *)c->io_host.get();
     memset(set, 0, slots * 8);
     const u32 mask = (u32)(slots - 1);
     for (u64 k = 0; k < n; k++) {
@@ -1796,7 +1722,7 @@ int bng_nat_flush(bng_ctx *c, const uint32_t *addrs, uint64_t n, uint64_t now_ns
     CU(c, cudaMemcpyAsync(c->io_dev, c->io_host, slots * 8, cudaMemcpyHostToDevice, c->L.stream));
     u32 *cnt = c->L.s.counters + 8; // scratch words 8.. are free between program runs
     CU(c, cudaMemsetAsync(cnt, 0, 16, c->L.stream));
-    CU(c, run_nat_flush(c->L, c->dev, AddrSet{(const u64 *)c->io_dev, mask}, now_ns, cnt));
+    CU(c, run_nat_flush(c->L, c->dev, AddrSet{(const u64 *)c->io_dev.get(), mask}, now_ns, cnt));
     u32 got[4] = {0, 0, 0, 0};
     CU(c, cudaMemcpyAsync(got, cnt, 16, cudaMemcpyDeviceToHost, c->L.stream));
     CU(c, cudaStreamSynchronize(c->L.stream));
@@ -1874,14 +1800,11 @@ static_assert(sizeof(bng_acct) == ACCT_WORDS * 8, "struct bng_acct is the device
 // The records (one per directory slot) and the per-frame attribution words, on first use.
 static int acct_alloc_locked(bng_ctx *c) {
     if (c->acct) return 0;
-    Scratch &s = c->L.s;
-    if (!s.attr) CU(c, cudaMalloc((void **)&s.attr, (size_t)s.cap * 4));
-    u64 *a = nullptr;
+    // a failure releases the whole batch scratch (all or none): the next batch grows it again for its own size
+    if (int r = scratch_locked(c, c->L.s.cap, true, c->li_ctl)) return r;
     const size_t bytes = ((size_t)c->dev.subdir.mask + 1) * sizeof(bng_acct);
-    if (cudaMalloc((void **)&a, bytes) != cudaSuccess) return fail(c, -ENOMEM, "accounting: %zu bytes of device memory", bytes);
-    c->allocs.push_back(a);
-    CU(c, cudaMemsetAsync(a, 0, bytes, c->L.stream));
-    c->acct = a;
+    if (!c->acct.grow(bytes)) return grow_failed(c, "accounting", bytes);
+    CU(c, cudaMemsetAsync(c->acct, 0, bytes, c->L.stream));
     return 0;
 }
 
@@ -1896,13 +1819,7 @@ static int64_t acct_dump_locked(bng_ctx *c, uint32_t *addrs_out, bng_acct *out, 
     if (cap == 0) return 0;
     const u64 ecap = std::min<u64>(cap, (u64)c->dev.subdir.mask + 1); // no more entries than slots
     const size_t aoff = ecap * sizeof(bng_acct), coff = (aoff + ecap * 4 + 15) & ~(size_t)15, need = coff + 16;
-    if (need > c->acct_dump_cap) {
-        if (c->acct_dump_buf) cudaFree(c->acct_dump_buf);
-        c->acct_dump_buf = nullptr;
-        c->acct_dump_cap = 0;
-        if (cudaMalloc((void **)&c->acct_dump_buf, need) != cudaSuccess) return fail(c, -ENOMEM, "acct_dump: out of device memory");
-        c->acct_dump_cap = need;
-    }
+    if (!c->acct_dump_buf.grow(need)) return grow_failed(c, "acct_dump", need);
     u8 *buf = c->acct_dump_buf;
     u32 *cnt = (u32 *)(buf + coff), n = 0;
     CU(c, cudaMemsetAsync(cnt, 0, 4, c->L.stream));
@@ -1943,7 +1860,7 @@ int bng_acct_read(bng_ctx *c, const uint32_t *addrs, uint64_t n, bng_acct *out, 
         if (int r = ensure_io(c, roff + k * 4)) return r;
         memcpy(c->io_host, addrs + done, k * 4);
         CU(c, cudaMemcpyAsync(c->io_dev, c->io_host, k * 4, cudaMemcpyHostToDevice, c->L.stream));
-        CU(c, run_acct_read(c->L, c->dev.subdir, c->acct, (const u32 *)c->io_dev, k, (u64 *)(c->io_dev + ooff), (int *)(c->io_dev + roff)));
+        CU(c, run_acct_read(c->L, c->dev.subdir, c->acct, (const u32 *)c->io_dev.get(), k, (u64 *)(c->io_dev + ooff), (int *)(c->io_dev + roff)));
         CU(c, cudaMemcpyAsync(c->io_host + ooff, c->io_dev + ooff, roff + k * 4 - ooff, cudaMemcpyDeviceToHost, c->L.stream));
         CU(c, cudaStreamSynchronize(c->L.stream));
         memcpy(out + done, c->io_host + ooff, k * sizeof(bng_acct));
@@ -1968,17 +1885,11 @@ static_assert(sizeof(bng_idle) == IDLE_WORDS * 8, "struct bng_idle has the size 
 // The records (one per directory slot, every field none) and the per-frame attribution words, on first use.
 static int idle_alloc_locked(bng_ctx *c) {
     if (c->idle) return 0;
-    Scratch &s = c->L.s;
-    if (!s.attr) CU(c, cudaMalloc((void **)&s.attr, (size_t)s.cap * 4));
-    u64 *a = nullptr;
+    // a failure releases the whole batch scratch (all or none): the next batch grows it again for its own size
+    if (int r = scratch_locked(c, c->L.s.cap, true, c->li_ctl)) return r;
     const size_t bytes = ((size_t)c->dev.subdir.mask + 1) * sizeof(bng_idle);
-    if (cudaMalloc((void **)&a, bytes) != cudaSuccess) {
-        cudaGetLastError();
-        return fail(c, -ENOMEM, "idle detection: %zu bytes of device memory", bytes);
-    }
-    c->allocs.push_back(a);
-    CU(c, cudaMemsetAsync(a, 0, bytes, c->L.stream));
-    c->idle = a;
+    if (!c->idle.grow(bytes)) return grow_failed(c, "idle detection", bytes);
+    CU(c, cudaMemsetAsync(c->idle, 0, bytes, c->L.stream));
     return 0;
 }
 
@@ -1999,7 +1910,7 @@ static int idle_timeouts_locked(bng_ctx *c, const uint32_t *addrs, const uint32_
         memcpy(c->io_host, addrs + done, k * 4);
         memcpy(c->io_host + toff, timeouts + done, k * 4);
         CU(c, cudaMemcpyAsync(c->io_dev, c->io_host, toff + k * 4, cudaMemcpyHostToDevice, c->L.stream));
-        CU(c, run_idle_timeout_set(c->L, c->dev.subdir, c->idle, (const u32 *)c->io_dev, (const u32 *)(c->io_dev + toff), k,
+        CU(c, run_idle_timeout_set(c->L, c->dev.subdir, c->idle, (const u32 *)c->io_dev.get(), (const u32 *)(c->io_dev + toff), k,
                                    (int *)(c->io_dev + roff)));
         if (results) CU(c, cudaMemcpyAsync(c->io_host + roff, c->io_dev + roff, k * 4, cudaMemcpyDeviceToHost, c->L.stream));
         CU(c, cudaStreamSynchronize(c->L.stream));
@@ -2017,7 +1928,7 @@ static int idle_read_locked(bng_ctx *c, const uint32_t *addrs, uint64_t n, bng_i
         if (int r = ensure_io(c, roff + k * 4)) return r;
         memcpy(c->io_host, addrs + done, k * 4);
         CU(c, cudaMemcpyAsync(c->io_dev, c->io_host, k * 4, cudaMemcpyHostToDevice, c->L.stream));
-        CU(c, run_idle_read(c->L, c->dev.subdir, c->idle, (const u32 *)c->io_dev, k, (u64 *)(c->io_dev + ooff), (int *)(c->io_dev + roff)));
+        CU(c, run_idle_read(c->L, c->dev.subdir, c->idle, (const u32 *)c->io_dev.get(), k, (u64 *)(c->io_dev + ooff), (int *)(c->io_dev + roff)));
         CU(c, cudaMemcpyAsync(c->io_host + ooff, c->io_dev + ooff, roff + k * 4 - ooff, cudaMemcpyDeviceToHost, c->L.stream));
         CU(c, cudaStreamSynchronize(c->L.stream));
         memcpy(out + done, c->io_host + ooff, k * sizeof(bng_idle));
@@ -2087,16 +1998,7 @@ int64_t bng_idle_scan(bng_ctx *c, uint64_t now_ns, uint32_t default_s, uint32_t 
     if (!c->idle) return 0; // no record exists yet: nobody can be idle
     const u64 ecap = std::min<u64>(cap, (u64)c->dev.subdir.mask + 1); // no more entries than slots
     const size_t aoff = ecap * sizeof(bng_idle), coff = (aoff + ecap * 4 + 15) & ~(size_t)15, need = coff + 16;
-    if (need > c->idle_scan_cap) {
-        if (c->idle_scan_buf) cudaFree(c->idle_scan_buf);
-        c->idle_scan_buf = nullptr;
-        c->idle_scan_cap = 0;
-        if (cudaMalloc((void **)&c->idle_scan_buf, need) != cudaSuccess) {
-            cudaGetLastError();
-            return fail(c, -ENOMEM, "idle_scan: out of device memory");
-        }
-        c->idle_scan_cap = need;
-    }
+    if (!c->idle_scan_buf.grow(need)) return grow_failed(c, "idle_scan", need);
     u8 *buf = c->idle_scan_buf;
     u32 *cnt = (u32 *)(buf + coff), n = 0;
     CU(c, cudaMemsetAsync(cnt, 0, 4, c->L.stream));
@@ -2117,15 +2019,6 @@ int64_t bng_idle_scan(bng_ctx *c, uint64_t now_ns, uint32_t default_s, uint32_t 
 static_assert(sizeof(bng_nat_sub_use) == 64 && sizeof(bng_nat_pub_use) == 64, "the census writes 16 u32 per record");
 static_assert(sizeof(bng_nat_usage_sum) == (NU_PUBS_FOUND + 1) * 8, "struct bng_nat_usage_sum is the head of the census's sum words");
 
-static int nu_malloc(bng_ctx *c, void **p, size_t bytes, const char *what) {
-    if (cudaMalloc(p, bytes) != cudaSuccess) {
-        cudaGetLastError();
-        *p = nullptr;
-        return fail(c, -ENOMEM, "nat_usage: %zu bytes of device memory for the %s", bytes, what);
-    }
-    return 0;
-}
-
 static u64 nu_pow2(u64 v) {
     u64 p = 64;
     while (p < v) p <<= 1;
@@ -2135,10 +2028,8 @@ static u64 nu_pow2(u64 v) {
 // the public-address table: pub_mask + 1 slots
 static int nu_pub_alloc(bng_ctx *c, u64 slots) {
     if (slots > (1ull << 32)) return fail(c, -ENOMEM, "nat_usage: %llu public-address slots", (unsigned long long)slots);
-    u64 *p = nullptr; // the old table stays when the new one does not fit
-    if (int r = nu_malloc(c, (void **)&p, slots * NU_PUB_WORDS * 8, "public-address table")) return r;
-    if (c->nu_pub) cudaFree(c->nu_pub);
-    c->nu_pub = p;
+    const size_t bytes = slots * NU_PUB_WORDS * 8; // the old table stays when the new one does not fit
+    if (cudaError_t e = c->nu_pub.grow_keep(bytes, 0, c->L.stream)) return grow_failed(c, "nat_usage", bytes, "public-address table", e);
     c->nu_pub_mask = (u32)(slots - 1);
     return 0;
 }
@@ -2152,15 +2043,10 @@ static int nu_alloc_locked(bng_ctx *c) {
     if (set_slots > (1ull << 30) || dir_slots > (1ull << 30))
         return fail(c, -ENOMEM, "nat_usage: %llu set slots / %llu directory slots exceed 2^30", (unsigned long long)set_slots,
                     (unsigned long long)dir_slots);
-    int r = nu_malloc(c, (void **)&c->nu_set, set_slots * 8, "triple set");
-    if (!r) r = nu_malloc(c, (void **)&c->nu_sub, dir_slots * NU_SUB_WORDS * 4, "subscriber counters");
-    if (!r) r = nu_pub_alloc(c, 1u << 16);
-    if (!r) r = nu_malloc(c, (void **)&c->nu_sum, NU_SUM_WORDS * 8, "summary");
-    if (r) {
-        for (void *p : {(void *)c->nu_set, (void *)c->nu_sub, (void *)c->nu_pub})
-            if (p) cudaFree(p);
-        c->nu_set = c->nu_pub = nullptr;
-        c->nu_sub = nullptr;
+    if (!devbuf::grow_all({{&c->nu_set, set_slots * 8}, {&c->nu_sub, dir_slots * NU_SUB_WORDS * 4}, {&c->nu_sum, NU_SUM_WORDS * 8}}))
+        return grow_failed(c, "nat_usage", set_slots * 8 + dir_slots * NU_SUB_WORDS * 4 + NU_SUM_WORDS * 8, "census");
+    if (int r = nu_pub_alloc(c, 1u << 16)) {
+        c->nu_set.reset(), c->nu_sub.reset(), c->nu_sum.reset();
         return r;
     }
     c->nu_set_mask = (u32)(set_slots - 1);
@@ -2181,16 +2067,11 @@ int bng_nat_usage(bng_ctx *c, uint32_t min_permille, bng_nat_usage_sum *sum, uin
     for (;;) {
         const u64 pcap = std::min<u64>(pub_cap, (u64)c->nu_pub_mask + 1);
         const u64 rec_b = (scap + pcap) * 64, need = rec_b + (scap + pcap) * 4;
-        if (need > c->nu_out_bytes) {
-            if (c->nu_out) cudaFree(c->nu_out);
-            c->nu_out_bytes = 0;
-            if ((r = nu_malloc(c, (void **)&c->nu_out, need, "records")) != 0) return r;
-            c->nu_out_bytes = need;
-        }
+        if (!c->nu_out.grow(need)) return grow_failed(c, "nat_usage", need, "records");
         NatUse u{};
         u.set = c->nu_set, u.set_mask = c->nu_set_mask, u.sub = c->nu_sub, u.pub = c->nu_pub, u.pub_mask = c->nu_pub_mask;
         u.sum = c->nu_sum;
-        u.sub_out = (u32 *)c->nu_out, u.pub_out = (u32 *)(c->nu_out + scap * 64);
+        u.sub_out = (u32 *)c->nu_out.get(), u.pub_out = (u32 *)(c->nu_out + scap * 64);
         u.sub_addrs = (u32 *)(c->nu_out + rec_b), u.pub_addrs = u.sub_addrs + scap;
         u.sub_cap = scap, u.pub_cap = pcap;
         const u64 dir_slots = (u64)c->dev.subdir.mask + 1;
@@ -2232,23 +2113,9 @@ int bng_nat_usage(bng_ctx *c, uint32_t min_permille, bng_nat_usage_sum *sum, uin
 static_assert(sizeof(bng_lease_pool_use) == 64 && sizeof(bng_lease_removed) == 64, "the lease kernels write 16 u32 per record");
 static_assert(sizeof(bng_lease_sum) == (LS_POOLS_FOUND + 1) * 8, "struct bng_lease_sum is the head of the census's sum words");
 
-static int ls_malloc(bng_ctx *c, void **p, size_t bytes, const char *what) {
-    if (cudaMalloc(p, bytes) != cudaSuccess) {
-        cudaGetLastError();
-        *p = nullptr;
-        return fail(c, -ENOMEM, "dhcp leases: %zu bytes of device memory for the %s", bytes, what);
-    }
-    return 0;
-}
-
 // the output records of either call (and the census's pool ids behind them): grow-only
 static int ls_out_locked(bng_ctx *c, u64 bytes) {
-    if (bytes <= c->ls_out_bytes) return 0;
-    if (c->ls_out) cudaFree(c->ls_out);
-    c->ls_out_bytes = 0;
-    if (int r = ls_malloc(c, (void **)&c->ls_out, bytes, "records")) return r;
-    c->ls_out_bytes = bytes;
-    return 0;
+    return c->ls_out.grow(bytes) ? 0 : grow_failed(c, "dhcp leases", bytes, "records");
 }
 
 // leases.cu reads the lease slots by fixed offsets
@@ -2264,10 +2131,8 @@ static int ls_layout_locked(bng_ctx *c) {
 static int ls_pools_alloc(bng_ctx *c, u64 unk_slots) {
     const u64 n = (u64)c->dev.ip_pools.mask + 1 + unk_slots;
     if (n > (1ull << 26)) return fail(c, -ENOMEM, "lease_census: %llu pool records", (unsigned long long)n);
-    u64 *p = nullptr; // the old records stay when the new ones do not fit
-    if (int r = ls_malloc(c, (void **)&p, n * LS_POOL_WORDS * 8, "pool records")) return r;
-    if (c->ls_pools) cudaFree(c->ls_pools);
-    c->ls_pools = p;
+    const size_t bytes = n * LS_POOL_WORDS * 8; // the old records stay when the new ones do not fit
+    if (cudaError_t e = c->ls_pools.grow_keep(bytes, 0, c->L.stream)) return grow_failed(c, "dhcp leases", bytes, "pool records", e);
     c->ls_unk_mask = (u32)(unk_slots - 1);
     return 0;
 }
@@ -2278,13 +2143,10 @@ static int ls_alloc_locked(bng_ctx *c) {
     const u64 keys = 3ull * ((u64)c->dev.sub_pools.max_entries + c->dev.vlan_pools.max_entries + c->dev.cid_subs.max_entries);
     const u64 set_slots = nu_pow2((keys * 4 + 2) / 3);
     if (set_slots > (1ull << 32)) return fail(c, -ENOMEM, "lease_census: %llu set slots", (unsigned long long)set_slots);
-    int r = ls_malloc(c, (void **)&c->ls_set, set_slots * 8, "address set");
-    if (!r) r = ls_pools_alloc(c, 1u << 14);
-    if (!r) r = ls_malloc(c, (void **)&c->ls_sum, LS_SUM_WORDS * 8, "summary");
-    if (r) {
-        for (void *p : {(void *)c->ls_set, (void *)c->ls_pools})
-            if (p) cudaFree(p);
-        c->ls_set = c->ls_pools = nullptr;
+    if (!devbuf::grow_all({{&c->ls_set, set_slots * 8}, {&c->ls_sum, LS_SUM_WORDS * 8}}))
+        return grow_failed(c, "dhcp leases", set_slots * 8 + LS_SUM_WORDS * 8, "census");
+    if (int r = ls_pools_alloc(c, 1u << 14)) {
+        c->ls_set.reset(), c->ls_sum.reset();
         return r;
     }
     c->ls_set_mask = (u32)(set_slots - 1);
@@ -2306,7 +2168,7 @@ int bng_dhcp_lease_census(bng_ctx *c, uint64_t now_ns, bng_lease_sum *sum, uint3
         const u64 recs = (u64)u.n_known + u.unk_mask + 1;
         u.cap = std::min<u64>(cap, recs); // no more records than record slots
         if ((r = ls_out_locked(c, u.cap * 68)) != 0) return r;
-        u.out = (u32 *)c->ls_out, u.ids_out = (u32 *)(c->ls_out + u.cap * 64);
+        u.out = (u32 *)c->ls_out.get(), u.ids_out = (u32 *)(c->ls_out + u.cap * 64);
         CU(c, cudaMemsetAsync(c->ls_set, 0, ((u64)c->ls_set_mask + 1) * 8, c->L.stream));
         CU(c, cudaMemsetAsync(c->ls_pools, 0, recs * LS_POOL_WORDS * 8, c->L.stream));
         CU(c, cudaMemsetAsync(c->ls_sum, 0, LS_SUM_WORDS * 8, c->L.stream));
@@ -2347,15 +2209,10 @@ int64_t bng_dhcp_lease_sweep(bng_ctx *c, uint64_t now_ns, uint32_t grace_s, bng_
     const u64 mac_slots = nu_pow2(2 * std::min<u64>(ecap, d.sub_pools.max_entries));
     if (mac_slots > (1ull << 32)) return fail(c, -ENOMEM, "lease_sweep: %llu MAC set slots", (unsigned long long)mac_slots);
     if ((r = ls_out_locked(c, ecap * 64)) != 0) return r;
-    if (mac_slots > c->ls_mac_slots) {
-        if (c->ls_macs) cudaFree(c->ls_macs);
-        c->ls_mac_slots = 0;
-        if ((r = ls_malloc(c, (void **)&c->ls_macs, (LS_W_WORDS + mac_slots) * 8, "MAC set")) != 0) return r;
-        c->ls_mac_slots = mac_slots;
-    }
+    if (!c->ls_macs.grow((LS_W_WORDS + mac_slots) * 8)) return grow_failed(c, "dhcp leases", (LS_W_WORDS + mac_slots) * 8, "MAC set");
     LeaseSweep w{};
     w.now_s = now_ns / 1000000000ull, w.grace_s = grace_s, w.cap = ecap;
-    w.out = (u32 *)c->ls_out, w.cnt = c->ls_macs, w.macs = c->ls_macs + LS_W_WORDS, w.mac_mask = (u32)(mac_slots - 1);
+    w.out = (u32 *)c->ls_out.get(), w.cnt = c->ls_macs, w.macs = c->ls_macs + LS_W_WORDS, w.mac_mask = (u32)(mac_slots - 1);
     CU(c, cudaMemsetAsync(c->ls_macs, 0, (LS_W_WORDS + mac_slots) * 8, c->L.stream));
     CU(c, run_lease_sweep(c->L, d, w));
     u64 cnt[LS_W_WORDS];
@@ -2395,21 +2252,14 @@ static_assert(sizeof(bng_li_record) == LI_HDR, "struct bng_li_record is the devi
 static int li_collect_locked(bng_ctx *c);
 static int li_ring_locked(bng_ctx *c, u32 snaplen, u32 cap) {
     const u32 rec = LI_HDR + ((snaplen + 15u) & ~15u);
-    u8 *ring = nullptr;
-    if (cudaMalloc((void **)&ring, (size_t)cap * rec) != cudaSuccess) {
-        cudaGetLastError();
-        return fail(c, -ENOMEM, "li_configure: %zu bytes of device memory", (size_t)cap * rec);
-    }
+    DevBuf<u8> ring;
+    if (!ring.grow((size_t)cap * rec)) return grow_failed(c, "li_configure", (size_t)cap * rec);
     if (c->li_ring) {
-        if (int r = li_collect_locked(c)) {
-            cudaFree(ring);
-            return r;
-        }
+        if (int r = li_collect_locked(c)) return r;
         c->li_lost_host += c->li_pending.size() / c->li_rec;
         c->li_pending.clear();
-        cudaFree(c->li_ring);
     }
-    c->li_ring = ring, c->li_cap = cap, c->li_rec = rec, c->li_snap = snaplen;
+    c->li_ring = std::move(ring), c->li_cap = cap, c->li_rec = rec, c->li_snap = snaplen;
     CU(c, cudaMemsetAsync(c->li_ctl, 0, 8, c->L.stream)); // no slot handed out
     return 0;
 }
@@ -2418,9 +2268,8 @@ static int li_ring_locked(bng_ctx *c, u32 snaplen, u32 cap) {
 // with the given size unless one exists.
 static int li_alloc_locked(bng_ctx *c, u32 snaplen = 1518, u32 cap = 1u << 15) {
     if (!c->li_ctl) {
-        Scratch &s = c->L.s;
-        if (!s.attr) CU(c, cudaMalloc((void **)&s.attr, (size_t)s.cap * 4));
-        CU(c, cudaMalloc((void **)&c->li_match, (size_t)s.cap * sizeof(uint2)));
+        // a failure releases the whole batch scratch (all or none): the next batch grows it again for its own size
+        if (int r = scratch_locked(c, c->L.s.cap, true, true)) return r;
         if (int r = dev_alloc(c, (void **)&c->li_words, LI_TSLOTS * 8, 0)) return r;
         if (int r = dev_alloc(c, (void **)&c->li_ids, LI_TSLOTS * 4, 0)) return r;
         u64 *ctl = nullptr;
@@ -2546,22 +2395,8 @@ uint64_t bng_li_lost(bng_ctx *c) {
 namespace {
 using blob::kAcct, blob::kLi, blob::kIdle;
 
-// a grow-only device buffer of at least `bytes`; keep: bytes at the start that survive the growth
-int dev_grow(bng_ctx *c, const char *what, u8 **p, u64 *cap, u64 bytes, u64 keep = 0) {
-    if (bytes <= *cap) return 0;
-    const u64 nb = std::max<u64>(bytes + bytes / 2, 1 << 20);
-    u8 *q = nullptr;
-    if (cudaMalloc((void **)&q, nb) != cudaSuccess) {
-        cudaGetLastError();
-        return fail(c, -ENOMEM, "%s: %llu bytes of device memory", what, (unsigned long long)nb);
-    }
-    if (keep) CU(c, cudaMemcpyAsync(q, *p, keep, cudaMemcpyDeviceToDevice, c->L.stream));
-    CU(c, cudaStreamSynchronize(c->L.stream));
-    if (*p) cudaFree(*p);
-    *p = q;
-    *cap = nb;
-    return 0;
-}
+// what the grow-only staging of an export allocates when it needs `bytes`: half as much again, at least 1 MiB
+u64 with_slack(u64 bytes) { return std::max<u64>(bytes + bytes / 2, 1 << 20); }
 
 // a non-event map, whole, as one section
 int map_section_locked(bng_ctx *c, MapReg *m, blob::Writer &w) {
@@ -2631,9 +2466,9 @@ int load_records_locked(bng_ctx *c, const u8 *addrs, const u8 *recs, u64 n, size
         memcpy(c->io_host + roff, recs + done * rs, k * rs);
         CU(c, cudaMemcpyAsync(c->io_dev, c->io_host, roff + k * rs, cudaMemcpyHostToDevice, c->L.stream));
         if (acct)
-            CU(c, run_acct_load(c->L, c->dev.subdir, c->acct, (const u32 *)c->io_dev, (const u64 *)(c->io_dev + roff), k));
+            CU(c, run_acct_load(c->L, c->dev.subdir, c->acct, (const u32 *)c->io_dev.get(), (const u64 *)(c->io_dev + roff), k));
         else
-            CU(c, run_idle_load(c->L, c->dev.subdir, c->idle, (const u32 *)c->io_dev, (const u64 *)(c->io_dev + roff), k));
+            CU(c, run_idle_load(c->L, c->dev.subdir, c->idle, (const u32 *)c->io_dev.get(), (const u64 *)(c->io_dev + roff), k));
         CU(c, cudaStreamSynchronize(c->L.stream));
     }
     return 0;
@@ -2773,14 +2608,14 @@ DeltaTbl delta_view(bng_ctx *c, const bng_ctx::DeltaShadow &s, u64 refresh, bool
     auto set = [&](u32 pos) { t.mask[pos / 8] |= 0xFFull << (8 * (pos % 8)); };
     if (s.map == kShadowIdle) { // idle records: the directory's address, then the timeout (no time word; clocks are not sent)
         const Tbl &d = c->dev.subdir;
-        t.slots = d.slots, t.slot_bytes = d.slot_bytes, t.vals = (const u8 *)c->idle, t.vstride = sizeof(bng_idle);
+        t.slots = d.slots, t.slot_bytes = d.slot_bytes, t.vals = (const u8 *)c->idle.get(), t.vstride = sizeof(bng_idle);
         t.kw = 1, t.key_size = 4, t.value_size = 4;
         for (u32 b = 0; b < 4; b++) set(8 + b);
         return t;
     }
     if (s.map < 0) { // accounting records: the directory's address, then the record
         const Tbl &d = c->dev.subdir;
-        t.slots = d.slots, t.slot_bytes = d.slot_bytes, t.vals = (const u8 *)c->acct, t.vstride = sizeof(bng_acct);
+        t.slots = d.slots, t.slot_bytes = d.slot_bytes, t.vals = (const u8 *)c->acct.get(), t.vstride = sizeof(bng_acct);
         t.kw = 1, t.key_size = 4, t.value_size = sizeof(bng_acct);
         for (u32 b = 0; b < sizeof(bng_acct); b++) set(8 + b);
         return t;
@@ -2815,30 +2650,20 @@ int delta_words(const Tbl &t, bool ses) { // shadow words of a slot: through the
 }
 
 int delta_shadow_locked(bng_ctx *c, int map, const Tbl &t, u32 sw) {
-    bng_ctx::DeltaShadow s{map, nullptr, (u64)t.mask + 1, sw};
-    const size_t bytes = s.nslots * sw * 8;
-    if (cudaMalloc((void **)&s.words, bytes) != cudaSuccess) {
-        cudaGetLastError();
-        return fail(c, -ENOMEM, "delta_enable: %zu bytes of device memory for the shadow of %s", bytes, map == kShadowAcct ? kAcct : (map == kShadowIdle ? kIdle : c->maps[map].name));
-    }
-    c->dshadow.push_back(s);
-    CU(c, cudaMemsetAsync(s.words, 0xFF, bytes, c->L.stream)); // every slot empty: nothing sent yet
-    if (s.nslots > c->dlist_slots) {
-        if (c->dlist) cudaFree(c->dlist);
-        c->dlist = nullptr;
-        c->dlist_slots = 0;
-        if (cudaMalloc((void **)&c->dlist, s.nslots * 8) != cudaSuccess) {
-            cudaGetLastError();
-            return fail(c, -ENOMEM, "delta_enable: out of device memory");
-        }
-        c->dlist_slots = s.nslots;
-    }
+    const u64 nslots = (u64)t.mask + 1;
+    const size_t bytes = nslots * sw * 8;
+    DevBuf<u64> words;
+    if (!words.grow(bytes))
+        return grow_failed(c, "delta_enable", bytes,
+                      (std::string("shadow of ") + (map == kShadowAcct ? kAcct : (map == kShadowIdle ? kIdle : c->maps[map].name))).c_str());
+    CU(c, cudaMemsetAsync(words, 0xFF, bytes, c->L.stream)); // every slot empty: nothing sent yet
+    c->dshadow.push_back({map, std::move(words), nslots, sw});
+    if (!c->dlist.grow(nslots * 8)) return grow_failed(c, "delta_enable", nslots * 8);
     return 0;
 }
 
 void delta_free_locked(bng_ctx *c) {
     cudaStreamSynchronize(c->L.stream);
-    for (auto &s : c->dshadow) cudaFree(s.words);
     c->dshadow.clear();
 }
 } // namespace
@@ -2924,8 +2749,11 @@ int bng_delta_export(bng_ctx *c, uint64_t refresh_ns, uint32_t flags, void *buf,
         CU(c, cudaMemcpyAsync(n, cnt, 8, cudaMemcpyDeviceToHost, c->L.stream));
         CU(c, cudaStreamSynchronize(c->L.stream));
         const u64 kb_del = (u64)n[0] * t.key_size, kb_up = (u64)n[1] * t.key_size, vb = (u64)n[1] * t.value_size;
-        if ((r = dev_grow(c, "delta_export", &c->demit, &c->demit_cap, kb_del + kb_up + vb)) != 0) return r;
-        if ((r = dev_grow(c, "delta_export", (u8 **)&c->dsent, &c->dsent_cap, (sent_used + n[0] + n[1]) * 4, sent_used * 4)) != 0) return r;
+        const u64 eb = kb_del + kb_up + vb, sb = (sent_used + n[0] + n[1]) * 4;
+        if (cudaError_t e = eb > c->demit.size() ? c->demit.grow_keep(with_slack(eb), 0, c->L.stream) : cudaSuccess)
+            return grow_failed(c, "delta_export", with_slack(eb), nullptr, e);
+        if (cudaError_t e = sb > c->dsent.size() ? c->dsent.grow_keep(with_slack(sb), sent_used * 4, c->L.stream) : cudaSuccess)
+            return grow_failed(c, "delta_export", with_slack(sb), nullptr, e);
         CU(c, run_delta_emit(c->L, t, del, n[0], up, n[1], c->demit, c->demit + kb_del, c->demit + kb_del + kb_up));
         if (n[0]) CU(c, cudaMemcpyAsync(c->dsent + sent_used, del, (u64)n[0] * 4, cudaMemcpyDeviceToDevice, c->L.stream));
         if (n[1]) CU(c, cudaMemcpyAsync(c->dsent + sent_used + n[0], up, (u64)n[1] * 4, cudaMemcpyDeviceToDevice, c->L.stream));
@@ -3102,11 +2930,7 @@ int bng_sub_export(bng_ctx *c, const uint32_t *addrs, uint64_t n_addrs, const ui
     const u64 ns = (u64)d.sessions.mask + 1, nr = (u64)d.reverse.mask + 1, ne = (u64)d.eim.mask + 1, n6s = (u64)c->v6.mask + 1;
     // the slot lists (4 bytes per slot of the three flow tables and subscriber_ipv6), allocated by the first export that
     // has addresses
-    if (na && !c->mv_lists && cudaMalloc((void **)&c->mv_lists, (ns + nr + ne + n6s) * 4) != cudaSuccess) {
-        cudaGetLastError();
-        c->mv_lists = nullptr;
-        return fail(c, -ENOMEM, "sub_export: %llu bytes of device memory", (unsigned long long)((ns + nr + ne + n6s) * 4));
-    }
+    if (na && !c->mv_lists.grow((ns + nr + ne + n6s) * 4)) return grow_failed(c, "sub_export", (ns + nr + ne + n6s) * 4);
     u32 *v6_list = c->mv_lists ? c->mv_lists + ns + nr + ne : nullptr;
     // staging: [in] address set, addresses, MACs, counters; [out] lookups by key, then the gathered flow entries
     MapReg *am[3], *mm[2], *fm[3];
@@ -3124,7 +2948,8 @@ int bng_sub_export(bng_ctx *c, const uint32_t *addrs, uint64_t n_addrs, const ui
     size_t nd_v = 0, nd_r = 0;
     if (nd) nd_v = at, nd_r = al256(at + nm * ndm->value_size), at = al256(nd_r + nm * 4);
     const size_t flow0 = at;
-    if (int r = dev_grow(c, "sub_export", &c->mv_buf, &c->mv_cap, flow0)) return r;
+    if (cudaError_t e = flow0 > c->mv_buf.size() ? c->mv_buf.grow_keep(with_slack(flow0), 0, c->L.stream) : cudaSuccess)
+        return grow_failed(c, "sub_export", with_slack(flow0), nullptr, e);
     // the inputs are built in the pinned staging buffer and copied on the context's stream, ahead of the kernels that
     // read them (as bng_nat_flush does)
     if (int r = ensure_io(c, out0)) return r;
@@ -3166,7 +2991,8 @@ int bng_sub_export(bng_ctx *c, const uint32_t *addrs, uint64_t n_addrs, const ui
     const u32 n6 = n4[4];
     const size_t v6k = at, v6v = al256(v6k + (size_t)n6 * LPM6_KEY), v6r = al256(v6v + (size_t)n6 * 4); // v6r: the detach's results
     if (n6) at = al256(v6r + (size_t)n6 * 4);
-    if (int r = dev_grow(c, "sub_export", &c->mv_buf, &c->mv_cap, at, flow0)) return r;
+    if (cudaError_t e = at > c->mv_buf.size() ? c->mv_buf.grow_keep(with_slack(at), flow0, c->L.stream) : cudaSuccess)
+        return grow_failed(c, "sub_export", with_slack(at), nullptr, e);
     dv = c->mv_buf;
     for (int k = 0; k < 3 && c->mv_lists; k++) {
         const u32 *lists[3] = {c->mv_lists, c->mv_lists + ns, c->mv_lists + ns + nr};
