@@ -614,9 +614,12 @@ __device__ __forceinline__ bool icmp_error_frame(const u8 *p, u32 dlen) {
 //   - its proposed port collides with an existing endpoint or with one an earlier frame of the chunk
 //     creates (allocate_port_from_block() would skip it, :450-459)
 //   - its proposed port lies past the end of the block (the counter wraps at that frame)
-// and nothing is committed (mask 0) when port parity is filtered or a flow table is within 64 entries of
-// max_entries: those chunks go frame by frame.
-// Exhaustion never happens on the cooperative path: every proposed port is inside the block.
+//   - its proposed port is 0 (the counter stood at 0: allocate_port_from_block() returns 0, which both callers
+//     take for exhaustion, :501-504, :697-705)
+// and nothing is committed (mask 0) when port parity is filtered, the counter is past 0xFFFF, or a flow table has
+// no room left for the prefix's inserts: those chunks go frame by frame.
+// Exhaustion never happens on the cooperative path: every proposed port is non-zero and not past the end of the
+// block.
 // ---------------------------------------------------------------------------
 // ICMPERR (bng_nat_icmp_errors_egress_enable): an ICMP error frame also ends the prefix; the sequential code looks up
 // the flow it quotes.
@@ -700,7 +703,8 @@ __device__ __forceinline__ u32 nat_chunk_coop(const DevCtx &c, BlockStats &bs, c
     if (nalloc) {
         if (next > 0xFFFFu) all_clash = true;
         port = next + __popc(amask & below);
-        if (alloc && port > port_end) clash = true; // the counter wraps here: that frame goes through the sequential code
+        // the counter wraps here, or hands out 0 (exhaustion): that frame goes through the sequential code
+        if (alloc && (port > port_end || port == 0)) clash = true;
     }
     // translation of every creating lane, and its nat_reverse key
     u32 nat_ip = 0;
