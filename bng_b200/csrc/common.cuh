@@ -84,7 +84,7 @@ struct Tbl {
 //   sector 1 [32,64)  last_seen 8 | orig_ip 4 | state word 4 | orig_port 2 | pad 6 | in_lo 8
 //            what a downstream hit adds (original tuple, TCP state, in-direction counters), and last_seen.
 //   sector 2 [64,96)  out_hi 8 | in_hi 8 | created 8 | dest_ip 4 | dest_port 2 | _pad1 2   (creation / carries / ABI)
-//   sector 3 [96,104) the struct's padding bytes (they cross the ABI verbatim)
+//   sector 3 [96,104) the struct's padding bytes (they cross the ABI verbatim); [104,112) SES_SIDE (ses_touch_exact)
 // `epoch` is not part of struct nat_session: it is the batch (low 16 bits of the batch sequence, 0 = never)
 // in which last_seen was last stored.  Every frame of a batch would store the same last_seen = now, so only
 // a frame that finds an older epoch stores it (and the epoch): one extra store per flow and batch instead of
@@ -115,6 +115,7 @@ enum {
     SES_DEST_PORT = 92, // u16, _pad1@94
     SES_PAD_A = 96,     // struct bytes 20..23
     SES_PAD_B = 100,    // struct bytes 76..79
+    SES_SIDE = 104,     // u64, dataplane-internal: per-frame clock values of a batch that replaces last_seen (ses_touch_exact)
 };
 // byte offset inside struct nat_session -> byte offset inside the slot
 __host__ __device__ __forceinline__ u32 ses_abi_to_slot(u32 a) {
@@ -140,28 +141,61 @@ __host__ __device__ __forceinline__ u32 ses_abi_to_slot(u32 a) {
 }
 __host__ __device__ __forceinline__ u32 ses_hi_of(u32 lo_off) { return lo_off == SES_OUT_LO ? (u32)SES_OUT_HI : (u32)SES_IN_HI; }
 #ifdef __CUDACC__
+// Rare half of ses_touch(): a per-frame clock, and a last_seen that no batch of that clock may have stored — epoch 0:
+// the control plane wrote it (bng_map_update, a restore, a hand-over import, a delta), possibly on another host's
+// clock — or one that this batch's first frame may be replacing right now (epoch == the batch's).  The reference
+// overwrites, so the last frame's `now` must end in last_seen, whatever was there.  The first frame claims the
+// epoch (a CAS on the word it shares with nat_port, which no frame changes) and replaces the stored value outright.
+// Every other frame records its `now` in the dataplane-only word SES_SIDE first and then raises last_seen; the
+// claimer folds SES_SIDE in after its exchange, so a frame whose raise landed before the exchange is not lost.
+// SES_SIDE starts at 0 wherever a session is written whole (nat_ses_fill, val_to_slot), and only frames raise it
+// after that; the clock is monotonic from batch to batch (include/bng_b200.h), so what it holds from earlier batches
+// is never above this batch's frames.
+static __device__ __noinline__ void ses_touch_exact(u8 *ses, u64 now, u32 seen, u32 epoch) {
+    unsigned long long *ls = (unsigned long long *)(ses + SES_LAST_SEEN), *side = (unsigned long long *)(ses + SES_SIDE);
+    if (seen == 0) {
+        u32 *pe = (u32 *)(ses + SES_NAT_PORT); // nat_port | epoch << 16
+        const u32 cur = *(volatile u32 *)pe;
+        if ((cur >> 16) == 0 && atomicCAS(pe, cur, (cur & 0xFFFFu) | (epoch << 16)) == cur) {
+            atomicExch(ls, (unsigned long long)now);
+            __threadfence();
+            const u64 s = *(volatile u64 *)side;
+            if (s > now) atomicMax(ls, (unsigned long long)s);
+            return;
+        }
+    }
+    atomicMax(side, (unsigned long long)now);
+    __threadfence();
+    atomicMax(ls, (unsigned long long)now);
+}
 // session->last_seen = now (bpf/nat44.c:677,881), once per flow and batch: `seen` is the epoch the caller
 // read with the probe, `epoch` the current batch's.
 // With per-frame timestamps (stamped) the frames of a batch carry different values and the LAST frame's must
-// stay: the clock is monotonic, so that is the maximum.
+// stay.  The clock is monotonic, so that is the maximum of the frames' values and of any earlier batch's stamp
+// (a non-zero epoch other than this batch's); anything else takes ses_touch_exact().
 __device__ __forceinline__ void ses_touch(u8 *ses, u64 now, u32 seen, u32 epoch, bool stamped = false) {
     if (stamped) {
-        atomicMax((unsigned long long *)(ses + SES_LAST_SEEN), (unsigned long long)now);
+        if (seen != 0 && seen != epoch)
+            atomicMax((unsigned long long *)(ses + SES_LAST_SEEN), (unsigned long long)now);
+        else
+            ses_touch_exact(ses, now, seen, epoch);
     } else if (seen != epoch) {
         *(u64 *)(ses + SES_LAST_SEEN) = now;
         *(u16 *)(ses + SES_EPOCH) = (u16)epoch;
     }
 }
 // Rare half of ses_count(): a low word wrapped.  c: the packet word carried into the byte word (undo
-// it there, count it in the high packet word); w: the byte word wrapped upwards.
+// it there, count it in the high packet word); w: the byte word wrapped upwards.  The high words of
+// packets and bytes are advanced with one 32-bit atomic each, so neither can carry into the other.
 static __device__ __noinline__ void ses_count_carry(u8 *ses, u32 lo_off, u32 c, u32 w) {
-    u64 add = w ? (1ull << 32) : 0;
+    u32 *hi = (u32 *)(ses + ses_hi_of(lo_off)); // hi[0]: packets[63:32], hi[1]: bytes[63:32]
+    u32 dbytes = w;
     if (c) {
-        add += 1;
         u64 old = atomicAdd((unsigned long long *)(ses + lo_off), 0xFFFFFFFF00000000ull); // byte word -= 1
-        if ((old >> 32) == 0) add -= 1ull << 32;                                         // ... which wrapped downwards
+        if ((old >> 32) == 0) dbytes -= 1;                                                // ... which wrapped downwards
+        atomicAdd(hi, 1u);
     }
-    if (add) atomicAdd((unsigned long long *)(ses + ses_hi_of(lo_off)), add);
+    if (dbytes) atomicAdd(hi + 1, dbytes);
 }
 // packets += 1, bytes += len on the counter pair at lo_off (SES_OUT_LO / SES_IN_LO): exact u64
 // arithmetic, every wrap of a low word is seen by exactly one caller through the value the atomic returns.

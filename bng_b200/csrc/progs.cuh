@@ -406,7 +406,8 @@ __device__ __forceinline__ void nat_ses_fill(u8 *ns, u32 nat_ip, u16 nat_port, u
     *(u64 *)(ns + SES_CREATED) = now;
     *(u32 *)(ns + SES_DEST_IP) = daddr;
     *(u32 *)(ns + SES_DEST_PORT) = (u32)dport; // dest_port, _pad1 = 0
-    *(u64 *)(ns + SES_PAD_A) = 0;              // the struct's padding bytes
+    // the struct's padding bytes and SES_SIDE (a claimed slot holds 0xFF bytes or an evicted flow's stamps), one store
+    *(uint4 *)(ns + SES_PAD_A) = make_uint4(0, 0, 0, 0);
 }
 
 // The parse of nat44_egress up to the session lookup (:569-665), shared by the sequential and the
@@ -761,6 +762,12 @@ __device__ __forceinline__ u32 nat_chunk_coop(const DevCtx &c, BlockStats &bs, c
         }
     }
 
+    // lanes of the prefix that reuse the same existing EIM mapping: the last of them (in frame order) stores last_used
+    // (:485 overwrites it, whatever it held)
+    const bool reuse = create && in && m;
+    const u32 gm = __match_any_sync(0xffffffffu, reuse ? (u64)m : (u64)lane | (1ull << 63));
+    const bool last_use = reuse && (31 - __clz(gm)) == (int)lane;
+
     // ---- commit: nothing below depends on another lane of the chunk ----
     if (nalloc_take && lane == 0) {
         const u32 nn = next + nalloc_take;
@@ -812,11 +819,8 @@ __device__ __forceinline__ u32 nat_chunk_coop(const DevCtx &c, BlockStats &bs, c
                 rs_new = rs && created;
             }
             back_ses = !ns_new, back_rev = !rs_new, back_eim = (!m && eim_on && !nm_new);
-            if (m) { // existing endpoint mapping (:482-487); two lanes may share it: the later frame's clock stays
-                if (stamped)
-                    atomicMax((unsigned long long *)(m + 24), (unsigned long long)now);
-                else
-                    *(u64 *)(m + 24) = now;
+            if (m) { // existing endpoint mapping (:482-487); lanes may share it: the last one's clock stays
+                if (last_use) *(u64 *)(m + 24) = now;
                 atomicAdd((u32 *)(m + 32), 1u);
                 n_hit = 1;
             } else if (eim_on) { // new mapping (:495-517)

@@ -29,6 +29,7 @@ __device__ __forceinline__ void val_to_slot(const Tbl &t, u8 *slot, const u8 *ab
     if (t.vlayout == VL_SESSION) {
         for (u32 i = 0; i < t.value_size; i++) slot[ses_abi_to_slot(i)] = abi[i];
         *(u16 *)(slot + SES_EPOCH) = 0; // last_seen came from the control plane: no batch has stamped it
+        *(u64 *)(slot + SES_SIDE) = 0;  // ... nor left a clock value in the side word (ses_touch_exact)
     } else {
         copy_bytes(slot + t.voff, abi, t.value_size);
         // token buckets: rate_bps (value offset 16) is mirrored next to the key, so that the per-frame
