@@ -141,35 +141,30 @@ static inline int acct_grid(const Launcher &L, u64 n, int per_sm) {
     return (int)(want < 1 ? 1 : (want < cap ? want : cap));
 }
 
+// (COUNT, STAMP) is (1, 1), (1, 0) or (0, 1): at least one of acct and idle is given
 template <int MODE, bool V6>
 static void launch_acct(Launcher &L, int grid, const Tbl &dir, const DevBatch &b, const u32 *attr, u64 *acct, u64 *idle, const Tbl &v6) {
-    if (acct && idle)
-        k_acct<MODE, true, true, V6><<<grid, ACCT_BLOCK, 0, L.stream>>>(dir, b, attr, acct, idle, v6);
-    else if (acct)
-        k_acct<MODE, true, false, V6><<<grid, ACCT_BLOCK, 0, L.stream>>>(dir, b, attr, acct, nullptr, v6);
-    else
-        k_acct<MODE, false, true, V6><<<grid, ACCT_BLOCK, 0, L.stream>>>(dir, b, attr, nullptr, idle, v6);
+    auto *k = acct && idle ? k_acct<MODE, true, true, V6> : acct ? k_acct<MODE, true, false, V6> : k_acct<MODE, false, true, V6>;
+    k<<<grid, ACCT_BLOCK, 0, L.stream>>>(dir, b, attr, acct, idle, v6);
 }
 
-template <bool V6>
-static void launch_acct_mode(Launcher &L, int grid, const Tbl &dir, const DevBatch &b, int mode, u64 *acct, u64 *idle, const Tbl &v6) {
-    if (mode == ACCT_ATTR)
-        launch_acct<ACCT_ATTR, V6>(L, grid, dir, b, L.acct_attr, acct, idle, v6);
-    else if (mode == ACCT_SRC)
-        launch_acct<ACCT_SRC, V6>(L, grid, dir, b, nullptr, acct, idle, v6);
-    else
-        launch_acct<ACCT_DST, V6>(L, grid, dir, b, nullptr, acct, idle, v6);
-}
+static std::string acct_name(bool v6) { return std::string("k_acct") + (v6 ? "<v6>" : ""); }
 
 cudaError_t run_acct(Launcher &L, const Tbl &dir, const DevBatch &b, int mode, u64 *acct, u64 *idle, const Tbl *v6) {
     const int grid = acct_grid(L, b.n, 8);
-    if (v6) {
-        prof_begin(L, "k_acct<v6>");
-        launch_acct_mode<true>(L, grid, dir, b, mode, acct, idle, *v6);
-    } else {
-        prof_begin(L, "k_acct");
-        launch_acct_mode<false>(L, grid, dir, b, mode, acct, idle, Tbl{});
-    }
+    with_flags(
+        [&](auto attr6) {
+            constexpr bool V6 = decltype(attr6)::value;
+            const Tbl t = V6 ? *v6 : Tbl{};
+            prof_begin(L, prof_name<acct_name, V6>());
+            if (mode == ACCT_ATTR)
+                launch_acct<ACCT_ATTR, V6>(L, grid, dir, b, L.acct_attr, acct, idle, t);
+            else if (mode == ACCT_SRC)
+                launch_acct<ACCT_SRC, V6>(L, grid, dir, b, nullptr, acct, idle, t);
+            else
+                launch_acct<ACCT_DST, V6>(L, grid, dir, b, nullptr, acct, idle, t);
+        },
+        v6 != nullptr);
     prof_end(L);
     L.launches++;
     return cudaGetLastError();

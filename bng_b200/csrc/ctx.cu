@@ -481,6 +481,14 @@ bool lpm_same(u32 pl, u32 a, u32 b) { // first pl bits equal, bytes in memory or
     return (x & mask) == 0;
 }
 
+// an opt-in switch of the context (bng_qos_ipv6_enable and its kind): in effect from the next run on
+int set_switch(bng_ctx *c, bool bng_ctx::*sw, int on) {
+    if (!c) return -EINVAL;
+    std::lock_guard<std::mutex> g(c->mu);
+    c->*sw = on != 0;
+    return 0;
+}
+
 } // namespace
 
 // ---- staged upserts ----
@@ -1213,6 +1221,13 @@ struct FrameRoom {
     u32 *need;
 };
 
+// Are ICMP errors translated by the flow they quote in this program?  nat44_ingress: bng_nat_icmp_errors_enable;
+// nat44_egress and the pipelines: bng_nat_icmp_errors_egress_enable.
+static bool icmp_errors(const bng_ctx *c, int prog) {
+    if (prog == P_NAT_IN) return c->nat_icmp;
+    return (prog == P_NAT_EG || prog == P_PIPE_UP || prog == P_PIPE_TC) && c->nat_icmp_eg;
+}
+
 static int dispatch(bng_ctx *c, int prog, const DevBatch &b, const LiSrc &src = LiSrc{}, const FrameRoom *room = nullptr) {
     cudaError_t e = cudaSuccess;
     const bool acct = c->acct && ((c->acct_progs >> prog) & 1);
@@ -1240,8 +1255,8 @@ static int dispatch(bng_ctx *c, int prog, const DevBatch &b, const LiSrc &src = 
     case P_ANTISPOOF: e = run_antispoof(c->L, c->dev, b, as6); break;
     case P_QOS_EG: e = run_qos(c->L, c->dev, b, true, qv6); break;
     case P_QOS_IN: e = run_qos(c->L, c->dev, b, false, qv6); break;
-    case P_NAT_EG: e = run_nat_egress(c->L, c->dev, b, c->nat_icmp_eg); break;
-    case P_NAT_IN: e = run_nat_ingress(c->L, c->dev, b, c->nat_icmp); break;
+    case P_NAT_EG: e = run_nat_egress(c->L, c->dev, b, icmp_errors(c, prog)); break;
+    case P_NAT_IN: e = run_nat_ingress(c->L, c->dev, b, icmp_errors(c, prog)); break;
     case P_NAT_HAIRPIN: e = run_nat_hairpin_xdp(c->L, c->dev, b); break;
     case P_DHCP: {
         // DHCPv6 needs the switch, a configured server and a binding: otherwise "on" launches what "off" does
@@ -1263,8 +1278,8 @@ static int dispatch(bng_ctx *c, int prog, const DevBatch &b, const LiSrc &src = 
         e = run_dhcp_fastpath(c->L, c->dev, b, v6 ? &d6 : nullptr, ndo ? &nd : nullptr);
         break;
     }
-    case P_PIPE_UP: e = run_pipeline_up(c->L, c->dev, b, qv6, as6, c->nat_icmp_eg); break;
-    case P_PIPE_TC: e = run_pipeline_tc(c->L, c->dev, b, qv6, as6, c->nat_icmp_eg); break;
+    case P_PIPE_UP: e = run_pipeline_up(c->L, c->dev, b, qv6, as6, icmp_errors(c, prog)); break;
+    case P_PIPE_TC: e = run_pipeline_tc(c->L, c->dev, b, qv6, as6, icmp_errors(c, prog)); break;
     default: return -EINVAL;
     }
     // after the program, before anything copies the frames out: the downstream modes read the rewritten headers
@@ -1341,10 +1356,7 @@ static int run_host_zero_copy(bng_ctx *c, int prog, bng_batch *bb, u8 *arena_dev
                                   c->s_in));
         } else {
             CU(c, run_gather_frames(c->s_in, c->L.num_sms, chunk_arena, bb->off16 ? c->zc_off[buf].get() : nullptr, c->zc_len[buf],
-                                    bb->stride, cn, hb, tc,
-                                    (prog == P_NAT_IN && c->nat_icmp) ||
-                                        ((prog == P_NAT_EG || prog == P_PIPE_UP || prog == P_PIPE_TC) && c->nat_icmp_eg),
-                                    c->zc_hdr[buf], c->zc_len0[buf]));
+                                    bb->stride, cn, hb, tc, icmp_errors(c, prog), c->zc_hdr[buf], c->zc_len0[buf]));
             c->L.launches++;
         }
         CU(c, cudaEventRecord(c->ev_in[buf], c->s_in));
@@ -3184,47 +3196,12 @@ int bng_stats_device_ptr(bng_ctx *c, void **dptr, uint32_t *n_u64) {
 
 uint64_t bng_launch_count(bng_ctx *c) { return c ? c->L.launches : 0; }
 
-int bng_dhcpv6_enable(bng_ctx *c, int on) {
-    if (!c) return -EINVAL;
-    std::lock_guard<std::mutex> g(c->mu);
-    c->dhcp6 = on != 0;
-    return 0;
-}
-
-int bng_nd_enable(bng_ctx *c, int on) {
-    if (!c) return -EINVAL;
-    std::lock_guard<std::mutex> g(c->mu);
-    c->nd = on != 0;
-    return 0;
-}
-
-int bng_qos_ipv6_enable(bng_ctx *c, int on) {
-    if (!c) return -EINVAL;
-    std::lock_guard<std::mutex> g(c->mu);
-    c->qos_v6 = on != 0;
-    return 0;
-}
-
-int bng_antispoof_ipv6_prefixes_enable(bng_ctx *c, int on) {
-    if (!c) return -EINVAL;
-    std::lock_guard<std::mutex> g(c->mu);
-    c->as_v6 = on != 0;
-    return 0;
-}
-
-int bng_nat_icmp_errors_enable(bng_ctx *c, int on) {
-    if (!c) return -EINVAL;
-    std::lock_guard<std::mutex> g(c->mu);
-    c->nat_icmp = on != 0;
-    return 0;
-}
-
-int bng_nat_icmp_errors_egress_enable(bng_ctx *c, int on) {
-    if (!c) return -EINVAL;
-    std::lock_guard<std::mutex> g(c->mu);
-    c->nat_icmp_eg = on != 0;
-    return 0;
-}
+int bng_dhcpv6_enable(bng_ctx *c, int on) { return set_switch(c, &bng_ctx::dhcp6, on); }
+int bng_nd_enable(bng_ctx *c, int on) { return set_switch(c, &bng_ctx::nd, on); }
+int bng_qos_ipv6_enable(bng_ctx *c, int on) { return set_switch(c, &bng_ctx::qos_v6, on); }
+int bng_antispoof_ipv6_prefixes_enable(bng_ctx *c, int on) { return set_switch(c, &bng_ctx::as_v6, on); }
+int bng_nat_icmp_errors_enable(bng_ctx *c, int on) { return set_switch(c, &bng_ctx::nat_icmp, on); }
+int bng_nat_icmp_errors_egress_enable(bng_ctx *c, int on) { return set_switch(c, &bng_ctx::nat_icmp_eg, on); }
 
 int bng_ipv6_prefix_lengths(bng_ctx *c, uint32_t *counts) {
     if (!c || !counts) return -EINVAL;

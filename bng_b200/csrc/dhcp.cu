@@ -831,22 +831,30 @@ __global__ void __launch_bounds__(DH_TILE) k_dhcp_fastpath(const __grid_constant
 // (A double-buffered variant — two staging slots per thread, the load of tile i+1 issued before the program runs on
 // tile i — was tried and dropped: it was slower.)
 
+static std::string dhcp_name(bool v6, bool nd) {
+    const std::string tags = std::string(v6 ? ",v6" : "") + (nd ? ",nd" : "");
+    return "k_dhcp_fastpath" + (tags.empty() ? tags : "<" + tags.substr(1) + ">");
+}
+
 cudaError_t run_dhcp_fastpath(Launcher &L, const DevCtx &c, const DevBatch &b, const Dhcp6Args *d6, const NdArgs *nd) {
     const int smem = DH_TILE * DH_SLOT;
-    int &set = nd ? L.nd_smem_set[d6 ? 1 : 0] : (d6 ? L.dhcp6_smem_set : L.dhcp_smem_set);
-    auto *k = nd ? (d6 ? k_dhcp_fastpath<true, true> : k_dhcp_fastpath<false, true>)
-                 : (d6 ? k_dhcp_fastpath<true, false> : k_dhcp_fastpath<false, false>);
-    if (!set) { // function attributes are per device: set on the device this context runs on
-        cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-        if (e != cudaSuccess) return e;
-        set = 1;
-    }
     long want = ((long)b.n + DH_TILE - 1) / DH_TILE;
     long cap = (long)L.num_sms * 4; // 4 x 50 KB of staging per SM (of the 228 KB an H100 SM has)
     int grid = (int)(want < cap ? (want < 1 ? 1 : want) : cap);
-    prof_begin(L, nd ? (d6 ? "k_dhcp_fastpath<v6,nd>" : "k_dhcp_fastpath<nd>") : (d6 ? "k_dhcp_fastpath<v6>" : "k_dhcp_fastpath"));
-    k<<<grid, DH_TILE, smem, L.stream>>>(c, b, d6 ? *d6 : Dhcp6Args{}, nd ? *nd : NdArgs{});
-    prof_end(L);
-    L.launches++;
-    return cudaGetLastError();
+    return with_flags(
+        [&](auto v6f, auto ndf) {
+            constexpr bool V6 = decltype(v6f)::value, ND = decltype(ndf)::value;
+            int &set = L.dhcp_smem_set[V6 * 2 + ND];
+            if (!set) { // function attributes are per device: set on the device this context runs on
+                cudaError_t e = cudaFuncSetAttribute(k_dhcp_fastpath<V6, ND>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+                if (e != cudaSuccess) return e;
+                set = 1;
+            }
+            prof_begin(L, prof_name<dhcp_name, V6, ND>());
+            k_dhcp_fastpath<V6, ND><<<grid, DH_TILE, smem, L.stream>>>(c, b, V6 ? *d6 : Dhcp6Args{}, ND ? *nd : NdArgs{});
+            prof_end(L);
+            L.launches++;
+            return cudaGetLastError();
+        },
+        d6 != nullptr, nd != nullptr);
 }

@@ -97,10 +97,11 @@ __global__ void __launch_bounds__(256) k_scatter_frames(u8 *__restrict__ arena, 
 // read requests and the scatter's small write TLPs share the upstream direction.  Copy-engine traffic (a header-split ring, moved with cudaMemcpyAsync) overlaps cleanly.
 cudaError_t run_gather_frames(cudaStream_t st, int blocks, const u8 *arena, const u32 *off16, const u32 *len, u32 stride,
                               u32 n, u32 slot, bool tc, bool icmp_errors, u8 *dst, u32 *need) {
-    if (tc && icmp_errors)
-        k_gather_frames<true><<<blocks, 256, 0, st>>>(arena, off16, len, stride, n, slot, 1u, dst, need);
-    else
-        k_gather_frames<false><<<blocks, 256, 0, st>>>(arena, off16, len, stride, n, slot, tc ? 1u : 0u, dst, need);
+    with_flags(
+        [&](auto icmp) {
+            k_gather_frames<decltype(icmp)::value><<<blocks, 256, 0, st>>>(arena, off16, len, stride, n, slot, tc ? 1u : 0u, dst, need);
+        },
+        tc && icmp_errors);
     return cudaGetLastError();
 }
 

@@ -1054,10 +1054,23 @@ static cudaError_t group_by_key(Launcher &L, u32 n, u64 key_space, u32 kshift, G
 // Room for the frame length above the ordering key?  (KEY_BITS covers the reference's capacities.)
 static inline u32 kshift_for(u64 key_space) { return bits_for(key_space) <= KEY_BITS ? KEY_BITS : 0; }
 
+static const char *tf(bool b) { return b ? "true" : "false"; }
+static std::string resolve_name(bool nat, bool qos, bool egress, bool tc, bool icmperr) {
+    return std::string("(k_resolve<") + tf(nat) + ", " + tf(qos) + ", " + tf(egress) + (tc ? ", tc" : "") + (icmperr ? ", icmperr" : "") + ">)";
+}
+// TC is printed when TC or ACCT is set, ACCT only when set, then a tag per optional stage
+static std::string classify_name(bool as, bool qos, bool tc, bool acct, bool v6, bool as6, bool icmperr) {
+    return std::string("(k_pipe_classify<") + tf(as) + ", " + tf(qos) + (tc || acct ? std::string(", ") + tf(tc) : "") +
+           (acct ? ", true" : "") + (v6 ? ", v6" : "") + (as6 ? ", as6" : "") + (icmperr ? ", icmperr" : "") + ">)";
+}
+static std::string antispoof_name(bool v6) { return std::string("k_antispoof") + (v6 ? "<v6>" : ""); }
+static std::string qos_name(bool v6) { return std::string("k_qos_classify") + (v6 ? "<v6>" : ""); }
+static std::string nat_ingress_name(bool icmperr) { return std::string("k_nat_ingress") + (icmperr ? "<icmperr>" : ""); }
+
 // k_resolve walks one group per block and a batch of n frames can hold n groups: the grid is sized for n blocks,
 // capped at what the GPU holds at once (the blocks loop over the groups).
 template <bool NAT, bool QOS, bool EGRESS, bool TC = false, bool ICMPERR = false>
-static void launch_resolve(Launcher &L, const DevCtx &c, const DevBatch &b, const Grouped &g, const char *name) {
+static void launch_resolve(Launcher &L, const DevCtx &c, const DevBatch &b, const Grouped &g) {
     int &per_sm = L.resolve_bps[ICMPERR * 16 + NAT * 8 + QOS * 4 + EGRESS * 2 + TC]; // resident blocks per SM of this instantiation
     if (!per_sm) {
         if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_resolve<NAT, QOS, EGRESS, TC, ICMPERR>, RS_TEAM, 0) != cudaSuccess ||
@@ -1066,17 +1079,19 @@ static void launch_resolve(Launcher &L, const DevCtx &c, const DevBatch &b, cons
     }
     long cap = (long)L.num_sms * per_sm, want = b.n ? b.n : 1;
     int grid = (int)(want < cap ? want : cap);
-    prof_begin(L, name);
+    prof_begin(L, prof_name<resolve_name, NAT, QOS, EGRESS, TC, ICMPERR>());
     launch_dep(k_resolve<NAT, QOS, EGRESS, TC, ICMPERR>, grid, RS_TEAM, L.stream, c, b, g, L.s.qslot, L.s.counters);
     prof_end(L);
     L.launches++;
 }
 
 cudaError_t run_antispoof(Launcher &L, const DevCtx &c, const DevBatch &b, const Tbl *as6) {
-    if (as6)
-        LAUNCH_AS("k_antispoof<v6>", k_antispoof<true>, b.n, 8, c, b, *as6);
-    else
-        LAUNCH_AS("k_antispoof", k_antispoof<false>, b.n, 8, c, b, Tbl{});
+    with_flags(
+        [&](auto v6) {
+            constexpr bool V6 = decltype(v6)::value;
+            LAUNCH_AS((prof_name<antispoof_name, V6>()), k_antispoof<V6>, b.n, 8, c, b, V6 ? *as6 : Tbl{});
+        },
+        as6 != nullptr);
     return cudaGetLastError();
 }
 
@@ -1084,82 +1099,57 @@ cudaError_t run_qos(Launcher &L, const DevCtx &c, const DevBatch &b0, bool egres
     const Tbl &t = egress ? c.qos_eg : c.qos_in;
     DevBatch b = b0;
     b.kshift = kshift_for((u64)t.mask + 1);
-    if (v6)
-        LAUNCH_AS("k_qos_classify<v6>", k_qos_classify<true>, b.n, 8, c, b, egress ? 1 : 0, L.s.key_a, L.s.val_a, L.s.counters, sort_T(L), *v6);
-    else
-        LAUNCH_AS("k_qos_classify", k_qos_classify<false>, b.n, 8, c, b, egress ? 1 : 0, L.s.key_a, L.s.val_a, L.s.counters, sort_T(L), Tbl{});
+    with_flags(
+        [&](auto shape6) {
+            constexpr bool V6 = decltype(shape6)::value;
+            LAUNCH_AS((prof_name<qos_name, V6>()), k_qos_classify<V6>, b.n, 8, c, b, egress ? 1 : 0, L.s.key_a, L.s.val_a, L.s.counters,
+                      sort_T(L), V6 ? *v6 : Tbl{});
+        },
+        v6 != nullptr);
     Grouped g;
     cudaError_t e = group_by_key(L, b.n, (u64)t.mask + 1, b.kshift, &g);
     if (e != cudaSuccess) return e;
-    if (egress)
-        launch_resolve<false, true, true>(L, c, b, g, "(k_resolve<false, true, true>)");
-    else
-        launch_resolve<false, true, false>(L, c, b, g, "(k_resolve<false, true, false>)");
+    with_flags([&](auto eg) { launch_resolve<false, true, decltype(eg)::value>(L, c, b, g); }, egress);
     return cudaGetLastError();
 }
 
 // The programs keyed on the subscriber directory (nat44_egress, pipeline_up, pipeline_tc): classify, group by
-// directory slot, resolve.  The names are what each launch is timed as; with accounting on, classify is the
-// ACCT instantiation and is timed under its own name.  v6 (the pipelines only): IPv6 frames are shaped, classify is
-// the V6 instantiation and is timed under its name with a ", v6>" suffix.  as6 (the pipelines only): antispoof allows
-// IPv6 sources in their subscriber's prefixes, classify is the AS6 instantiation, timed with an ", as6>" suffix.
-struct ClassifyNames {
-    const char *plain, *acct, *v6, *acct_v6, *as6, *acct_as6, *v6_as6, *acct_v6_as6;
-};
-template <bool AS, bool QOS, bool TC, bool ACCT, bool V6, bool AS6 = false, bool ICMPERR = false>
-static void launch_classify(Launcher &L, const DevCtx &c, const DevBatch &b, const char *name, const Tbl &v6) {
-    LAUNCH_AS(name, (k_pipe_classify<AS, QOS, TC, ACCT, V6, AS6, ICMPERR>), b.n, CLASSIFY_BPS(AS), c, b, L.s.key_a, L.s.val_a, L.s.counters,
-              sort_T(L), ACCT ? L.acct_attr : nullptr, v6);
-}
-// ICMPERR (bng_nat_icmp_errors_egress_enable): the ICMPERR instantiations of classify and resolve, timed under their
-// names with an ", icmperr>" suffix.
-template <bool AS, bool QOS, bool TC, bool ICMPERR = false>
-static cudaError_t run_dir_prog(Launcher &L, const DevCtx &c, const DevBatch &b0, const ClassifyNames &nm, const char *resolve_name,
-                                const Tbl *v6, const Tbl *as6) {
+// directory slot, resolve.  With accounting on (L.acct_attr), classify is the ACCT instantiation.  v6 (the pipelines
+// only): IPv6 frames are shaped, classify is the V6 instantiation.  as6 (the pipelines only): antispoof allows IPv6
+// sources in their subscriber's prefixes, classify is the AS6 instantiation.  icmperr
+// (bng_nat_icmp_errors_egress_enable): the ICMPERR instantiations of classify and resolve.
+template <bool AS, bool QOS, bool TC>
+static cudaError_t run_dir_prog(Launcher &L, const DevCtx &c, const DevBatch &b0, const Tbl *v6, const Tbl *as6, bool icmperr) {
     DevBatch b = b0;
     b.kshift = kshift_for((u64)c.subdir.mask + 1);
-    if (AS && as6) { // (AS6 = AS: nat44_egress has no antispoof stage and is never given the table)
-        if (QOS && v6) {
-            if (L.acct_attr)
-                launch_classify<AS, QOS, TC, true, QOS, AS, ICMPERR>(L, c, b, nm.acct_v6_as6, *as6);
-            else
-                launch_classify<AS, QOS, TC, false, QOS, AS, ICMPERR>(L, c, b, nm.v6_as6, *as6);
-        } else if (L.acct_attr) {
-            launch_classify<AS, QOS, TC, true, false, AS, ICMPERR>(L, c, b, nm.acct_as6, *as6);
-        } else {
-            launch_classify<AS, QOS, TC, false, false, AS, ICMPERR>(L, c, b, nm.as6, *as6);
-        }
-    } else if (QOS && v6) { // (V6 = QOS: nat44_egress has no bucket and is never given the table)
-        if (L.acct_attr)
-            launch_classify<AS, QOS, TC, true, QOS, false, ICMPERR>(L, c, b, nm.acct_v6, *v6);
-        else
-            launch_classify<AS, QOS, TC, false, QOS, false, ICMPERR>(L, c, b, nm.v6, *v6);
-    } else if (L.acct_attr) {
-        launch_classify<AS, QOS, TC, true, false, false, ICMPERR>(L, c, b, nm.acct, Tbl{});
-    } else {
-        launch_classify<AS, QOS, TC, false, false, false, ICMPERR>(L, c, b, nm.plain, Tbl{});
-    }
+    // (nat44_egress has neither a bucket nor antispoof and is never given the tables)
+    with_flags(
+        [&](auto acct, auto shape6, auto spoof6, auto icmp) {
+            constexpr bool ACCT = decltype(acct)::value, V6 = decltype(shape6)::value, AS6 = decltype(spoof6)::value,
+                           ICMPERR = decltype(icmp)::value;
+            LAUNCH_AS((prof_name<classify_name, AS, QOS, TC, ACCT, V6, AS6, ICMPERR>()), (k_pipe_classify<AS, QOS, TC, ACCT, V6, AS6, ICMPERR>),
+                      b.n, CLASSIFY_BPS(AS), c, b, L.s.key_a, L.s.val_a, L.s.counters, sort_T(L), L.acct_attr,
+                      AS6 ? *as6 : (V6 ? *v6 : Tbl{}));
+        },
+        L.acct_attr != nullptr, only<QOS>(v6 != nullptr), only<AS>(as6 != nullptr), icmperr);
     Grouped g;
     cudaError_t e = group_by_key(L, b.n, (u64)c.subdir.mask + 1, b.kshift, &g);
     if (e != cudaSuccess) return e;
-    launch_resolve<true, QOS, false, TC, ICMPERR>(L, c, b, g, resolve_name);
+    with_flags([&](auto icmp) { launch_resolve<true, QOS, false, TC, decltype(icmp)::value>(L, c, b, g); }, icmperr);
     return cudaGetLastError();
 }
 
 cudaError_t run_nat_egress(Launcher &L, const DevCtx &c, const DevBatch &b, bool icmp_errors_eg) {
-    if (icmp_errors_eg)
-        return run_dir_prog<false, false, false, true>(
-            L, c, b, {"(k_pipe_classify<false, false, icmperr>)", "(k_pipe_classify<false, false, false, true, icmperr>)"},
-            "(k_resolve<true, false, false, icmperr>)", nullptr, nullptr);
-    return run_dir_prog<false, false, false>(L, c, b, {"(k_pipe_classify<false, false>)", "(k_pipe_classify<false, false, false, true>)"},
-                                             "(k_resolve<true, false, false>)", nullptr, nullptr);
+    return run_dir_prog<false, false, false>(L, c, b, nullptr, nullptr, icmp_errors_eg);
 }
 
 cudaError_t run_nat_ingress(Launcher &L, const DevCtx &c, const DevBatch &b, bool icmp_errors) {
-    if (icmp_errors)
-        LAUNCH_AS("k_nat_ingress<icmperr>", k_nat_ingress<true>, b.n, 6, c, b);
-    else
-        LAUNCH_AS("k_nat_ingress", k_nat_ingress<false>, b.n, 6, c, b);
+    with_flags(
+        [&](auto icmp) {
+            constexpr bool ICMPERR = decltype(icmp)::value;
+            LAUNCH_AS((prof_name<nat_ingress_name, ICMPERR>()), k_nat_ingress<ICMPERR>, b.n, 6, c, b);
+        },
+        icmp_errors);
     return cudaGetLastError();
 }
 
@@ -1169,36 +1159,9 @@ cudaError_t run_nat_hairpin_xdp(Launcher &L, const DevCtx &c, const DevBatch &b)
 }
 
 cudaError_t run_pipeline_up(Launcher &L, const DevCtx &c, const DevBatch &b, const Tbl *v6, const Tbl *as6, bool icmp_errors_eg) {
-    if (icmp_errors_eg)
-        return run_dir_prog<true, true, false, true>(
-            L, c, b,
-            {"(k_pipe_classify<true, true, icmperr>)", "(k_pipe_classify<true, true, false, true, icmperr>)",
-             "(k_pipe_classify<true, true, v6, icmperr>)", "(k_pipe_classify<true, true, false, true, v6, icmperr>)",
-             "(k_pipe_classify<true, true, as6, icmperr>)", "(k_pipe_classify<true, true, false, true, as6, icmperr>)",
-             "(k_pipe_classify<true, true, v6, as6, icmperr>)", "(k_pipe_classify<true, true, false, true, v6, as6, icmperr>)"},
-            "(k_resolve<true, true, false, icmperr>)", v6, as6);
-    return run_dir_prog<true, true, false>(L, c, b,
-                                           {"(k_pipe_classify<true, true>)", "(k_pipe_classify<true, true, false, true>)",
-                                            "(k_pipe_classify<true, true, v6>)", "(k_pipe_classify<true, true, false, true, v6>)",
-                                            "(k_pipe_classify<true, true, as6>)", "(k_pipe_classify<true, true, false, true, as6>)",
-                                            "(k_pipe_classify<true, true, v6, as6>)", "(k_pipe_classify<true, true, false, true, v6, as6>)"},
-                                           "(k_resolve<true, true, false>)", v6, as6);
+    return run_dir_prog<true, true, false>(L, c, b, v6, as6, icmp_errors_eg);
 }
 
 cudaError_t run_pipeline_tc(Launcher &L, const DevCtx &c, const DevBatch &b, const Tbl *v6, const Tbl *as6, bool icmp_errors_eg) {
-    if (icmp_errors_eg)
-        return run_dir_prog<true, true, true, true>(
-            L, c, b,
-            {"(k_pipe_classify<true, true, true, icmperr>)", "(k_pipe_classify<true, true, true, true, icmperr>)",
-             "(k_pipe_classify<true, true, true, v6, icmperr>)", "(k_pipe_classify<true, true, true, true, v6, icmperr>)",
-             "(k_pipe_classify<true, true, true, as6, icmperr>)", "(k_pipe_classify<true, true, true, true, as6, icmperr>)",
-             "(k_pipe_classify<true, true, true, v6, as6, icmperr>)", "(k_pipe_classify<true, true, true, true, v6, as6, icmperr>)"},
-            "(k_resolve<true, true, false, tc, icmperr>)", v6, as6);
-    return run_dir_prog<true, true, true>(L, c, b,
-                                          {"(k_pipe_classify<true, true, true>)", "(k_pipe_classify<true, true, true, true>)",
-                                           "(k_pipe_classify<true, true, true, v6>)", "(k_pipe_classify<true, true, true, true, v6>)",
-                                           "(k_pipe_classify<true, true, true, as6>)", "(k_pipe_classify<true, true, true, true, as6>)",
-                                           "(k_pipe_classify<true, true, true, v6, as6>)",
-                                           "(k_pipe_classify<true, true, true, true, v6, as6>)"},
-                                          "(k_resolve<true, true, false, tc>)", v6, as6);
+    return run_dir_prog<true, true, true>(L, c, b, v6, as6, icmp_errors_eg);
 }

@@ -1,7 +1,40 @@
 // bng_b200 — internal interface between the C-ABI layer (ctx.cu) and the
 // kernel translation units.
 #pragma once
+#include <string>
+#include <type_traits>
+
 #include "common.cuh"
+
+// Picks a kernel instantiation from runtime switches: calls f with each runtime bool lifted to std::true_type or
+// std::false_type, which f reads as decltype(x)::value.  An argument that already is a std::bool_constant passes
+// through, so a caller pins the combinations that cannot occur (only<>) and they are never instantiated.
+template <class F>
+decltype(auto) with_flags(F &&f) {
+    return f();
+}
+template <class F, class A, class... R>
+decltype(auto) with_flags(F &&f, A a, R... r) {
+    auto rest = [&](auto x) { return with_flags([&](auto... y) { return f(x, y...); }, r...); };
+    if constexpr (std::is_same_v<A, bool>)
+        return a ? rest(std::true_type{}) : rest(std::false_type{});
+    else
+        return rest(a);
+}
+// the switch b where the instantiation has the stage it selects (C), else always off
+template <bool C>
+auto only(bool b) {
+    if constexpr (C)
+        return b;
+    else
+        return std::false_type{};
+}
+// The profile name of an instantiation, built once by name(F...) and kept for the process: prof_begin keeps the pointer.
+template <auto name, bool... F>
+const char *prof_name() {
+    static const std::string s = name(F...);
+    return s.c_str();
+}
 
 struct Scratch {
     u32 *key_a, *key_b, *val_a, *val_b; // ordering keys / frame indices, unsorted and grouped
@@ -27,9 +60,7 @@ struct Launcher {
     unsigned long long launches;
     // per-context (= per-device) launch configuration, filled on first use: nothing here may be process-wide,
     // one process can hold contexts on several GPUs
-    int dhcp_smem_set;  // cudaFuncAttributeMaxDynamicSharedMemorySize applied on this context's device
-    int dhcp6_smem_set; // ... and to k_dhcp_fastpath<v6>
-    int nd_smem_set[2]; // ... and to k_dhcp_fastpath<nd>, <v6,nd>
+    int dhcp_smem_set[4]; // cudaFuncAttributeMaxDynamicSharedMemorySize applied on this context's device, by <V6, ND> bits
     int resolve_bps[32]; // resident blocks per SM of the k_resolve instantiations, by <NAT, QOS, EGRESS, TC, ICMPERR> bits
     int prof;
     ProfPending pend[32];

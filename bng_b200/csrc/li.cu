@@ -156,21 +156,17 @@ static inline int li_grid(const Launcher &L, u64 n, int per_sm) {
     return (int)(want < 1 ? 1 : (want < cap ? want : cap));
 }
 
+static std::string li_name(bool up, bool v6) { return std::string("k_li_capture<") + (up ? "up" : "down") + (v6 ? ",v6" : "") + ">"; }
+
 cudaError_t run_li_capture(Launcher &L, const LiRing &r, const DevBatch &b, const LiSrc &src, bool up, const Tbl *v6) {
     const int grid = li_grid(L, b.n, 8);
-    if (up && v6) {
-        prof_begin(L, "k_li_capture<up,v6>");
-        k_li_capture<true, true><<<grid, LI_BLOCK, 0, L.stream>>>(r, b, src, *v6);
-    } else if (up) {
-        prof_begin(L, "k_li_capture<up>");
-        k_li_capture<true, false><<<grid, LI_BLOCK, 0, L.stream>>>(r, b, src, Tbl{});
-    } else if (v6) {
-        prof_begin(L, "k_li_capture<down,v6>");
-        k_li_capture<false, true><<<grid, LI_BLOCK, 0, L.stream>>>(r, b, src, *v6);
-    } else {
-        prof_begin(L, "k_li_capture<down>");
-        k_li_capture<false, false><<<grid, LI_BLOCK, 0, L.stream>>>(r, b, src, Tbl{});
-    }
+    with_flags(
+        [&](auto upf, auto attr6) {
+            constexpr bool UP = decltype(upf)::value, V6 = decltype(attr6)::value;
+            prof_begin(L, prof_name<li_name, UP, V6>());
+            k_li_capture<UP, V6><<<grid, LI_BLOCK, 0, L.stream>>>(r, b, src, V6 ? *v6 : Tbl{});
+        },
+        up, v6 != nullptr);
     prof_end(L);
     L.launches++;
     return cudaGetLastError();
