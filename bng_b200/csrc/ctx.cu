@@ -25,6 +25,7 @@
 #include "blob.hpp"
 #include "devbuf.hpp"
 #include "kernels.h"
+#include "stage.hpp"
 
 namespace {
 
@@ -225,11 +226,25 @@ u32 zc_chunk_frames() { // frames per chunk of the zero-copy pipeline; BNG_ZC_CH
     return 1u << lg;
 }
 
-u32 pow2_at_least(u64 v) {
-    u64 p = 1;
+// the least power of two >= v and >= 64: the slots of a table, a census set or an address set
+u64 pow2_slots(u64 v) {
+    u64 p = 64;
     while (p < v) p <<= 1;
-    return (u32)p;
+    return p;
 }
+
+// The slots of an address set of n addresses (load 1/2 at most), and an address put into a set whose words start
+// zeroed: its slot, the one it has already when it is a member.
+u64 aset_slots(u64 n) { return pow2_slots(2 * n); }
+u32 aset_insert(u64 *words, u32 mask, u32 addr) {
+    u32 i = aset_home(addr, mask);
+    while (words[i] && (u32)words[i] != addr) i = (i + 1) & mask;
+    words[i] = ADDRSET_LIVE | addr;
+    return i;
+}
+
+// the half of the subscriber directory a table feeds (run_table_op): 1 subscriber_nat, 2 qos_ingress, 0 none
+int dir_role(const bng_ctx *c, const Tbl *t) { return t == &c->dev.sub_nat ? 1 : (t == &c->dev.qos_in ? 2 : 0); }
 
 int dev_alloc(bng_ctx *c, void **p, size_t bytes, int fill) {
     CU(c, cudaMalloc(p, bytes ? bytes : 16));
@@ -240,7 +255,7 @@ int dev_alloc(bng_ctx *c, void **p, size_t bytes, int fill) {
 
 int make_table(bng_ctx *c, Tbl *t, u32 key_size, u32 value_size, u32 voff, u32 max_entries, u32 vlayout = 0,
                u32 slot_bytes = 0, u32 sparsity = 2) {
-    u32 cap = pow2_at_least(std::max<u64>(64, (u64)max_entries * sparsity));
+    const u32 cap = (u32)pow2_slots((u64)max_entries * sparsity);
     t->mask = cap - 1;
     t->home_mask = cap - 1;
     t->voff = voff;
@@ -284,6 +299,21 @@ int ensure_io(bng_ctx *c, size_t bytes) {
     const size_t nb = std::max<size_t>(bytes, 1 << 20);
     if (!devbuf::grow_all({{&c->io_dev, nb}, {&c->io_host, nb}})) return grow_failed(c, "staging", 2 * nb);
     return 0;
+}
+
+// n items through the staging buffers on the context's stream (stage::round_trip)
+template <class Launch, class Done = std::nullptr_t>
+int staged(bng_ctx *c, u64 n, u64 chunk, std::initializer_list<stage::In> in, std::initializer_list<stage::Out> out, Launch launch,
+           Done chunk_done = nullptr) {
+    int r = 0;
+    auto bufs = [&](size_t bytes, u8 **dev, u8 **host) {
+        if ((r = ensure_io(c, bytes)) != 0) return false;
+        *dev = c->io_dev, *host = c->io_host;
+        return true;
+    };
+    const cudaError_t e = stage::round_trip(n, chunk, in, out, c->L.stream, bufs, launch, chunk_done);
+    if (r) return r;
+    return e == cudaSuccess ? 0 : fail(c, -EIO, "staging: %s", cudaGetErrorString(e));
 }
 
 MapReg *get_map(bng_ctx *c, int id) {
@@ -431,36 +461,26 @@ bool nd_bad_config(const u8 *v) {
 // ---- control-plane commands on hash maps ----
 int hash_cmd(bng_ctx *c, MapReg *m, int op, const void *keys, void *vals, u64 n, u32 flags, int *first_err, u64 *n_err = nullptr) {
     const Tbl &t = *m->tbl;
-    const u64 chunk_max = 1u << 18;
+    const bool upd = op == TOP_UPDATE, look = op == TOP_LOOKUP;
+    const int role = dir_role(c, m->tbl);
     *first_err = 0;
-    for (u64 done = 0; done < n; done += chunk_max) {
-        u64 k = std::min(chunk_max, n - done);
-        size_t kb = k * t.key_size, vb = k * t.value_size, rb = k * 4;
-        size_t koff = 0, voff = (kb + 255) & ~(size_t)255, roff = (voff + vb + 255) & ~(size_t)255;
-        int r = ensure_io(c, roff + rb);
-        if (r) return r;
-        memcpy(c->io_host + koff, (const u8 *)keys + done * t.key_size, kb);
-        if (op == TOP_UPDATE) memcpy(c->io_host + voff, (const u8 *)vals + done * t.value_size, vb);
-        size_t up = op == TOP_UPDATE ? voff + vb : kb;
-        CU(c, cudaMemcpyAsync(c->io_dev, c->io_host, up, cudaMemcpyHostToDevice, c->L.stream));
-        const int role = m->tbl == &c->dev.sub_nat ? 1 : (m->tbl == &c->dev.qos_in ? 2 : 0);
-        CU(c, run_table_op(c->L, t, op, c->io_dev + koff, c->io_dev + voff, (int *)(c->io_dev + roff), k, flags, c->dev.subdir,
-                           role, c->acct, c->idle));
-        size_t dfrom = op == TOP_LOOKUP ? voff : roff;
-        CU(c, cudaMemcpyAsync(c->io_host + dfrom, c->io_dev + dfrom, roff + rb - dfrom, cudaMemcpyDeviceToHost, c->L.stream));
-        CU(c, cudaStreamSynchronize(c->L.stream));
-        const int *res = (const int *)(c->io_host + roff);
+    // columns: keys, update's values | lookup's values, results
+    auto launch = [&](u8 *const *d, u64 k) {
+        return run_table_op(c->L, t, op, d[0], upd ? d[1] : d[2], (int *)d[3], k, flags, c->dev.subdir, role, c->acct, c->idle);
+    };
+    auto chunk_done = [&](const u8 *const *h, u64 done, u64 k) {
+        const int *res = (const int *)h[3];
         for (u64 i = 0; i < k; i++)
             if (res[i]) {
                 if (!*first_err) *first_err = res[i];
                 if (n_err) ++*n_err;
+            } else if (look) { // a miss leaves the caller's value as it was
+                memcpy((u8 *)vals + (done + i) * t.value_size, h[2] + i * t.value_size, t.value_size);
             }
-        if (op == TOP_LOOKUP) {
-            for (u64 i = 0; i < k; i++)
-                if (!res[i])
-                    memcpy((u8 *)vals + (done + i) * t.value_size, c->io_host + voff + i * t.value_size, t.value_size);
-        }
-    }
+    };
+    if (int r = staged(c, n, 1u << 18, {{keys, t.key_size}, {upd ? vals : nullptr, upd ? t.value_size : 0}},
+                       {{nullptr, look ? t.value_size : 0}, {nullptr, 4}}, launch, chunk_done))
+        return r;
     if (m->tbl == &c->v6 && op != TOP_LOOKUP) return v6_refresh_locked(c);
     if (m->tbl == &c->d6b && op != TOP_LOOKUP) return d6_refresh_locked(c);
     if (m->tbl == &c->ndb && op != TOP_LOOKUP) return nd_refresh_locked(c);
@@ -1061,8 +1081,7 @@ int bng_map_clear(bng_ctx *c, int map) {
     if (m->tbl == &c->v6) c->v6_live = 0;
     if (m->tbl == &c->d6b) c->d6_live = 0;
     if (m->tbl == &c->ndb) c->nd_live = 0;
-    if (m->tbl == &c->dev.sub_nat || m->tbl == &c->dev.qos_in)
-        CU(c, run_dir_clear_half(c->L, c->dev.subdir, m->tbl == &c->dev.sub_nat ? 1 : 2));
+    if (const int role = dir_role(c, m->tbl)) CU(c, run_dir_clear_half(c->L, c->dev.subdir, role));
     CU(c, cudaStreamSynchronize(c->L.stream));
     if (feeds_small_tabs(m)) c->small_dirty = true;
     return 0;
@@ -1717,8 +1736,7 @@ int bng_nat_flush(bng_ctx *c, const uint32_t *addrs, uint64_t n, uint64_t now_ns
     std::lock_guard<std::mutex> g(c->mu);
     cudaSetDevice(c->device);
     if (n == 0) return flush_staged_locked(c, -1);
-    u64 slots = 64;
-    while (slots < 2 * n) slots *= 2;
+    const u64 slots = aset_slots(n);
     if (slots > (1ull << 32)) return fail(c, -EINVAL, "nat_flush: %llu addresses", (unsigned long long)n);
     int r = flow_pass_begin_locked(c);
     if (r) return r;
@@ -1726,11 +1744,7 @@ int bng_nat_flush(bng_ctx *c, const uint32_t *addrs, uint64_t n, uint64_t now_ns
     u64 *set = (u64 *)c->io_host.get();
     memset(set, 0, slots * 8);
     const u32 mask = (u32)(slots - 1);
-    for (u64 k = 0; k < n; k++) {
-        u32 i = aset_home(addrs[k], mask);
-        while (set[i] && (u32)set[i] != addrs[k]) i = (i + 1) & mask;
-        set[i] = ADDRSET_LIVE | addrs[k];
-    }
+    for (u64 k = 0; k < n; k++) aset_insert(set, mask, addrs[k]);
     CU(c, cudaMemcpyAsync(c->io_dev, c->io_host, slots * 8, cudaMemcpyHostToDevice, c->L.stream));
     u32 *cnt = c->L.s.counters + 8; // scratch words 8.. are free between program runs
     CU(c, cudaMemsetAsync(cnt, 0, 16, c->L.stream));
@@ -1830,20 +1844,12 @@ static int acct_flush_locked(bng_ctx *c) {
 static int64_t acct_dump_locked(bng_ctx *c, uint32_t *addrs_out, bng_acct *out, uint64_t cap) {
     if (cap == 0) return 0;
     const u64 ecap = std::min<u64>(cap, (u64)c->dev.subdir.mask + 1); // no more entries than slots
-    const size_t aoff = ecap * sizeof(bng_acct), coff = (aoff + ecap * 4 + 15) & ~(size_t)15, need = coff + 16;
+    const size_t need = stage::Dump(ecap, sizeof(bng_acct)).l.end;
     if (!c->acct_dump_buf.grow(need)) return grow_failed(c, "acct_dump", need);
-    u8 *buf = c->acct_dump_buf;
-    u32 *cnt = (u32 *)(buf + coff), n = 0;
-    CU(c, cudaMemsetAsync(cnt, 0, 4, c->L.stream));
-    CU(c, run_acct_dump(c->L, c->dev.subdir, c->acct, (u32 *)(buf + aoff), (u64 *)buf, cnt, ecap));
-    CU(c, cudaMemcpyAsync(&n, cnt, 4, cudaMemcpyDeviceToHost, c->L.stream));
-    CU(c, cudaStreamSynchronize(c->L.stream));
-    const u64 got = std::min<u64>(n, ecap);
-    if (got) {
-        CU(c, cudaMemcpy(out, buf, got * sizeof(bng_acct), cudaMemcpyDeviceToHost));
-        CU(c, cudaMemcpy(addrs_out, buf + aoff, got * 4, cudaMemcpyDeviceToHost));
-    }
-    return (int64_t)got;
+    auto launch = [&](u8 *recs, u32 *addrs, u32 *cnt) { return run_acct_dump(c->L, c->dev.subdir, c->acct, addrs, (u64 *)recs, cnt, ecap); };
+    u32 n = 0;
+    CU(c, stage::counted_dump(c->acct_dump_buf, ecap, sizeof(bng_acct), out, addrs_out, &n, c->L.stream, launch));
+    return (int64_t)std::min<u64>(n, ecap);
 }
 
 int bng_acct_enable(bng_ctx *c, int prog, int on) {
@@ -1865,20 +1871,9 @@ int bng_acct_read(bng_ctx *c, const uint32_t *addrs, uint64_t n, bng_acct *out, 
     std::lock_guard<std::mutex> g(c->mu);
     cudaSetDevice(c->device);
     if (int fr = acct_flush_locked(c)) return fr;
-    const u64 chunk_max = 1u << 16;
-    for (u64 done = 0; done < n; done += chunk_max) {
-        const u64 k = std::min(chunk_max, n - done);
-        const size_t ooff = (k * 4 + 255) & ~(size_t)255, roff = ooff + k * sizeof(bng_acct);
-        if (int r = ensure_io(c, roff + k * 4)) return r;
-        memcpy(c->io_host, addrs + done, k * 4);
-        CU(c, cudaMemcpyAsync(c->io_dev, c->io_host, k * 4, cudaMemcpyHostToDevice, c->L.stream));
-        CU(c, run_acct_read(c->L, c->dev.subdir, c->acct, (const u32 *)c->io_dev.get(), k, (u64 *)(c->io_dev + ooff), (int *)(c->io_dev + roff)));
-        CU(c, cudaMemcpyAsync(c->io_host + ooff, c->io_dev + ooff, roff + k * 4 - ooff, cudaMemcpyDeviceToHost, c->L.stream));
-        CU(c, cudaStreamSynchronize(c->L.stream));
-        memcpy(out + done, c->io_host + ooff, k * sizeof(bng_acct));
-        memcpy(results + done, c->io_host + roff, k * 4);
-    }
-    return 0;
+    return staged(c, n, 1u << 16, {{addrs, 4}}, {{out, sizeof(bng_acct)}, {results, 4}}, [&](u8 *const *d, u64 k) {
+        return run_acct_read(c->L, c->dev.subdir, c->acct, (const u32 *)d[0], k, (u64 *)d[1], (int *)d[2]);
+    });
 }
 
 int64_t bng_acct_dump(bng_ctx *c, uint32_t *addrs_out, bng_acct *out, uint64_t cap) {
@@ -1914,39 +1909,16 @@ static int idle_restart_locked(bng_ctx *c) {
 // timeouts of n addresses from host memory, chunked through the staging buffers; results may be nullptr
 static int idle_timeouts_locked(bng_ctx *c, const uint32_t *addrs, const uint32_t *timeouts, uint64_t n, int32_t *results) {
     if (int r = idle_alloc_locked(c)) return r;
-    const u64 chunk_max = 1u << 18;
-    for (u64 done = 0; done < n; done += chunk_max) {
-        const u64 k = std::min(chunk_max, n - done);
-        const size_t toff = (k * 4 + 255) & ~(size_t)255, roff = toff * 2;
-        if (int r = ensure_io(c, roff + k * 4)) return r;
-        memcpy(c->io_host, addrs + done, k * 4);
-        memcpy(c->io_host + toff, timeouts + done, k * 4);
-        CU(c, cudaMemcpyAsync(c->io_dev, c->io_host, toff + k * 4, cudaMemcpyHostToDevice, c->L.stream));
-        CU(c, run_idle_timeout_set(c->L, c->dev.subdir, c->idle, (const u32 *)c->io_dev.get(), (const u32 *)(c->io_dev + toff), k,
-                                   (int *)(c->io_dev + roff)));
-        if (results) CU(c, cudaMemcpyAsync(c->io_host + roff, c->io_dev + roff, k * 4, cudaMemcpyDeviceToHost, c->L.stream));
-        CU(c, cudaStreamSynchronize(c->L.stream));
-        if (results) memcpy(results + done, c->io_host + roff, k * 4);
-    }
-    return 0;
+    return staged(c, n, 1u << 18, {{addrs, 4}, {timeouts, 4}}, {{results, 4}}, [&](u8 *const *d, u64 k) {
+        return run_idle_timeout_set(c->L, c->dev.subdir, c->idle, (const u32 *)d[0], (const u32 *)d[1], k, (int *)d[2]);
+    });
 }
 
 // records of n addresses from host memory, chunked through the staging buffers
 static int idle_read_locked(bng_ctx *c, const uint32_t *addrs, uint64_t n, bng_idle *out, int32_t *results) {
-    const u64 chunk_max = 1u << 16;
-    for (u64 done = 0; done < n; done += chunk_max) {
-        const u64 k = std::min(chunk_max, n - done);
-        const size_t ooff = (k * 4 + 255) & ~(size_t)255, roff = ooff + k * sizeof(bng_idle);
-        if (int r = ensure_io(c, roff + k * 4)) return r;
-        memcpy(c->io_host, addrs + done, k * 4);
-        CU(c, cudaMemcpyAsync(c->io_dev, c->io_host, k * 4, cudaMemcpyHostToDevice, c->L.stream));
-        CU(c, run_idle_read(c->L, c->dev.subdir, c->idle, (const u32 *)c->io_dev.get(), k, (u64 *)(c->io_dev + ooff), (int *)(c->io_dev + roff)));
-        CU(c, cudaMemcpyAsync(c->io_host + ooff, c->io_dev + ooff, roff + k * 4 - ooff, cudaMemcpyDeviceToHost, c->L.stream));
-        CU(c, cudaStreamSynchronize(c->L.stream));
-        memcpy(out + done, c->io_host + ooff, k * sizeof(bng_idle));
-        memcpy(results + done, c->io_host + roff, k * 4);
-    }
-    return 0;
+    return staged(c, n, 1u << 16, {{addrs, 4}}, {{out, sizeof(bng_idle)}, {results, 4}}, [&](u8 *const *d, u64 k) {
+        return run_idle_read(c->L, c->dev.subdir, c->idle, (const u32 *)d[0], k, (u64 *)d[1], (int *)d[2]);
+    });
 }
 
 // (address, timeout) of every record, by address, for the snapshot: the directory's addresses (k_acct_dump lists them
@@ -2009,19 +1981,13 @@ int64_t bng_idle_scan(bng_ctx *c, uint64_t now_ns, uint32_t default_s, uint32_t 
     if (int fr = acct_flush_locked(c)) return fr;
     if (!c->idle) return 0; // no record exists yet: nobody can be idle
     const u64 ecap = std::min<u64>(cap, (u64)c->dev.subdir.mask + 1); // no more entries than slots
-    const size_t aoff = ecap * sizeof(bng_idle), coff = (aoff + ecap * 4 + 15) & ~(size_t)15, need = coff + 16;
+    const size_t need = stage::Dump(ecap, sizeof(bng_idle)).l.end;
     if (!c->idle_scan_buf.grow(need)) return grow_failed(c, "idle_scan", need);
-    u8 *buf = c->idle_scan_buf;
-    u32 *cnt = (u32 *)(buf + coff), n = 0;
-    CU(c, cudaMemsetAsync(cnt, 0, 4, c->L.stream));
-    CU(c, run_idle_scan(c->L, c->dev.subdir, c->idle, now_ns, default_s, flags, (u32 *)(buf + aoff), (u64 *)buf, cnt, ecap));
-    CU(c, cudaMemcpyAsync(&n, cnt, 4, cudaMemcpyDeviceToHost, c->L.stream));
-    CU(c, cudaStreamSynchronize(c->L.stream));
-    const u64 got = std::min<u64>(n, ecap);
-    if (got) {
-        CU(c, cudaMemcpy(out, buf, got * sizeof(bng_idle), cudaMemcpyDeviceToHost));
-        CU(c, cudaMemcpy(addrs_out, buf + aoff, got * 4, cudaMemcpyDeviceToHost));
-    }
+    auto launch = [&](u8 *recs, u32 *addrs, u32 *cnt) {
+        return run_idle_scan(c->L, c->dev.subdir, c->idle, now_ns, default_s, flags, addrs, (u64 *)recs, cnt, ecap);
+    };
+    u32 n = 0;
+    CU(c, stage::counted_dump(c->idle_scan_buf, ecap, sizeof(bng_idle), out, addrs_out, &n, c->L.stream, launch));
     return (int64_t)n;
 }
 
@@ -2030,12 +1996,6 @@ int64_t bng_idle_scan(bng_ctx *c, uint64_t now_ns, uint32_t default_s, uint32_t 
 // ---------------------------------------------------------------------------
 static_assert(sizeof(bng_nat_sub_use) == 64 && sizeof(bng_nat_pub_use) == 64, "the census writes 16 u32 per record");
 static_assert(sizeof(bng_nat_usage_sum) == (NU_PUBS_FOUND + 1) * 8, "struct bng_nat_usage_sum is the head of the census's sum words");
-
-static u64 nu_pow2(u64 v) {
-    u64 p = 64;
-    while (p < v) p <<= 1;
-    return p;
-}
 
 // the public-address table: pub_mask + 1 slots
 static int nu_pub_alloc(bng_ctx *c, u64 slots) {
@@ -2050,7 +2010,7 @@ static int nu_pub_alloc(bng_ctx *c, u64 slots) {
 static int nu_alloc_locked(bng_ctx *c) {
     if (c->nu_sum) return 0;
     const u64 keys = 4ull * ((u64)c->dev.sessions.max_entries + c->dev.eim.max_entries);
-    const u64 set_slots = nu_pow2((keys * 4 + 2) / 3);
+    const u64 set_slots = pow2_slots((keys * 4 + 2) / 3);
     const u64 dir_slots = (u64)c->dev.subdir.mask + 1;
     if (set_slots > (1ull << 30) || dir_slots > (1ull << 30))
         return fail(c, -ENOMEM, "nat_usage: %llu set slots / %llu directory slots exceed 2^30", (unsigned long long)set_slots,
@@ -2097,7 +2057,7 @@ int bng_nat_usage(bng_ctx *c, uint32_t min_permille, bng_nat_usage_sum *sum, uin
         if (sum_w[NU_SET_FULL]) return fail(c, -EIO, "nat_usage: the triple set is full");
         if (sum_w[NU_OVERFLOW]) { // more public addresses than half the table: grow it past the reservations and count again
             prof_collect(c->L);
-            if ((r = nu_pub_alloc(c, nu_pow2(2 * sum_w[NU_PUB_RESERVED]))) != 0) return r;
+            if ((r = nu_pub_alloc(c, pow2_slots(2 * sum_w[NU_PUB_RESERVED]))) != 0) return r;
             continue;
         }
         CU(c, run_nat_usage_emit(c->L, c->dev, u, min_permille));
@@ -2153,7 +2113,7 @@ static int ls_pools_alloc(bng_ctx *c, u64 unk_slots) {
 static int ls_alloc_locked(bng_ctx *c) {
     if (c->ls_sum) return 0;
     const u64 keys = 3ull * ((u64)c->dev.sub_pools.max_entries + c->dev.vlan_pools.max_entries + c->dev.cid_subs.max_entries);
-    const u64 set_slots = nu_pow2((keys * 4 + 2) / 3);
+    const u64 set_slots = pow2_slots((keys * 4 + 2) / 3);
     if (set_slots > (1ull << 32)) return fail(c, -ENOMEM, "lease_census: %llu set slots", (unsigned long long)set_slots);
     if (!devbuf::grow_all({{&c->ls_set, set_slots * 8}, {&c->ls_sum, LS_SUM_WORDS * 8}}))
         return grow_failed(c, "dhcp leases", set_slots * 8 + LS_SUM_WORDS * 8, "census");
@@ -2190,7 +2150,7 @@ int bng_dhcp_lease_census(bng_ctx *c, uint64_t now_ns, bng_lease_sum *sum, uint3
         if (sum_w[LS_SET_FULL]) return fail(c, -EIO, "lease_census: the address set is full");
         if (sum_w[LS_OVERFLOW]) { // more unknown pool_ids than half the hash: grow it past the claims and count again
             prof_collect(c->L);
-            if ((r = ls_pools_alloc(c, nu_pow2(4 * sum_w[LS_UNK_CLAIMED]))) != 0) return r;
+            if ((r = ls_pools_alloc(c, pow2_slots(4 * sum_w[LS_UNK_CLAIMED]))) != 0) return r;
             continue;
         }
         CU(c, run_lease_pools(c->L, c->dev, u));
@@ -2218,7 +2178,7 @@ int64_t bng_dhcp_lease_sweep(bng_ctx *c, uint64_t now_ns, uint32_t grace_s, bng_
     DevCtx &d = c->dev;
     // no more entries can be due than the three maps hold
     const u64 ecap = std::min<u64>(cap, (u64)d.sub_pools.max_entries + d.vlan_pools.max_entries + d.cid_subs.max_entries);
-    const u64 mac_slots = nu_pow2(2 * std::min<u64>(ecap, d.sub_pools.max_entries));
+    const u64 mac_slots = pow2_slots(2 * std::min<u64>(ecap, d.sub_pools.max_entries));
     if (mac_slots > (1ull << 32)) return fail(c, -ENOMEM, "lease_sweep: %llu MAC set slots", (unsigned long long)mac_slots);
     if ((r = ls_out_locked(c, ecap * 64)) != 0) return r;
     if (!c->ls_macs.grow((LS_W_WORDS + mac_slots) * 8)) return grow_failed(c, "dhcp leases", (LS_W_WORDS + mac_slots) * 8, "MAC set");
@@ -2293,17 +2253,11 @@ static int li_alloc_locked(bng_ctx *c, u32 snaplen = 1518, u32 cap = 1u << 15) {
 
 // The device copy of the targets (bng_prog_run, when they changed): an AddrSet of a power of two >= 2n slots.
 static int li_upload_locked(bng_ctx *c) {
-    u32 slots = 64;
-    while (slots < 2 * c->li_targets.size()) slots *= 2;
+    const u32 slots = (u32)aset_slots(c->li_targets.size());
     std::vector<u64> words(slots, 0);
     std::vector<u32> ids(slots, 0);
     const u32 mask = slots - 1;
-    for (const auto &t : c->li_targets) {
-        u32 i = aset_home(t.first, mask);
-        while (words[i]) i = (i + 1) & mask;
-        words[i] = ADDRSET_LIVE | t.first;
-        ids[i] = t.second;
-    }
+    for (const auto &t : c->li_targets) ids[aset_insert(words.data(), mask, t.first)] = t.second;
     // pageable sources: the copies are staged before the calls return, so the vectors may go
     CU(c, cudaMemcpyAsync(c->li_words, words.data(), (size_t)slots * 8, cudaMemcpyHostToDevice, c->L.stream));
     CU(c, cudaMemcpyAsync(c->li_ids, ids.data(), (size_t)slots * 4, cudaMemcpyHostToDevice, c->L.stream));
@@ -2462,28 +2416,15 @@ int records_reset_locked(bng_ctx *c) {
     return 0;
 }
 
-size_t al256(size_t v) { return (v + 255) & ~(size_t)255; }
-
 // n (address, record) pairs into the addresses' directory slots, chunked through the staging buffers: accounting
 // records (rs = sizeof(bng_acct)) or whole idle records (rs = sizeof(bng_idle))
 int load_records_locked(bng_ctx *c, const u8 *addrs, const u8 *recs, u64 n, size_t rs) {
     const bool acct = rs == sizeof(bng_acct);
     if (int r = acct ? acct_alloc_locked(c) : idle_alloc_locked(c)) return r;
-    const u64 chunk_max = 1u << 16;
-    for (u64 done = 0; done < n; done += chunk_max) {
-        const u64 k = std::min(chunk_max, n - done);
-        const size_t roff = al256(k * 4);
-        if (int r = ensure_io(c, roff + k * rs)) return r;
-        memcpy(c->io_host, addrs + done * 4, k * 4);
-        memcpy(c->io_host + roff, recs + done * rs, k * rs);
-        CU(c, cudaMemcpyAsync(c->io_dev, c->io_host, roff + k * rs, cudaMemcpyHostToDevice, c->L.stream));
-        if (acct)
-            CU(c, run_acct_load(c->L, c->dev.subdir, c->acct, (const u32 *)c->io_dev.get(), (const u64 *)(c->io_dev + roff), k));
-        else
-            CU(c, run_idle_load(c->L, c->dev.subdir, c->idle, (const u32 *)c->io_dev.get(), (const u64 *)(c->io_dev + roff), k));
-        CU(c, cudaStreamSynchronize(c->L.stream));
-    }
-    return 0;
+    return staged(c, n, 1u << 16, {{addrs, 4}, {recs, rs}}, {}, [&](u8 *const *d, u64 k) {
+        return acct ? run_acct_load(c->L, c->dev.subdir, c->acct, (const u32 *)d[0], (const u64 *)d[1], k)
+                    : run_idle_load(c->L, c->dev.subdir, c->idle, (const u32 *)d[0], (const u64 *)d[1], k);
+    });
 }
 
 // n (address, target id) pairs into the interception targets; replace: they are the only targets afterwards
@@ -2935,8 +2876,7 @@ int bng_sub_export(bng_ctx *c, const uint32_t *addrs, uint64_t n_addrs, const ui
             if (seen.insert(macs[i]).second) M.push_back(macs[i]);
     }
     const u64 na = A.size(), nm = M.size();
-    u64 slots = 64;
-    while (slots < 2 * na) slots *= 2;
+    const u64 slots = aset_slots(na);
     if (slots > (1ull << 32)) return fail(c, -EINVAL, "sub_export: %llu addresses", (unsigned long long)na);
     const DevCtx &d = c->dev;
     const u64 ns = (u64)d.sessions.mask + 1, nr = (u64)d.reverse.mask + 1, ne = (u64)d.eim.mask + 1, n6s = (u64)c->v6.mask + 1;
@@ -2948,18 +2888,20 @@ int bng_sub_export(bng_ctx *c, const uint32_t *addrs, uint64_t n_addrs, const ui
     MapReg *am[3], *mm[2], *fm[3];
     for (int k = 0; k < 3; k++) am[k] = get_map(c, bng_map_id(c, kMoveAddrMaps[k])), fm[k] = get_map(c, bng_map_id(c, kMoveFlowMaps[k]));
     for (int k = 0; k < 2; k++) mm[k] = get_map(c, bng_map_id(c, kMoveMacMaps[k]));
-    const size_t aoff = al256(slots * 8), moff = al256(aoff + na * 4), coff = al256(moff + nm * 8), out0 = al256(coff + 32);
-    size_t at = out0, am_v[3], am_r[3], mm_v[2], mm_r[2], acct_v = 0, acct_r = 0, idle_v = 0, idle_r = 0;
-    for (int k = 0; k < 3; k++) am_v[k] = at, am_r[k] = al256(at + na * am[k]->value_size), at = al256(am_r[k] + na * 4);
-    for (int k = 0; k < 2; k++) mm_v[k] = at, mm_r[k] = al256(at + nm * mm[k]->value_size), at = al256(mm_r[k] + nm * 4);
-    if (c->acct) acct_v = at, acct_r = al256(at + na * sizeof(bng_acct)), at = al256(acct_r + na * 4);
-    if (c->idle) idle_v = at, idle_r = al256(at + na * sizeof(bng_idle)), at = al256(idle_r + na * 4);
+    stage::Layout l;
+    l.take(slots * 8); // the address set, at 0
+    const size_t aoff = l.take(na * 4), moff = l.take(nm * 8), coff = l.take(32), out0 = l.take(0);
+    size_t am_v[3], am_r[3], mm_v[2], mm_r[2], acct_v = 0, acct_r = 0, idle_v = 0, idle_r = 0;
+    for (int k = 0; k < 3; k++) am_v[k] = l.take(na * am[k]->value_size), am_r[k] = l.take(na * 4);
+    for (int k = 0; k < 2; k++) mm_v[k] = l.take(nm * mm[k]->value_size), mm_r[k] = l.take(nm * 4);
+    if (c->acct) acct_v = l.take(na * sizeof(bng_acct)), acct_r = l.take(na * 4);
+    if (c->idle) idle_v = l.take(na * sizeof(bng_idle)), idle_r = l.take(na * 4);
     // nd_bindings by MAC, only while it has entries: an export from a context that never used it launches nothing more
     MapReg *ndm = get_map(c, bng_map_id(c, "nd_bindings"));
     const bool nd = nm && c->nd_live;
     size_t nd_v = 0, nd_r = 0;
-    if (nd) nd_v = at, nd_r = al256(at + nm * ndm->value_size), at = al256(nd_r + nm * 4);
-    const size_t flow0 = at;
+    if (nd) nd_v = l.take(nm * ndm->value_size), nd_r = l.take(nm * 4);
+    const size_t flow0 = l.end;
     if (cudaError_t e = flow0 > c->mv_buf.size() ? c->mv_buf.grow_keep(with_slack(flow0), 0, c->L.stream) : cudaSuccess)
         return grow_failed(c, "sub_export", with_slack(flow0), nullptr, e);
     // the inputs are built in the pinned staging buffer and copied on the context's stream, ahead of the kernels that
@@ -2969,11 +2911,7 @@ int bng_sub_export(bng_ctx *c, const uint32_t *addrs, uint64_t n_addrs, const ui
     memset(in, 0, out0);
     u64 *set = (u64 *)in;
     const u32 mask = (u32)(slots - 1);
-    for (u32 a : A) {
-        u32 i = aset_home(a, mask);
-        while (set[i]) i = (i + 1) & mask;
-        set[i] = ADDRSET_LIVE | a;
-    }
+    for (u32 a : A) aset_insert(set, mask, a);
     if (na) memcpy(in + aoff, A.data(), na * 4);
     if (nm) memcpy(in + moff, M.data(), nm * 8);
     u8 *dv = c->mv_buf;
@@ -2995,14 +2933,11 @@ int bng_sub_export(bng_ctx *c, const uint32_t *addrs, uint64_t n_addrs, const ui
     CU(c, cudaStreamSynchronize(c->L.stream));
     // the delta exporter's gather turns the slot lists into ABI keys and values
     size_t fk[3], fv[3];
-    at = flow0;
-    for (int k = 0; k < 3; k++) {
-        const Tbl &t = *fm[k]->tbl;
-        fk[k] = at, fv[k] = at + (size_t)n4[k] * t.key_size, at = al256(fv[k] + (size_t)n4[k] * t.value_size);
-    }
+    for (int k = 0; k < 3; k++) fk[k] = l.take((size_t)n4[k] * fm[k]->tbl->key_size), fv[k] = l.take((size_t)n4[k] * fm[k]->tbl->value_size);
     const u32 n6 = n4[4];
-    const size_t v6k = at, v6v = al256(v6k + (size_t)n6 * LPM6_KEY), v6r = al256(v6v + (size_t)n6 * 4); // v6r: the detach's results
-    if (n6) at = al256(v6r + (size_t)n6 * 4);
+    size_t v6k = 0, v6v = 0, v6r = 0; // v6r: the detach's results
+    if (n6) v6k = l.take((size_t)n6 * LPM6_KEY), v6v = l.take((size_t)n6 * 4), v6r = l.take((size_t)n6 * 4);
+    const size_t at = l.end;
     if (cudaError_t e = at > c->mv_buf.size() ? c->mv_buf.grow_keep(with_slack(at), flow0, c->L.stream) : cudaSuccess)
         return grow_failed(c, "sub_export", with_slack(at), nullptr, e);
     dv = c->mv_buf;
@@ -3085,9 +3020,8 @@ int bng_sub_export(bng_ctx *c, const uint32_t *addrs, uint64_t n_addrs, const ui
     if (c->mv_lists) CU(c, run_move_detach(c->L, d, c->mv_lists, n4));
     for (int k = 0; k < 5; k++) {
         MapReg *m = k < 3 ? am[k] : mm[k - 3];
-        const int role = m->tbl == &d.sub_nat ? 1 : (m->tbl == &d.qos_in ? 2 : 0);
         CU(c, run_table_op(c->L, *m->tbl, TOP_DELETE, dv + (k < 3 ? aoff : moff), nullptr, (int *)(dv + (k < 3 ? am_r[k] : mm_r[k - 3])),
-                           k < 3 ? na : nm, 0, d.subdir, role, c->acct, c->idle));
+                           k < 3 ? na : nm, 0, d.subdir, dir_role(c, m->tbl), c->acct, c->idle));
     }
     if (n6) CU(c, run_table_op(c->L, c->v6, TOP_DELETE, dv + v6k, nullptr, (int *)(dv + v6r), n6, 0, d.subdir, 0, nullptr, nullptr));
     if (nd_sec) CU(c, run_table_op(c->L, c->ndb, TOP_DELETE, dv + moff, nullptr, (int *)(dv + nd_r), nm, 0, d.subdir, 0, nullptr, nullptr));
